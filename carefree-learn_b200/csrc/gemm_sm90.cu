@@ -1,15 +1,30 @@
 // Persistent warp-specialised bf16 GEMM for sm_90a:  C[M,N] = A[M,K] * B[N,K]^T  (fp32 accumulate in registers)
 //
-//   warp 8          : TMA producer (cp.async.bulk.tensor -> 128B-swizzled smem ring of 4 stages x (A 16 KB + B 32 KB))
-//   warpgroups 0, 1 : consumers.  Warpgroup c owns rows [64 c, 64 c + 64) of the 128 x 256 tile: wgmma m64n256k16 straight
-//                     from the smem ring (one k-block = 4 instructions), the accumulator (128 fp32 per thread) stays in
-//                     registers, and the fused epilogue reads it from there and writes bf16 / fp32 pairs to global memory.
+//   warpgroups 0, 1 : MMA.  Warpgroup c owns rows [64 c, 64 c + 64) of the 128 x 256 tile: wgmma m64n256k16 straight
+//                     from the smem ring (one k-block = 4 instructions); the accumulator (128 fp32 per thread) stays in
+//                     registers.
+//   TMA producer    : one thread; cp.async.bulk.tensor -> 128B-swizzled smem ring of STAGES x (A 16 KB + B 32 KB).
+//
+// Fused epilogues (every variant but the split-K partials) run on their own warpgroup, overlapped with the next tile's
+// MMAs: at the end of a tile the MMA warpgroups write t = bf16(acc + bias) -- the first thing every such variant computes --
+// into a 64 KB staging tile in shared memory and go straight on to the next tile's k-loop; the epilogue warpgroup reads
+// t back row by row and does the rest (GELU / dual output, fp32 residual, dGELU on h, M / N edges) with 16-byte global
+// accesses.  Roles (384 threads):
+//   warps 0-7   the two MMA warpgroups
+//   warp 8      the TMA producer (lane 0)
+//   warps 9-11  the epilogue
+// ptxas compiles the whole kernel under one register cap (launch bounds: 65536 / 384 -> 168), which the 128-register
+// accumulator plus the wgmma operands need; setmaxnreg cannot raise it, so a 512-thread layout (cap 128) with a full
+// fourth warpgroup does not compile, and at 384 threads every role already fits in the 64K register file.
+// Shared memory: 3 stages (144 KB) + staging (64 KB) + barriers.  The split-K partial variant (wgrad: K per unit is in
+// the thousands, its epilogue a small share) keeps the epilogue in the MMA warpgroups, 4 stages and 288 threads.
 //
 // One wgmma group stays in flight: the stage of k-block i is handed back to the producer once the MMAs of k-block i + 1
 // have been issued and those of k-block i have retired.  Both operands may be K-major (row-major [rows, K]) or MN-major
 // (row-major [K, rows]); the latter is what the backward GEMMs need (dgrad reads W[N,K] with the reduction over N, wgrad
 // reads dY and X with the reduction over tokens) -- wgmma reads either layout through its transpose bits, so no
-// transposed copies are ever materialised.
+// transposed copies are ever materialised.  The majors are template parameters: a runtime choice inside the k-loop
+// makes ptxas fence the accumulator around every branch.
 //
 // This one kernel serves every dense layer on the hot path of the reference's transformer block
 // (SURVEY.md section 2b, K1/K4/K8/K10/K11/K12/K14):
@@ -29,21 +44,29 @@ namespace b200 {
 constexpr int BM = 128;
 constexpr int BN = 256;
 constexpr int BK = 64;
-constexpr int STAGES = 4;
 constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB
 constexpr int B_STAGE_BYTES = BN * BK * 2;  // 32 KB
 constexpr int MN_BOX_BYTES = 64 * BK * 2;   // one MN-major TMA box: 64 (MN) x 64 (K) bf16 = 8 KB
-constexpr int GEMM_THREADS = 288;           // 2 consumer warpgroups + 1 producer warp
-constexpr int SMEM_B_OFF = STAGES * A_STAGE_BYTES;
-constexpr int SMEM_BAR_OFF = SMEM_B_OFF + STAGES * B_STAGE_BYTES;
-constexpr int GEMM_SMEM_USED = SMEM_BAR_OFF + 128;
-constexpr int GEMM_SMEM_BYTES = GEMM_SMEM_USED + 1024;  // + the manual 1 KB alignment of the base
-static_assert(GEMM_SMEM_BYTES <= 232448, "GEMM shared-memory layout does not fit the 227 KB of an H100 SM");
+constexpr int STAGING_ROW_BYTES = BN * 2;   // one bf16 row of the staging tile
+constexpr int STAGING_BYTES = BM * STAGING_ROW_BYTES;  // 64 KB
+
+// Kernel layout by epilogue: OVERLAP = separate epilogue warpgroup (everything but the split-K partials).
+template <int EPI>
+struct GemmCfg {
+    static constexpr bool OVERLAP = EPI != EPI_PARTIAL_F32;
+    static constexpr int STAGES = OVERLAP ? 3 : 4;
+    static constexpr int THREADS = OVERLAP ? 384 : 288;
+    static constexpr int EPI_WARPS = 3;  // warps 9-11
+    static constexpr int B_OFF = STAGES * A_STAGE_BYTES;
+    static constexpr int STAGING_OFF = B_OFF + STAGES * B_STAGE_BYTES;
+    static constexpr int BAR_OFF = STAGING_OFF + (OVERLAP ? STAGING_BYTES : 0);
+    static constexpr int SMEM_BYTES = BAR_OFF + 128 + 1024;  // + the manual 1 KB alignment of the base
+    static_assert(SMEM_BYTES <= 232448, "GEMM shared-memory layout does not fit the 227 KB of an H100 SM");
+};
 
 struct GemmParams {
     int M, N, K;
     int num_m_tiles, num_n_tiles, splits, num_kb;
-    int a_mn, b_mn;  // 1 = MN-major operand
     const __nv_bfloat16* bias;  // [N] bf16 or nullptr
     void* out0;                 // epilogue outputs / aux operand: plain pointers, leading dimension ldo (elements)
     void* out1;
@@ -66,105 +89,137 @@ __device__ __forceinline__ void decode_unit(const GemmParams& p, int u, int& m_t
     kb1 = static_cast<int>((static_cast<long long>(p.num_kb) * (sp + 1)) / p.splits);
 }
 
-// one k-block (BK = 64 = four k16 steps) of this warpgroup's 64 x 256 accumulator
+// one k-block (BK = 64 = four k16 steps) of this warpgroup's 64 x 256 accumulator; scale_d = 0 on a unit's first k-block
+// starts the accumulator from zero (no register zeroing between the wgmma groups)
 template <int TA, int TB>
-__device__ __forceinline__ void mma_kblock(float (&acc)[128], uint32_t a_base, uint32_t b_base) {
+__device__ __forceinline__ void mma_kblock(float (&acc)[128], uint32_t a_base, uint32_t b_base, uint32_t scale_d) {
 #pragma unroll
     for (int kk = 0; kk < BK / 16; ++kk) {
         const uint64_t ad = TA ? make_smem_desc(a_base + kk * 2048, MN_BOX_BYTES, 1024, kSwz128) : make_smem_desc(a_base + kk * 32, 16, 1024, kSwz128);
         const uint64_t bd = TB ? make_smem_desc(b_base + kk * 2048, MN_BOX_BYTES, 1024, kSwz128) : make_smem_desc(b_base + kk * 32, 16, 1024, kSwz128);
-        if constexpr (TA == 0 && TB == 0) wgmma_m64n256k16_ss_t00(acc, ad, bd, 1u);
-        if constexpr (TA == 0 && TB == 1) wgmma_m64n256k16_ss_t01(acc, ad, bd, 1u);
-        if constexpr (TA == 1 && TB == 0) wgmma_m64n256k16_ss_t10(acc, ad, bd, 1u);
-        if constexpr (TA == 1 && TB == 1) wgmma_m64n256k16_ss_t11(acc, ad, bd, 1u);
+        const uint32_t sd = kk == 0 ? scale_d : 1u;
+        if constexpr (TA == 0 && TB == 0) wgmma_m64n256k16_ss_t00(acc, ad, bd, sd);
+        if constexpr (TA == 0 && TB == 1) wgmma_m64n256k16_ss_t01(acc, ad, bd, sd);
+        if constexpr (TA == 1 && TB == 0) wgmma_m64n256k16_ss_t10(acc, ad, bd, sd);
+        if constexpr (TA == 1 && TB == 1) wgmma_m64n256k16_ss_t11(acc, ad, bd, sd);
     }
 }
 
-// Fused epilogue of two horizontally adjacent accumulator elements (row, col), (row, col + 1).  ok0 / ok1: inside [M, N].
+// split-K partial of two horizontally adjacent accumulator elements (row, col), (row, col + 1).  ok0 / ok1: inside [M, N].
+__device__ __forceinline__ void store_partial_pair(const GemmParams& p, int sp, int row, int col, float v0, float v1, bool ok0, bool ok1) {
+    float* dst = reinterpret_cast<float*>(p.out0) + (static_cast<long long>(sp) * p.M + row) * p.ldo + col;
+    if (ok1) *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
+    else if (ok0) dst[0] = v0;
+}
+
+// Fused epilogue of 8 consecutive elements (row, col .. col + 7) of one output row; t = bf16(acc + bias) as 4 bf16 pairs.
+// n_ok: how many of the 8 columns are inside N (8 on every interior chunk).  Element for element the same arithmetic as
+// the per-pair epilogue it replaces, so results are bit-identical.
 template <int EPI, bool QUICK>
-__device__ __forceinline__ void epi_pair(const GemmParams& p, int sp, int row, int col, float v0, float v1, bool ok0, bool ok1) {
-    const long long ldo = p.ldo;
-    const long long off = static_cast<long long>(row) * ldo + col;
-    if constexpr (EPI == EPI_PARTIAL_F32) {
-        float* dst = reinterpret_cast<float*>(p.out0) + static_cast<long long>(sp) * p.M * ldo + off;
-        if (ok1) *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
-        else if (ok0) dst[0] = v0;
-        return;
-    }
-    float b0 = 0.f, b1 = 0.f;
-    if constexpr (EPI != EPI_DGELU_BF16) {
-        if (p.bias != nullptr) {
-            b0 = __bfloat162float(p.bias[col]);
-            if (ok1) b1 = __bfloat162float(p.bias[col + 1]);
-        }
-    }
-    const uint32_t t = pack_bf16x2(v0 + b0, v1 + b1);  // bf16(acc + bias): what every variant consumes
+__device__ __forceinline__ void epi_chunk(const GemmParams& p, int row, int col, const uint32_t (&t)[4], int n_ok) {
+    const long long off = static_cast<long long>(row) * p.ldo + col;
+    uint32_t o[4];  // the bf16 output (out0) of the bf16 variants
     if constexpr (EPI == EPI_BIAS_BF16) {
-        __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.out0) + off;
-        if (ok1) *reinterpret_cast<uint32_t*>(dst) = t;
-        else if (ok0) dst[0] = __ushort_as_bfloat16(static_cast<unsigned short>(t));
+#pragma unroll
+        for (int i = 0; i < 4; ++i) o[i] = t[i];
     } else if constexpr (EPI == EPI_BIAS_GELU_BF16) {
         // out0 = h (rounded pre-activation), out1 = bf16(gelu(h)): GELU sees the ROUNDED h, like eager
-        float g0, g1;
-        if constexpr (!QUICK) {
-            gelu_erf2(bf16lo(t), bf16hi(t), g0, g1);
-        } else {
-            g0 = quick_gelu_bf16(bf16lo(t));
-            g1 = quick_gelu_bf16(bf16hi(t));
+        uint32_t g[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            float g0, g1;
+            if constexpr (!QUICK) {
+                gelu_erf2(bf16lo(t[i]), bf16hi(t[i]), g0, g1);
+            } else {
+                g0 = quick_gelu_bf16(bf16lo(t[i]));
+                g1 = quick_gelu_bf16(bf16hi(t[i]));
+            }
+            g[i] = pack_bf16x2(g0, g1);
+            o[i] = t[i];
         }
-        const uint32_t g = pack_bf16x2(g0, g1);
-        __nv_bfloat16* d0 = reinterpret_cast<__nv_bfloat16*>(p.out0) + off;
         __nv_bfloat16* d1 = reinterpret_cast<__nv_bfloat16*>(p.out1) + off;
-        if (ok1) {
-            *reinterpret_cast<uint32_t*>(d0) = t;
-            *reinterpret_cast<uint32_t*>(d1) = g;
-        } else if (ok0) {
-            d0[0] = __ushort_as_bfloat16(static_cast<unsigned short>(t));
-            d1[0] = __ushort_as_bfloat16(static_cast<unsigned short>(g));
+        if (n_ok == 8) {
+            *reinterpret_cast<uint4*>(d1) = make_uint4(g[0], g[1], g[2], g[3]);
+        } else {
+#pragma unroll
+            for (int e = 0; e < 8; ++e)
+                if (e < n_ok) d1[e] = __ushort_as_bfloat16(static_cast<unsigned short>(g[e >> 1] >> (16 * (e & 1))));
         }
     } else if constexpr (EPI == EPI_BIAS_RESID_F32) {
         // out0(fp32) = aux(fp32) + float(bf16(acc + bias))     (aux may alias out0)
         const float* src = reinterpret_cast<const float*>(p.aux) + off;
         float* dst = reinterpret_cast<float*>(p.out0) + off;
-        if (ok1) {
-            float2 a = *reinterpret_cast<const float2*>(src);
-            a.x += bf16lo(t);
-            a.y += bf16hi(t);
-            *reinterpret_cast<float2*>(dst) = a;
-        } else if (ok0) {
-            dst[0] = src[0] + bf16lo(t);
+        if (n_ok == 8) {
+            float4 a = reinterpret_cast<const float4*>(src)[0];
+            float4 b = reinterpret_cast<const float4*>(src)[1];
+            a.x += bf16lo(t[0]); a.y += bf16hi(t[0]); a.z += bf16lo(t[1]); a.w += bf16hi(t[1]);
+            b.x += bf16lo(t[2]); b.y += bf16hi(t[2]); b.z += bf16lo(t[3]); b.w += bf16hi(t[3]);
+            reinterpret_cast<float4*>(dst)[0] = a;
+            reinterpret_cast<float4*>(dst)[1] = b;
+        } else {
+#pragma unroll
+            for (int e = 0; e < 8; ++e)
+                if (e < n_ok) dst[e] = src[e] + ((e & 1) ? bf16hi(t[e >> 1]) : bf16lo(t[e >> 1]));
         }
     } else {  // EPI_DGELU_BF16: out0 = bf16( float(bf16(acc)) * gelu'(h) ),  h = aux (bf16)
         const __nv_bfloat16* hsrc = reinterpret_cast<const __nv_bfloat16*>(p.aux) + off;
-        uint32_t hw = 0;
-        if (ok1) hw = *reinterpret_cast<const uint32_t*>(hsrc);
-        else if (ok0) hw = static_cast<uint32_t>(__bfloat16_as_ushort(hsrc[0]));
-        uint32_t o;
-        if constexpr (!QUICK) {
-            float g0, g1;
-            gelu_erf_grad2(bf16lo(hw), bf16hi(hw), g0, g1);
-            o = pack_bf16x2(bf16lo(t) * g0, bf16hi(t) * g1);
+        uint32_t hw[4] = {0u, 0u, 0u, 0u};
+        if (n_ok == 8) {
+            const uint4 h = *reinterpret_cast<const uint4*>(hsrc);
+            hw[0] = h.x; hw[1] = h.y; hw[2] = h.z; hw[3] = h.w;
         } else {
-            o = pack_bf16x2(quick_gelu_bf16_grad(bf16lo(hw), bf16lo(t)), quick_gelu_bf16_grad(bf16hi(hw), bf16hi(t)));
+#pragma unroll
+            for (int e = 0; e < 8; ++e)
+                if (e < n_ok) hw[e >> 1] |= static_cast<uint32_t>(__bfloat16_as_ushort(hsrc[e])) << (16 * (e & 1));
         }
-        __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.out0) + off;
-        if (ok1) *reinterpret_cast<uint32_t*>(dst) = o;
-        else if (ok0) dst[0] = __ushort_as_bfloat16(static_cast<unsigned short>(o));
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            if constexpr (!QUICK) {
+                float g0, g1;
+                gelu_erf_grad2(bf16lo(hw[i]), bf16hi(hw[i]), g0, g1);
+                o[i] = pack_bf16x2(bf16lo(t[i]) * g0, bf16hi(t[i]) * g1);
+            } else {
+                o[i] = pack_bf16x2(quick_gelu_bf16_grad(bf16lo(hw[i]), bf16lo(t[i])), quick_gelu_bf16_grad(bf16hi(hw[i]), bf16hi(t[i])));
+            }
+        }
     }
+    if constexpr (EPI != EPI_BIAS_RESID_F32) {
+        __nv_bfloat16* d0 = reinterpret_cast<__nv_bfloat16*>(p.out0) + off;
+        if (n_ok == 8) {
+            *reinterpret_cast<uint4*>(d0) = make_uint4(o[0], o[1], o[2], o[3]);
+        } else {
+#pragma unroll
+            for (int e = 0; e < 8; ++e)
+                if (e < n_ok) d0[e] = __ushort_as_bfloat16(static_cast<unsigned short>(o[e >> 1] >> (16 * (e & 1))));
+        }
+    }
+}
+
+// Staging tile: 128 rows x 256 bf16, 512 B per row; the 16-byte chunk c of row r sits at chunk c ^ (r & 7) of that row.
+// The MMA warpgroups' 4-byte writes (8 rows x 4 lanes per chunk column) and the epilogue's 16-byte row reads (a warp reads
+// one whole row) are both free of bank conflicts.
+__device__ __forceinline__ uint32_t staging_offset(int r, int chunk) {
+    return static_cast<uint32_t>(r) * STAGING_ROW_BYTES + (static_cast<uint32_t>(chunk ^ (r & 7)) << 4);
 }
 
 // QUICK (GELU / dGELU variants only): QuickGELU instead of the exact erf GELU.  A template parameter, not a runtime flag,
 // so the other variants carry none of its registers.
-template <int EPI, bool QUICK = false>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
+// TA / TB: 1 = that operand is MN-major.
+template <int EPI, bool QUICK, int TA, int TB>
+__global__ void __launch_bounds__(GemmCfg<EPI>::THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+    using Cfg = GemmCfg<EPI>;
+    constexpr int STAGES = Cfg::STAGES;
     extern __shared__ uint8_t smem_raw[];
     // 1 KB alignment (the 128B swizzle pattern repeats every 1024 bytes) as an OFFSET from the __shared__ array
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* sA = smem;
-    uint8_t* sB = smem + SMEM_B_OFF;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + SMEM_BAR_OFF);
+    uint8_t* sB = smem + Cfg::B_OFF;
+    uint8_t* staging = smem + Cfg::STAGING_OFF;
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::BAR_OFF);
     uint64_t* empty_bar = full_bar + STAGES;
+    uint64_t* staging_full = empty_bar + STAGES;  // the MMA warpgroups have written a tile's t
+    uint64_t* staging_empty = staging_full + 1;   // the epilogue warpgroup has read it
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -175,9 +230,48 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             mbar_init(&full_bar[i], 1);
             mbar_init(&empty_bar[i], 2);  // one arrival per consumer warpgroup
         }
+        if constexpr (Cfg::OVERLAP) {
+            mbar_init(staging_full, 256);  // every MMA thread, after its own staging writes
+            mbar_init(staging_empty, 32 * Cfg::EPI_WARPS);  // every epilogue thread, after its last staging read of the tile
+        }
         fence_mbar_init();
     }
     __syncthreads();
+
+    if constexpr (Cfg::OVERLAP) {
+        if (warp > 8) {
+            // ===================================== epilogue warps =====================================
+            uint32_t sphase = 0;
+            for (int u = blockIdx.x; u < total_units; u += gridDim.x) {
+                int m_t, n_t, sp, kb0, kb1;
+                decode_unit(p, u, m_t, n_t, sp, kb0, kb1);
+                const int col = n_t * BN + lane * 8;
+                const int n_ok = min(8, max(0, p.N - col));
+                const int rows = min(BM, p.M - m_t * BM);
+                if constexpr (EPI == EPI_DGELU_BF16 || EPI == EPI_BIAS_RESID_F32) {
+                    // pull the tile's aux rows into L2 while its MMAs still run: three warps cannot hide HBM latency alone.
+                    // Rows are 16-byte aligned and padded to ldo >= the 16-byte-rounded width, so no byte past a row is named.
+                    constexpr int eb = EPI == EPI_BIAS_RESID_F32 ? 4 : 2;
+                    const int n0 = n_t * BN;
+                    const uint32_t bytes = static_cast<uint32_t>((min(BN, p.N - n0) * eb + 15) & ~15);
+                    const uint8_t* aux = reinterpret_cast<const uint8_t*>(p.aux);
+                    for (int r = threadIdx.x - 9 * 32; r < rows; r += 32 * Cfg::EPI_WARPS)
+                        bulk_prefetch_l2(aux + (static_cast<long long>(m_t * BM + r) * p.ldo + n0) * eb, bytes);
+                }
+                mbar_wait(staging_full, sphase);
+                // epilogue warp w takes rows w, w + 3, ...: one 512-byte row per warp access, 16 bytes per lane
+#pragma unroll 4
+                for (int r = warp - 9; r < rows; r += Cfg::EPI_WARPS) {
+                    const uint4 v = *reinterpret_cast<const uint4*>(staging + staging_offset(r, lane));
+                    const uint32_t t[4] = {v.x, v.y, v.z, v.w};
+                    if (n_ok > 0) epi_chunk<EPI, QUICK>(p, m_t * BM + r, col, t, n_ok);
+                }
+                mbar_arrive(staging_empty);
+                sphase ^= 1u;
+            }
+            return;
+        }
+    }
 
     if (warp == 8) {
         // ===================================== TMA producer =====================================
@@ -202,7 +296,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                         const int hw = p.conv_h * p.conv_w;
                         const int bimg = m0 / hw, y0 = (m0 - bimg * hw) / p.conv_w;
                         tma_load_4d(a_dst, &tmA, &full_bar[stage], c0, kx - 1, y0 + ky - 1, bimg);
-                    } else if (!p.a_mn) {
+                    } else if constexpr (!TA) {
                         tma_load_2d(a_dst, &tmA, &full_bar[stage], kb * BK, m0);
                     } else {
 #pragma unroll
@@ -222,7 +316,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                             // (boxes past N = 9 Cin: tap >= 9 lands outside the image -> zero fill, bytes still credited)
                             tma_load_4d(b_dst + i * MN_BOX_BYTES, &tmB, &full_bar[stage], c0, kx - 1, tap < 9 ? y0 + ky - 1 : -65536, bimg);
                         }
-                    } else if (!p.b_mn) {
+                    } else if constexpr (!TB) {
                         tma_load_2d(b_dst, &tmB, &full_bar[stage], kb * BK, n0);
                     } else {
 #pragma unroll
@@ -236,33 +330,25 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         return;
     }
 
-    // ===================================== consumer warpgroups ==================================
+    // ===================================== MMA warpgroups ==================================
     const int wg = warp >> 2;        // 0 / 1: which 64-row half of the tile
     const int wq = warp & 3;         // warp inside the warpgroup: 16 accumulator rows each
     const bool leader = (threadIdx.x & 127) == 0;
     // a K-major A tile is 128 rows of 128 B, an MN-major one two 8 KB boxes of 64 rows: the half starts 8 KB in either way
     const uint32_t a_half = static_cast<uint32_t>(wg) * 8192u;
     int stage = 0;
-    uint32_t phase = 0;
+    uint32_t phase = 0, sphase = 0;
     for (int u = blockIdx.x; u < total_units; u += gridDim.x) {
         int m_t, n_t, sp, kb0, kb1;
         decode_unit(p, u, m_t, n_t, sp, kb0, kb1);
         float acc[128];
-#pragma unroll
-        for (int i = 0; i < 128; ++i) acc[i] = 0.f;
         int prev = -1;
         for (int kb = kb0; kb < kb1; ++kb) {
             mbar_wait(&full_bar[stage], phase);
             const uint32_t a_base = smem_u32(sA + stage * A_STAGE_BYTES) + a_half;
             const uint32_t b_base = smem_u32(sB + stage * B_STAGE_BYTES);
             wgmma_fence();
-            if (p.a_mn) {
-                if (p.b_mn) mma_kblock<1, 1>(acc, a_base, b_base);
-                else mma_kblock<1, 0>(acc, a_base, b_base);
-            } else {
-                if (p.b_mn) mma_kblock<0, 1>(acc, a_base, b_base);
-                else mma_kblock<0, 0>(acc, a_base, b_base);
-            }
+            mma_kblock<TA, TB>(acc, a_base, b_base, kb == kb0 ? 0u : 1u);
             wgmma_commit();
             wgmma_wait<1>();  // the k-block before this one has been read completely: its stage goes back to the producer
             if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
@@ -273,25 +359,42 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         reg_fence(acc);
         if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
 
-        // ---- epilogue straight from the accumulator fragment ----
-        const int row0 = m_t * BM + wg * 64 + wq * 16 + (lane >> 2);
+        const int rl = wg * 64 + wq * 16 + (lane >> 2);  // accumulator rows rl, rl + 8 of the tile
         const int colq = n_t * BN + (lane & 3) * 2;
-        const bool interior = (m_t * BM + BM <= p.M) && (n_t * BN + BN <= p.N);
-        if (interior) {
+        if constexpr (Cfg::OVERLAP) {
+            // ---- handoff: t = bf16(acc + bias) into the staging tile, the rest on the epilogue warpgroup ----
+            mbar_wait(staging_empty, sphase ^ 1u);
 #pragma unroll
             for (int j = 0; j < 32; ++j) {
-                epi_pair<EPI, QUICK>(p, sp, row0, colq + j * 8, acc[4 * j], acc[4 * j + 1], true, true);
-                epi_pair<EPI, QUICK>(p, sp, row0 + 8, colq + j * 8, acc[4 * j + 2], acc[4 * j + 3], true, true);
+                const int col = colq + j * 8;
+                float b0 = 0.f, b1 = 0.f;
+                if constexpr (EPI != EPI_DGELU_BF16) {
+                    if (p.bias != nullptr) {
+                        if (col < p.N) b0 = __bfloat162float(p.bias[col]);
+                        if (col + 1 < p.N) b1 = __bfloat162float(p.bias[col + 1]);
+                    }
+                }
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const uint32_t t = pack_bf16x2(acc[4 * j + 2 * h] + b0, acc[4 * j + 2 * h + 1] + b1);
+                    *reinterpret_cast<uint32_t*>(staging + staging_offset(rl + h * 8, j) + (lane & 3) * 4) = t;
+                }
             }
+            mbar_arrive(staging_full);
+            sphase ^= 1u;
         } else {
+            // ---- split-K partials straight from the accumulator fragment ----
+            const int row0 = m_t * BM + rl;
+            const bool interior = (m_t * BM + BM <= p.M) && (n_t * BN + BN <= p.N);
 #pragma unroll
             for (int j = 0; j < 32; ++j) {
                 const int col = colq + j * 8;
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                     const int row = row0 + h * 8;
-                    const bool rok = row < p.M;
-                    epi_pair<EPI, QUICK>(p, sp, row, col, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], rok && col < p.N, rok && col + 1 < p.N);
+                    const bool rok = interior || row < p.M;
+                    store_partial_pair(p, sp, row, col, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], rok && (interior || col < p.N),
+                                       rok && (interior || col + 1 < p.N));
                 }
             }
         }
@@ -392,29 +495,51 @@ extern "C" int b200_set_persistent_ctas(int n, int launches) {
 // only recorded and returned.
 static int g_gemm_multicast = 0;
 
-template <int EPI, bool QUICK>
+template <int EPI, bool QUICK, int TA, int TB>
 static int launch_gemm_impl(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int grid, cudaStream_t stream) {
+    using Cfg = GemmCfg<EPI>;
     static bool configured[64] = {};  // the opt-in to > 48 KB of dynamic shared memory is per function AND per device
     cudaError_t e;
     const int dev = current_device_slot();
     if (!configured[dev]) {
-        e = cudaFuncSetAttribute(gemm_bf16_kernel<EPI, QUICK>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM_BYTES);
+        e = cudaFuncSetAttribute(gemm_bf16_kernel<EPI, QUICK, TA, TB>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
         if (e != cudaSuccess) return set_error(B200_ERR_LAUNCH, cudaGetErrorString(e));
         configured[dev] = true;
     }
-    gemm_bf16_kernel<EPI, QUICK><<<grid, GEMM_THREADS, GEMM_SMEM_BYTES, stream>>>(tmA, tmB, p);
+    gemm_bf16_kernel<EPI, QUICK, TA, TB><<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
     e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(B200_ERR_LAUNCH, cudaGetErrorString(e));
     count_launch(1);
     return 0;
 }
 
+// Operand majors each epilogue is compiled for: (0,0) forward and conv, (0,1) dgrad, (1,1) wgrad, conv wgrad and CLIP's db.
+// The plain bias epilogue takes all four (ops.gemm's general form).
+template <int EPI, int TA, int TB>
+constexpr bool kHasMajors = EPI == EPI_BIAS_BF16 ||
+                            (TA == 0 && TB == 0 && (EPI == EPI_BIAS_GELU_BF16 || EPI == EPI_BIAS_RESID_F32)) ||
+                            (TA == 0 && TB == 1 && EPI == EPI_DGELU_BF16) || (TA == 1 && TB == 1 && EPI == EPI_PARTIAL_F32);
+
+template <int EPI, bool QUICK, int TA, int TB>
+static int launch_majors(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int grid, cudaStream_t stream) {
+    if constexpr (kHasMajors<EPI, TA, TB>) return launch_gemm_impl<EPI, QUICK, TA, TB>(tmA, tmB, p, grid, stream);
+    else return set_error(B200_ERR_ARG, "gemm: operand majors not supported by this epilogue");
+}
+
+template <int EPI, bool QUICK>
+static int launch_quick(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int a_mn, int b_mn, int grid,
+                        cudaStream_t stream) {
+    if (!a_mn) return b_mn ? launch_majors<EPI, QUICK, 0, 1>(tmA, tmB, p, grid, stream) : launch_majors<EPI, QUICK, 0, 0>(tmA, tmB, p, grid, stream);
+    return b_mn ? launch_majors<EPI, QUICK, 1, 1>(tmA, tmB, p, grid, stream) : launch_majors<EPI, QUICK, 1, 0>(tmA, tmB, p, grid, stream);
+}
+
 template <int EPI>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int grid, cudaStream_t stream) {
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int a_mn, int b_mn, int grid,
+                       cudaStream_t stream) {
     if constexpr (EPI == EPI_BIAS_GELU_BF16 || EPI == EPI_DGELU_BF16) {
-        if (p.act != 0) return launch_gemm_impl<EPI, true>(tmA, tmB, p, grid, stream);
+        if (p.act != 0) return launch_quick<EPI, true>(tmA, tmB, p, a_mn, b_mn, grid, stream);
     }
-    return launch_gemm_impl<EPI, false>(tmA, tmB, p, grid, stream);
+    return launch_quick<EPI, false>(tmA, tmB, p, a_mn, b_mn, grid, stream);
 }
 
 }  // namespace b200
@@ -525,23 +650,22 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
     p.num_n_tiles = (N + BN - 1) / BN;
     p.splits = splits;
     p.num_kb = num_kb;
-    p.a_mn = a_mn_major ? 1 : 0;
-    p.b_mn = b_mn_major ? 1 : 0;
     p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
     p.out0 = out0;
     p.out1 = out1;
     p.aux = aux;
     p.ldo = ldo;
     const long long units = static_cast<long long>(p.num_m_tiles) * p.num_n_tiles * splits;
+    const int a_mn = a_mn_major ? 1 : 0, b_mn = b_mn_major ? 1 : 0;
     int grid = persistent_ctas();
     if (max_ctas > 0 && max_ctas < grid) grid = max_ctas;
     if (units < grid) grid = static_cast<int>(units);
     switch (epilogue) {
-        case EPI_BIAS_BF16: return launch_gemm<EPI_BIAS_BF16>(tmA, tmB, p, grid, stream);
-        case EPI_BIAS_GELU_BF16: return launch_gemm<EPI_BIAS_GELU_BF16>(tmA, tmB, p, grid, stream);
-        case EPI_BIAS_RESID_F32: return launch_gemm<EPI_BIAS_RESID_F32>(tmA, tmB, p, grid, stream);
-        case EPI_DGELU_BF16: return launch_gemm<EPI_DGELU_BF16>(tmA, tmB, p, grid, stream);
-        case EPI_PARTIAL_F32: return launch_gemm<EPI_PARTIAL_F32>(tmA, tmB, p, grid, stream);
+        case EPI_BIAS_BF16: return launch_gemm<EPI_BIAS_BF16>(tmA, tmB, p, a_mn, b_mn, grid, stream);
+        case EPI_BIAS_GELU_BF16: return launch_gemm<EPI_BIAS_GELU_BF16>(tmA, tmB, p, a_mn, b_mn, grid, stream);
+        case EPI_BIAS_RESID_F32: return launch_gemm<EPI_BIAS_RESID_F32>(tmA, tmB, p, a_mn, b_mn, grid, stream);
+        case EPI_DGELU_BF16: return launch_gemm<EPI_DGELU_BF16>(tmA, tmB, p, a_mn, b_mn, grid, stream);
+        case EPI_PARTIAL_F32: return launch_gemm<EPI_PARTIAL_F32>(tmA, tmB, p, a_mn, b_mn, grid, stream);
         default: return set_error(B200_ERR_ARG, "gemm: unknown epilogue");
     }
 }

@@ -55,6 +55,9 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
     return ok != 0;
 }
 // Bounded wait: a protocol bug traps (launch fails with an error) instead of hanging the GPU.
+// The wait must stay free of function calls: it sits between wgmma groups in the consumer k-loops, and any call there
+// (printf is one) makes ptxas serialise every wgmma of the kernel (warning C7510; csrc/Makefile fails the build on it).
+// B200_MBAR_TIMEOUT_PRINTF reports which block / thread timed out, for debugging builds only.
 #ifndef B200_MBAR_TIMEOUT_CYCLES
 #define B200_MBAR_TIMEOUT_CYCLES (4000000000ll)  // ~2 s at 1.98 GHz
 #endif
@@ -64,7 +67,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     uint32_t spins = 0;
     while (!mbar_try_wait(bar, parity)) {
         if ((++spins & 0x3ffu) == 0u && (clock64() - t0) > B200_MBAR_TIMEOUT_CYCLES) {
+#ifdef B200_MBAR_TIMEOUT_PRINTF
             printf("b200: mbarrier timeout block %d thread %d parity %u\n", blockIdx.x, threadIdx.x, parity);
+#endif
             __trap();
         }
     }
