@@ -47,6 +47,9 @@ SIGNATURES: Dict[str, Any] = {
     "b200_set_attention_bwd_version": (c_int, [c_int]),
     "b200_set_attention_prefetch": (c_int, [c_int]),
     "b200_attention_bwd": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_float, c_int, _P, _P]),
+    "b200_attention_long_fwd": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_float, c_int, _P]),
+    "b200_attention_long_bwd_workspace_floats": (_LL, [c_int, c_int, c_int]),
+    "b200_attention_long_bwd": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_float, c_int, _P, _P, _P]),
     "b200_fcnn_step": (
         c_int,
         [_P, _P, _P, _P, _P, _P, c_int, c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int), c_int, c_int, c_float, c_float,

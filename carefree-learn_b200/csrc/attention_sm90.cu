@@ -5,7 +5,8 @@
 //   F.scaled_dot_product_attention (via sdp_attn)               cflearn/toolkit.py:911-974
 //   output.transpose(1,2).contiguous()                          cflearn/modules/core/attentions.py:270
 // and their autograd.  T <= 256 (197 for ViT-B/16, 50 / 77 for CLIP) so every K / V tile of a head fits in shared memory
-// at once: no online-softmax rescaling is needed and a warpgroup holds whole score rows in registers.
+// at once: no online-softmax rescaling is needed and a warpgroup holds whole score rows in registers.  Longer sequences (up
+// to 16384) go to the streamed kernels at the end of this file (attn_long_*), which reuse these helpers.
 //
 // Every product is a warpgroup MMA (wgmma m64n64k16, fp32 accumulators in registers).  Operands that come from memory are
 // TMA-loaded 128B-swizzled tiles (a 3-D tensor map over qkv: rows >= T are zero-filled); operands that were just computed
@@ -384,6 +385,482 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// streamed kernels for long sequences (1 <= T <= 16384)
+// ------------------------------------------------------------------------------------------------
+// The kernels above hold a head's whole K / V (or Q / dO) in shared memory, loaded as ONE TMA box of tp <= 256 rows.
+// The kernels below keep one side of the product resident and stream the other through a ring of 64-row TMA blocks with
+// full / empty mbarriers (FlashAttention-2 scheme, the pipeline of the GEMM in gemm_sm90.cu):
+//   forward   one CTA per (image, head, 128-query tile): Q resident, K / V streamed, online softmax in fp32
+//   delta     delta = rowsum(dO o O) in fp32, one value per (image, head, query), into the workspace
+//   dK / dV   one CTA per (image, head, 128-key tile): K / V resident, Q / dO streamed with their lse / delta rows
+//   dQ        one CTA per (image, head, 128-query tile): Q / dO / lse / delta resident, K / V streamed
+//   dbias     per-64-row-tile column sums of the stored dq | dk | dv, summed per image in a fixed order
+// Warp 8 is the TMA producer; warpgroup g in {0, 1} owns rows [64 g, 64 g + 64) of the CTA's tile.  Causal CTAs stop at
+// the diagonal.  Nothing is accumulated with atomics: two runs give bit-identical results.
+constexpr int LA_THREADS = 288;  // two consumer warpgroups + the producer warp
+constexpr int LA_STAGES = 4;
+constexpr int LA_MAX_T = 16384;
+
+__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
+// forward: 80 KB + barriers, so that two CTAs (four consumer warpgroups) share an SM
+constexpr int LF_SQ = 0;                                   // 16 KB: the 128-query tile
+constexpr int LF_SKV = 16384;                              // per stage: K block, V block (8 KB each)
+constexpr int LF_BAR = LF_SKV + LA_STAGES * 2 * TILE_BYTES;  // full[S], empty[S], q
+constexpr int LF_SMEM = LF_BAR + 128 + 1024;
+
+__global__ void __launch_bounds__(LA_THREADS, 2)
+attn_long_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __restrict__ out, float* __restrict__ lse_out,
+                     const AttnParams p) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + LF_BAR);
+    uint64_t* empty = full + LA_STAGES;
+    uint64_t* bar_q = empty + LA_STAGES;
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const int n_mt = (p.T + 127) / 128;
+    const int mt = blockIdx.x % n_mt;
+    const int bh = blockIdx.x / n_mt;
+    const int h = bh % p.H;
+    const int b = bh / p.H;
+    const int n_cons = mt * 128 + 64 < p.T ? 2 : 1;  // warpgroups with at least one query row < T
+    const int nkb_all = (p.T + 63) / 64;
+    const int nkb = p.causal ? min(nkb_all, 2 * mt + n_cons) : nkb_all;  // key blocks this CTA streams
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < LA_STAGES; ++s) {
+            mbar_init(&full[s], 1);
+            mbar_init(&empty[s], 4 * n_cons);  // one arrival per consumer warp
+        }
+        mbar_init(bar_q, 1);
+        fence_mbar_init();
+    }
+    __syncthreads();
+
+    if (warp == 8) {
+        // ---- producer: Q once, then the K / V blocks through the ring ----
+        if (lane == 0) {
+            tma_prefetch_desc(&tmQKV);
+            mbar_expect_tx(bar_q, static_cast<uint32_t>(n_cons) * TILE_BYTES);
+            for (int g = 0; g < n_cons; ++g) tma_load_3d(smem + LF_SQ + g * TILE_BYTES, &tmQKV, bar_q, h * 64, mt * 128 + g * 64, b);
+            for (int kb = 0; kb < nkb; ++kb) {
+                const int s = kb % LA_STAGES;
+                mbar_wait(&empty[s], ((kb / LA_STAGES) & 1) ^ 1u);
+                uint8_t* dst = smem + LF_SKV + s * 2 * TILE_BYTES;
+                mbar_expect_tx(&full[s], 2u * TILE_BYTES);
+                tma_load_3d(dst, &tmQKV, &full[s], p.D + h * 64, kb * 64, b);
+                tma_load_3d(dst + TILE_BYTES, &tmQKV, &full[s], 2 * p.D + h * 64, kb * 64, b);
+            }
+        }
+        return;
+    }
+    const int g = warp >> 2;
+    if (g >= n_cons) return;  // (a warpgroup of padding rows only)
+    const int rl = (warp & 3) * 16 + (lane >> 2);
+    const int jq = (lane & 3) * 2;
+    const int q0 = mt * 128 + g * 64;
+    const int i0 = q0 + rl;  // this thread's query rows: i0 and i0 + 8
+    const int diag = q0 / 64;  // the key block on the diagonal of this warpgroup's queries
+    const int nkb_g = p.causal ? min(nkb, diag + 1) : nkb;
+    const float sl2 = p.scale * kLog2e;
+    const uint32_t q_base = smem_u32(smem + LF_SQ) + g * TILE_BYTES;
+
+    float o[32];
+#pragma unroll
+    for (int e = 0; e < 32; ++e) o[e] = 0.f;
+    // running row max (raw scores) and this thread's share of the row sum; every row has a valid key in block 0, so m is
+    // finite from the first block on
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+    mbar_wait(bar_q, 0);
+    for (int kb = 0; kb < nkb; ++kb) {
+        const int s = kb % LA_STAGES;
+        mbar_wait(&full[s], (kb / LA_STAGES) & 1);
+        if (kb < nkb_g) {
+            const uint32_t k_base = smem_u32(smem + LF_SKV + s * 2 * TILE_BYTES);
+            float sc[32];
+            wgmma_fence();
+            mma_tile_kk(sc, q_base, k_base);
+            wgmma_commit();
+            wgmma_wait<0>();
+            reg_fence(sc);
+            if (kb * 64 + 64 > p.T || (p.causal && kb == diag)) {
+                // keys >= T were zero-filled by TMA and score 0, not -inf; causal: keys after the query
+#pragma unroll
+                for (int e = 0; e < 32; ++e) {
+                    const int hr = (e >> 1) & 1;
+                    const int j = kb * 64 + (e >> 2) * 8 + jq + (e & 1);
+                    if (!(j < p.T && (!p.causal || j <= i0 + 8 * hr))) sc[e] = -INFINITY;
+                }
+            }
+            float mn[2] = {m[0], m[1]};
+#pragma unroll
+            for (int e = 0; e < 32; ++e) mn[(e >> 1) & 1] = fmaxf(mn[(e >> 1) & 1], sc[e]);
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr) {
+                mn[hr] = fmaxf(mn[hr], __shfl_xor_sync(0xffffffffu, mn[hr], 1));
+                mn[hr] = fmaxf(mn[hr], __shfl_xor_sync(0xffffffffu, mn[hr], 2));
+            }
+            const float alpha[2] = {fast_ex2((m[0] - mn[0]) * sl2), fast_ex2((m[1] - mn[1]) * sl2)};  // 0 on the first block
+            const float m2[2] = {mn[0] * sl2, mn[1] * sl2};
+            float rs[2] = {0.f, 0.f};
+#pragma unroll
+            for (int e = 0; e < 32; ++e) {
+                const int hr = (e >> 1) & 1;
+                const float pv = fast_ex2(fmaf(sc[e], sl2, -m2[hr]));  // exp2(-inf) = 0 for masked keys
+                sc[e] = pv;
+                rs[hr] += pv;
+            }
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr) {
+                l[hr] = fmaf(l[hr], alpha[hr], rs[hr]);
+                m[hr] = mn[hr];
+            }
+#pragma unroll
+            for (int e = 0; e < 32; ++e) o[e] *= alpha[(e >> 1) & 1];
+            // O += P V: P from registers (bf16), V MN-major from the stage
+            wgmma_fence();
+#pragma unroll
+            for (int st = 0; st < 4; ++st) {
+                uint32_t a[4];
+                a_frag(sc, st, a);
+                wgmma_m64n64k16_rs_tb(o, a, mnmajor_desc(k_base + TILE_BYTES + st * 2048), 1u);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            reg_fence(o);
+        }
+        if (lane == 0) mbar_arrive(&empty[s]);
+    }
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+        l[hr] += __shfl_xor_sync(0xffffffffu, l[hr], 1);
+        l[hr] += __shfl_xor_sync(0xffffffffu, l[hr], 2);
+    }
+    const float inv[2] = {1.0f / l[0], 1.0f / l[1]};
+#pragma unroll
+    for (int e = 0; e < 32; ++e) o[e] *= inv[(e >> 1) & 1];
+    store_tile(o, 1.0f, out + (static_cast<long long>(b) * p.T) * p.D + h * 64, p.D, i0, p.T, lane, nullptr);
+    if ((lane & 3) == 0) {
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+            const int i = i0 + 8 * hr;
+            if (i < p.T) lse_out[(static_cast<long long>(b) * p.H + h) * p.T + i] = m[hr] * p.scale + logf(l[hr]);
+        }
+    }
+}
+
+// delta[b, h, i] = sum_d dO[b, i, h, d] O[b, i, h, d] in fp32: one (row, head) per thread, 128 contiguous bytes of each
+__global__ void attn_long_delta_kernel(const __nv_bfloat16* __restrict__ o_in, const __nv_bfloat16* __restrict__ do_in,
+                                       float* __restrict__ delta, int B, int T, int H) {
+    const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (idx >= static_cast<long long>(B) * T * H) return;
+    const int h = static_cast<int>(idx % H);
+    const long long row = idx / H;
+    const int b = static_cast<int>(row / T), i = static_cast<int>(row % T);
+    const uint4* po = reinterpret_cast<const uint4*>(o_in + idx * 64);
+    const uint4* pd = reinterpret_cast<const uint4*>(do_in + idx * 64);
+    float dl = 0.f;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        const uint4 a = __ldg(po + k), gg = __ldg(pd + k);
+        dl += bf16lo(a.x) * bf16lo(gg.x) + bf16hi(a.x) * bf16hi(gg.x) + bf16lo(a.y) * bf16lo(gg.y) + bf16hi(a.y) * bf16hi(gg.y) +
+              bf16lo(a.z) * bf16lo(gg.z) + bf16hi(a.z) * bf16hi(gg.z) + bf16lo(a.w) * bf16lo(gg.w) + bf16hi(a.w) * bf16hi(gg.w);
+    }
+    delta[(static_cast<long long>(b) * H + h) * T + i] = dl;
+}
+
+// Column-sum partials: [B * H][ceil(T / 64) row tiles][dq | dk | dv][64], each slot written by exactly one warpgroup.
+// Sums the 64-column partials of the 4 warps of warpgroup g (cs: [4][64], written by store_tile) in a fixed order.
+__device__ __forceinline__ float wg_colsum(const float* cs, int c) { return ((cs[c] + cs[64 + c]) + cs[128 + c]) + cs[192 + c]; }
+
+// dK / dV: 96 KB of tiles + lse / delta rows + column sums
+constexpr int LK_SK = 0;                                     // 16 KB: the 128-key tile
+constexpr int LK_SV = 16384;                                 // 16 KB
+constexpr int LK_SQD = 32768;                                // per stage: Q block, dO block
+constexpr int LK_ROW = LK_SQD + LA_STAGES * 2 * TILE_BYTES;  // per stage: lse * log2(e) [64], delta [64]
+constexpr int LK_CS = LK_ROW + LA_STAGES * 512;              // [dk | dv][warpgroup][warp][64] column sums
+constexpr int LK_BAR = LK_CS + 2 * 8 * 64 * 4;
+constexpr int LK_SMEM = LK_BAR + 128 + 1024;
+
+__global__ void __launch_bounds__(LA_THREADS, 1)
+attn_long_dkdv_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmDO,
+                      const float* __restrict__ lse_in, const float* __restrict__ delta_in, __nv_bfloat16* __restrict__ dqkv,
+                      float* __restrict__ csum_part, const AttnParams p) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + LK_BAR);
+    uint64_t* empty = full + LA_STAGES;
+    uint64_t* bar_kv = empty + LA_STAGES;
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const int n_kt = (p.T + 127) / 128;
+    const int kt = blockIdx.x % n_kt;
+    const int bh = blockIdx.x / n_kt;
+    const int h = bh % p.H;
+    const int b = bh / p.H;
+    const int n_cons = kt * 128 + 64 < p.T ? 2 : 1;
+    const int nqb = (p.T + 63) / 64;
+    const int qb0 = p.causal ? 2 * kt : 0;  // causal: query blocks wholly before the key tile contribute nothing
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < LA_STAGES; ++s) {
+            mbar_init(&full[s], 1 + 32);  // the producer's expect_tx + one arrival per producer lane after its lse / delta stores
+            mbar_init(&empty[s], 4 * n_cons);
+        }
+        mbar_init(bar_kv, 1);
+        fence_mbar_init();
+    }
+    __syncthreads();
+
+    if (warp == 8) {
+        // ---- producer: K / V once, then Q / dO blocks (TMA) and their lse / delta rows (lanes) through the ring ----
+        if (lane == 0) {
+            tma_prefetch_desc(&tmQKV);
+            tma_prefetch_desc(&tmDO);
+            mbar_expect_tx(bar_kv, 2u * n_cons * TILE_BYTES);
+            for (int g = 0; g < n_cons; ++g) {
+                tma_load_3d(smem + LK_SK + g * TILE_BYTES, &tmQKV, bar_kv, p.D + h * 64, kt * 128 + g * 64, b);
+                tma_load_3d(smem + LK_SV + g * TILE_BYTES, &tmQKV, bar_kv, 2 * p.D + h * 64, kt * 128 + g * 64, b);
+            }
+        }
+        const float* lse_bh = lse_in + static_cast<long long>(bh) * p.T;
+        const float* delta_bh = delta_in + static_cast<long long>(bh) * p.T;
+        for (int qb = qb0, it = 0; qb < nqb; ++qb, ++it) {
+            const int s = it % LA_STAGES;
+            mbar_wait(&empty[s], ((it / LA_STAGES) & 1) ^ 1u);
+            if (lane == 0) {
+                uint8_t* dst = smem + LK_SQD + s * 2 * TILE_BYTES;
+                mbar_expect_tx(&full[s], 2u * TILE_BYTES);
+                tma_load_3d(dst, &tmQKV, &full[s], h * 64, qb * 64, b);
+                tma_load_3d(dst + TILE_BYTES, &tmDO, &full[s], h * 64, qb * 64, b);
+            }
+            float* row = reinterpret_cast<float*>(smem + LK_ROW + s * 512);
+#pragma unroll
+            for (int k = 0; k < 2; ++k) {
+                const int r = lane + 32 * k, i = qb * 64 + r;
+                // padded query rows: lse = +inf makes P = dS = 0 (their Q / dO rows are zero-filled as well)
+                row[r] = i < p.T ? __ldg(lse_bh + i) * kLog2e : INFINITY;
+                row[64 + r] = i < p.T ? __ldg(delta_bh + i) : 0.f;
+            }
+            mbar_arrive(&full[s]);
+        }
+        return;
+    }
+    const int g = warp >> 2;
+    if (g >= n_cons) return;
+    const int wq = warp & 3;
+    const int rl = wq * 16 + (lane >> 2);  // accumulator rows rl, rl + 8: keys
+    const int jq = (lane & 3) * 2;         // accumulator columns 8 n + jq (+ 1): queries
+    const int k0 = kt * 128 + g * 64;
+    const int key0 = k0 + rl;
+    const int diag = k0 / 64;
+    const int qb_g = p.causal ? diag : 0;
+    const float sl2 = p.scale * kLog2e;
+    const uint32_t k_base = smem_u32(smem + LK_SK) + g * TILE_BYTES, v_base = smem_u32(smem + LK_SV) + g * TILE_BYTES;
+    const bool key_edge = k0 + 64 > p.T;
+
+    float dv[32], dk[32];
+#pragma unroll
+    for (int e = 0; e < 32; ++e) { dv[e] = 0.f; dk[e] = 0.f; }
+    mbar_wait(bar_kv, 0);
+    for (int qb = qb0, it = 0; qb < nqb; ++qb, ++it) {
+        const int s = it % LA_STAGES;
+        mbar_wait(&full[s], (it / LA_STAGES) & 1);
+        if (qb >= qb_g) {
+            const uint32_t q_st = smem_u32(smem + LK_SQD + s * 2 * TILE_BYTES), do_st = q_st + TILE_BYTES;
+            const float* row = reinterpret_cast<const float*>(smem + LK_ROW + s * 512);
+            float st[32], dpt[32];
+            wgmma_fence();
+            mma_tile_kk(st, k_base, q_st);    // S^T = K Q^T
+            mma_tile_kk(dpt, v_base, do_st);  // dP^T = V dO^T
+            wgmma_commit();
+            wgmma_wait<0>();
+            reg_fence(st);
+            reg_fence(dpt);
+            const bool edge = key_edge || (p.causal && qb == diag);
+#pragma unroll
+            for (int e = 0; e < 32; ++e) {
+                const int key = key0 + ((e >> 1) & 1) * 8;
+                const int ii = (e >> 2) * 8 + jq + (e & 1);
+                float pv = fast_ex2(fmaf(st[e], sl2, -row[ii]));
+                if (edge && !(key < p.T && (!p.causal || key <= qb * 64 + ii))) pv = 0.f;
+                st[e] = pv;
+                dpt[e] = pv * (dpt[e] - row[64 + ii]);
+            }
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                uint32_t a[4];
+                a_frag(st, k, a);
+                wgmma_m64n64k16_rs_tb(dv, a, mnmajor_desc(do_st + k * 2048), 1u);  // dV += P^T dO
+                a_frag(dpt, k, a);
+                wgmma_m64n64k16_rs_tb(dk, a, mnmajor_desc(q_st + k * 2048), 1u);   // dK += dS^T Q
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            reg_fence(dv);
+            reg_fence(dk);
+        }
+        if (lane == 0) mbar_arrive(&empty[s]);
+    }
+    const long long D3 = 3ll * p.D;
+    __nv_bfloat16* g0 = dqkv + (static_cast<long long>(b) * p.T) * D3 + h * 64;
+    float* cs = reinterpret_cast<float*>(smem + LK_CS);
+    const bool sums = csum_part != nullptr;
+    store_tile(dk, p.scale, g0 + p.D, D3, key0, p.T, lane, sums ? cs + ((0 * 2 + g) * 4 + wq) * 64 : nullptr);
+    store_tile(dv, 1.0f, g0 + 2 * p.D, D3, key0, p.T, lane, sums ? cs + ((1 * 2 + g) * 4 + wq) * 64 : nullptr);
+    if (sums) {
+        named_bar_sync(1 + g, 128);
+        const int t = threadIdx.x & 127, sec = t >> 6, c = t & 63;
+        float* dst = csum_part + (static_cast<long long>(bh) * ((p.T + 63) / 64) + diag) * 192;
+        dst[(1 + sec) * 64 + c] = wg_colsum(cs + (sec * 2 + g) * 4 * 64, c);
+    }
+}
+
+// dQ: 96 KB of tiles + column sums
+constexpr int LQ_SQ = 0;                                  // 16 KB: the 128-query tile
+constexpr int LQ_SDO = 16384;                             // 16 KB
+constexpr int LQ_SKV = 32768;                             // per stage: K block, V block
+constexpr int LQ_CS = LQ_SKV + LA_STAGES * 2 * TILE_BYTES;  // [warpgroup][warp][64] column sums
+constexpr int LQ_BAR = LQ_CS + 8 * 64 * 4;
+constexpr int LQ_SMEM = LQ_BAR + 128 + 1024;
+
+__global__ void __launch_bounds__(LA_THREADS, 1)
+attn_long_dq_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmDO,
+                    const float* __restrict__ lse_in, const float* __restrict__ delta_in, __nv_bfloat16* __restrict__ dqkv,
+                    float* __restrict__ csum_part, const AttnParams p) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + LQ_BAR);
+    uint64_t* empty = full + LA_STAGES;
+    uint64_t* bar_q = empty + LA_STAGES;
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const int n_qt = (p.T + 127) / 128;
+    const int qt = blockIdx.x % n_qt;
+    const int bh = blockIdx.x / n_qt;
+    const int h = bh % p.H;
+    const int b = bh / p.H;
+    const int n_cons = qt * 128 + 64 < p.T ? 2 : 1;
+    const int nkb_all = (p.T + 63) / 64;
+    const int nkb = p.causal ? min(nkb_all, 2 * qt + n_cons) : nkb_all;
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < LA_STAGES; ++s) {
+            mbar_init(&full[s], 1);
+            mbar_init(&empty[s], 4 * n_cons);
+        }
+        mbar_init(bar_q, 1);
+        fence_mbar_init();
+    }
+    __syncthreads();
+
+    if (warp == 8) {
+        if (lane == 0) {
+            tma_prefetch_desc(&tmQKV);
+            tma_prefetch_desc(&tmDO);
+            mbar_expect_tx(bar_q, 2u * n_cons * TILE_BYTES);
+            for (int g = 0; g < n_cons; ++g) {
+                tma_load_3d(smem + LQ_SQ + g * TILE_BYTES, &tmQKV, bar_q, h * 64, qt * 128 + g * 64, b);
+                tma_load_3d(smem + LQ_SDO + g * TILE_BYTES, &tmDO, bar_q, h * 64, qt * 128 + g * 64, b);
+            }
+            for (int kb = 0; kb < nkb; ++kb) {
+                const int s = kb % LA_STAGES;
+                mbar_wait(&empty[s], ((kb / LA_STAGES) & 1) ^ 1u);
+                uint8_t* dst = smem + LQ_SKV + s * 2 * TILE_BYTES;
+                mbar_expect_tx(&full[s], 2u * TILE_BYTES);
+                tma_load_3d(dst, &tmQKV, &full[s], p.D + h * 64, kb * 64, b);
+                tma_load_3d(dst + TILE_BYTES, &tmQKV, &full[s], 2 * p.D + h * 64, kb * 64, b);
+            }
+        }
+        return;
+    }
+    const int g = warp >> 2;
+    if (g >= n_cons) return;
+    const int wq = warp & 3;
+    const int rl = wq * 16 + (lane >> 2);
+    const int jq = (lane & 3) * 2;
+    const int q0 = qt * 128 + g * 64;
+    const int i0 = q0 + rl;
+    const int diag = q0 / 64;
+    const int nkb_g = p.causal ? min(nkb, diag + 1) : nkb;
+    const float sl2 = p.scale * kLog2e;
+    const uint32_t q_base = smem_u32(smem + LQ_SQ) + g * TILE_BYTES, do_base = smem_u32(smem + LQ_SDO) + g * TILE_BYTES;
+    float l2[2], de[2];
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+        const int i = i0 + 8 * hr;
+        const long long at = static_cast<long long>(bh) * p.T + i;
+        l2[hr] = i < p.T ? __ldg(lse_in + at) * kLog2e : INFINITY;  // padded query rows: P = dS = 0
+        de[hr] = i < p.T ? __ldg(delta_in + at) : 0.f;
+    }
+
+    float dq[32];
+#pragma unroll
+    for (int e = 0; e < 32; ++e) dq[e] = 0.f;
+    mbar_wait(bar_q, 0);
+    for (int kb = 0; kb < nkb; ++kb) {
+        const int s = kb % LA_STAGES;
+        mbar_wait(&full[s], (kb / LA_STAGES) & 1);
+        if (kb < nkb_g) {
+            const uint32_t k_st = smem_u32(smem + LQ_SKV + s * 2 * TILE_BYTES), v_st = k_st + TILE_BYTES;
+            float sc[32], dp[32];
+            wgmma_fence();
+            mma_tile_kk(sc, q_base, k_st);   // S = Q K^T
+            mma_tile_kk(dp, do_base, v_st);  // dP = dO V^T
+            wgmma_commit();
+            wgmma_wait<0>();
+            reg_fence(sc);
+            reg_fence(dp);
+            const bool edge = kb * 64 + 64 > p.T || (p.causal && kb == diag);
+#pragma unroll
+            for (int e = 0; e < 32; ++e) {
+                const int hr = (e >> 1) & 1;
+                const int j = kb * 64 + (e >> 2) * 8 + jq + (e & 1);
+                float pv = fast_ex2(fmaf(sc[e], sl2, -l2[hr]));
+                if (edge && !(j < p.T && (!p.causal || j <= i0 + 8 * hr))) pv = 0.f;
+                dp[e] = pv * (dp[e] - de[hr]);
+            }
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                uint32_t a[4];
+                a_frag(dp, k, a);
+                wgmma_m64n64k16_rs_tb(dq, a, mnmajor_desc(k_st + k * 2048), 1u);  // dQ += dS K
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            reg_fence(dq);
+        }
+        if (lane == 0) mbar_arrive(&empty[s]);
+    }
+    const long long D3 = 3ll * p.D;
+    float* cs = reinterpret_cast<float*>(smem + LQ_CS);
+    const bool sums = csum_part != nullptr;
+    store_tile(dq, p.scale, dqkv + (static_cast<long long>(b) * p.T) * D3 + h * 64, D3, i0, p.T, lane,
+               sums ? cs + (g * 4 + wq) * 64 : nullptr);
+    if (sums) {
+        named_bar_sync(1 + g, 128);
+        const int t = threadIdx.x & 127;
+        if (t < 64) csum_part[(static_cast<long long>(bh) * ((p.T + 63) / 64) + diag) * 192 + t] = wg_colsum(cs + g * 4 * 64, t);
+    }
+}
+
+// dbias_part[b, sec * D + h * 64 + c] = sum over the 64-row tiles of (b, h), in tile order
+__global__ void attn_long_dbias_kernel(const float* __restrict__ csum_part, float* __restrict__ dbias_part, int B, int H, int n64) {
+    const int D = H * 64;
+    const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (idx >= 3ll * B * D) return;
+    const int b = static_cast<int>(idx / (3 * D));
+    const int r = static_cast<int>(idx % (3 * D));
+    const int sec = r / D, h = (r % D) / 64, c = r & 63;
+    const float* src = csum_part + (static_cast<long long>(b) * H + h) * n64 * 192 + sec * 64 + c;
+    float t = 0.f;
+    for (int k = 0; k < n64; ++k) t += src[k * 192];
+    dbias_part[idx] = t;
+}
+
 }  // namespace b200
 
 using namespace b200;
@@ -479,4 +956,90 @@ extern "C" int b200_set_attention_bwd_version(int version) {
     const int old = g_attn_bwd_version;
     g_attn_bwd_version = (version >= 1 && version <= 3) ? version : 0;
     return old;
+}
+
+// ---- streamed kernels: any 1 <= T <= 16384 ----
+static int attn_long_check(int B, int T, int H, int Dh) {
+    if (B <= 0 || T <= 0 || H <= 0) return set_error(B200_ERR_ARG, "attention_long: non-positive size");
+    if (Dh != 64) return set_error(B200_ERR_ARG, "attention_long: head dim must be 64");
+    if (T > LA_MAX_T) return set_error(B200_ERR_ARG, "attention_long: T must be <= 16384");
+    return 0;
+}
+
+// the dynamic shared-memory attribute belongs to the (function, device) pair
+template <typename Kernel>
+static int attn_long_configure(Kernel kernel, int smem, bool (&configured)[64]) {
+    const int dev = current_device_slot();
+    if (configured[dev]) return 0;
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) return set_error(B200_ERR_LAUNCH, cudaGetErrorString(e));
+    configured[dev] = true;
+    return 0;
+}
+
+// 64 x 64 boxes (128B-swizzled) over a [B, T, cols] bf16 tensor: rows >= T of an image are zero-filled
+static int attn_long_tmap(CUtensorMap* tm, const void* base, int cols, int T, int B) {
+    uint64_t dims[3] = {static_cast<uint64_t>(cols), static_cast<uint64_t>(T), static_cast<uint64_t>(B)};
+    uint64_t strides[2] = {static_cast<uint64_t>(cols) * 2, static_cast<uint64_t>(cols) * 2 * static_cast<uint64_t>(T)};
+    uint32_t box[3] = {64, 64, 1};
+    return make_tmap(tm, base, 2, 3, dims, strides, box, 128);
+}
+
+extern "C" int b200_attention_long_fwd(const void* qkv_bf16, void* out_bf16, float* lse, int B, int T, int H, int Dh,
+                                       float scale, int causal, cudaStream_t stream) {
+    int rc = attn_long_check(B, T, H, Dh);
+    if (rc) return rc;
+    if (qkv_bf16 == nullptr || out_bf16 == nullptr || lse == nullptr) return set_error(B200_ERR_ARG, "attention_long_fwd: null pointer");
+    const int D = H * 64;
+    CUtensorMap tmQKV;
+    if ((rc = attn_long_tmap(&tmQKV, qkv_bf16, 3 * D, T, B)) != 0) return rc;
+    static bool configured[64] = {};
+    if ((rc = attn_long_configure(attn_long_fwd_kernel, LF_SMEM, configured)) != 0) return rc;
+    AttnParams p;
+    p.B = B; p.T = T; p.H = H; p.D = D; p.tp = (T + 63) / 64 * 64; p.scale = scale; p.causal = causal;
+    const int n_mt = (T + 127) / 128;
+    attn_long_fwd_kernel<<<B * H * n_mt, LA_THREADS, LF_SMEM, stream>>>(tmQKV, reinterpret_cast<__nv_bfloat16*>(out_bf16), lse, p);
+    return check_launch("attention_long_fwd");
+}
+
+extern "C" long long b200_attention_long_bwd_workspace_floats(int B, int T, int H) {
+    if (B <= 0 || T <= 0 || H <= 0) return 0;
+    // delta [B, H, T] + column-sum partials [B, H, ceil(T / 64)][3][64]
+    return static_cast<long long>(B) * H * (static_cast<long long>(T) + (T + 63) / 64 * 192ll);
+}
+
+extern "C" int b200_attention_long_bwd(const void* qkv_bf16, const void* out_bf16, const void* dout_bf16, const float* lse,
+                                       void* dqkv_bf16, int B, int T, int H, int Dh, float scale, int causal,
+                                       float* dbias_part, float* workspace, cudaStream_t stream) {
+    int rc = attn_long_check(B, T, H, Dh);
+    if (rc) return rc;
+    if (qkv_bf16 == nullptr || out_bf16 == nullptr || dout_bf16 == nullptr || lse == nullptr || dqkv_bf16 == nullptr || workspace == nullptr)
+        return set_error(B200_ERR_ARG, "attention_long_bwd: null pointer");
+    const int D = H * 64;
+    CUtensorMap tmQKV, tmDO;
+    if ((rc = attn_long_tmap(&tmQKV, qkv_bf16, 3 * D, T, B)) != 0) return rc;
+    if ((rc = attn_long_tmap(&tmDO, dout_bf16, D, T, B)) != 0) return rc;
+    static bool configured_kv[64] = {}, configured_q[64] = {};
+    if ((rc = attn_long_configure(attn_long_dkdv_kernel, LK_SMEM, configured_kv)) != 0) return rc;
+    if ((rc = attn_long_configure(attn_long_dq_kernel, LQ_SMEM, configured_q)) != 0) return rc;
+    AttnParams p;
+    p.B = B; p.T = T; p.H = H; p.D = D; p.tp = (T + 63) / 64 * 64; p.scale = scale; p.causal = causal;
+    float* delta = workspace;
+    float* csum_part = dbias_part != nullptr ? workspace + static_cast<long long>(B) * H * T : nullptr;
+    const long long rows = static_cast<long long>(B) * T * H;
+    attn_long_delta_kernel<<<static_cast<unsigned>((rows + 255) / 256), 256, 0, stream>>>(
+        reinterpret_cast<const __nv_bfloat16*>(out_bf16), reinterpret_cast<const __nv_bfloat16*>(dout_bf16), delta, B, T, H);
+    if ((rc = check_launch("attention_long_bwd (delta)")) != 0) return rc;
+    const int n_t = (T + 127) / 128;
+    __nv_bfloat16* dqkv = reinterpret_cast<__nv_bfloat16*>(dqkv_bf16);
+    attn_long_dkdv_kernel<<<B * H * n_t, LA_THREADS, LK_SMEM, stream>>>(tmQKV, tmDO, lse, delta, dqkv, csum_part, p);
+    if ((rc = check_launch("attention_long_bwd (dk, dv)")) != 0) return rc;
+    attn_long_dq_kernel<<<B * H * n_t, LA_THREADS, LQ_SMEM, stream>>>(tmQKV, tmDO, lse, delta, dqkv, csum_part, p);
+    if ((rc = check_launch("attention_long_bwd (dq)")) != 0) return rc;
+    if (dbias_part != nullptr) {
+        const long long n = 3ll * B * D;
+        attn_long_dbias_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(csum_part, dbias_part, B, H, (T + 63) / 64);
+        if ((rc = check_launch("attention_long_bwd (dbias)")) != 0) return rc;
+    }
+    return 0;
 }

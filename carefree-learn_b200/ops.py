@@ -192,6 +192,10 @@ def layernorm_bwd(
 # ----------------------------------------------------------------------------------------------------------------
 # attention
 # ----------------------------------------------------------------------------------------------------------------
+ATTENTION_MAX_T = 16384   # longest sequence the attention kernels accept
+ATTENTION_RESIDENT_MAX_T = 256  # up to here a whole head fits in shared memory; longer sequences use the streamed kernels
+
+
 def attention_fwd(qkv: Tensor, B: int, T: int, H: int, *, scale: Optional[float] = None, causal: bool = False) -> Tuple[Tensor, Tensor]:
     _need_cuda(qkv)
     D = H * 64
@@ -200,7 +204,8 @@ def attention_fwd(qkv: Tensor, B: int, T: int, H: int, *, scale: Optional[float]
     out = torch.empty((B * T, D), dtype=torch.bfloat16, device=qkv.device)
     lse = torch.empty((B, H, T), dtype=torch.float32, device=qkv.device)
     sc = float(scale) if scale is not None else 0.125
-    call("b200_attention_fwd", qkv.data_ptr(), out.data_ptr(), lse.data_ptr(), B, T, H, 64, sc, int(causal), _stream())
+    name = "b200_attention_fwd" if T <= ATTENTION_RESIDENT_MAX_T else "b200_attention_long_fwd"
+    call(name, qkv.data_ptr(), out.data_ptr(), lse.data_ptr(), B, T, H, 64, sc, int(causal), _stream())
     return out, lse
 
 
@@ -214,8 +219,13 @@ def attention_bwd(qkv: Tensor, out: Tensor, dout: Tensor, lse: Tensor, B: int, T
         dqkv = torch.empty((B * T, 3 * D), dtype=torch.bfloat16, device=qkv.device)
     sc = float(scale) if scale is not None else 0.125
     part = WORKSPACE.get(qkv.device, B * 3 * D, "attn_dbias") if dbias is not None else None
-    call("b200_attention_bwd", qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr(), dqkv.data_ptr(), B, T, H, 64, sc, int(causal),
-         _ptr(part), _stream())
+    if T <= ATTENTION_RESIDENT_MAX_T:
+        call("b200_attention_bwd", qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr(), dqkv.data_ptr(), B, T, H, 64, sc, int(causal),
+             _ptr(part), _stream())
+    else:
+        ws = WORKSPACE.get(qkv.device, int(_cabi.lib().b200_attention_long_bwd_workspace_floats(B, T, H)), "attn_long")
+        call("b200_attention_long_bwd", qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr(), dqkv.data_ptr(), B, T, H, 64, sc,
+             int(causal), _ptr(part), ws.data_ptr(), _stream())
     if dbias is not None:
         call("b200_colsum_finish", part.data_ptr(), 3 * D, B, 3 * D, dbias.data_ptr(), 1, 0, _stream())
     return dqkv

@@ -170,8 +170,8 @@ class ViTGeometry:
             raise NotImplementedError(f"FeedForward activation {activation!r} is outside the fused path (GELU, quick_gelu)")
         if output_dim is not None and (output_dim % 8 != 0 or num_classes is not None):
             raise NotImplementedError("output_dim must be a multiple of 8 and cannot be combined with a classifier head")
-        if self.T > 256:
-            raise NotImplementedError("sequence length > 256 tokens is not supported by the fused attention yet")
+        if self.T > ops.ATTENTION_MAX_T:
+            raise NotImplementedError(f"sequence length > {ops.ATTENTION_MAX_T} tokens is not supported by the fused attention")
 
     @property
     def head_norm_key(self) -> str:  # mixed_stacks/api.py:383-395: PreNorm(head) vs head then head_norm

@@ -132,6 +132,17 @@ int b200_set_attention_prefetch(int enable);
 int b200_attention_bwd(const void* qkv_bf16, const void* out_bf16, const void* dout_bf16, const float* lse,
                        void* dqkv_bf16, int B, int T, int H, int Dh, float scale, int causal, float* dbias_part,
                        cudaStream_t stream);
+/* The same attention for long sequences: 1 <= T <= 16384, Dh = 64, the same layouts, outputs and causal flag as
+ * b200_attention_fwd / _bwd.  These kernels stream K / V (forward, dQ) or Q / dO (dK / dV) through shared memory in
+ * 64-row blocks with an online softmax, so no head has to fit in shared memory at once.  Deterministic (no atomics).
+ * workspace (backward, required): b200_attention_long_bwd_workspace_floats(B, T, H) floats of device scratch.
+ * dbias_part (optional): the same per-image column sums as b200_attention_bwd writes. */
+int b200_attention_long_fwd(const void* qkv_bf16, void* out_bf16, float* lse, int B, int T, int H, int Dh, float scale,
+                            int causal, cudaStream_t stream);
+long long b200_attention_long_bwd_workspace_floats(int B, int T, int H);
+int b200_attention_long_bwd(const void* qkv_bf16, const void* out_bf16, const void* dout_bf16, const float* lse,
+                            void* dqkv_bf16, int B, int T, int H, int Dh, float scale, int causal, float* dbias_part,
+                            float* workspace, cudaStream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * FCNN (cflearn/modules/ml/fcnn.py:12-59: Mapping(Linear + ReLU) x n, then nn.Linear) -- one launch per training
