@@ -50,6 +50,12 @@ SIGNATURES: Dict[str, Any] = {
     "b200_attention_long_fwd": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_float, c_int, _P]),
     "b200_attention_long_bwd_workspace_floats": (_LL, [c_int, c_int, c_int]),
     "b200_attention_long_bwd": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_float, c_int, _P, _P, _P]),
+    "b200_cross_attention_fwd": (c_int, [_P, _LL, _P, _P, _LL, _P, _LL, _P, c_int, c_int, c_int, c_int, c_int, c_float, c_int, _P]),
+    "b200_cross_attention_bwd_workspace_floats": (_LL, [c_int, c_int, c_int, c_int, c_int]),
+    "b200_cross_attention_bwd": (
+        c_int,
+        [_P, _LL, _P, _P, _LL, _P, _LL, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_float, c_int, _P, _P],
+    ),
     "b200_fcnn_step": (
         c_int,
         [_P, _P, _P, _P, _P, _P, c_int, c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int), c_int, c_int, c_float, c_float,

@@ -1,0 +1,128 @@
+"""The SD-v1.5 UNet's ``CrossAttention`` (cflearn/modules/core/attentions.py:498-569) on the native kernels.
+
+``CrossAttentionB200`` is a drop-in for the reference module: same constructor keywords, the same fp32 parameters under the
+same ``state_dict`` keys (``to_q.weight``, ``to_k.weight``, ``to_v.weight``, ``out_linear.0.weight``, ``out_linear.0.bias``).
+Its forward and backward are one ``autograd.Function``; every product is the wgmma GEMM (``ops.gemm`` / ``ops.wgrad``) or the
+streamed attention (``ops.cross_attention_fwd/_bwd``), which reads q / k / v as column slices of the projection outputs:
+
+    self-attention (context None):  qkv = x [Wq; Wk; Wv]^T  (one GEMM, N = 3L)   dx = dqkv [Wq; Wk; Wv]  (one GEMM, K = 3L)
+    cross-attention:                q = x Wq^T, kv = context [Wk; Wv]^T          dx = dq Wq, dcontext = dkv [Wk; Wv]
+    then attention (scale Dh^-0.5), out_linear with bias; weight gradients by split-K wgrad, the bias gradient by a column sum.
+
+Semantics are eager's under bf16 autocast: each input is cast to bf16 once, q / k / v, the attention output and the module
+output are bf16, weight and bias gradients are rounded to bf16 like eager's, and input gradients come back in the input's
+dtype.  Rounding points that differ from eager: in self-attention the three contributions to the input gradient are summed in
+fp32 inside the packed dgrad GEMM and rounded once, where eager rounds each to bf16 and adds them (in bf16 for a bf16 input);
+likewise the k and v contributions to the context gradient.  Dropout > 0 and attention masks are refused.
+"""
+from __future__ import annotations
+
+from typing import Optional
+
+import torch
+from torch import Tensor, nn
+
+from . import ops
+from ._cabi import B200Error
+
+
+def _bf(t: Tensor) -> Tensor:
+    return t.to(torch.bfloat16).contiguous()
+
+
+class _CrossAttentionFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, net: Tensor, context: Optional[Tensor], wq: Tensor, wk: Tensor, wv: Tensor, wo: Tensor, bo: Tensor, heads: int):  # type: ignore[override]
+        B, Tq, Dq = net.shape
+        L = wq.shape[0]
+        x = _bf(net.reshape(B * Tq, Dq))
+        if context is None:
+            w_in = _bf(torch.cat([wq, wk, wv], 0))
+            qkv = ops.gemm(x, w_in)
+            q, k, v = qkv[:, :L], qkv[:, L:2 * L], qkv[:, 2 * L:]
+            c, w_kv = None, None
+        else:
+            c = _bf(context.reshape(-1, context.shape[-1]))
+            w_in, w_kv = _bf(wq), _bf(torch.cat([wk, wv], 0))
+            q = ops.gemm(x, w_in)
+            kv = ops.gemm(c, w_kv)
+            k, v = kv[:, :L], kv[:, L:]
+        o, lse = ops.cross_attention_fwd(q, k, v, B, heads)
+        w_o = _bf(wo)
+        y = ops.gemm(o, w_o, bias=_bf(bo))
+        ctx.save_for_backward(x, c, q, k, v, o, lse, w_in, w_kv, w_o)
+        ctx.meta = (B, heads, net.dtype, net.shape, None if context is None else (context.dtype, context.shape))
+        return y.view(B, Tq, Dq)
+
+    @staticmethod
+    def backward(ctx, dy: Tensor):  # type: ignore[override]
+        x, c, q, k, v, o, lse, w_in, w_kv, w_o = ctx.saved_tensors
+        B, heads, net_dtype, net_shape, ctx_meta = ctx.meta
+        M, Dq = x.shape
+        L = q.shape[1]
+        dy = _bf(dy.reshape(M, Dq))
+        dwo = torch.empty(w_o.shape, dtype=torch.float32, device=dy.device)
+        dbo = torch.empty(Dq, dtype=torch.float32, device=dy.device)
+        ops.wgrad(dy, o, dwo)
+        ops.colsum(dy, dbo)
+        do = ops.gemm(dy, w_o, b_mn_major=True)
+        if c is None:
+            dqkv = torch.empty((M, 3 * L), dtype=torch.bfloat16, device=dy.device)
+            ops.cross_attention_bwd(q, k, v, o, do, lse, B, heads, dq=dqkv[:, :L], dk=dqkv[:, L:2 * L], dv=dqkv[:, 2 * L:])
+            dw = torch.empty((3 * L, Dq), dtype=torch.float32, device=dy.device)
+            ops.wgrad(dqkv, x, dw)
+            dwq, dwk, dwv = dw[:L], dw[L:2 * L], dw[2 * L:]
+            dx = ops.gemm(dqkv, w_in, b_mn_major=True)
+            dctx = None
+        else:
+            dq = torch.empty((M, L), dtype=torch.bfloat16, device=dy.device)
+            dkv = torch.empty((c.shape[0], 2 * L), dtype=torch.bfloat16, device=dy.device)
+            ops.cross_attention_bwd(q, k, v, o, do, lse, B, heads, dq=dq, dk=dkv[:, :L], dv=dkv[:, L:])
+            dwq = torch.empty((L, Dq), dtype=torch.float32, device=dy.device)
+            dwkv = torch.empty((2 * L, c.shape[1]), dtype=torch.float32, device=dy.device)
+            ops.wgrad(dq, x, dwq)
+            ops.wgrad(dkv, c, dwkv)
+            dwk, dwv = dwkv[:L], dwkv[L:]
+            dx = ops.gemm(dq, w_in, b_mn_major=True)
+            dctx = ops.gemm(dkv, w_kv, b_mn_major=True).to(ctx_meta[0]).view(ctx_meta[1])
+        return dx.to(net_dtype).view(net_shape), dctx, dwq, dwk, dwv, dwo, dbo, None
+
+
+class _Linear(nn.Module):
+    """Parameter holder with nn.Linear's parameter names and shapes (the reference's HijackLinear)."""
+
+    def __init__(self, in_dim: int, out_dim: int, bias: bool) -> None:
+        super().__init__()
+        self.weight = nn.Parameter(torch.empty(out_dim, in_dim))
+        self.bias = nn.Parameter(torch.empty(out_dim)) if bias else None
+        ref = nn.Linear(in_dim, out_dim, bias=bias)  # nn.Linear's initialisation
+        with torch.no_grad():
+            self.weight.copy_(ref.weight)
+            if bias:
+                self.bias.copy_(ref.bias)
+
+
+class CrossAttentionB200(nn.Module):
+    """Drop-in for cflearn's ``CrossAttention`` on the native kernels (bf16 compute, fp32 parameters; CUDA only)."""
+
+    def __init__(self, *, query_dim: int, context_dim: Optional[int] = None, num_heads: int = 8, head_dim: int = 64,
+                 dropout: float = 0.0) -> None:
+        super().__init__()
+        if dropout > 0.0:
+            raise NotImplementedError("CrossAttentionB200: dropout > 0 is not supported")
+        self.has_context = context_dim is not None
+        latent_dim = head_dim * num_heads
+        context_dim = context_dim or query_dim
+        self.num_heads = num_heads
+        self.to_q = _Linear(query_dim, latent_dim, bias=False)
+        self.to_k = _Linear(context_dim, latent_dim, bias=False)
+        self.to_v = _Linear(context_dim, latent_dim, bias=False)
+        self.out_linear = nn.Sequential(_Linear(latent_dim, query_dim, bias=True), nn.Dropout(dropout))
+
+    def forward(self, net: Tensor, *, context: Optional[Tensor] = None, mask: Optional[Tensor] = None) -> Tensor:
+        if mask is not None:
+            raise NotImplementedError("CrossAttentionB200: attention masks are not supported")
+        if not net.is_cuda:
+            raise B200Error("CrossAttentionB200 needs CUDA tensors (there is no CPU fallback)")
+        lin = self.out_linear[0]
+        return _CrossAttentionFn.apply(net, context, self.to_q.weight, self.to_k.weight, self.to_v.weight, lin.weight, lin.bias, self.num_heads)

@@ -61,8 +61,10 @@ __device__ __forceinline__ void a_frag(const float (&v)[32], int s, uint32_t (&a
 }
 // Stores a warpgroup's 64 x 64 accumulator (rows row0 + {0, 8} per thread, see ptx.cuh) times `sc` as bf16 at g0 + row *
 // stride; rows >= nrows are skipped.  csum (optional): this warp's fp32 column sums of the bf16 values written, 64 floats.
+// kCols: columns >= ncols are skipped as well (a head dim padded to whole 64-column boxes).
+template <bool kCols = false>
 __device__ __forceinline__ void store_tile(const float (&v)[32], float sc, __nv_bfloat16* g0, long long stride, int row0, int nrows,
-                                           int lane, float* csum) {
+                                           int lane, float* csum, int ncols = 64) {
     const int c0 = (lane & 3) * 2;
     float cs[16];
 #pragma unroll
@@ -71,7 +73,7 @@ __device__ __forceinline__ void store_tile(const float (&v)[32], float sc, __nv_
         for (int h = 0; h < 2; ++h) {
             const int row = row0 + h * 8;
             const uint32_t t = pack_bf16x2(v[4 * j + 2 * h] * sc, v[4 * j + 2 * h + 1] * sc);
-            const bool ok = row < nrows;
+            const bool ok = row < nrows && (!kCols || j * 8 + c0 < ncols);
             if (ok) *reinterpret_cast<uint32_t*>(g0 + row * stride + j * 8 + c0) = t;
             if (h == 0) { cs[2 * j] = 0.f; cs[2 * j + 1] = 0.f; }
             if (ok) { cs[2 * j] += bf16lo(t); cs[2 * j + 1] += bf16hi(t); }
@@ -386,52 +388,130 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant
 }
 
 // ------------------------------------------------------------------------------------------------
-// streamed kernels for long sequences (1 <= T <= 16384)
+// streamed kernels (1 <= Tq, Tk <= 16384, head dim Dh <= 160, separate Q / K / V operands)
 // ------------------------------------------------------------------------------------------------
 // The kernels above hold a head's whole K / V (or Q / dO) in shared memory, loaded as ONE TMA box of tp <= 256 rows.
 // The kernels below keep one side of the product resident and stream the other through a ring of 64-row TMA blocks with
 // full / empty mbarriers (FlashAttention-2 scheme, the pipeline of the GEMM in gemm_sm90.cu):
 //   forward   one CTA per (image, head, 128-query tile): Q resident, K / V streamed, online softmax in fp32
 //   delta     delta = rowsum(dO o O) in fp32, one value per (image, head, query), into the workspace
-//   dK / dV   one CTA per (image, head, 128-key tile): K / V resident, Q / dO streamed with their lse / delta rows
+//   dK / dV   one CTA per (image, head, key tile[, query chunk]): K / V resident, Q / dO streamed with their lse / delta rows
 //   dQ        one CTA per (image, head, 128-query tile): Q / dO / lse / delta resident, K / V streamed
-//   dbias     per-64-row-tile column sums of the stored dq | dk | dv, summed per image in a fixed order
-// Warp 8 is the TMA producer; warpgroup g in {0, 1} owns rows [64 g, 64 g + 64) of the CTA's tile.  Causal CTAs stop at
-// the diagonal.  Nothing is accumulated with atomics: two runs give bit-identical results.
+//   dbias     per-64-row-tile column sums of the stored dq | dk | dv, summed per image in a fixed order (packed layout only)
+// Q is [B, Tq, ldq] with head h at column h * Dh, K / V are [B, Tk, ldkv]; the packed qkv tensor is q = qkv, k = qkv + D,
+// v = qkv + 2 D with ld = 3 D.  Every operand is read through a 4-D tensor map {Dh, H, T, B} with 64 x 64 boxes, so columns
+// >= Dh and rows >= T arrive as zeros.  The kernels are instantiated per k16-step count KS of S = Q K^T and dP = dO V^T
+// (attn_long_ksteps: ceil(Dh / 16) up to Dh 80, then 8 and 10), the head dim is padded to NB = ceil(KS / 4) whole 64-column
+// boxes, and outputs skip the padding.
+// Warp 8 is the TMA producer; warpgroup g in {0, 1} owns rows [64 g, 64 g + 64) of the CTA's tile (the NB > 1 dK / dV kernel
+// splits its work differently, see there).  Causal CTAs (Tq == Tk) stop at the diagonal.  Nothing is accumulated with
+// atomics: two runs give bit-identical results.
 constexpr int LA_THREADS = 288;  // two consumer warpgroups + the producer warp
-constexpr int LA_STAGES = 4;
 constexpr int LA_MAX_T = 16384;
+constexpr int LA_MAX_DH = 160;
+constexpr int LA_SMS = 132;  // H100 SXM: a dK / dV grid smaller than this is split over the queries
+
+struct LongParams {
+    int B, Tq, Tk, H, Dh;
+    long long ldq, ldkv, ldo;  // leading dims (elements) of q / dq, k / v / dk / dv, out / dout
+    float scale;
+    int causal;
+    int qb_chunk;  // dK / dV: 64-query blocks per chunk
+    int nchunk;    // dK / dV: query chunks; > 1 writes fp32 partials that attn_long_dkdv_reduce_kernel sums in chunk order
+};
+
+// Shared-memory layouts per padded head dim.  Stage counts keep every kernel <= 227 KB; NB = 1 fits two forward CTAs per SM.
+template <int NB>
+struct LongCfg {
+    static constexpr int BOX = NB * TILE_BYTES;  // one 64-row block over the padded head dim
+    // forward: 128-query tile, per stage a K block and a V block
+    static constexpr int F_STAGES = NB == 3 ? 3 : 4;
+    static constexpr int F_Q = 0;
+    static constexpr int F_KV = 2 * BOX;
+    static constexpr int F_BAR = F_KV + F_STAGES * 2 * BOX;  // full[S], empty[S], q
+    static constexpr int F_SMEM = F_BAR + 128 + 1024;
+    // dK / dV: NB = 1 keeps a 128-key tile, a warpgroup per 64 keys, each accumulating dK and dV.  For NB > 1 those two
+    // accumulators (2 x 32 NB fp32 per thread) plus S^T and dP^T exceed the register budget, so both warpgroups share a 64-key
+    // tile: warpgroup 0 computes P^T and dV += P^T dO, warpgroup 1 dP^T, dS^T and dK += dS^T Q, and P^T is handed from 0 to 1
+    // through shared memory in fp32 (K_PB) -- two GEMMs per warpgroup, nothing recomputed.
+    static constexpr int K_ROWS = NB == 1 ? 128 : 64;
+    static constexpr int K_STAGES = NB == 3 ? 3 : 4;
+    static constexpr int K_K = 0;
+    static constexpr int K_V = K_ROWS / 64 * BOX;
+    static constexpr int K_QD = 2 * K_V;                          // per stage: Q block, dO block
+    static constexpr int K_ROW = K_QD + K_STAGES * 2 * BOX;       // per stage: lse * log2(e) [64], delta [64]
+    static constexpr int K_CS = K_ROW + K_STAGES * 512;           // NB = 1: [dk | dv][warpgroup][warp][64] column sums
+    static constexpr int K_PB = K_CS + (NB == 1 ? 2 * 8 * 64 * 4 : 0);  // NB > 1: P^T, [32 values][128 threads] fp32
+    static constexpr int K_BAR = K_PB + (NB == 1 ? 0 : 32 * 128 * 4);
+    static constexpr int K_SMEM = K_BAR + 128 + 1024;
+    // dQ: 128-query tile of Q and dO, per stage a K block and a V block
+    static constexpr int Q_STAGES = NB == 3 ? 2 : 4;
+    static constexpr int Q_Q = 0;
+    static constexpr int Q_DO = 2 * BOX;
+    static constexpr int Q_KV = 4 * BOX;
+    static constexpr int Q_CS = Q_KV + Q_STAGES * 2 * BOX;  // [warpgroup][warp][64] column sums
+    static constexpr int Q_BAR = Q_CS + 8 * 64 * 4;
+    static constexpr int Q_SMEM = Q_BAR + 128 + 1024;
+};
+static_assert(LongCfg<1>::F_SMEM == 83072 && LongCfg<1>::K_SMEM == 105600 && LongCfg<1>::Q_SMEM == 101504, "Dh 64 layouts");
+static_assert(LongCfg<3>::F_SMEM <= 232448 && LongCfg<3>::K_SMEM <= 232448 && LongCfg<3>::Q_SMEM <= 232448, "227 KB");
+static_assert(LongCfg<2>::F_SMEM <= 232448 && LongCfg<2>::K_SMEM <= 232448 && LongCfg<2>::Q_SMEM <= 232448, "227 KB");
 
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
+    asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 
-// forward: 80 KB + barriers, so that two CTAs (four consumer warpgroups) share an SM
-constexpr int LF_SQ = 0;                                   // 16 KB: the 128-query tile
-constexpr int LF_SKV = 16384;                              // per stage: K block, V block (8 KB each)
-constexpr int LF_BAR = LF_SKV + LA_STAGES * 2 * TILE_BYTES;  // full[S], empty[S], q
-constexpr int LF_SMEM = LF_BAR + 128 + 1024;
+// acc = A B^T over the first KS k16 steps of the padded head dim: A and B are 64-row blocks of K-major 64-column boxes
+template <int KS>
+__device__ __forceinline__ void mma_rows_kk(float (&acc)[32], uint32_t a_base, uint32_t b_base) {
+#pragma unroll
+    for (int kk = 0; kk < KS; ++kk) {
+        const uint32_t off = (kk >> 2) * TILE_BYTES + (kk & 3) * 32;
+        wgmma_m64n64k16_ss(acc, kmajor_desc(a_base + off), kmajor_desc(b_base + off), kk > 0 ? 1u : 0u);
+    }
+}
 
-__global__ void __launch_bounds__(LA_THREADS, 2)
-attn_long_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __restrict__ out, float* __restrict__ lse_out,
-                     const AttnParams p) {
+// fp32 copy of a warpgroup's 64 x 64 accumulator: rows < nrows, columns < ncols, at p0 + row * ld
+__device__ __forceinline__ void store_part(const float (&v)[32], float* p0, int ld, int row0, int nrows, int ncols, int lane) {
+    const int c0 = (lane & 3) * 2;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = row0 + h * 8;
+            if (row < nrows && j * 8 + c0 < ncols)
+                *reinterpret_cast<float2*>(p0 + static_cast<long long>(row) * ld + j * 8 + c0) = make_float2(v[4 * j + 2 * h], v[4 * j + 2 * h + 1]);
+        }
+    }
+}
+
+template <int KS>
+__global__ void __launch_bounds__(LA_THREADS, KS <= 4 ? 2 : 1)
+attn_long_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
+                     __nv_bfloat16* __restrict__ out, float* __restrict__ lse_out, const LongParams p) {
+    constexpr int NB = (KS + 3) / 4;
+    using C = LongCfg<NB>;
+    constexpr int S = C::F_STAGES;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + LF_BAR);
-    uint64_t* empty = full + LA_STAGES;
-    uint64_t* bar_q = empty + LA_STAGES;
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + C::F_BAR);
+    uint64_t* empty = full + S;
+    uint64_t* bar_q = empty + S;
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const int n_mt = (p.T + 127) / 128;
+    const int n_mt = (p.Tq + 127) / 128;
     const int mt = blockIdx.x % n_mt;
     const int bh = blockIdx.x / n_mt;
     const int h = bh % p.H;
     const int b = bh / p.H;
-    const int n_cons = mt * 128 + 64 < p.T ? 2 : 1;  // warpgroups with at least one query row < T
-    const int nkb_all = (p.T + 63) / 64;
+    const int n_cons = mt * 128 + 64 < p.Tq ? 2 : 1;  // warpgroups with at least one query row < Tq
+    const int nkb_all = (p.Tk + 63) / 64;
     const int nkb = p.causal ? min(nkb_all, 2 * mt + n_cons) : nkb_all;  // key blocks this CTA streams
     if (threadIdx.x == 0) {
-        for (int s = 0; s < LA_STAGES; ++s) {
+        for (int s = 0; s < S; ++s) {
             mbar_init(&full[s], 1);
             mbar_init(&empty[s], 4 * n_cons);  // one arrival per consumer warp
         }
@@ -443,16 +523,22 @@ attn_long_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* _
     if (warp == 8) {
         // ---- producer: Q once, then the K / V blocks through the ring ----
         if (lane == 0) {
-            tma_prefetch_desc(&tmQKV);
-            mbar_expect_tx(bar_q, static_cast<uint32_t>(n_cons) * TILE_BYTES);
-            for (int g = 0; g < n_cons; ++g) tma_load_3d(smem + LF_SQ + g * TILE_BYTES, &tmQKV, bar_q, h * 64, mt * 128 + g * 64, b);
+            tma_prefetch_desc(&tmQ);
+            tma_prefetch_desc(&tmK);
+            tma_prefetch_desc(&tmV);
+            mbar_expect_tx(bar_q, static_cast<uint32_t>(n_cons) * C::BOX);
+            for (int g = 0; g < n_cons; ++g)
+                for (int c = 0; c < NB; ++c)
+                    tma_load_4d(smem + C::F_Q + (g * NB + c) * TILE_BYTES, &tmQ, bar_q, c * 64, h, mt * 128 + g * 64, b);
             for (int kb = 0; kb < nkb; ++kb) {
-                const int s = kb % LA_STAGES;
-                mbar_wait(&empty[s], ((kb / LA_STAGES) & 1) ^ 1u);
-                uint8_t* dst = smem + LF_SKV + s * 2 * TILE_BYTES;
-                mbar_expect_tx(&full[s], 2u * TILE_BYTES);
-                tma_load_3d(dst, &tmQKV, &full[s], p.D + h * 64, kb * 64, b);
-                tma_load_3d(dst + TILE_BYTES, &tmQKV, &full[s], 2 * p.D + h * 64, kb * 64, b);
+                const int s = kb % S;
+                mbar_wait(&empty[s], ((kb / S) & 1) ^ 1u);
+                uint8_t* dst = smem + C::F_KV + s * 2 * C::BOX;
+                mbar_expect_tx(&full[s], 2u * C::BOX);
+                for (int c = 0; c < NB; ++c) {
+                    tma_load_4d(dst + c * TILE_BYTES, &tmK, &full[s], c * 64, h, kb * 64, b);
+                    tma_load_4d(dst + C::BOX + c * TILE_BYTES, &tmV, &full[s], c * 64, h, kb * 64, b);
+                }
             }
         }
         return;
@@ -466,33 +552,35 @@ attn_long_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* _
     const int diag = q0 / 64;  // the key block on the diagonal of this warpgroup's queries
     const int nkb_g = p.causal ? min(nkb, diag + 1) : nkb;
     const float sl2 = p.scale * kLog2e;
-    const uint32_t q_base = smem_u32(smem + LF_SQ) + g * TILE_BYTES;
+    const uint32_t q_base = smem_u32(smem + C::F_Q) + g * C::BOX;
 
-    float o[32];
+    float o[NB][32];
 #pragma unroll
-    for (int e = 0; e < 32; ++e) o[e] = 0.f;
+    for (int c = 0; c < NB; ++c)
+#pragma unroll
+        for (int e = 0; e < 32; ++e) o[c][e] = 0.f;
     // running row max (raw scores) and this thread's share of the row sum; every row has a valid key in block 0, so m is
     // finite from the first block on
     float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
     mbar_wait(bar_q, 0);
     for (int kb = 0; kb < nkb; ++kb) {
-        const int s = kb % LA_STAGES;
-        mbar_wait(&full[s], (kb / LA_STAGES) & 1);
+        const int s = kb % S;
+        mbar_wait(&full[s], (kb / S) & 1);
         if (kb < nkb_g) {
-            const uint32_t k_base = smem_u32(smem + LF_SKV + s * 2 * TILE_BYTES);
+            const uint32_t k_base = smem_u32(smem + C::F_KV + s * 2 * C::BOX);
             float sc[32];
             wgmma_fence();
-            mma_tile_kk(sc, q_base, k_base);
+            mma_rows_kk<KS>(sc, q_base, k_base);
             wgmma_commit();
             wgmma_wait<0>();
             reg_fence(sc);
-            if (kb * 64 + 64 > p.T || (p.causal && kb == diag)) {
-                // keys >= T were zero-filled by TMA and score 0, not -inf; causal: keys after the query
+            if (kb * 64 + 64 > p.Tk || (p.causal && kb == diag)) {
+                // keys >= Tk were zero-filled by TMA and score 0, not -inf; causal: keys after the query
 #pragma unroll
                 for (int e = 0; e < 32; ++e) {
                     const int hr = (e >> 1) & 1;
                     const int j = kb * 64 + (e >> 2) * 8 + jq + (e & 1);
-                    if (!(j < p.T && (!p.causal || j <= i0 + 8 * hr))) sc[e] = -INFINITY;
+                    if (!(j < p.Tk && (!p.causal || j <= i0 + 8 * hr))) sc[e] = -INFINITY;
                 }
             }
             float mn[2] = {m[0], m[1]};
@@ -519,18 +607,22 @@ attn_long_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* _
                 m[hr] = mn[hr];
             }
 #pragma unroll
-            for (int e = 0; e < 32; ++e) o[e] *= alpha[(e >> 1) & 1];
+            for (int c = 0; c < NB; ++c)
+#pragma unroll
+                for (int e = 0; e < 32; ++e) o[c][e] *= alpha[(e >> 1) & 1];
             // O += P V: P from registers (bf16), V MN-major from the stage
             wgmma_fence();
 #pragma unroll
             for (int st = 0; st < 4; ++st) {
                 uint32_t a[4];
                 a_frag(sc, st, a);
-                wgmma_m64n64k16_rs_tb(o, a, mnmajor_desc(k_base + TILE_BYTES + st * 2048), 1u);
+#pragma unroll
+                for (int c = 0; c < NB; ++c) wgmma_m64n64k16_rs_tb(o[c], a, mnmajor_desc(k_base + C::BOX + c * TILE_BYTES + st * 2048), 1u);
             }
             wgmma_commit();
             wgmma_wait<0>();
-            reg_fence(o);
+#pragma unroll
+            for (int c = 0; c < NB; ++c) reg_fence(o[c]);
         }
         if (lane == 0) mbar_arrive(&empty[s]);
     }
@@ -540,31 +632,34 @@ attn_long_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* _
         l[hr] += __shfl_xor_sync(0xffffffffu, l[hr], 2);
     }
     const float inv[2] = {1.0f / l[0], 1.0f / l[1]};
+    __nv_bfloat16* g0 = out + static_cast<long long>(b) * p.Tq * p.ldo + h * p.Dh;
 #pragma unroll
-    for (int e = 0; e < 32; ++e) o[e] *= inv[(e >> 1) & 1];
-    store_tile(o, 1.0f, out + (static_cast<long long>(b) * p.T) * p.D + h * 64, p.D, i0, p.T, lane, nullptr);
+    for (int c = 0; c < NB; ++c) {
+#pragma unroll
+        for (int e = 0; e < 32; ++e) o[c][e] *= inv[(e >> 1) & 1];
+        store_tile<true>(o[c], 1.0f, g0 + c * 64, p.ldo, i0, p.Tq, lane, nullptr, p.Dh - c * 64);
+    }
     if ((lane & 3) == 0) {
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
             const int i = i0 + 8 * hr;
-            if (i < p.T) lse_out[(static_cast<long long>(b) * p.H + h) * p.T + i] = m[hr] * p.scale + logf(l[hr]);
+            if (i < p.Tq) lse_out[static_cast<long long>(bh) * p.Tq + i] = m[hr] * p.scale + logf(l[hr]);
         }
     }
 }
 
-// delta[b, h, i] = sum_d dO[b, i, h, d] O[b, i, h, d] in fp32: one (row, head) per thread, 128 contiguous bytes of each
+// delta[b, h, i] = sum_d dO[b, i, h, d] O[b, i, h, d] in fp32: one (row, head) per thread, 2 Dh contiguous bytes of each
 __global__ void attn_long_delta_kernel(const __nv_bfloat16* __restrict__ o_in, const __nv_bfloat16* __restrict__ do_in,
-                                       float* __restrict__ delta, int B, int T, int H) {
+                                       float* __restrict__ delta, int B, int T, int H, int Dh, long long ldo) {
     const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (idx >= static_cast<long long>(B) * T * H) return;
     const int h = static_cast<int>(idx % H);
     const long long row = idx / H;
     const int b = static_cast<int>(row / T), i = static_cast<int>(row % T);
-    const uint4* po = reinterpret_cast<const uint4*>(o_in + idx * 64);
-    const uint4* pd = reinterpret_cast<const uint4*>(do_in + idx * 64);
+    const uint4* po = reinterpret_cast<const uint4*>(o_in + row * ldo + h * Dh);
+    const uint4* pd = reinterpret_cast<const uint4*>(do_in + row * ldo + h * Dh);
     float dl = 0.f;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
+    for (int k = 0; k < Dh / 8; ++k) {
         const uint4 a = __ldg(po + k), gg = __ldg(pd + k);
         dl += bf16lo(a.x) * bf16lo(gg.x) + bf16hi(a.x) * bf16hi(gg.x) + bf16lo(a.y) * bf16lo(gg.y) + bf16hi(a.y) * bf16hi(gg.y) +
               bf16lo(a.z) * bf16lo(gg.z) + bf16hi(a.z) * bf16hi(gg.z) + bf16lo(a.w) * bf16lo(gg.w) + bf16hi(a.w) * bf16hi(gg.w);
@@ -576,38 +671,39 @@ __global__ void attn_long_delta_kernel(const __nv_bfloat16* __restrict__ o_in, c
 // Sums the 64-column partials of the 4 warps of warpgroup g (cs: [4][64], written by store_tile) in a fixed order.
 __device__ __forceinline__ float wg_colsum(const float* cs, int c) { return ((cs[c] + cs[64 + c]) + cs[128 + c]) + cs[192 + c]; }
 
-// dK / dV: 96 KB of tiles + lse / delta rows + column sums
-constexpr int LK_SK = 0;                                     // 16 KB: the 128-key tile
-constexpr int LK_SV = 16384;                                 // 16 KB
-constexpr int LK_SQD = 32768;                                // per stage: Q block, dO block
-constexpr int LK_ROW = LK_SQD + LA_STAGES * 2 * TILE_BYTES;  // per stage: lse * log2(e) [64], delta [64]
-constexpr int LK_CS = LK_ROW + LA_STAGES * 512;              // [dk | dv][warpgroup][warp][64] column sums
-constexpr int LK_BAR = LK_CS + 2 * 8 * 64 * 4;
-constexpr int LK_SMEM = LK_BAR + 128 + 1024;
-
+// dK / dV.  CTA = (query chunk, key tile, image, head) with the chunk fastest.  With one chunk dK / dV are stored as bf16; with
+// several, chunk c writes its fp32 sums to part[dk | dv][c][B * H][Tk][Dh] and attn_long_dkdv_reduce_kernel finishes them.
+template <int KS>
 __global__ void __launch_bounds__(LA_THREADS, 1)
-attn_long_dkdv_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmDO,
-                      const float* __restrict__ lse_in, const float* __restrict__ delta_in, __nv_bfloat16* __restrict__ dqkv,
-                      float* __restrict__ csum_part, const AttnParams p) {
+attn_long_dkdv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
+                      const __grid_constant__ CUtensorMap tmDO, const float* __restrict__ lse_in, const float* __restrict__ delta_in,
+                      __nv_bfloat16* __restrict__ dk_out, __nv_bfloat16* __restrict__ dv_out, float* __restrict__ part,
+                      float* __restrict__ csum_part, const LongParams p) {
+    constexpr int NB = (KS + 3) / 4;
+    using C = LongCfg<NB>;
+    constexpr int S = C::K_STAGES;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + LK_BAR);
-    uint64_t* empty = full + LA_STAGES;
-    uint64_t* bar_kv = empty + LA_STAGES;
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + C::K_BAR);
+    uint64_t* empty = full + S;
+    uint64_t* bar_kv = empty + S;
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const int n_kt = (p.T + 127) / 128;
-    const int kt = blockIdx.x % n_kt;
-    const int bh = blockIdx.x / n_kt;
+    const int n_kt = (p.Tk + C::K_ROWS - 1) / C::K_ROWS;
+    const int chunk = blockIdx.x % p.nchunk;
+    const int kt = (blockIdx.x / p.nchunk) % n_kt;
+    const int bh = blockIdx.x / p.nchunk / n_kt;
     const int h = bh % p.H;
     const int b = bh / p.H;
-    const int n_cons = kt * 128 + 64 < p.T ? 2 : 1;
-    const int nqb = (p.T + 63) / 64;
-    const int qb0 = p.causal ? 2 * kt : 0;  // causal: query blocks wholly before the key tile contribute nothing
+    const int n_kb = (NB == 1 && kt * 128 + 64 < p.Tk) ? 2 : 1;  // resident 64-key blocks
+    const int nqb = (p.Tq + 63) / 64;
+    // causal: query blocks wholly before the key tile contribute nothing
+    const int qb_lo = max(chunk * p.qb_chunk, p.causal ? kt * (C::K_ROWS / 64) : 0);
+    const int qb_hi = min(nqb, (chunk + 1) * p.qb_chunk);
     if (threadIdx.x == 0) {
-        for (int s = 0; s < LA_STAGES; ++s) {
+        for (int s = 0; s < S; ++s) {
             mbar_init(&full[s], 1 + 32);  // the producer's expect_tx + one arrival per producer lane after its lse / delta stores
-            mbar_init(&empty[s], 4 * n_cons);
+            mbar_init(&empty[s], NB == 1 ? 4 * n_kb : 8);
         }
         mbar_init(bar_kv, 1);
         fence_mbar_init();
@@ -617,137 +713,246 @@ attn_long_dkdv_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_co
     if (warp == 8) {
         // ---- producer: K / V once, then Q / dO blocks (TMA) and their lse / delta rows (lanes) through the ring ----
         if (lane == 0) {
-            tma_prefetch_desc(&tmQKV);
+            tma_prefetch_desc(&tmQ);
+            tma_prefetch_desc(&tmK);
+            tma_prefetch_desc(&tmV);
             tma_prefetch_desc(&tmDO);
-            mbar_expect_tx(bar_kv, 2u * n_cons * TILE_BYTES);
-            for (int g = 0; g < n_cons; ++g) {
-                tma_load_3d(smem + LK_SK + g * TILE_BYTES, &tmQKV, bar_kv, p.D + h * 64, kt * 128 + g * 64, b);
-                tma_load_3d(smem + LK_SV + g * TILE_BYTES, &tmQKV, bar_kv, 2 * p.D + h * 64, kt * 128 + g * 64, b);
-            }
+            mbar_expect_tx(bar_kv, 2u * n_kb * C::BOX);
+            for (int g = 0; g < n_kb; ++g)
+                for (int c = 0; c < NB; ++c) {
+                    tma_load_4d(smem + C::K_K + (g * NB + c) * TILE_BYTES, &tmK, bar_kv, c * 64, h, kt * C::K_ROWS + g * 64, b);
+                    tma_load_4d(smem + C::K_V + (g * NB + c) * TILE_BYTES, &tmV, bar_kv, c * 64, h, kt * C::K_ROWS + g * 64, b);
+                }
         }
-        const float* lse_bh = lse_in + static_cast<long long>(bh) * p.T;
-        const float* delta_bh = delta_in + static_cast<long long>(bh) * p.T;
-        for (int qb = qb0, it = 0; qb < nqb; ++qb, ++it) {
-            const int s = it % LA_STAGES;
-            mbar_wait(&empty[s], ((it / LA_STAGES) & 1) ^ 1u);
+        const float* lse_bh = lse_in + static_cast<long long>(bh) * p.Tq;
+        const float* delta_bh = delta_in + static_cast<long long>(bh) * p.Tq;
+        for (int qb = qb_lo, it = 0; qb < qb_hi; ++qb, ++it) {
+            const int s = it % S;
+            mbar_wait(&empty[s], ((it / S) & 1) ^ 1u);
             if (lane == 0) {
-                uint8_t* dst = smem + LK_SQD + s * 2 * TILE_BYTES;
-                mbar_expect_tx(&full[s], 2u * TILE_BYTES);
-                tma_load_3d(dst, &tmQKV, &full[s], h * 64, qb * 64, b);
-                tma_load_3d(dst + TILE_BYTES, &tmDO, &full[s], h * 64, qb * 64, b);
+                uint8_t* dst = smem + C::K_QD + s * 2 * C::BOX;
+                mbar_expect_tx(&full[s], 2u * C::BOX);
+                for (int c = 0; c < NB; ++c) {
+                    tma_load_4d(dst + c * TILE_BYTES, &tmQ, &full[s], c * 64, h, qb * 64, b);
+                    tma_load_4d(dst + C::BOX + c * TILE_BYTES, &tmDO, &full[s], c * 64, h, qb * 64, b);
+                }
             }
-            float* row = reinterpret_cast<float*>(smem + LK_ROW + s * 512);
+            float* row = reinterpret_cast<float*>(smem + C::K_ROW + s * 512);
 #pragma unroll
             for (int k = 0; k < 2; ++k) {
                 const int r = lane + 32 * k, i = qb * 64 + r;
                 // padded query rows: lse = +inf makes P = dS = 0 (their Q / dO rows are zero-filled as well)
-                row[r] = i < p.T ? __ldg(lse_bh + i) * kLog2e : INFINITY;
-                row[64 + r] = i < p.T ? __ldg(delta_bh + i) : 0.f;
+                row[r] = i < p.Tq ? __ldg(lse_bh + i) * kLog2e : INFINITY;
+                row[64 + r] = i < p.Tq ? __ldg(delta_bh + i) : 0.f;
             }
             mbar_arrive(&full[s]);
         }
         return;
     }
     const int g = warp >> 2;
-    if (g >= n_cons) return;
     const int wq = warp & 3;
     const int rl = wq * 16 + (lane >> 2);  // accumulator rows rl, rl + 8: keys
     const int jq = (lane & 3) * 2;         // accumulator columns 8 n + jq (+ 1): queries
-    const int k0 = kt * 128 + g * 64;
-    const int key0 = k0 + rl;
-    const int diag = k0 / 64;
-    const int qb_g = p.causal ? diag : 0;
     const float sl2 = p.scale * kLog2e;
-    const uint32_t k_base = smem_u32(smem + LK_SK) + g * TILE_BYTES, v_base = smem_u32(smem + LK_SV) + g * TILE_BYTES;
-    const bool key_edge = k0 + 64 > p.T;
+    const long long n_part = static_cast<long long>(p.nchunk) * p.B * p.H * p.Tk * p.Dh;  // floats per dk / dv partial set
+    const long long kv_row0 = static_cast<long long>(b) * p.Tk;
 
-    float dv[32], dk[32];
+    if constexpr (NB == 1) {
+        if (g >= n_kb) return;
+        const int k0 = kt * 128 + g * 64;
+        const int key0 = k0 + rl;
+        const int diag = k0 / 64;
+        const int qb_g = p.causal ? diag : 0;
+        const uint32_t k_base = smem_u32(smem + C::K_K) + g * TILE_BYTES, v_base = smem_u32(smem + C::K_V) + g * TILE_BYTES;
+        const bool key_edge = k0 + 64 > p.Tk;
+
+        float dv[32], dk[32];
 #pragma unroll
-    for (int e = 0; e < 32; ++e) { dv[e] = 0.f; dk[e] = 0.f; }
-    mbar_wait(bar_kv, 0);
-    for (int qb = qb0, it = 0; qb < nqb; ++qb, ++it) {
-        const int s = it % LA_STAGES;
-        mbar_wait(&full[s], (it / LA_STAGES) & 1);
-        if (qb >= qb_g) {
-            const uint32_t q_st = smem_u32(smem + LK_SQD + s * 2 * TILE_BYTES), do_st = q_st + TILE_BYTES;
-            const float* row = reinterpret_cast<const float*>(smem + LK_ROW + s * 512);
-            float st[32], dpt[32];
+        for (int e = 0; e < 32; ++e) { dv[e] = 0.f; dk[e] = 0.f; }
+        mbar_wait(bar_kv, 0);
+        for (int qb = qb_lo, it = 0; qb < qb_hi; ++qb, ++it) {
+            const int s = it % S;
+            mbar_wait(&full[s], (it / S) & 1);
+            if (qb >= qb_g) {
+                const uint32_t q_st = smem_u32(smem + C::K_QD + s * 2 * C::BOX), do_st = q_st + C::BOX;
+                const float* row = reinterpret_cast<const float*>(smem + C::K_ROW + s * 512);
+                float st[32], dpt[32];
+                wgmma_fence();
+                mma_rows_kk<KS>(st, k_base, q_st);    // S^T = K Q^T
+                mma_rows_kk<KS>(dpt, v_base, do_st);  // dP^T = V dO^T
+                wgmma_commit();
+                wgmma_wait<0>();
+                reg_fence(st);
+                reg_fence(dpt);
+                const bool edge = key_edge || (p.causal && qb == diag);
+#pragma unroll
+                for (int e = 0; e < 32; ++e) {
+                    const int key = key0 + ((e >> 1) & 1) * 8;
+                    const int ii = (e >> 2) * 8 + jq + (e & 1);
+                    float pv = fast_ex2(fmaf(st[e], sl2, -row[ii]));
+                    if (edge && !(key < p.Tk && (!p.causal || key <= qb * 64 + ii))) pv = 0.f;
+                    st[e] = pv;
+                    asm volatile("" ::: "memory");  // keeps ptxas' schedule (and register count, 164) of the Dh-64 kernel
+                    dpt[e] = pv * (dpt[e] - row[64 + ii]);
+                }
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    uint32_t a[4];
+                    a_frag(st, k, a);
+                    wgmma_m64n64k16_rs_tb(dv, a, mnmajor_desc(do_st + k * 2048), 1u);  // dV += P^T dO
+                    a_frag(dpt, k, a);
+                    wgmma_m64n64k16_rs_tb(dk, a, mnmajor_desc(q_st + k * 2048), 1u);   // dK += dS^T Q
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                reg_fence(dv);
+                reg_fence(dk);
+            }
+            if (lane == 0) mbar_arrive(&empty[s]);
+        }
+        if (p.nchunk > 1) {
+            const long long at = ((static_cast<long long>(chunk) * p.B * p.H + bh) * p.Tk) * p.Dh;
+            store_part(dk, part + at, p.Dh, key0, p.Tk, p.Dh, lane);
+            store_part(dv, part + n_part + at, p.Dh, key0, p.Tk, p.Dh, lane);
+            return;
+        }
+        float* cs = reinterpret_cast<float*>(smem + C::K_CS);
+        const bool sums = csum_part != nullptr;
+        const long long off = kv_row0 * p.ldkv + h * p.Dh;
+        store_tile<true>(dk, p.scale, dk_out + off, p.ldkv, key0, p.Tk, lane, sums ? cs + ((0 * 2 + g) * 4 + wq) * 64 : nullptr, p.Dh);
+        store_tile<true>(dv, 1.0f, dv_out + off, p.ldkv, key0, p.Tk, lane, sums ? cs + ((1 * 2 + g) * 4 + wq) * 64 : nullptr, p.Dh);
+        if (sums) {
+            named_bar_sync(1 + g, 128);
+            const int t = threadIdx.x & 127, sec = t >> 6, c = t & 63;
+            float* dst = csum_part + (static_cast<long long>(bh) * ((p.Tq + 63) / 64) + diag) * 192;
+            dst[(1 + sec) * 64 + c] = wg_colsum(cs + (sec * 2 + g) * 4 * 64, c);
+        }
+    } else {
+        // both warpgroups on keys [64 kt, 64 kt + 64): 0 -> P^T, dV;  1 -> dP^T, dS^T, dK.  P^T goes through K_PB, guarded by
+        // named barriers 3 (P^T written) and 4 (P^T read, the buffer may be overwritten)
+        const int key0 = kt * 64 + rl;
+        const uint32_t k_base = smem_u32(smem + C::K_K), v_base = smem_u32(smem + C::K_V);
+        const bool key_edge = kt * 64 + 64 > p.Tk;
+        float* pb = reinterpret_cast<float*>(smem + C::K_PB) + (threadIdx.x & 127);
+        float acc[NB][32];
+#pragma unroll
+        for (int c = 0; c < NB; ++c)
+#pragma unroll
+            for (int e = 0; e < 32; ++e) acc[c][e] = 0.f;
+        mbar_wait(bar_kv, 0);
+        for (int qb = qb_lo, it = 0; qb < qb_hi; ++qb, ++it) {
+            const int s = it % S;
+            mbar_wait(&full[s], (it / S) & 1);
+            const uint32_t q_st = smem_u32(smem + C::K_QD + s * 2 * C::BOX), do_st = q_st + C::BOX;
+            const float* row = reinterpret_cast<const float*>(smem + C::K_ROW + s * 512);
+            float x[32];
             wgmma_fence();
-            mma_tile_kk(st, k_base, q_st);    // S^T = K Q^T
-            mma_tile_kk(dpt, v_base, do_st);  // dP^T = V dO^T
+            if (g == 0)
+                mma_rows_kk<KS>(x, k_base, q_st);   // S^T = K Q^T
+            else
+                mma_rows_kk<KS>(x, v_base, do_st);  // dP^T = V dO^T
             wgmma_commit();
             wgmma_wait<0>();
-            reg_fence(st);
-            reg_fence(dpt);
-            const bool edge = key_edge || (p.causal && qb == diag);
+            reg_fence(x);
+            if (g == 0) {
+                const bool edge = key_edge || (p.causal && qb == kt);
 #pragma unroll
-            for (int e = 0; e < 32; ++e) {
-                const int key = key0 + ((e >> 1) & 1) * 8;
-                const int ii = (e >> 2) * 8 + jq + (e & 1);
-                float pv = fast_ex2(fmaf(st[e], sl2, -row[ii]));
-                if (edge && !(key < p.T && (!p.causal || key <= qb * 64 + ii))) pv = 0.f;
-                st[e] = pv;
-                dpt[e] = pv * (dpt[e] - row[64 + ii]);
+                for (int e = 0; e < 32; ++e) {
+                    const int key = key0 + ((e >> 1) & 1) * 8;
+                    const int ii = (e >> 2) * 8 + jq + (e & 1);
+                    float pv = fast_ex2(fmaf(x[e], sl2, -row[ii]));
+                    if (edge && !(key < p.Tk && (!p.causal || key <= qb * 64 + ii))) pv = 0.f;
+                    x[e] = pv;
+                }
+                if (qb > qb_lo) named_bar_sync(4, 256);
+#pragma unroll
+                for (int e = 0; e < 32; ++e) pb[e * 128] = x[e];
+                named_bar_arrive(3, 256);
+            } else {
+                named_bar_sync(3, 256);
+#pragma unroll
+                for (int e = 0; e < 32; ++e) x[e] = pb[e * 128] * (x[e] - row[64 + (e >> 2) * 8 + jq + (e & 1)]);
+                if (qb + 1 < qb_hi) named_bar_arrive(4, 256);
             }
+            const uint32_t b_st = g == 0 ? do_st : q_st;  // dV += P^T dO  |  dK += dS^T Q
             wgmma_fence();
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
                 uint32_t a[4];
-                a_frag(st, k, a);
-                wgmma_m64n64k16_rs_tb(dv, a, mnmajor_desc(do_st + k * 2048), 1u);  // dV += P^T dO
-                a_frag(dpt, k, a);
-                wgmma_m64n64k16_rs_tb(dk, a, mnmajor_desc(q_st + k * 2048), 1u);   // dK += dS^T Q
+                a_frag(x, k, a);
+#pragma unroll
+                for (int c = 0; c < NB; ++c) wgmma_m64n64k16_rs_tb(acc[c], a, mnmajor_desc(b_st + c * TILE_BYTES + k * 2048), 1u);
             }
             wgmma_commit();
             wgmma_wait<0>();
-            reg_fence(dv);
-            reg_fence(dk);
+#pragma unroll
+            for (int c = 0; c < NB; ++c) reg_fence(acc[c]);
+            if (lane == 0) mbar_arrive(&empty[s]);
         }
-        if (lane == 0) mbar_arrive(&empty[s]);
-    }
-    const long long D3 = 3ll * p.D;
-    __nv_bfloat16* g0 = dqkv + (static_cast<long long>(b) * p.T) * D3 + h * 64;
-    float* cs = reinterpret_cast<float*>(smem + LK_CS);
-    const bool sums = csum_part != nullptr;
-    store_tile(dk, p.scale, g0 + p.D, D3, key0, p.T, lane, sums ? cs + ((0 * 2 + g) * 4 + wq) * 64 : nullptr);
-    store_tile(dv, 1.0f, g0 + 2 * p.D, D3, key0, p.T, lane, sums ? cs + ((1 * 2 + g) * 4 + wq) * 64 : nullptr);
-    if (sums) {
-        named_bar_sync(1 + g, 128);
-        const int t = threadIdx.x & 127, sec = t >> 6, c = t & 63;
-        float* dst = csum_part + (static_cast<long long>(bh) * ((p.T + 63) / 64) + diag) * 192;
-        dst[(1 + sec) * 64 + c] = wg_colsum(cs + (sec * 2 + g) * 4 * 64, c);
+        if (p.nchunk > 1) {
+            float* dst = part + (g == 0 ? n_part : 0) + ((static_cast<long long>(chunk) * p.B * p.H + bh) * p.Tk) * p.Dh;
+#pragma unroll
+            for (int c = 0; c < NB; ++c) store_part(acc[c], dst + c * 64, p.Dh, key0, p.Tk, p.Dh - c * 64, lane);
+            return;
+        }
+        __nv_bfloat16* dst = (g == 0 ? dv_out : dk_out) + kv_row0 * p.ldkv + h * p.Dh;
+        const float sc = g == 0 ? 1.0f : p.scale;
+#pragma unroll
+        for (int c = 0; c < NB; ++c) store_tile<true>(acc[c], sc, dst + c * 64, p.ldkv, key0, p.Tk, lane, nullptr, p.Dh - c * 64);
     }
 }
 
-// dQ: 96 KB of tiles + column sums
-constexpr int LQ_SQ = 0;                                  // 16 KB: the 128-query tile
-constexpr int LQ_SDO = 16384;                             // 16 KB
-constexpr int LQ_SKV = 32768;                             // per stage: K block, V block
-constexpr int LQ_CS = LQ_SKV + LA_STAGES * 2 * TILE_BYTES;  // [warpgroup][warp][64] column sums
-constexpr int LQ_BAR = LQ_CS + 8 * 64 * 4;
-constexpr int LQ_SMEM = LQ_BAR + 128 + 1024;
+// dK / dV of a query-split grid: the chunk partials summed in chunk order, dK scaled, rounded to bf16 once
+__global__ void attn_long_dkdv_reduce_kernel(const float* __restrict__ part, __nv_bfloat16* __restrict__ dk, __nv_bfloat16* __restrict__ dv,
+                                             int B, int H, int Tk, int Dh, long long ldkv, int nchunk, float scale) {
+    const long long n = static_cast<long long>(B) * H * Tk * Dh;
+    const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (idx >= 2 * n) return;
+    const int which = idx >= n ? 1 : 0;
+    const long long r = idx - which * n;
+    const int d = static_cast<int>(r % Dh);
+    const long long key_row = r / Dh;  // (b * H + h) * Tk + key
+    const int key = static_cast<int>(key_row % Tk);
+    const int bh = static_cast<int>(key_row / Tk);
+    const float* src = part + which * nchunk * n + r;
+    float t = 0.f;
+    for (int c = 0; c < nchunk; ++c) t += src[c * n];
+    __nv_bfloat16* dst = which ? dv : dk;
+    dst[(static_cast<long long>(bh / H) * Tk + key) * ldkv + (bh % H) * Dh + d] = __float2bfloat16_rn(which ? t : t * scale);
+}
 
-__global__ void __launch_bounds__(LA_THREADS, 1)
-attn_long_dq_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmDO,
-                    const float* __restrict__ lse_in, const float* __restrict__ delta_in, __nv_bfloat16* __restrict__ dqkv,
-                    float* __restrict__ csum_part, const AttnParams p) {
+// dQ.  For Dh > 64 the dQ accumulators (32 NB fp32) plus S and dP do not fit the 168 registers per thread that 288 threads
+// leave, so those instances run 256 threads without the producer warp: thread 0 issues the loads, each K / V block as soon as
+// every consumer warp has released the stage it goes into.
+template <int KS>
+constexpr int dq_threads() { return KS <= 4 ? LA_THREADS : 256; }
+
+template <int KS>
+__global__ void __launch_bounds__(dq_threads<KS>(), 1)
+attn_long_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
+                    const __grid_constant__ CUtensorMap tmDO, const float* __restrict__ lse_in, const float* __restrict__ delta_in,
+                    __nv_bfloat16* __restrict__ dq_out, float* __restrict__ csum_part, const LongParams p) {
+    constexpr int NB = (KS + 3) / 4;
+    using C = LongCfg<NB>;
+    constexpr int S = C::Q_STAGES;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + LQ_BAR);
-    uint64_t* empty = full + LA_STAGES;
-    uint64_t* bar_q = empty + LA_STAGES;
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + C::Q_BAR);
+    uint64_t* empty = full + S;
+    uint64_t* bar_q = empty + S;
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const int n_qt = (p.T + 127) / 128;
+    const int n_qt = (p.Tq + 127) / 128;
     const int qt = blockIdx.x % n_qt;
     const int bh = blockIdx.x / n_qt;
     const int h = bh % p.H;
     const int b = bh / p.H;
-    const int n_cons = qt * 128 + 64 < p.T ? 2 : 1;
-    const int nkb_all = (p.T + 63) / 64;
+    const int n_cons = qt * 128 + 64 < p.Tq ? 2 : 1;
+    const int nkb_all = (p.Tk + 63) / 64;
     const int nkb = p.causal ? min(nkb_all, 2 * qt + n_cons) : nkb_all;
     if (threadIdx.x == 0) {
-        for (int s = 0; s < LA_STAGES; ++s) {
+        for (int s = 0; s < S; ++s) {
             mbar_init(&full[s], 1);
             mbar_init(&empty[s], 4 * n_cons);
         }
@@ -756,26 +961,37 @@ attn_long_dq_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_cons
     }
     __syncthreads();
 
-    if (warp == 8) {
-        if (lane == 0) {
-            tma_prefetch_desc(&tmQKV);
-            tma_prefetch_desc(&tmDO);
-            mbar_expect_tx(bar_q, 2u * n_cons * TILE_BYTES);
-            for (int g = 0; g < n_cons; ++g) {
-                tma_load_3d(smem + LQ_SQ + g * TILE_BYTES, &tmQKV, bar_q, h * 64, qt * 128 + g * 64, b);
-                tma_load_3d(smem + LQ_SDO + g * TILE_BYTES, &tmDO, bar_q, h * 64, qt * 128 + g * 64, b);
-            }
-            for (int kb = 0; kb < nkb; ++kb) {
-                const int s = kb % LA_STAGES;
-                mbar_wait(&empty[s], ((kb / LA_STAGES) & 1) ^ 1u);
-                uint8_t* dst = smem + LQ_SKV + s * 2 * TILE_BYTES;
-                mbar_expect_tx(&full[s], 2u * TILE_BYTES);
-                tma_load_3d(dst, &tmQKV, &full[s], p.D + h * 64, kb * 64, b);
-                tma_load_3d(dst + TILE_BYTES, &tmQKV, &full[s], 2 * p.D + h * 64, kb * 64, b);
-            }
+    auto load_kv = [&](int kb) {  // K / V block kb into stage kb % S (its empty barrier already waited on)
+        const int s = kb % S;
+        uint8_t* dst = smem + C::Q_KV + s * 2 * C::BOX;
+        mbar_expect_tx(&full[s], 2u * C::BOX);
+        for (int c = 0; c < NB; ++c) {
+            tma_load_4d(dst + c * TILE_BYTES, &tmK, &full[s], c * 64, h, kb * 64, b);
+            tma_load_4d(dst + C::BOX + c * TILE_BYTES, &tmV, &full[s], c * 64, h, kb * 64, b);
         }
-        return;
+    };
+    const bool issuer = dq_threads<KS>() == LA_THREADS ? (warp == 8 && lane == 0) : threadIdx.x == 0;
+    if (issuer) {
+        tma_prefetch_desc(&tmQ);
+        tma_prefetch_desc(&tmK);
+        tma_prefetch_desc(&tmV);
+        tma_prefetch_desc(&tmDO);
+        mbar_expect_tx(bar_q, 2u * n_cons * C::BOX);
+        for (int g = 0; g < n_cons; ++g)
+            for (int c = 0; c < NB; ++c) {
+                tma_load_4d(smem + C::Q_Q + (g * NB + c) * TILE_BYTES, &tmQ, bar_q, c * 64, h, qt * 128 + g * 64, b);
+                tma_load_4d(smem + C::Q_DO + (g * NB + c) * TILE_BYTES, &tmDO, bar_q, c * 64, h, qt * 128 + g * 64, b);
+            }
+        if constexpr (dq_threads<KS>() == LA_THREADS) {  // the producer warp streams every block through the ring
+            for (int kb = 0; kb < nkb; ++kb) {
+                mbar_wait(&empty[kb % S], ((kb / S) & 1) ^ 1u);
+                load_kv(kb);
+            }
+        } else {
+            for (int kb = 0; kb < min(nkb, S); ++kb) load_kv(kb);  // the ring starts empty
+        }
     }
+    if (warp == 8) return;
     const int g = warp >> 2;
     if (g >= n_cons) return;
     const int wq = warp & 3;
@@ -786,40 +1002,42 @@ attn_long_dq_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_cons
     const int diag = q0 / 64;
     const int nkb_g = p.causal ? min(nkb, diag + 1) : nkb;
     const float sl2 = p.scale * kLog2e;
-    const uint32_t q_base = smem_u32(smem + LQ_SQ) + g * TILE_BYTES, do_base = smem_u32(smem + LQ_SDO) + g * TILE_BYTES;
+    const uint32_t q_base = smem_u32(smem + C::Q_Q) + g * C::BOX, do_base = smem_u32(smem + C::Q_DO) + g * C::BOX;
     float l2[2], de[2];
 #pragma unroll
     for (int hr = 0; hr < 2; ++hr) {
         const int i = i0 + 8 * hr;
-        const long long at = static_cast<long long>(bh) * p.T + i;
-        l2[hr] = i < p.T ? __ldg(lse_in + at) * kLog2e : INFINITY;  // padded query rows: P = dS = 0
-        de[hr] = i < p.T ? __ldg(delta_in + at) : 0.f;
+        const long long at = static_cast<long long>(bh) * p.Tq + i;
+        l2[hr] = i < p.Tq ? __ldg(lse_in + at) * kLog2e : INFINITY;  // padded query rows: P = dS = 0
+        de[hr] = i < p.Tq ? __ldg(delta_in + at) : 0.f;
     }
 
-    float dq[32];
+    float dq[NB][32];
 #pragma unroll
-    for (int e = 0; e < 32; ++e) dq[e] = 0.f;
+    for (int c = 0; c < NB; ++c)
+#pragma unroll
+        for (int e = 0; e < 32; ++e) dq[c][e] = 0.f;
     mbar_wait(bar_q, 0);
     for (int kb = 0; kb < nkb; ++kb) {
-        const int s = kb % LA_STAGES;
-        mbar_wait(&full[s], (kb / LA_STAGES) & 1);
+        const int s = kb % S;
+        mbar_wait(&full[s], (kb / S) & 1);
         if (kb < nkb_g) {
-            const uint32_t k_st = smem_u32(smem + LQ_SKV + s * 2 * TILE_BYTES), v_st = k_st + TILE_BYTES;
+            const uint32_t k_st = smem_u32(smem + C::Q_KV + s * 2 * C::BOX), v_st = k_st + C::BOX;
             float sc[32], dp[32];
             wgmma_fence();
-            mma_tile_kk(sc, q_base, k_st);   // S = Q K^T
-            mma_tile_kk(dp, do_base, v_st);  // dP = dO V^T
+            mma_rows_kk<KS>(sc, q_base, k_st);   // S = Q K^T
+            mma_rows_kk<KS>(dp, do_base, v_st);  // dP = dO V^T
             wgmma_commit();
             wgmma_wait<0>();
             reg_fence(sc);
             reg_fence(dp);
-            const bool edge = kb * 64 + 64 > p.T || (p.causal && kb == diag);
+            const bool edge = kb * 64 + 64 > p.Tk || (p.causal && kb == diag);
 #pragma unroll
             for (int e = 0; e < 32; ++e) {
                 const int hr = (e >> 1) & 1;
                 const int j = kb * 64 + (e >> 2) * 8 + jq + (e & 1);
                 float pv = fast_ex2(fmaf(sc[e], sl2, -l2[hr]));
-                if (edge && !(j < p.T && (!p.causal || j <= i0 + 8 * hr))) pv = 0.f;
+                if (edge && !(j < p.Tk && (!p.causal || j <= i0 + 8 * hr))) pv = 0.f;
                 dp[e] = pv * (dp[e] - de[hr]);
             }
             wgmma_fence();
@@ -827,23 +1045,30 @@ attn_long_dq_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_cons
             for (int k = 0; k < 4; ++k) {
                 uint32_t a[4];
                 a_frag(dp, k, a);
-                wgmma_m64n64k16_rs_tb(dq, a, mnmajor_desc(k_st + k * 2048), 1u);  // dQ += dS K
+#pragma unroll
+                for (int c = 0; c < NB; ++c) wgmma_m64n64k16_rs_tb(dq[c], a, mnmajor_desc(k_st + c * TILE_BYTES + k * 2048), 1u);  // dQ += dS K
             }
             wgmma_commit();
             wgmma_wait<0>();
-            reg_fence(dq);
+#pragma unroll
+            for (int c = 0; c < NB; ++c) reg_fence(dq[c]);
         }
         if (lane == 0) mbar_arrive(&empty[s]);
+        if (dq_threads<KS>() != LA_THREADS && threadIdx.x == 0 && kb + S < nkb) {
+            mbar_wait(&empty[s], (kb / S) & 1);
+            load_kv(kb + S);
+        }
     }
-    const long long D3 = 3ll * p.D;
-    float* cs = reinterpret_cast<float*>(smem + LQ_CS);
+    float* cs = reinterpret_cast<float*>(smem + C::Q_CS);
     const bool sums = csum_part != nullptr;
-    store_tile(dq, p.scale, dqkv + (static_cast<long long>(b) * p.T) * D3 + h * 64, D3, i0, p.T, lane,
-               sums ? cs + (g * 4 + wq) * 64 : nullptr);
+    __nv_bfloat16* g0 = dq_out + static_cast<long long>(b) * p.Tq * p.ldq + h * p.Dh;
+#pragma unroll
+    for (int c = 0; c < NB; ++c)
+        store_tile<true>(dq[c], p.scale, g0 + c * 64, p.ldq, i0, p.Tq, lane, sums && c == 0 ? cs + (g * 4 + wq) * 64 : nullptr, p.Dh - c * 64);
     if (sums) {
         named_bar_sync(1 + g, 128);
         const int t = threadIdx.x & 127;
-        if (t < 64) csum_part[(static_cast<long long>(bh) * ((p.T + 63) / 64) + diag) * 192 + t] = wg_colsum(cs + g * 4 * 64, t);
+        if (t < 64) csum_part[(static_cast<long long>(bh) * ((p.Tq + 63) / 64) + diag) * 192 + t] = wg_colsum(cs + g * 4 * 64, t);
     }
 }
 
@@ -958,7 +1183,7 @@ extern "C" int b200_set_attention_bwd_version(int version) {
     return old;
 }
 
-// ---- streamed kernels: any 1 <= T <= 16384 ----
+// ---- streamed kernels: any 1 <= Tq, Tk <= 16384, Dh <= 160 ----
 static int attn_long_check(int B, int T, int H, int Dh) {
     if (B <= 0 || T <= 0 || H <= 0) return set_error(B200_ERR_ARG, "attention_long: non-positive size");
     if (Dh != 64) return set_error(B200_ERR_ARG, "attention_long: head dim must be 64");
@@ -977,12 +1202,130 @@ static int attn_long_configure(Kernel kernel, int smem, bool (&configured)[64]) 
     return 0;
 }
 
-// 64 x 64 boxes (128B-swizzled) over a [B, T, cols] bf16 tensor: rows >= T of an image are zero-filled
-static int attn_long_tmap(CUtensorMap* tm, const void* base, int cols, int T, int B) {
-    uint64_t dims[3] = {static_cast<uint64_t>(cols), static_cast<uint64_t>(T), static_cast<uint64_t>(B)};
-    uint64_t strides[2] = {static_cast<uint64_t>(cols) * 2, static_cast<uint64_t>(cols) * 2 * static_cast<uint64_t>(T)};
-    uint32_t box[3] = {64, 64, 1};
-    return make_tmap(tm, base, 2, 3, dims, strides, box, 128);
+// {Dh, H, T, B} over a [B, T, ld] bf16 tensor whose head h starts at column h * Dh; 64 x 64 boxes (128B-swizzled): columns
+// >= Dh and rows >= T of an image are zero-filled
+static int attn_long_tmap(CUtensorMap* tm, const void* base, long long ld, int Dh, int H, int T, int B) {
+    uint64_t dims[4] = {static_cast<uint64_t>(Dh), static_cast<uint64_t>(H), static_cast<uint64_t>(T), static_cast<uint64_t>(B)};
+    uint64_t strides[3] = {static_cast<uint64_t>(Dh) * 2, static_cast<uint64_t>(ld) * 2, static_cast<uint64_t>(ld) * 2 * static_cast<uint64_t>(T)};
+    uint32_t box[4] = {64, 1, 64, 1};
+    return make_tmap(tm, base, 2, 4, dims, strides, box, 128);
+}
+
+// A dK / dV CTA walks every query block of its (image, head).  When B * H * (key tiles) cannot fill the SMs -- cross-attention
+// on a 77-token context -- the queries are split into chunks of whole 64-row blocks instead.  Returns the chunk count.
+static int attn_long_dkdv_chunks(int B, int Tq, int Tk, int H, int Dh, int* qb_chunk) {
+    const int rows = Dh <= 64 ? LongCfg<1>::K_ROWS : LongCfg<2>::K_ROWS;
+    const long long ctas = static_cast<long long>(B) * H * ((Tk + rows - 1) / rows);
+    const int nqb = (Tq + 63) / 64;
+    const int want = static_cast<int>(min(static_cast<long long>(nqb), ctas >= LA_SMS ? 1ll : LA_SMS / ctas));
+    *qb_chunk = (nqb + want - 1) / want;
+    return (nqb + *qb_chunk - 1) / *qb_chunk;
+}
+
+static LongParams attn_long_params(int B, int Tq, int Tk, int H, int Dh, long long ldq, long long ldkv, long long ldo, float scale, int causal) {
+    LongParams p;
+    p.B = B; p.Tq = Tq; p.Tk = Tk; p.H = H; p.Dh = Dh;
+    p.ldq = ldq; p.ldkv = ldkv; p.ldo = ldo; p.scale = scale; p.causal = causal;
+    p.qb_chunk = (Tq + 63) / 64; p.nchunk = 1;
+    return p;
+}
+
+// k16 steps of S = Q K^T / dP = dO V^T per head dim: exact up to Dh 80 (the SD UNet's 40, ViT's 64, 80), then Dh 128 and 160
+static int attn_long_ksteps(int Dh) {
+    const int ks = (Dh + 15) / 16;
+    return ks <= 2 ? 2 : ks <= 5 ? ks : ks <= 8 ? 8 : 10;
+}
+
+template <int KS>
+static int attn_long_fwd_launch(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, void* out, float* lse,
+                                const LongParams& p, cudaStream_t stream) {
+    constexpr int NB = (KS + 3) / 4;
+    static bool configured[64] = {};
+    int rc = attn_long_configure(attn_long_fwd_kernel<KS>, LongCfg<NB>::F_SMEM, configured);
+    if (rc) return rc;
+    const int n_mt = (p.Tq + 127) / 128;
+    attn_long_fwd_kernel<KS><<<p.B * p.H * n_mt, LA_THREADS, LongCfg<NB>::F_SMEM, stream>>>(tmQ, tmK, tmV, reinterpret_cast<__nv_bfloat16*>(out), lse, p);
+    return check_launch("attention_long_fwd");
+}
+
+template <int KS>
+static int attn_long_bwd_launch(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const CUtensorMap& tmDO, const float* lse,
+                                const float* delta, void* dq, void* dk, void* dv, float* part, float* csum_part, const LongParams& p,
+                                cudaStream_t stream) {
+    using C = LongCfg<(KS + 3) / 4>;
+    static bool configured_kv[64] = {}, configured_q[64] = {};
+    int rc;
+    if ((rc = attn_long_configure(attn_long_dkdv_kernel<KS>, C::K_SMEM, configured_kv)) != 0) return rc;
+    if ((rc = attn_long_configure(attn_long_dq_kernel<KS>, C::Q_SMEM, configured_q)) != 0) return rc;
+    const int n_kt = (p.Tk + C::K_ROWS - 1) / C::K_ROWS;
+    attn_long_dkdv_kernel<KS><<<p.B * p.H * n_kt * p.nchunk, LA_THREADS, C::K_SMEM, stream>>>(
+        tmQ, tmK, tmV, tmDO, lse, delta, reinterpret_cast<__nv_bfloat16*>(dk), reinterpret_cast<__nv_bfloat16*>(dv), part, csum_part, p);
+    if ((rc = check_launch("attention_long_bwd (dk, dv)")) != 0) return rc;
+    const int n_qt = (p.Tq + 127) / 128;
+    attn_long_dq_kernel<KS><<<p.B * p.H * n_qt, dq_threads<KS>(), C::Q_SMEM, stream>>>(tmQ, tmK, tmV, tmDO, lse, delta,
+                                                                                reinterpret_cast<__nv_bfloat16*>(dq), csum_part, p);
+    return check_launch("attention_long_bwd (dq)");
+}
+
+static int attn_long_fwd_run(const void* q, long long ldq, const void* k, const void* v, long long ldkv, void* out, long long ldo, float* lse,
+                             int B, int Tq, int Tk, int H, int Dh, float scale, int causal, cudaStream_t stream) {
+    CUtensorMap tmQ, tmK, tmV;
+    int rc;
+    if ((rc = attn_long_tmap(&tmQ, q, ldq, Dh, H, Tq, B)) != 0) return rc;
+    if ((rc = attn_long_tmap(&tmK, k, ldkv, Dh, H, Tk, B)) != 0) return rc;
+    if ((rc = attn_long_tmap(&tmV, v, ldkv, Dh, H, Tk, B)) != 0) return rc;
+    const LongParams p = attn_long_params(B, Tq, Tk, H, Dh, ldq, ldkv, ldo, scale, causal);
+    switch (attn_long_ksteps(Dh)) {
+        case 2: return attn_long_fwd_launch<2>(tmQ, tmK, tmV, out, lse, p, stream);
+        case 3: return attn_long_fwd_launch<3>(tmQ, tmK, tmV, out, lse, p, stream);
+        case 4: return attn_long_fwd_launch<4>(tmQ, tmK, tmV, out, lse, p, stream);
+        case 5: return attn_long_fwd_launch<5>(tmQ, tmK, tmV, out, lse, p, stream);
+        case 8: return attn_long_fwd_launch<8>(tmQ, tmK, tmV, out, lse, p, stream);
+        default: return attn_long_fwd_launch<10>(tmQ, tmK, tmV, out, lse, p, stream);
+    }
+}
+
+// workspace: delta [B, H, Tq] (rounded up to 4 floats), then either the packed layout's column-sum partials (dbias_part) or,
+// for a query-split dK / dV grid (split != 0 only), the fp32 partials [dk | dv][chunk][B, H, Tk, Dh]
+static int attn_long_bwd_run(const void* q, long long ldq, const void* k, const void* v, long long ldkv, const void* out, long long ldo,
+                             const void* dout, const float* lse, void* dq, void* dk, void* dv, int B, int Tq, int Tk, int H, int Dh, float scale,
+                             int causal, float* dbias_part, float* workspace, bool split, cudaStream_t stream) {
+    CUtensorMap tmQ, tmK, tmV, tmDO;
+    int rc;
+    if ((rc = attn_long_tmap(&tmQ, q, ldq, Dh, H, Tq, B)) != 0) return rc;
+    if ((rc = attn_long_tmap(&tmK, k, ldkv, Dh, H, Tk, B)) != 0) return rc;
+    if ((rc = attn_long_tmap(&tmV, v, ldkv, Dh, H, Tk, B)) != 0) return rc;
+    if ((rc = attn_long_tmap(&tmDO, dout, ldo, Dh, H, Tq, B)) != 0) return rc;
+    LongParams p = attn_long_params(B, Tq, Tk, H, Dh, ldq, ldkv, ldo, scale, causal);
+    if (split) p.nchunk = attn_long_dkdv_chunks(B, Tq, Tk, H, Dh, &p.qb_chunk);
+    float* delta = workspace;
+    float* csum_part = dbias_part != nullptr ? workspace + static_cast<long long>(B) * H * Tq : nullptr;
+    float* part = p.nchunk > 1 ? workspace + (static_cast<long long>(B) * H * Tq + 3) / 4 * 4 : nullptr;
+    const long long rows = static_cast<long long>(B) * Tq * H;
+    attn_long_delta_kernel<<<static_cast<unsigned>((rows + 255) / 256), 256, 0, stream>>>(
+        reinterpret_cast<const __nv_bfloat16*>(out), reinterpret_cast<const __nv_bfloat16*>(dout), delta, B, Tq, H, Dh, ldo);
+    if ((rc = check_launch("attention_long_bwd (delta)")) != 0) return rc;
+    switch (attn_long_ksteps(Dh)) {
+        case 2: rc = attn_long_bwd_launch<2>(tmQ, tmK, tmV, tmDO, lse, delta, dq, dk, dv, part, csum_part, p, stream); break;
+        case 3: rc = attn_long_bwd_launch<3>(tmQ, tmK, tmV, tmDO, lse, delta, dq, dk, dv, part, csum_part, p, stream); break;
+        case 4: rc = attn_long_bwd_launch<4>(tmQ, tmK, tmV, tmDO, lse, delta, dq, dk, dv, part, csum_part, p, stream); break;
+        case 5: rc = attn_long_bwd_launch<5>(tmQ, tmK, tmV, tmDO, lse, delta, dq, dk, dv, part, csum_part, p, stream); break;
+        case 8: rc = attn_long_bwd_launch<8>(tmQ, tmK, tmV, tmDO, lse, delta, dq, dk, dv, part, csum_part, p, stream); break;
+        default: rc = attn_long_bwd_launch<10>(tmQ, tmK, tmV, tmDO, lse, delta, dq, dk, dv, part, csum_part, p, stream); break;
+    }
+    if (rc) return rc;
+    if (p.nchunk > 1) {
+        const long long n = 2ll * B * H * Tk * Dh;
+        attn_long_dkdv_reduce_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(
+            part, reinterpret_cast<__nv_bfloat16*>(dk), reinterpret_cast<__nv_bfloat16*>(dv), B, H, Tk, Dh, ldkv, p.nchunk, scale);
+        if ((rc = check_launch("attention_long_bwd (dk, dv reduce)")) != 0) return rc;
+    }
+    if (dbias_part != nullptr) {
+        const long long n = 3ll * B * H * 64;
+        attn_long_dbias_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(csum_part, dbias_part, B, H, (Tq + 63) / 64);
+        if ((rc = check_launch("attention_long_bwd (dbias)")) != 0) return rc;
+    }
+    return 0;
 }
 
 extern "C" int b200_attention_long_fwd(const void* qkv_bf16, void* out_bf16, float* lse, int B, int T, int H, int Dh,
@@ -991,15 +1334,8 @@ extern "C" int b200_attention_long_fwd(const void* qkv_bf16, void* out_bf16, flo
     if (rc) return rc;
     if (qkv_bf16 == nullptr || out_bf16 == nullptr || lse == nullptr) return set_error(B200_ERR_ARG, "attention_long_fwd: null pointer");
     const int D = H * 64;
-    CUtensorMap tmQKV;
-    if ((rc = attn_long_tmap(&tmQKV, qkv_bf16, 3 * D, T, B)) != 0) return rc;
-    static bool configured[64] = {};
-    if ((rc = attn_long_configure(attn_long_fwd_kernel, LF_SMEM, configured)) != 0) return rc;
-    AttnParams p;
-    p.B = B; p.T = T; p.H = H; p.D = D; p.tp = (T + 63) / 64 * 64; p.scale = scale; p.causal = causal;
-    const int n_mt = (T + 127) / 128;
-    attn_long_fwd_kernel<<<B * H * n_mt, LA_THREADS, LF_SMEM, stream>>>(tmQKV, reinterpret_cast<__nv_bfloat16*>(out_bf16), lse, p);
-    return check_launch("attention_long_fwd");
+    const __nv_bfloat16* qkv = reinterpret_cast<const __nv_bfloat16*>(qkv_bf16);
+    return attn_long_fwd_run(qkv, 3 * D, qkv + D, qkv + 2 * D, 3 * D, out_bf16, D, lse, B, T, T, H, 64, scale, causal, stream);
 }
 
 extern "C" long long b200_attention_long_bwd_workspace_floats(int B, int T, int H) {
@@ -1016,30 +1352,58 @@ extern "C" int b200_attention_long_bwd(const void* qkv_bf16, const void* out_bf1
     if (qkv_bf16 == nullptr || out_bf16 == nullptr || dout_bf16 == nullptr || lse == nullptr || dqkv_bf16 == nullptr || workspace == nullptr)
         return set_error(B200_ERR_ARG, "attention_long_bwd: null pointer");
     const int D = H * 64;
-    CUtensorMap tmQKV, tmDO;
-    if ((rc = attn_long_tmap(&tmQKV, qkv_bf16, 3 * D, T, B)) != 0) return rc;
-    if ((rc = attn_long_tmap(&tmDO, dout_bf16, D, T, B)) != 0) return rc;
-    static bool configured_kv[64] = {}, configured_q[64] = {};
-    if ((rc = attn_long_configure(attn_long_dkdv_kernel, LK_SMEM, configured_kv)) != 0) return rc;
-    if ((rc = attn_long_configure(attn_long_dq_kernel, LQ_SMEM, configured_q)) != 0) return rc;
-    AttnParams p;
-    p.B = B; p.T = T; p.H = H; p.D = D; p.tp = (T + 63) / 64 * 64; p.scale = scale; p.causal = causal;
-    float* delta = workspace;
-    float* csum_part = dbias_part != nullptr ? workspace + static_cast<long long>(B) * H * T : nullptr;
-    const long long rows = static_cast<long long>(B) * T * H;
-    attn_long_delta_kernel<<<static_cast<unsigned>((rows + 255) / 256), 256, 0, stream>>>(
-        reinterpret_cast<const __nv_bfloat16*>(out_bf16), reinterpret_cast<const __nv_bfloat16*>(dout_bf16), delta, B, T, H);
-    if ((rc = check_launch("attention_long_bwd (delta)")) != 0) return rc;
-    const int n_t = (T + 127) / 128;
+    const __nv_bfloat16* qkv = reinterpret_cast<const __nv_bfloat16*>(qkv_bf16);
     __nv_bfloat16* dqkv = reinterpret_cast<__nv_bfloat16*>(dqkv_bf16);
-    attn_long_dkdv_kernel<<<B * H * n_t, LA_THREADS, LK_SMEM, stream>>>(tmQKV, tmDO, lse, delta, dqkv, csum_part, p);
-    if ((rc = check_launch("attention_long_bwd (dk, dv)")) != 0) return rc;
-    attn_long_dq_kernel<<<B * H * n_t, LA_THREADS, LQ_SMEM, stream>>>(tmQKV, tmDO, lse, delta, dqkv, csum_part, p);
-    if ((rc = check_launch("attention_long_bwd (dq)")) != 0) return rc;
-    if (dbias_part != nullptr) {
-        const long long n = 3ll * B * D;
-        attn_long_dbias_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(csum_part, dbias_part, B, H, (T + 63) / 64);
-        if ((rc = check_launch("attention_long_bwd (dbias)")) != 0) return rc;
-    }
+    return attn_long_bwd_run(qkv, 3 * D, qkv + D, qkv + 2 * D, 3 * D, out_bf16, D, dout_bf16, lse, dqkv, dqkv + D, dqkv + 2 * D, B, T, T, H, 64,
+                             scale, causal, dbias_part, workspace, false, stream);
+}
+
+// ---- separate Q / K / V (cross-attention, head dims 8 ... 160) on the same streamed kernels ----
+static bool misaligned16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15u) != 0; }
+
+static int cross_check(int B, int Tq, int Tk, int H, int Dh, int causal, long long ldq, long long ldkv, long long ldo) {
+    if (B <= 0 || H <= 0) return set_error(B200_ERR_ARG, "cross_attention: non-positive size");
+    if (Tq < 1 || Tk < 1 || Tq > LA_MAX_T || Tk > LA_MAX_T) return set_error(B200_ERR_ARG, "cross_attention: Tq and Tk must be in [1, 16384]");
+    if (Dh < 8 || Dh > LA_MAX_DH || Dh % 8 != 0) return set_error(B200_ERR_ARG, "cross_attention: head dim must be a multiple of 8 in [8, 160]");
+    if (causal && Tq != Tk) return set_error(B200_ERR_ARG, "cross_attention: causal needs Tq == Tk");
+    const long long width = static_cast<long long>(H) * Dh;
+    if (ldq < width || ldkv < width || ldo < width) return set_error(B200_ERR_ARG, "cross_attention: leading dim < H * Dh");
+    if (ldq % 8 != 0 || ldkv % 8 != 0 || ldo % 8 != 0) return set_error(B200_ERR_ALIGN, "cross_attention: leading dims must be multiples of 8");
     return 0;
+}
+
+extern "C" int b200_cross_attention_fwd(const void* q, long long ldq, const void* k, const void* v, long long ldkv, void* out, long long ldo,
+                                        float* lse, int B, int Tq, int Tk, int H, int Dh, float scale, int causal, cudaStream_t stream) {
+    int rc = cross_check(B, Tq, Tk, H, Dh, causal, ldq, ldkv, ldo);
+    if (rc) return rc;
+    if (q == nullptr || k == nullptr || v == nullptr || out == nullptr || lse == nullptr)
+        return set_error(B200_ERR_ARG, "cross_attention_fwd: null pointer");
+    if (misaligned16(q) || misaligned16(k) || misaligned16(v) || misaligned16(out) || misaligned16(lse))
+        return set_error(B200_ERR_ALIGN, "cross_attention_fwd: pointers must be 16-byte aligned");
+    return attn_long_fwd_run(q, ldq, k, v, ldkv, out, ldo, lse, B, Tq, Tk, H, Dh, scale, causal, stream);
+}
+
+extern "C" long long b200_cross_attention_bwd_workspace_floats(int B, int Tq, int Tk, int H, int Dh) {
+    if (B <= 0 || Tq <= 0 || Tk <= 0 || H <= 0 || Dh <= 0) return 0;
+    int qb_chunk;
+    const int nchunk = attn_long_dkdv_chunks(B, Tq, Tk, H, Dh, &qb_chunk);
+    // delta [B, H, Tq] rounded up to 4 floats, then the fp32 dk | dv partials of a query-split grid
+    const long long delta = (static_cast<long long>(B) * H * Tq + 3) / 4 * 4;
+    return delta + (nchunk > 1 ? 2ll * nchunk * B * H * Tk * Dh : 0ll);
+}
+
+extern "C" int b200_cross_attention_bwd(const void* q, long long ldq, const void* k, const void* v, long long ldkv, const void* out,
+                                        long long ldo, const void* dout, const float* lse, void* dq, void* dk, void* dv, int B, int Tq, int Tk,
+                                        int H, int Dh, float scale, int causal, float* workspace, cudaStream_t stream) {
+    int rc = cross_check(B, Tq, Tk, H, Dh, causal, ldq, ldkv, ldo);
+    if (rc) return rc;
+    if (q == nullptr || k == nullptr || v == nullptr || out == nullptr || dout == nullptr || lse == nullptr || dq == nullptr || dk == nullptr ||
+        dv == nullptr)
+        return set_error(B200_ERR_ARG, "cross_attention_bwd: null pointer");
+    if (workspace == nullptr) return set_error(B200_ERR_ARG, "cross_attention_bwd: workspace is required");
+    if (misaligned16(q) || misaligned16(k) || misaligned16(v) || misaligned16(out) || misaligned16(dout) || misaligned16(lse) ||
+        misaligned16(dq) || misaligned16(dk) || misaligned16(dv) || misaligned16(workspace))
+        return set_error(B200_ERR_ALIGN, "cross_attention_bwd: pointers must be 16-byte aligned");
+    return attn_long_bwd_run(q, ldq, k, v, ldkv, out, ldo, dout, lse, dq, dk, dv, B, Tq, Tk, H, Dh, scale, causal, nullptr, workspace, true,
+                             stream);
 }

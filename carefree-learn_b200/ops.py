@@ -231,6 +231,56 @@ def attention_bwd(qkv: Tensor, out: Tensor, dout: Tensor, lse: Tensor, B: int, T
     return dqkv
 
 
+def _rows_view(t: Tensor, name: str) -> int:
+    if t.dtype != torch.bfloat16 or t.dim() != 2 or t.stride(1) != 1:
+        raise B200Error(f"cross_attention: {name} must be a 2-D bf16 view with unit inner stride")
+    return t.stride(0)
+
+
+def cross_attention_fwd(q: Tensor, k: Tensor, v: Tensor, B: int, H: int, *, scale: Optional[float] = None,
+                        causal: bool = False) -> Tuple[Tensor, Tensor]:
+    """Attention with separate operands: q [B*Tq, >= H*Dh], k / v [B*Tk, >= H*Dh] (bf16 2-D views with unit inner stride, e.g.
+    column slices of one packed projection), head h at columns [h*Dh, (h+1)*Dh).  Returns (out bf16 [B*Tq, H*Dh], lse f32 [B, H, Tq])."""
+    _need_cuda(q, k, v)
+    ldq, ldk, ldv = _rows_view(q, "q"), _rows_view(k, "k"), _rows_view(v, "v")
+    if ldk != ldv or k.shape != v.shape:
+        raise B200Error("cross_attention: k and v must share shape and leading dim")
+    L = q.shape[1]
+    if L % H != 0 or k.shape[1] != L or q.shape[0] % B != 0 or k.shape[0] % B != 0:
+        raise B200Error("cross_attention: q / k / v widths must be H * Dh and rows a multiple of B")
+    Tq, Tk, Dh = q.shape[0] // B, k.shape[0] // B, L // H
+    out = torch.empty((B * Tq, L), dtype=torch.bfloat16, device=q.device)
+    lse = torch.empty((B, H, Tq), dtype=torch.float32, device=q.device)
+    sc = float(scale) if scale is not None else Dh ** -0.5
+    call("b200_cross_attention_fwd", q.data_ptr(), ldq, k.data_ptr(), v.data_ptr(), ldk, out.data_ptr(), out.stride(0), lse.data_ptr(),
+         B, Tq, Tk, H, Dh, sc, int(causal), _stream())
+    return out, lse
+
+
+def cross_attention_bwd(q: Tensor, k: Tensor, v: Tensor, out: Tensor, dout: Tensor, lse: Tensor, B: int, H: int, *,
+                        scale: Optional[float] = None, causal: bool = False, dq: Optional[Tensor] = None, dk: Optional[Tensor] = None,
+                        dv: Optional[Tensor] = None) -> Tuple[Tensor, Tensor, Tensor]:
+    """(dq, dk, dv) of ``cross_attention_fwd``.  dq / dk / dv may be given as views (dq with q's leading dim, dk / dv with k's), e.g.
+    column slices of one packed [M, 3L] gradient for self-attention; otherwise they are allocated contiguous."""
+    _need_cuda(q, k, v, out, dout, lse)
+    ldq, ldk = _rows_view(q, "q"), _rows_view(k, "k")
+    if _rows_view(dout, "dout") != _rows_view(out, "out"):
+        raise B200Error("cross_attention_bwd: dout must share out's leading dim")
+    L = q.shape[1]
+    Tq, Tk, Dh = q.shape[0] // B, k.shape[0] // B, L // H
+    if dq is None and dk is None and dv is None and ldq == L and ldk == L:
+        dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+    if dq is None or dk is None or dv is None:
+        raise B200Error("cross_attention_bwd: give all of dq, dk, dv or none (with contiguous q / k / v)")
+    if _rows_view(dq, "dq") != ldq or _rows_view(dk, "dk") != ldk or _rows_view(dv, "dv") != ldk:
+        raise B200Error("cross_attention_bwd: dq must share q's leading dim, dk / dv k's")
+    sc = float(scale) if scale is not None else Dh ** -0.5
+    ws = WORKSPACE.get(q.device, int(_cabi.lib().b200_cross_attention_bwd_workspace_floats(B, Tq, Tk, H, Dh)), "cross_attn")
+    call("b200_cross_attention_bwd", q.data_ptr(), ldq, k.data_ptr(), v.data_ptr(), ldk, out.data_ptr(), out.stride(0), dout.data_ptr(),
+         lse.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), B, Tq, Tk, H, Dh, sc, int(causal), ws.data_ptr(), _stream())
+    return dq, dk, dv
+
+
 # ----------------------------------------------------------------------------------------------------------------
 # patch embedding glue, loss, casts
 # ----------------------------------------------------------------------------------------------------------------

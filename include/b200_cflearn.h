@@ -143,6 +143,20 @@ long long b200_attention_long_bwd_workspace_floats(int B, int T, int H);
 int b200_attention_long_bwd(const void* qkv_bf16, const void* out_bf16, const void* dout_bf16, const float* lse,
                             void* dqkv_bf16, int B, int T, int H, int Dh, float scale, int causal, float* dbias_part,
                             float* workspace, cudaStream_t stream);
+/* Attention with separate Q / K / V and head dims 8 ... 160 (multiple of 8) on the same streamed kernels: the SD-v1.5 UNet's
+ * CrossAttention, cflearn/modules/core/attentions.py:534-569 (heads folded into the batch, then sdp_attn ->
+ * F.scaled_dot_product_attention at cflearn/toolkit.py:959-963).  q: bf16 [B, Tq, ldq], k / v: bf16 [B, Tk, ldkv], head h at
+ * columns [h * Dh, h * Dh + Dh); out: bf16 [B, Tq, ldo]; lse: f32 [B, H, Tq].  1 <= Tq, Tk <= 16384; causal only with Tq == Tk.
+ * Leading dims are multiples of 8 and >= H * Dh, pointers 16-byte aligned, so q / k / v may be column slices of one packed
+ * projection output (self-attention: q = qkv, k = qkv + H * Dh, v = qkv + 2 * H * Dh, ld = 3 * H * Dh).
+ * Backward: dout uses ldo, dq uses ldq, dk / dv use ldkv (so dq / dk / dv may be views of one packed gradient buffer).
+ * workspace (required): b200_cross_attention_bwd_workspace_floats(B, Tq, Tk, H, Dh) floats.  Deterministic (no atomics). */
+int b200_cross_attention_fwd(const void* q, long long ldq, const void* k, const void* v, long long ldkv, void* out, long long ldo,
+                             float* lse, int B, int Tq, int Tk, int H, int Dh, float scale, int causal, cudaStream_t stream);
+long long b200_cross_attention_bwd_workspace_floats(int B, int Tq, int Tk, int H, int Dh);
+int b200_cross_attention_bwd(const void* q, long long ldq, const void* k, const void* v, long long ldkv, const void* out,
+                             long long ldo, const void* dout, const float* lse, void* dq, void* dk, void* dv, int B, int Tq, int Tk,
+                             int H, int Dh, float scale, int causal, float* workspace, cudaStream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * FCNN (cflearn/modules/ml/fcnn.py:12-59: Mapping(Linear + ReLU) x n, then nn.Linear) -- one launch per training
