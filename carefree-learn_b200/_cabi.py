@@ -39,6 +39,8 @@ SIGNATURES: Dict[str, Any] = {
         c_int,
         [_P, c_int, _P, _LL, _P, _P, _P, _P, _P, _LL, _P, _P, c_int, POINTER(c_int), c_int, c_int, c_int, _P],
     ),
+    "b200_layernorm_bf16_fwd": (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_float, _P]),
+    "b200_layernorm_bf16_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, c_int, POINTER(c_int), c_int, c_int, _P]),
     "b200_colsum_bf16": (c_int, [_P, _LL, c_int, c_int, _P, c_int, POINTER(c_int), _P]),
     "b200_colsum_finish": (c_int, [_P, _LL, c_int, c_int, _P, c_int, c_int, _P]),
     "b200_colsum_finish2": (c_int, [_P, _LL, c_int, c_int, _P, c_int, c_int, _P, c_int, c_int, _P]),

@@ -2,7 +2,8 @@
 
 ``CrossAttentionB200`` is a drop-in for the reference module: same constructor keywords, the same fp32 parameters under the
 same ``state_dict`` keys (``to_q.weight``, ``to_k.weight``, ``to_v.weight``, ``out_linear.0.weight``, ``out_linear.0.bias``).
-Its forward and backward are one ``autograd.Function``; every product is the wgmma GEMM (``ops.gemm`` / ``ops.wgrad``) or the
+Its forward and backward are one ``autograd.Function`` over ``attention_forward`` / ``attention_backward``, which the
+SpatialTransformerBlock (``spatial_transformer.py``) calls as well; every product is the wgmma GEMM (``ops.gemm`` / ``ops.wgrad``) or the
 streamed attention (``ops.cross_attention_fwd/_bwd``), which reads q / k / v as column slices of the projection outputs:
 
     self-attention (context None):  qkv = x [Wq; Wk; Wv]^T  (one GEMM, N = 3L)   dx = dqkv [Wq; Wk; Wv]  (one GEMM, K = 3L)
@@ -17,7 +18,7 @@ likewise the k and v contributions to the context gradient.  Dropout > 0 and att
 """
 from __future__ import annotations
 
-from typing import Optional
+from typing import Optional, Tuple
 
 import torch
 from torch import Tensor, nn
@@ -30,61 +31,84 @@ def _bf(t: Tensor) -> Tensor:
     return t.to(torch.bfloat16).contiguous()
 
 
+def attention_forward(x: Tensor, c: Optional[Tensor], wq: Tensor, wk: Tensor, wv: Tensor, wo: Tensor, bo: Tensor, B: int, heads: int,
+                      resid: Optional[Tensor] = None) -> Tuple[Tensor, tuple]:
+    """Projections, attention and out_linear of one CrossAttention.  x: bf16 [B*Tq, Dq]; c: bf16 [B*Tk, Dc], or None for
+    self-attention; fp32 weights.  ``resid`` (bf16 [B*Tq, Dq]): the module output is added to it in out_linear's epilogue,
+    y = bf16(bf16(out_linear) + resid) -- the bf16 residual add that follows every attention of a SpatialTransformerBlock.
+    Returns (y bf16 [B*Tq, Dq], what ``attention_backward`` needs: a flat tuple of tensors and Nones, for save_for_backward)."""
+    L = wq.shape[0]
+    if c is None:
+        w_in = _bf(torch.cat([wq, wk, wv], 0))
+        qkv = ops.gemm(x, w_in)
+        q, k, v = qkv[:, :L], qkv[:, L:2 * L], qkv[:, 2 * L:]
+        w_kv = None
+    else:
+        w_in, w_kv = _bf(wq), _bf(torch.cat([wk, wv], 0))
+        q = ops.gemm(x, w_in)
+        kv = ops.gemm(c, w_kv)
+        k, v = kv[:, :L], kv[:, L:]
+    o, lse = ops.cross_attention_fwd(q, k, v, B, heads)
+    w_o = _bf(wo)
+    if resid is None:
+        y = ops.gemm(o, w_o, bias=_bf(bo))
+    else:
+        y = ops.gemm(o, w_o, bias=_bf(bo), epilogue=ops.EPI_BIAS_RESID_BF16, aux=resid)
+    return y, (x, c, q, k, v, o, lse, w_in, w_kv, w_o)
+
+
+def attention_backward(saved: tuple, dy: Tensor, B: int, heads: int):
+    """Backward of ``attention_forward`` for dy bf16 [B*Tq, Dq] (the gradient of y; with ``resid`` the residual's own
+    gradient is dy as well, which the caller adds).  Returns (dx bf16, dc bf16 or None, dwq, dwk, dwv, dwo, dbo), the weight
+    and bias gradients fp32 and rounded to bf16 like eager's."""
+    x, c, q, k, v, o, lse, w_in, w_kv, w_o = saved
+    M, Dq = x.shape
+    L = q.shape[1]
+    dwo = torch.empty(w_o.shape, dtype=torch.float32, device=dy.device)
+    dbo = torch.empty(Dq, dtype=torch.float32, device=dy.device)
+    ops.wgrad(dy, o, dwo)
+    ops.colsum(dy, dbo)
+    do = ops.gemm(dy, w_o, b_mn_major=True)
+    if c is None:
+        dqkv = torch.empty((M, 3 * L), dtype=torch.bfloat16, device=dy.device)
+        ops.cross_attention_bwd(q, k, v, o, do, lse, B, heads, dq=dqkv[:, :L], dk=dqkv[:, L:2 * L], dv=dqkv[:, 2 * L:])
+        dw = torch.empty((3 * L, Dq), dtype=torch.float32, device=dy.device)
+        ops.wgrad(dqkv, x, dw)
+        dwq, dwk, dwv = dw[:L], dw[L:2 * L], dw[2 * L:]
+        dx = ops.gemm(dqkv, w_in, b_mn_major=True)
+        dc = None
+    else:
+        dq = torch.empty((M, L), dtype=torch.bfloat16, device=dy.device)
+        dkv = torch.empty((c.shape[0], 2 * L), dtype=torch.bfloat16, device=dy.device)
+        ops.cross_attention_bwd(q, k, v, o, do, lse, B, heads, dq=dq, dk=dkv[:, :L], dv=dkv[:, L:])
+        dwq = torch.empty((L, Dq), dtype=torch.float32, device=dy.device)
+        dwkv = torch.empty((2 * L, c.shape[1]), dtype=torch.float32, device=dy.device)
+        ops.wgrad(dq, x, dwq)
+        ops.wgrad(dkv, c, dwkv)
+        dwk, dwv = dwkv[:L], dwkv[L:]
+        dx = ops.gemm(dq, w_in, b_mn_major=True)
+        dc = ops.gemm(dkv, w_kv, b_mn_major=True)
+    return dx, dc, dwq, dwk, dwv, dwo, dbo
+
+
 class _CrossAttentionFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, net: Tensor, context: Optional[Tensor], wq: Tensor, wk: Tensor, wv: Tensor, wo: Tensor, bo: Tensor, heads: int):  # type: ignore[override]
         B, Tq, Dq = net.shape
-        L = wq.shape[0]
         x = _bf(net.reshape(B * Tq, Dq))
-        if context is None:
-            w_in = _bf(torch.cat([wq, wk, wv], 0))
-            qkv = ops.gemm(x, w_in)
-            q, k, v = qkv[:, :L], qkv[:, L:2 * L], qkv[:, 2 * L:]
-            c, w_kv = None, None
-        else:
-            c = _bf(context.reshape(-1, context.shape[-1]))
-            w_in, w_kv = _bf(wq), _bf(torch.cat([wk, wv], 0))
-            q = ops.gemm(x, w_in)
-            kv = ops.gemm(c, w_kv)
-            k, v = kv[:, :L], kv[:, L:]
-        o, lse = ops.cross_attention_fwd(q, k, v, B, heads)
-        w_o = _bf(wo)
-        y = ops.gemm(o, w_o, bias=_bf(bo))
-        ctx.save_for_backward(x, c, q, k, v, o, lse, w_in, w_kv, w_o)
+        c = None if context is None else _bf(context.reshape(-1, context.shape[-1]))
+        y, saved = attention_forward(x, c, wq, wk, wv, wo, bo, B, heads)
+        ctx.save_for_backward(*saved)
         ctx.meta = (B, heads, net.dtype, net.shape, None if context is None else (context.dtype, context.shape))
         return y.view(B, Tq, Dq)
 
     @staticmethod
     def backward(ctx, dy: Tensor):  # type: ignore[override]
-        x, c, q, k, v, o, lse, w_in, w_kv, w_o = ctx.saved_tensors
         B, heads, net_dtype, net_shape, ctx_meta = ctx.meta
-        M, Dq = x.shape
-        L = q.shape[1]
-        dy = _bf(dy.reshape(M, Dq))
-        dwo = torch.empty(w_o.shape, dtype=torch.float32, device=dy.device)
-        dbo = torch.empty(Dq, dtype=torch.float32, device=dy.device)
-        ops.wgrad(dy, o, dwo)
-        ops.colsum(dy, dbo)
-        do = ops.gemm(dy, w_o, b_mn_major=True)
-        if c is None:
-            dqkv = torch.empty((M, 3 * L), dtype=torch.bfloat16, device=dy.device)
-            ops.cross_attention_bwd(q, k, v, o, do, lse, B, heads, dq=dqkv[:, :L], dk=dqkv[:, L:2 * L], dv=dqkv[:, 2 * L:])
-            dw = torch.empty((3 * L, Dq), dtype=torch.float32, device=dy.device)
-            ops.wgrad(dqkv, x, dw)
-            dwq, dwk, dwv = dw[:L], dw[L:2 * L], dw[2 * L:]
-            dx = ops.gemm(dqkv, w_in, b_mn_major=True)
-            dctx = None
-        else:
-            dq = torch.empty((M, L), dtype=torch.bfloat16, device=dy.device)
-            dkv = torch.empty((c.shape[0], 2 * L), dtype=torch.bfloat16, device=dy.device)
-            ops.cross_attention_bwd(q, k, v, o, do, lse, B, heads, dq=dq, dk=dkv[:, :L], dv=dkv[:, L:])
-            dwq = torch.empty((L, Dq), dtype=torch.float32, device=dy.device)
-            dwkv = torch.empty((2 * L, c.shape[1]), dtype=torch.float32, device=dy.device)
-            ops.wgrad(dq, x, dwq)
-            ops.wgrad(dkv, c, dwkv)
-            dwk, dwv = dwkv[:L], dwkv[L:]
-            dx = ops.gemm(dq, w_in, b_mn_major=True)
-            dctx = ops.gemm(dkv, w_kv, b_mn_major=True).to(ctx_meta[0]).view(ctx_meta[1])
+        saved = ctx.saved_tensors
+        M, Dq = saved[0].shape
+        dx, dc, dwq, dwk, dwv, dwo, dbo = attention_backward(saved, _bf(dy.reshape(M, Dq)), B, heads)
+        dctx = None if dc is None else dc.to(ctx_meta[0]).view(ctx_meta[1])
         return dx.to(net_dtype).view(net_shape), dctx, dwq, dwk, dwv, dwo, dbo, None
 
 

@@ -14,6 +14,9 @@ enum : int {
     EPI_BIAS_RESID_F32 = B200_EPI_BIAS_RESID_F32,
     EPI_DGELU_BF16 = B200_EPI_DGELU_BF16,
     EPI_PARTIAL_F32 = B200_EPI_PARTIAL_F32,
+    EPI_BIAS_GEGLU_BF16 = B200_EPI_BIAS_GEGLU_BF16,
+    EPI_DGEGLU_BF16 = B200_EPI_DGEGLU_BF16,
+    EPI_BIAS_RESID_BF16 = B200_EPI_BIAS_RESID_BF16,
 };
 
 int set_error(int code, const char* msg);  // records msg (thread-local) and returns code

@@ -8,8 +8,8 @@
 // Fused epilogues (every variant but the split-K partials) run on their own warpgroup, overlapped with the next tile's
 // MMAs: at the end of a tile the MMA warpgroups write t = bf16(acc + bias) -- the first thing every such variant computes --
 // into a 64 KB staging tile in shared memory and go straight on to the next tile's k-loop; the epilogue warpgroup reads
-// t back row by row and does the rest (GELU / dual output, fp32 residual, dGELU on h, M / N edges) with 16-byte global
-// accesses.  Roles (384 threads):
+// t back row by row and does the rest (GELU / dual output, fp32 or bf16 residual, dGELU on h, GEGLU / dGEGLU, M / N edges)
+// with 16-byte global accesses.  Roles (384 threads):
 //   warps 0-7   the two MMA warpgroups
 //   warp 8      the TMA producer (lane 0)
 //   warps 9-11  the epilogue
@@ -161,6 +161,41 @@ __device__ __forceinline__ void epi_chunk(const GemmParams& p, int row, int col,
             for (int e = 0; e < 8; ++e)
                 if (e < n_ok) dst[e] = src[e] + ((e & 1) ? bf16hi(t[e >> 1]) : bf16lo(t[e >> 1]));
         }
+    } else if constexpr (EPI == EPI_BIAS_RESID_BF16) {
+        // out0(bf16) = bf16(float(bf16(acc + bias)) + float(aux(bf16)))     (aux may alias out0)
+        const __nv_bfloat16* src = reinterpret_cast<const __nv_bfloat16*>(p.aux) + off;
+        uint32_t rw[4] = {0u, 0u, 0u, 0u};
+        if (n_ok == 8) {
+            const uint4 r = *reinterpret_cast<const uint4*>(src);
+            rw[0] = r.x; rw[1] = r.y; rw[2] = r.z; rw[3] = r.w;
+        } else {
+#pragma unroll
+            for (int e = 0; e < 8; ++e)
+                if (e < n_ok) rw[e >> 1] |= static_cast<uint32_t>(__bfloat16_as_ushort(src[e])) << (16 * (e & 1));
+        }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) o[i] = pack_bf16x2(bf16lo(t[i]) + bf16lo(rw[i]), bf16hi(t[i]) + bf16hi(rw[i]));
+    } else if constexpr (EPI == EPI_DGEGLU_BF16) {
+        // t = bf16(da) at columns col.. of F; aux = hg [M, 2F]: h at col, gate at F + col.  out0 = dhg: dh at col, dgate at F + col.
+        // (F % 8 == 0, so a chunk is either whole or outside: the caller only passes n_ok == 8.)
+        const int F = p.N >> 1;
+        const __nv_bfloat16* hg = reinterpret_cast<const __nv_bfloat16*>(p.aux) + off;
+        const uint4 hv = *reinterpret_cast<const uint4*>(hg);
+        const uint4 gv = *reinterpret_cast<const uint4*>(hg + F);
+        const uint32_t hw[4] = {hv.x, hv.y, hv.z, hv.w};
+        const uint32_t gw[4] = {gv.x, gv.y, gv.z, gv.w};
+        uint32_t dgate[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const float d0 = bf16lo(t[i]), d1 = bf16hi(t[i]);
+            float g0, g1, q0, q1;
+            gelu_erf2(bf16lo(gw[i]), bf16hi(gw[i]), g0, g1);
+            o[i] = pack_bf16x2(d0 * bf16_round(g0), d1 * bf16_round(g1));              // dh = bf16(da * g)
+            const float dg0 = bf16_round(d0 * bf16lo(hw[i])), dg1 = bf16_round(d1 * bf16hi(hw[i]));  // dg = bf16(da * h)
+            gelu_erf_grad2(bf16lo(gw[i]), bf16hi(gw[i]), q0, q1);
+            dgate[i] = pack_bf16x2(dg0 * q0, dg1 * q1);                                  // dgate = bf16(gelu'(gate) * dg)
+        }
+        *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out0) + off + F) = make_uint4(dgate[0], dgate[1], dgate[2], dgate[3]);
     } else {  // EPI_DGELU_BF16: out0 = bf16( float(bf16(acc)) * gelu'(h) ),  h = aux (bf16)
         const __nv_bfloat16* hsrc = reinterpret_cast<const __nv_bfloat16*>(p.aux) + off;
         uint32_t hw[4] = {0u, 0u, 0u, 0u};
@@ -193,6 +228,25 @@ __device__ __forceinline__ void epi_chunk(const GemmParams& p, int row, int col,
                 if (e < n_ok) d0[e] = __ushort_as_bfloat16(static_cast<unsigned short>(o[e >> 1] >> (16 * (e & 1))));
         }
     }
+}
+
+// GEGLU forward of 8 consecutive columns f .. f + 7 of F: th = bf16(acc + bias) of h, tg that of the gate.  out0 = hg in the
+// reference's column order (h at f, gate at F + f), out1 = a = bf16(h * bf16(gelu(gate))) (dense [M, F]).
+__device__ __forceinline__ void epi_geglu(const GemmParams& p, int row, int f, const uint4& th, const uint4& tg) {
+    const int F = p.N >> 1;
+    const uint32_t hw[4] = {th.x, th.y, th.z, th.w};
+    const uint32_t gw[4] = {tg.x, tg.y, tg.z, tg.w};
+    uint32_t a[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        float g0, g1;
+        gelu_erf2(bf16lo(gw[i]), bf16hi(gw[i]), g0, g1);
+        a[i] = pack_bf16x2(bf16lo(hw[i]) * bf16_round(g0), bf16hi(hw[i]) * bf16_round(g1));
+    }
+    __nv_bfloat16* d0 = reinterpret_cast<__nv_bfloat16*>(p.out0) + static_cast<long long>(row) * p.ldo + f;
+    *reinterpret_cast<uint4*>(d0) = th;
+    *reinterpret_cast<uint4*>(d0 + F) = tg;
+    *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out1) + static_cast<long long>(row) * F + f) = make_uint4(a[0], a[1], a[2], a[3]);
 }
 
 // Staging tile: 128 rows x 256 bf16, 512 B per row; the 16-byte chunk c of row r sits at chunk c ^ (r & 7) of that row.
@@ -246,9 +300,9 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 int m_t, n_t, sp, kb0, kb1;
                 decode_unit(p, u, m_t, n_t, sp, kb0, kb1);
                 const int col = n_t * BN + lane * 8;
-                const int n_ok = min(8, max(0, p.N - col));
+                const int n_ok = min(8, max(0, (EPI == EPI_DGEGLU_BF16 ? p.N >> 1 : p.N) - col));  // dGEGLU's GEMM is F wide
                 const int rows = min(BM, p.M - m_t * BM);
-                if constexpr (EPI == EPI_DGELU_BF16 || EPI == EPI_BIAS_RESID_F32) {
+                if constexpr (EPI == EPI_DGELU_BF16 || EPI == EPI_BIAS_RESID_F32 || EPI == EPI_BIAS_RESID_BF16) {
                     // pull the tile's aux rows into L2 while its MMAs still run: three warps cannot hide HBM latency alone.
                     // Rows are 16-byte aligned and padded to ldo >= the 16-byte-rounded width, so no byte past a row is named.
                     constexpr int eb = EPI == EPI_BIAS_RESID_F32 ? 4 : 2;
@@ -258,13 +312,38 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                     for (int r = threadIdx.x - 9 * 32; r < rows; r += 32 * Cfg::EPI_WARPS)
                         bulk_prefetch_l2(aux + (static_cast<long long>(m_t * BM + r) * p.ldo + n0) * eb, bytes);
                 }
+                if constexpr (EPI == EPI_DGEGLU_BF16) {  // the same for both halves of hg: h at n0, the gate at F + n0
+                    const int F = p.N >> 1, n0 = n_t * BN;
+                    const uint32_t bytes = static_cast<uint32_t>(min(BN, F - n0) * 2);
+                    const __nv_bfloat16* aux = reinterpret_cast<const __nv_bfloat16*>(p.aux);
+                    for (int r = threadIdx.x - 9 * 32; r < rows; r += 32 * Cfg::EPI_WARPS) {
+                        const __nv_bfloat16* src = aux + static_cast<long long>(m_t * BM + r) * p.ldo + n0;
+                        bulk_prefetch_l2(src, bytes);
+                        bulk_prefetch_l2(src + F, bytes);
+                    }
+                }
                 mbar_wait(staging_full, sphase);
-                // epilogue warp w takes rows w, w + 3, ...: one 512-byte row per warp access, 16 bytes per lane
+                if constexpr (EPI == EPI_BIAS_GEGLU_BF16) {
+                    // the tile's 256 columns are 128 h columns and the matching 128 gate columns: a half-warp takes one row,
+                    // lane l & 15 the h chunk l & 15 and the gate chunk 16 + (l & 15) -- one 8-column piece of out0's two
+                    // halves and of out1 each
+                    const int hl = lane & 15;
+                    const int f = n_t * (BN / 2) + hl * 8;
+                    const bool ok = f < (p.N >> 1);
+#pragma unroll 2
+                    for (int r = 2 * (warp - 9) + (lane >> 4); r < rows; r += 2 * Cfg::EPI_WARPS) {
+                        const uint4 th = *reinterpret_cast<const uint4*>(staging + staging_offset(r, hl));
+                        const uint4 tg = *reinterpret_cast<const uint4*>(staging + staging_offset(r, 16 + hl));
+                        if (ok) epi_geglu(p, m_t * BM + r, f, th, tg);
+                    }
+                } else {
+                    // epilogue warp w takes rows w, w + 3, ...: one 512-byte row per warp access, 16 bytes per lane
 #pragma unroll 4
-                for (int r = warp - 9; r < rows; r += Cfg::EPI_WARPS) {
-                    const uint4 v = *reinterpret_cast<const uint4*>(staging + staging_offset(r, lane));
-                    const uint32_t t[4] = {v.x, v.y, v.z, v.w};
-                    if (n_ok > 0) epi_chunk<EPI, QUICK>(p, m_t * BM + r, col, t, n_ok);
+                    for (int r = warp - 9; r < rows; r += Cfg::EPI_WARPS) {
+                        const uint4 v = *reinterpret_cast<const uint4*>(staging + staging_offset(r, lane));
+                        const uint32_t t[4] = {v.x, v.y, v.z, v.w};
+                        if (n_ok > 0) epi_chunk<EPI, QUICK>(p, m_t * BM + r, col, t, n_ok);
+                    }
                 }
                 mbar_arrive(staging_empty);
                 sphase ^= 1u;
@@ -316,6 +395,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                             // (boxes past N = 9 Cin: tap >= 9 lands outside the image -> zero fill, bytes still credited)
                             tma_load_4d(b_dst + i * MN_BOX_BYTES, &tmB, &full_bar[stage], c0, kx - 1, tap < 9 ? y0 + ky - 1 : -65536, bimg);
                         }
+                    } else if constexpr (EPI == EPI_BIAS_GEGLU_BF16) {
+                        // W1 behind a 3-D map {K, F, 2}: one box = 128 h rows then the matching 128 gate rows (rows past F
+                        // zero-filled), so the B tile holds [h | gate] of the same 128 columns
+                        tma_load_3d(b_dst, &tmB, &full_bar[stage], kb * BK, n_t * (BN / 2), 0);
                     } else if constexpr (!TB) {
                         tma_load_2d(b_dst, &tmB, &full_bar[stage], kb * BK, n0);
                     } else {
@@ -368,7 +451,16 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             for (int j = 0; j < 32; ++j) {
                 const int col = colq + j * 8;
                 float b0 = 0.f, b1 = 0.f;
-                if constexpr (EPI != EPI_DGELU_BF16) {
+                if constexpr (EPI == EPI_BIAS_GEGLU_BF16) {
+                    // tile column c < 128: h column n_t * 128 + c; c >= 128: gate column F + n_t * 128 + c - 128
+                    // (the bias is required; f is even and F % 8 == 0, so f < F covers f + 1 too: one 4-byte load of the pair)
+                    const int f = colq - n_t * (BN / 2) + (j & 15) * 8;  // colq = n_t * BN + (lane & 3) * 2
+                    if (f < (p.N >> 1)) {
+                        const uint32_t bp = *reinterpret_cast<const uint32_t*>(p.bias + (j < 16 ? f : f + (p.N >> 1)));
+                        b0 = bf16lo(bp);
+                        b1 = bf16hi(bp);
+                    }
+                } else if constexpr (EPI != EPI_DGELU_BF16 && EPI != EPI_DGEGLU_BF16) {
                     if (p.bias != nullptr) {
                         if (col < p.N) b0 = __bfloat162float(p.bias[col]);
                         if (col + 1 < p.N) b1 = __bfloat162float(p.bias[col + 1]);
@@ -419,6 +511,31 @@ static PFN_encodeTiled get_encode_fn() {
     return fn;
 }
 
+// The tensor-map encode is a driver call and needs a current context.  A host thread that has not yet made a runtime call
+// that binds one has none -- autograd's device thread, for example, when one of our GEMMs is the first CUDA work of a
+// backward.  cudaSetDevice on the runtime's current device makes that device's primary context current; it is skipped
+// whenever a context already is.
+typedef CUresult (*PFN_ctxGetCurrent)(CUcontext*);
+
+static int ensure_current_context() {
+    static PFN_ctxGetCurrent get = nullptr;
+    if (get == nullptr) {
+        void* p = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        cudaError_t e = cudaGetDriverEntryPoint("cuCtxGetCurrent", &p, cudaEnableDefault, &q);
+        if (e != cudaSuccess || q != cudaDriverEntryPointSuccess || p == nullptr)
+            return set_error(B200_ERR_DRIVER, "cuCtxGetCurrent entry point unavailable");
+        get = reinterpret_cast<PFN_ctxGetCurrent>(p);
+    }
+    CUcontext c = nullptr;
+    if (get(&c) == CUDA_SUCCESS && c != nullptr) return 0;
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaSetDevice(dev);
+    if (e != cudaSuccess) return set_error(B200_ERR_DRIVER, cudaGetErrorString(e));
+    return 0;
+}
+
 // rank-2/3 tiled map; dims/box innermost first; strides in BYTES for dims 1.. (rank-1 entries)
 int make_tmap(CUtensorMap* out, const void* base, int elem_bytes, int rank, const uint64_t* dims,
               const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes) {
@@ -442,6 +559,7 @@ int make_tmap(CUtensorMap* out, const void* base, int elem_bytes, int rank, cons
     if ((reinterpret_cast<uintptr_t>(base) & 15u) != 0) return set_error(B200_ERR_ALIGN, "tensor base not 16 B aligned");
     for (int i = 0; i + 1 < rank; ++i)
         if (gstr[i] % 16 != 0) return set_error(B200_ERR_ALIGN, "tensor stride not a multiple of 16 B");
+    if (const int rc = ensure_current_context()) return rc;
     CUresult r = fn(out, dt, static_cast<cuuint32_t>(rank), const_cast<void*>(base), gdim, gstr, bx, es,
                     CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -514,11 +632,14 @@ static int launch_gemm_impl(const CUtensorMap& tmA, const CUtensorMap& tmB, cons
 }
 
 // Operand majors each epilogue is compiled for: (0,0) forward and conv, (0,1) dgrad, (1,1) wgrad, conv wgrad and CLIP's db.
-// The plain bias epilogue takes all four (ops.gemm's general form).
+// The plain bias epilogue takes all four (ops.gemm's general form).  GEGLU and the bf16 residual are forward epilogues (0,0),
+// dGEGLU a dgrad one (0,1).
 template <int EPI, int TA, int TB>
 constexpr bool kHasMajors = EPI == EPI_BIAS_BF16 ||
-                            (TA == 0 && TB == 0 && (EPI == EPI_BIAS_GELU_BF16 || EPI == EPI_BIAS_RESID_F32)) ||
-                            (TA == 0 && TB == 1 && EPI == EPI_DGELU_BF16) || (TA == 1 && TB == 1 && EPI == EPI_PARTIAL_F32);
+                            (TA == 0 && TB == 0 && (EPI == EPI_BIAS_GELU_BF16 || EPI == EPI_BIAS_RESID_F32 ||
+                                                    EPI == EPI_BIAS_GEGLU_BF16 || EPI == EPI_BIAS_RESID_BF16)) ||
+                            (TA == 0 && TB == 1 && (EPI == EPI_DGELU_BF16 || EPI == EPI_DGEGLU_BF16)) ||
+                            (TA == 1 && TB == 1 && EPI == EPI_PARTIAL_F32);
 
 template <int EPI, bool QUICK, int TA, int TB>
 static int launch_majors(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int grid, cudaStream_t stream) {
@@ -590,6 +711,23 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
     if (epilogue != EPI_PARTIAL_F32 && splits != 1) return set_error(B200_ERR_ARG, "gemm: split-K needs EPI_PARTIAL_F32");
     const int num_kb = (K + BK - 1) / BK;
     if (splits > num_kb) splits = num_kb;
+    const bool geglu = epilogue == EPI_BIAS_GEGLU_BF16 || epilogue == EPI_DGEGLU_BF16;
+    if (geglu || epilogue == EPI_BIAS_RESID_BF16) {
+        // checked before any tensor map is encoded: these fail the same way with or without a device
+        if (cg != nullptr) return set_error(B200_ERR_ARG, "gemm: the GEGLU / bf16-residual epilogues are not offered for convolutions");
+        if (epilogue == EPI_DGEGLU_BF16 ? (a_mn_major || !b_mn_major) : (a_mn_major || b_mn_major))
+            return set_error(B200_ERR_ARG, "gemm: operand majors not supported by this epilogue");
+        if (geglu && N % 16 != 0) return set_error(B200_ERR_ARG, "gemm: GEGLU epilogues need N = 2F with F % 8 == 0");
+        if (ldo < N) return set_error(B200_ERR_ARG, "gemm: ldo < N");
+        if (epilogue == EPI_BIAS_GEGLU_BF16 && out1 == nullptr) return set_error(B200_ERR_ARG, "gemm: GEGLU epilogue needs out1 (a, [M, F])");
+        if (epilogue != EPI_BIAS_GEGLU_BF16 && aux == nullptr) return set_error(B200_ERR_ARG, "gemm: epilogue needs aux");
+        if (epilogue == EPI_DGEGLU_BF16 && bias != nullptr) return set_error(B200_ERR_ARG, "gemm: dGEGLU takes no bias");
+        if (epilogue == EPI_BIAS_GEGLU_BF16 && (bias == nullptr || (reinterpret_cast<uintptr_t>(bias) & 3u) != 0))
+            return set_error(B200_ERR_ARG, "gemm: GEGLU epilogue needs a 4-byte aligned bias [2F]");
+        if ((static_cast<unsigned long long>(ldo) * 2) % 16 != 0) return set_error(B200_ERR_ALIGN, "gemm: ldo rows must be 16-byte aligned");
+        if (((reinterpret_cast<uintptr_t>(out0) | reinterpret_cast<uintptr_t>(out1) | reinterpret_cast<uintptr_t>(aux)) & 15u) != 0)
+            return set_error(B200_ERR_ALIGN, "gemm: out0 / out1 / aux not 16-byte aligned");
+    }
 
     CUtensorMap tmA, tmB;
     int rc;
@@ -620,9 +758,17 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
                               static_cast<uint64_t>(cg->H) * cg->W * cg->Cin * 2};
             uint32_t b4[4] = {64, static_cast<uint32_t>(cg->W), static_cast<uint32_t>(hb), 1};
             if ((rc = make_tmap(&tmB, B, 2, 4, d4, s4, b4, 128)) != 0) return rc;
+        } else if (epilogue == EPI_BIAS_GEGLU_BF16) {
+            // W1 [2F, ldb] as {K, F, 2}: one box is 128 rows of the h half and the same 128 rows of the gate half
+            const uint64_t F = static_cast<uint64_t>(N / 2);
+            uint64_t d3[3] = {static_cast<uint64_t>(K), F, 2};
+            uint64_t s3[2] = {static_cast<uint64_t>(ldb) * 2, F * static_cast<uint64_t>(ldb) * 2};
+            uint32_t b3[3] = {BK, BN / 2, 2};
+            if ((rc = make_tmap(&tmB, B, 2, 3, d3, s3, b3, 128)) != 0) return rc;
         } else {
-        if (!b_mn_major) { d[0] = K; d[1] = N; bx[0] = BK; bx[1] = BN; }
-        else             { d[0] = N; d[1] = K; bx[0] = 64; bx[1] = BK; }
+        const int nb = epilogue == EPI_DGEGLU_BF16 ? N / 2 : N;  // dGEGLU: the GEMM itself is F wide
+        if (!b_mn_major) { d[0] = K; d[1] = nb; bx[0] = BK; bx[1] = BN; }
+        else             { d[0] = nb; d[1] = K; bx[0] = 64; bx[1] = BK; }
         s[0] = static_cast<uint64_t>(ldb) * 2;
         if ((rc = make_tmap(&tmB, B, 2, 2, d, s, bx, 128)) != 0) return rc;
         }
@@ -647,7 +793,10 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
     p.conv_cin = cg != nullptr ? cg->Cin : 0;
     p.M = M; p.N = N; p.K = K;
     p.num_m_tiles = (M + BM - 1) / BM;
-    p.num_n_tiles = (N + BN - 1) / BN;
+    // GEGLU's N tile holds 128 h columns and their 128 gate columns; dGEGLU's GEMM is F = N / 2 wide
+    const int tile_n = epilogue == EPI_BIAS_GEGLU_BF16 ? BN / 2 : BN;
+    const int n_cols = geglu ? N / 2 : N;
+    p.num_n_tiles = (n_cols + tile_n - 1) / tile_n;
     p.splits = splits;
     p.num_kb = num_kb;
     p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
@@ -666,6 +815,9 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
         case EPI_BIAS_RESID_F32: return launch_gemm<EPI_BIAS_RESID_F32>(tmA, tmB, p, a_mn, b_mn, grid, stream);
         case EPI_DGELU_BF16: return launch_gemm<EPI_DGELU_BF16>(tmA, tmB, p, a_mn, b_mn, grid, stream);
         case EPI_PARTIAL_F32: return launch_gemm<EPI_PARTIAL_F32>(tmA, tmB, p, a_mn, b_mn, grid, stream);
+        case EPI_BIAS_GEGLU_BF16: return launch_gemm<EPI_BIAS_GEGLU_BF16>(tmA, tmB, p, a_mn, b_mn, grid, stream);
+        case EPI_DGEGLU_BF16: return launch_gemm<EPI_DGEGLU_BF16>(tmA, tmB, p, a_mn, b_mn, grid, stream);
+        case EPI_BIAS_RESID_BF16: return launch_gemm<EPI_BIAS_RESID_BF16>(tmA, tmB, p, a_mn, b_mn, grid, stream);
         default: return set_error(B200_ERR_ARG, "gemm: unknown epilogue");
     }
 }

@@ -245,6 +245,171 @@ __global__ void __launch_bounds__(256, 2) layernorm_bwd_kernel(const void* __res
 }
 
 // ------------------------------------------------------------------------------------------------
+// LayerNorm over bf16 rows (the SD-UNet SpatialTransformer's residual stream is bf16 under autocast): one warp per row,
+// 8 bf16 (16 bytes) per lane access, the row kept packed in registers; dim % 8 == 0, dim <= 256 * NV.
+// Forward: y = bf16(LN_fp32(x)), fp32 mean / rstd.
+// ------------------------------------------------------------------------------------------------
+constexpr int LNB_MAX_V8 = 8;  // 16-byte chunks per lane: dim <= 2048
+
+template <int NV>
+__global__ void __launch_bounds__(256) layernorm_bf16_fwd_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ gamma,
+                                                                 const float* __restrict__ beta, __nv_bfloat16* __restrict__ y,
+                                                                 float* __restrict__ mean_out, float* __restrict__ rstd_out, int rows,
+                                                                 int dim, float eps) {
+    const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (row >= rows) return;
+    const __nv_bfloat16* xr = x + static_cast<long long>(row) * dim;
+    uint4 v[NV];
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < NV; ++i) {
+        const int c = (lane + 32 * i) * 8;
+        v[i] = c < dim ? *reinterpret_cast<const uint4*>(xr + c) : make_uint4(0u, 0u, 0u, 0u);
+        const uint32_t w[4] = {v[i].x, v[i].y, v[i].z, v[i].w};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) s += bf16lo(w[k]) + bf16hi(w[k]);
+    }
+    const float inv_n = 1.0f / static_cast<float>(dim);
+    const float mean = warp_sum(s) * inv_n;
+    float ss = 0.f;
+#pragma unroll
+    for (int i = 0; i < NV; ++i) {
+        const int c = (lane + 32 * i) * 8;
+        if (c < dim) {
+            const uint32_t w[4] = {v[i].x, v[i].y, v[i].z, v[i].w};
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const float a = bf16lo(w[k]) - mean, b = bf16hi(w[k]) - mean;
+                ss += a * a + b * b;
+            }
+        }
+    }
+    const float rstd = rsqrtf(warp_sum(ss) * inv_n + eps);
+    if (lane == 0) {
+        mean_out[row] = mean;
+        rstd_out[row] = rstd;
+    }
+    __nv_bfloat16* yr = y + static_cast<long long>(row) * dim;
+#pragma unroll
+    for (int i = 0; i < NV; ++i) {
+        const int c = (lane + 32 * i) * 8;
+        if (c < dim) {
+            const float4 g0 = *reinterpret_cast<const float4*>(gamma + c), g1 = *reinterpret_cast<const float4*>(gamma + c + 4);
+            const float4 b0 = *reinterpret_cast<const float4*>(beta + c), b1 = *reinterpret_cast<const float4*>(beta + c + 4);
+            const float g[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
+            const float b[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+            const uint32_t w[4] = {v[i].x, v[i].y, v[i].z, v[i].w};
+            uint32_t o[4];
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+                o[k] = pack_bf16x2((bf16lo(w[k]) - mean) * rstd * g[2 * k] + b[2 * k], (bf16hi(w[k]) - mean) * rstd * g[2 * k + 1] + b[2 * k + 1]);
+            *reinterpret_cast<uint4*>(yr + c) = make_uint4(o[0], o[1], o[2], o[3]);
+        }
+    }
+}
+
+// Backward: dx = bf16(float(dres) + float(bf16(LN'(dy)))) -- eager's cast back to the bf16 input, then the bf16 addition of
+// the residual branch's gradient (dres == nullptr: no addition).  Warps stride over rows; each warp keeps running dgamma /
+// dbeta sums of its rows in its own shared-memory rows (lane-private columns: no synchronisation, and no accumulator
+// registers), which the block reduces in warp order into part[blockIdx][0:dim] / [dim:2 dim].  A fixed grid and fixed
+// summation orders make the result deterministic.
+template <int NV>
+__global__ void __launch_bounds__(256) layernorm_bf16_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x,
+                                                                 const float* __restrict__ gamma, const float* __restrict__ mean_in,
+                                                                 const float* __restrict__ rstd_in, const __nv_bfloat16* __restrict__ dres,
+                                                                 __nv_bfloat16* __restrict__ dx, float* __restrict__ part, int rows, int dim) {
+    extern __shared__ float sred[];  // [8 warps][2][dim]
+    const int wib = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const int warps_per_block = blockDim.x >> 5;
+    float* sg = sred + wib * 2 * dim;
+    float* sb = sg + dim;
+    for (int c = lane * 4; c < dim; c += 128) {
+        *reinterpret_cast<float4*>(sg + c) = make_float4(0.f, 0.f, 0.f, 0.f);
+        *reinterpret_cast<float4*>(sb + c) = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    __syncwarp();
+    const float fn = static_cast<float>(dim);
+    for (int row = blockIdx.x * warps_per_block + wib; row < rows; row += gridDim.x * warps_per_block) {
+        const long long off = static_cast<long long>(row) * dim;
+        uint4 xv[NV], dv[NV], rv[NV];
+#pragma unroll
+        for (int i = 0; i < NV; ++i) {  // every load of the row in flight before any is used
+            const int c = (lane + 32 * i) * 8;
+            if (c < dim) {
+                xv[i] = *reinterpret_cast<const uint4*>(x + off + c);
+                dv[i] = *reinterpret_cast<const uint4*>(dy + off + c);
+                rv[i] = dres != nullptr ? *reinterpret_cast<const uint4*>(dres + off + c) : make_uint4(0u, 0u, 0u, 0u);
+            }
+        }
+        const float mean = mean_in[row];
+        const float rstd = rstd_in[row];
+        float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+        for (int i = 0; i < NV; ++i) {
+            const int c = (lane + 32 * i) * 8;
+            if (c < dim) {
+                const uint32_t xw[4] = {xv[i].x, xv[i].y, xv[i].z, xv[i].w};
+                const uint32_t dw[4] = {dv[i].x, dv[i].y, dv[i].z, dv[i].w};
+                float4 ag[2], ab[2];
+                ag[0] = *reinterpret_cast<float4*>(sg + c); ag[1] = *reinterpret_cast<float4*>(sg + c + 4);
+                ab[0] = *reinterpret_cast<float4*>(sb + c); ab[1] = *reinterpret_cast<float4*>(sb + c + 4);
+                float* pg = reinterpret_cast<float*>(ag);
+                float* pb = reinterpret_cast<float*>(ab);
+#pragma unroll
+                for (int k = 0; k < 8; ++k) {
+                    const uint32_t xk = xw[k >> 1], dk = dw[k >> 1];
+                    const float xh = ((k & 1) ? bf16hi(xk) : bf16lo(xk)) - mean;
+                    const float d = (k & 1) ? bf16hi(dk) : bf16lo(dk);
+                    const float xn = xh * rstd;
+                    const float gd = d * gamma[c + k];
+                    s1 += gd;
+                    s2 += gd * xn;
+                    pg[k] += d * xn;
+                    pb[k] += d;
+                }
+                *reinterpret_cast<float4*>(sg + c) = ag[0]; *reinterpret_cast<float4*>(sg + c + 4) = ag[1];
+                *reinterpret_cast<float4*>(sb + c) = ab[0]; *reinterpret_cast<float4*>(sb + c + 4) = ab[1];
+            }
+        }
+        s1 = warp_sum(s1);
+        s2 = warp_sum(s2);
+        const float term = rstd / fn;
+#pragma unroll
+        for (int i = 0; i < NV; ++i) {
+            const int c = (lane + 32 * i) * 8;
+            if (c < dim) {
+                const uint32_t xw[4] = {xv[i].x, xv[i].y, xv[i].z, xv[i].w};
+                const uint32_t dw[4] = {dv[i].x, dv[i].y, dv[i].z, dv[i].w};
+                const uint32_t rw[4] = {rv[i].x, rv[i].y, rv[i].z, rv[i].w};
+                float o[8];
+#pragma unroll
+                for (int k = 0; k < 8; ++k) {
+                    const uint32_t xk = xw[k >> 1], dk = dw[k >> 1], rk = rw[k >> 1];
+                    const float xn = (((k & 1) ? bf16hi(xk) : bf16lo(xk)) - mean) * rstd;
+                    const float d = (k & 1) ? bf16hi(dk) : bf16lo(dk);
+                    const float g = bf16_round((fn * (d * gamma[c + k]) - s1 - xn * s2) * term);  // bf16(LN'(dy))
+                    o[k] = dres != nullptr ? g + ((k & 1) ? bf16hi(rk) : bf16lo(rk)) : g;
+                }
+                *reinterpret_cast<uint4*>(dx + off + c) =
+                    make_uint4(pack_bf16x2(o[0], o[1]), pack_bf16x2(o[2], o[3]), pack_bf16x2(o[4], o[5]), pack_bf16x2(o[6], o[7]));
+            }
+        }
+    }
+    __syncthreads();
+    for (int c = threadIdx.x; c < dim; c += blockDim.x) {
+        float a = 0.f, b = 0.f;
+        for (int w = 0; w < warps_per_block; ++w) {
+            a += sred[(w * 2 + 0) * dim + c];
+            b += sred[(w * 2 + 1) * dim + c];
+        }
+        part[static_cast<long long>(blockIdx.x) * 2 * dim + c] = a;
+        part[static_cast<long long>(blockIdx.x) * 2 * dim + dim + c] = b;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // column sums of a bf16 matrix: grid (col chunks of 256, row slices); block (32, 8)
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) colsum_bf16_kernel(const __nv_bfloat16* __restrict__ x, long long ld, int rows,
@@ -793,11 +958,66 @@ static int ln_bwd_launch(const void* dy, const float* x, long long ld_x, const f
     return ln_bwd_launch2<NV, false, false>(dy, x, ld_x, gamma, mean, rstd, dres, dx_out, ld_dx, dx_bf16, part, nparts, rows, dim, st);
 }
 
+template <int NV>
+static int lnb_fwd_launch(const void* x, const float* gamma, const float* beta, void* y, float* mean, float* rstd, int rows, int dim,
+                          float eps, cudaStream_t st) {
+    layernorm_bf16_fwd_kernel<NV><<<(rows + 7) / 8, 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(x), gamma, beta,
+                                                                   reinterpret_cast<__nv_bfloat16*>(y), mean, rstd, rows, dim, eps);
+    return check_launch("layernorm_bf16_fwd");
+}
+template <int NV>
+static int lnb_bwd_launch(const void* dy, const void* x, const float* gamma, const float* mean, const float* rstd, const void* dres,
+                          void* dx, float* part, int nparts, int rows, int dim, cudaStream_t st) {
+    const size_t smem = static_cast<size_t>(8) * 2 * dim * sizeof(float);
+    if (smem > 48 * 1024) cudaFuncSetAttribute(layernorm_bf16_bwd_kernel<NV>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    layernorm_bf16_bwd_kernel<NV><<<nparts, 256, smem, st>>>(
+        reinterpret_cast<const __nv_bfloat16*>(dy), reinterpret_cast<const __nv_bfloat16*>(x), gamma, mean, rstd,
+        reinterpret_cast<const __nv_bfloat16*>(dres), reinterpret_cast<__nv_bfloat16*>(dx), part, rows, dim);
+    return check_launch("layernorm_bf16_bwd");
+}
+
+static bool misaligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) != 0; }
+
 }  // namespace b200
 
 using namespace b200;
 
 extern "C" int b200_abi_version(void) { return B200_ABI_VERSION; }
+
+extern "C" int b200_layernorm_bf16_fwd(const void* x, const float* gamma, const float* beta, void* y, float* mean, float* rstd, int rows,
+                                       int dim, float eps, cudaStream_t stream) {
+    if (rows <= 0 || dim <= 0 || dim % 8 != 0 || dim > 256 * LNB_MAX_V8)
+        return set_error(B200_ERR_ARG, "layernorm_bf16_fwd: need rows > 0, 0 < dim <= 2048, dim % 8 == 0");
+    if (!x || !gamma || !beta || !y || !mean || !rstd) return set_error(B200_ERR_ARG, "layernorm_bf16_fwd: null pointer");
+    if (misaligned16(x) || misaligned16(gamma) || misaligned16(beta) || misaligned16(y))
+        return set_error(B200_ERR_ALIGN, "layernorm_bf16_fwd: x / gamma / beta / y not 16-byte aligned");
+    const int nv = (dim + 255) / 256;
+    if (nv <= 2) return lnb_fwd_launch<2>(x, gamma, beta, y, mean, rstd, rows, dim, eps, stream);
+    if (nv <= 4) return lnb_fwd_launch<4>(x, gamma, beta, y, mean, rstd, rows, dim, eps, stream);
+    if (nv <= 5) return lnb_fwd_launch<5>(x, gamma, beta, y, mean, rstd, rows, dim, eps, stream);
+    return lnb_fwd_launch<8>(x, gamma, beta, y, mean, rstd, rows, dim, eps, stream);
+}
+
+extern "C" int b200_layernorm_bf16_bwd(const void* dy, const void* x, const float* gamma, const float* mean, const float* rstd,
+                                       const void* dres, void* dx, float* dgb_part, int max_parts, int* nparts_out, int rows, int dim,
+                                       cudaStream_t stream) {
+    if (rows <= 0 || dim <= 0 || dim % 8 != 0 || dim > 256 * LNB_MAX_V8)
+        return set_error(B200_ERR_ARG, "layernorm_bf16_bwd: need rows > 0, 0 < dim <= 2048, dim % 8 == 0");
+    if (!dy || !x || !gamma || !mean || !rstd || !dx || !dgb_part) return set_error(B200_ERR_ARG, "layernorm_bf16_bwd: null pointer");
+    if (max_parts < 1) return set_error(B200_ERR_ARG, "layernorm_bf16_bwd: max_parts < 1");
+    if (misaligned16(dy) || misaligned16(x) || misaligned16(gamma) || misaligned16(dx) || (dres != nullptr && misaligned16(dres)))
+        return set_error(B200_ERR_ALIGN, "layernorm_bf16_bwd: dy / x / gamma / dres / dx not 16-byte aligned");
+    int nparts = num_sms() * 2;
+    const int need = (rows + 7) / 8;
+    if (nparts > need) nparts = need;
+    if (nparts > max_parts) nparts = max_parts;
+    if (nparts_out) *nparts_out = nparts;
+    const int nv = (dim + 255) / 256;
+    if (nv <= 2) return lnb_bwd_launch<2>(dy, x, gamma, mean, rstd, dres, dx, dgb_part, nparts, rows, dim, stream);
+    if (nv <= 4) return lnb_bwd_launch<4>(dy, x, gamma, mean, rstd, dres, dx, dgb_part, nparts, rows, dim, stream);
+    if (nv <= 5) return lnb_bwd_launch<5>(dy, x, gamma, mean, rstd, dres, dx, dgb_part, nparts, rows, dim, stream);
+    return lnb_bwd_launch<8>(dy, x, gamma, mean, rstd, dres, dx, dgb_part, nparts, rows, dim, stream);
+}
 extern "C" const char* b200_last_error(void) { return g_err; }
 extern "C" long long b200_launch_count(void) { return g_launches.load(); }
 

@@ -22,6 +22,9 @@ EPI_DGELU_BF16 = 3
 EPI_PARTIAL_F32 = 4
 EPI_BIAS_QGELU_BF16 = 5  # QuickGELU (CLIP towers) flavours of 1 and 3
 EPI_DQGELU_BF16 = 6
+EPI_BIAS_GEGLU_BF16 = 7   # GEGLU: out0 = hg [M, 2F], out1 = a = h * gelu(gate) [M, F]  (b = W1 [2F, K])
+EPI_DGEGLU_BF16 = 8       # its backward through the FF2 dgrad: out0 = dhg [M, 2F] from aux = hg  (b = W2 MN-major [K, F])
+EPI_BIAS_RESID_BF16 = 9   # out0 = bf16(bf16(acc + bias) + aux), the bf16 residual stream (aux may alias out0)
 
 _MAX_PARTS = 1024
 
@@ -91,6 +94,9 @@ def gemm(
         N, Kb = b.shape
     if K != Kb:
         raise B200Error(f"gemm reduction mismatch: {K} vs {Kb}")
+    # dGEGLU: the product da is F wide, its input hg and output dhg 2F wide -- the C-ABI's N is 2F for both GEGLU epilogues
+    if epilogue == EPI_DGEGLU_BF16:
+        N = 2 * N
     f32_out = epilogue in (EPI_BIAS_RESID_F32, EPI_PARTIAL_F32)
     if out0 is None:
         if epilogue == EPI_PARTIAL_F32:
@@ -101,6 +107,15 @@ def gemm(
     if out0.dtype != (torch.float32 if f32_out else torch.bfloat16):
         raise B200Error("gemm: out0 dtype does not match the epilogue")
     ldo = out0.stride(-2)
+    if epilogue in (EPI_BIAS_GEGLU_BF16, EPI_DGEGLU_BF16, EPI_BIAS_RESID_BF16):
+        if tuple(out0.shape) != (M, N) or out0.stride(1) != 1:
+            raise B200Error("gemm: out0 must be an [M, N] view with unit inner stride")
+        if epilogue == EPI_BIAS_GEGLU_BF16 and (out1 is None or out1.dtype != torch.bfloat16 or tuple(out1.shape) != (M, N // 2)
+                                                or not out1.is_contiguous()):
+            raise B200Error("gemm: the GEGLU epilogue needs out1 = contiguous bf16 [M, F]")
+        if epilogue != EPI_BIAS_GEGLU_BF16 and (aux is None or aux.dtype != torch.bfloat16 or tuple(aux.shape) != (M, N)
+                                                or aux.stride(0) != ldo or aux.stride(1) != 1):
+            raise B200Error("gemm: this epilogue needs a bf16 aux [M, N] with out0's leading dim")
     call(
         "b200_gemm_bf16",
         a.data_ptr(), a.stride(0), int(a_mn_major),
@@ -108,6 +123,18 @@ def gemm(
         M, N, K, epilogue, _ptr(bias), out0.data_ptr(), _ptr(out1), _ptr(aux), ldo, splits, max_ctas, _stream(),
     )
     return out0
+
+
+def geglu(x: Tensor, w1: Tensor, b1: Tensor, *, max_ctas: int = 0) -> Tuple[Tensor, Tensor]:
+    """GEGLU's projection and gate in one GEMM: x [M, K] bf16, w1 [2F, K] bf16 (h rows, then gate rows), b1 [2F] bf16.
+    Returns (hg [M, 2F] = bf16(x w1^T + b1), a [M, F] = bf16(h * bf16(gelu(gate))))."""
+    _need_cuda(x, w1, b1)
+    F2 = w1.shape[0]
+    if F2 % 16 != 0:
+        raise B200Error("geglu: need F % 8 == 0")
+    a = torch.empty((x.shape[0], F2 // 2), dtype=torch.bfloat16, device=x.device)
+    hg = gemm(x, w1, bias=b1, epilogue=EPI_BIAS_GEGLU_BF16, out1=a, max_ctas=max_ctas)
+    return hg, a
 
 
 _NUM_SMS: Dict[int, int] = {}
@@ -187,6 +214,63 @@ def layernorm_bwd(
         call("b200_colsum_finish", part.data_ptr() + 4 * dim, nw * dim, nparts.value, dim, dbeta.data_ptr(), 0, int(accumulate), _stream())
     if dx_colsum is not None:
         call("b200_colsum_finish", part.data_ptr() + 8 * dim, nw * dim, nparts.value, dim, dx_colsum.data_ptr(), 1, int(accumulate), _stream())
+
+
+def _dense_bf16(t: Tensor, name: str) -> None:
+    if t.dtype != torch.bfloat16 or t.dim() != 2 or not t.is_contiguous():
+        raise B200Error(f"layernorm_bf16: {name} must be a contiguous bf16 [rows, dim] tensor")
+
+
+def _dense_f32(t: Tensor, n: int, name: str) -> None:
+    if t.dtype != torch.float32 or tuple(t.shape) != (n,) or not t.is_contiguous():
+        raise B200Error(f"layernorm_bf16: {name} must be a contiguous fp32 [{n}] tensor")
+
+
+def layernorm_bf16_fwd(x: Tensor, gamma: Tensor, beta: Tensor, eps: float) -> Tuple[Tensor, Tensor, Tensor]:
+    """LayerNorm of bf16 rows x [rows, dim] with fp32 statistics: (y = bf16(LN(x)), mean f32 [rows], rstd f32 [rows]).
+    gamma / beta: contiguous fp32 [dim]."""
+    _need_cuda(x, gamma, beta)
+    _dense_bf16(x, "x")
+    rows, dim = x.shape
+    _dense_f32(gamma, dim, "gamma")
+    _dense_f32(beta, dim, "beta")
+    y = torch.empty_like(x)
+    mean = torch.empty(rows, dtype=torch.float32, device=x.device)
+    rstd = torch.empty(rows, dtype=torch.float32, device=x.device)
+    call("b200_layernorm_bf16_fwd", x.data_ptr(), gamma.data_ptr(), beta.data_ptr(), y.data_ptr(), mean.data_ptr(), rstd.data_ptr(),
+         rows, dim, float(eps), _stream())
+    return y, mean, rstd
+
+
+def layernorm_bf16_bwd(dy: Tensor, x: Tensor, gamma: Tensor, mean: Tensor, rstd: Tensor, *, dres: Optional[Tensor] = None,
+                       dgamma: Optional[Tensor] = None, dbeta: Optional[Tensor] = None, accumulate: bool = False) -> Tuple[Tensor, Tensor, Tensor]:
+    """(dx, dgamma, dbeta): dx = bf16(dres + bf16(LN'(dy))) bf16 [rows, dim]; dgamma / dbeta fp32 [dim] (``accumulate``: added)."""
+    _need_cuda(dy, x, gamma, mean, rstd, dres)
+    _dense_bf16(dy, "dy")
+    _dense_bf16(x, "x")
+    if dres is not None:
+        _dense_bf16(dres, "dres")
+    rows, dim = x.shape
+    if dy.shape != x.shape or (dres is not None and dres.shape != x.shape):
+        raise B200Error("layernorm_bf16_bwd: dy / dres must have x's shape")
+    _dense_f32(gamma, dim, "gamma")
+    _dense_f32(mean, rows, "mean")
+    _dense_f32(rstd, rows, "rstd")
+    dx = torch.empty_like(x)
+    if dgamma is None:
+        dgamma = torch.empty(dim, dtype=torch.float32, device=x.device)
+        dbeta = torch.empty(dim, dtype=torch.float32, device=x.device)
+        accumulate = False
+    _need_cuda(dgamma, dbeta)
+    _dense_f32(dgamma, dim, "dgamma")
+    _dense_f32(dbeta, dim, "dbeta")
+    part = WORKSPACE.get(x.device, 2 * _MAX_PARTS * dim, "lnbwd")
+    nparts = ctypes.c_int(0)
+    call("b200_layernorm_bf16_bwd", dy.data_ptr(), x.data_ptr(), gamma.data_ptr(), mean.data_ptr(), rstd.data_ptr(), _ptr(dres),
+         dx.data_ptr(), part.data_ptr(), _MAX_PARTS, ctypes.byref(nparts), rows, dim, _stream())
+    call("b200_colsum_finish", part.data_ptr(), 2 * dim, nparts.value, dim, dgamma.data_ptr(), 0, int(accumulate), _stream())
+    call("b200_colsum_finish", part.data_ptr() + 4 * dim, 2 * dim, nparts.value, dim, dbeta.data_ptr(), 0, int(accumulate), _stream())
+    return dx, dgamma, dbeta
 
 
 # ----------------------------------------------------------------------------------------------------------------

@@ -9,8 +9,9 @@
 
 Rounding points are eager's under bf16 autocast (oracle/unet_oracle.py::res_block): GroupNorm / SiLU in fp32 with one bf16
 rounding at the conv input, every conv / Linear output rounded to bf16, the two residual adds in bf16.  This is the
-forward only -- the UNet's attention at T = 4096 keys, GEGLU, up / down-sampling, the weight gradients of the convolution
-and the module / training step are the open part of row N3.
+forward only.  The UNet's attention (``attention.CrossAttentionB200``) and its SpatialTransformer with GEGLU
+(``spatial_transformer.SpatialTransformerB200``) train natively; the ResBlock backward, up / down-sampling and the
+module / training step are the open part of row N3.
 """
 from __future__ import annotations
 

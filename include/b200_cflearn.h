@@ -47,7 +47,18 @@ enum {
     B200_EPI_PARTIAL_F32 = 4,    /* out0[f32][split, M, N] = partial accumulators (split-K)                      */
     B200_EPI_BIAS_QGELU_BF16 = 5, /* like 1 with QuickGELU x * sigmoid(1.702 x) (CLIP, activations.py:151-153), rounded to
                                     bf16 after each of eager's three elementwise ops                              */
-    B200_EPI_DQGELU_BF16 = 6      /* like 3: autograd of those three ops with eager's bf16 rounding after each kernel */
+    B200_EPI_DQGELU_BF16 = 6,     /* like 3: autograd of those three ops with eager's bf16 rounding after each kernel */
+    /* GEGLU (cflearn/modules/core/activations.py:157-164): N = 2F, the rows of W1 = [h rows 0..F-1 ; gate rows F..2F-1]
+     * (the reference layout), F % 8 == 0.  out0 = hg = bf16(acc + bias) [M, ldo] (2F columns, the reference's column order);
+     * out1 = a = bf16(float(h) * float(bf16(gelu_erf(gate)))), DENSE [M, F] (row stride F).  bias bf16 [2F], required.
+     * A and B K-major. */
+    B200_EPI_BIAS_GEGLU_BF16 = 7,
+    /* its backward through the FF2 dgrad: the GEMM is da = dy . W2 with W2 MN-major [K, ldb] of F columns, but N = 2F as
+     * above; aux = hg [M, ldo], out0 = dhg [M, ldo]:  dh = bf16(float(bf16(da)) * g), dg = bf16(float(bf16(da)) * h),
+     * dgate = bf16(gelu_erf'(gate) * float(dg)), g = bf16(gelu_erf(gate)) -- eager's three roundings.  No bias. */
+    B200_EPI_DGEGLU_BF16 = 8,
+    /* out0[bf16] = bf16(float(bf16(acc + bias)) + float(aux[bf16]))   (aux may alias out0): the bf16 residual stream */
+    B200_EPI_BIAS_RESID_BF16 = 9
 };
 
 int b200_abi_version(void);
@@ -59,7 +70,8 @@ long long b200_launch_count(void);
  * Dense layers: C[M,N] = A[M,K] . B[N,K]^T on the tensor cores (wgmma: bf16 in, fp32 accumulate in registers).
  *   a_mn_major = 0: A is row-major [M, lda] (K contiguous);  1: A is row-major [K, lda] (M contiguous).
  *   b_mn_major = 0: B is row-major [N, ldb] (K contiguous);  1: B is row-major [K, ldb] (N contiguous).
- *   bias: bf16 [N] or NULL.  ldo: leading dimension (elements) of out0/out1/aux.  N % 8 == 0.
+ *   bias: bf16 [N] or NULL.  ldo: leading dimension (elements) of out0/out1/aux (but see the GEGLU epilogues: their
+ *   out1 is dense).  N % 8 == 0.  out0 / out1 / aux 16-byte aligned.
  *   splits > 1 only with B200_EPI_PARTIAL_F32 (out0 is f32 [splits, M, ldo]).  max_ctas <= 0: all SMs.
  * Replaces F.linear at cflearn/modules/core/customs.py:85-89 (Linear.forward), the packed-QKV projection at
  * cflearn/modules/core/attentions.py:214, FeedForward's Linear->GELU->Linear at
@@ -101,6 +113,19 @@ int b200_layernorm_bwd(const void* dy, int dy_is_f32, const float* x, long long 
                        const float* rstd, const float* dres, float* dx_out, long long ld_dx, void* dx_bf16,
                        float* dgb_part, int max_parts, int* nparts_out, int rows, int dim, int dx_colsum,
                        cudaStream_t stream);
+
+/* LayerNorm over BF16 rows: the SD-v1.5 UNet's SpatialTransformerBlock norms (mixed_stacks/api.py:800-812), whose residual
+ * stream is bf16 under autocast.  x, y, dy, dres, dx: bf16 [rows, dim] dense; gamma, beta f32 [dim]; 0 < dim <= 2048,
+ * dim % 8 == 0; x / y / dy / dres / dx / gamma / beta 16-byte aligned.
+ *   forward : y = bf16(LN_fp32(x)); mean, rstd f32 [rows].
+ *   backward: dx = bf16(float(dres) + float(bf16(LN'(dy))))  (dres NULL: dx = bf16(LN'(dy))) -- eager's cast back to the bf16
+ *             input followed by the bf16 accumulation of the residual branch.  dgb_part: f32 [nparts, 2 * dim] ([.., 0:dim]
+ *             dgamma, [.., dim:2 dim] dbeta partials; finish with b200_colsum_finish, unrounded).  Deterministic. */
+int b200_layernorm_bf16_fwd(const void* x_bf16, const float* gamma, const float* beta, void* y_bf16, float* mean, float* rstd,
+                            int rows, int dim, float eps, cudaStream_t stream);
+int b200_layernorm_bf16_bwd(const void* dy_bf16, const void* x_bf16, const float* gamma, const float* mean, const float* rstd,
+                            const void* dres_bf16, void* dx_bf16, float* dgb_part, int max_parts, int* nparts_out, int rows, int dim,
+                            cudaStream_t stream);
 
 /* column sums: part[p][c] = sum over a slice of rows of x[r][c]  (x bf16 or f32), then finish() reduces the
  * parts.  Bias gradients of every Linear (autograd of customs.py:89) and LN gamma/beta gradients. */
