@@ -44,6 +44,8 @@ SIGNATURES: Dict[str, Any] = {
     "b200_colsum_bf16": (c_int, [_P, _LL, c_int, c_int, _P, c_int, POINTER(c_int), _P]),
     "b200_colsum_finish": (c_int, [_P, _LL, c_int, c_int, _P, c_int, c_int, _P]),
     "b200_colsum_finish2": (c_int, [_P, _LL, c_int, c_int, _P, c_int, c_int, _P, c_int, c_int, _P]),
+    "b200_colsum_per_image_workspace_floats": (_LL, [c_int, c_int, c_int]),
+    "b200_colsum_per_image_bf16": (c_int, [_P, c_int, c_int, c_int, _P, _P, _P, _P]),
     "b200_attention_fwd": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_float, c_int, _P]),
     "b200_set_attention_fwd_version": (c_int, [c_int]),
     "b200_set_attention_bwd_version": (c_int, [c_int]),

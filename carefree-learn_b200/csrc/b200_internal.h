@@ -17,6 +17,8 @@ enum : int {
     EPI_BIAS_GEGLU_BF16 = B200_EPI_BIAS_GEGLU_BF16,
     EPI_DGEGLU_BF16 = B200_EPI_DGEGLU_BF16,
     EPI_BIAS_RESID_BF16 = B200_EPI_BIAS_RESID_BF16,
+    EPI_BIAS_ADD_PER_IMAGE_BF16 = B200_EPI_BIAS_ADD_PER_IMAGE_BF16,
+    EPI_BIAS_RESID_CLAMP_BF16 = B200_EPI_BIAS_RESID_CLAMP_BF16,
 };
 
 int set_error(int code, const char* msg);  // records msg (thread-local) and returns code

@@ -161,9 +161,11 @@ __device__ __forceinline__ void epi_chunk(const GemmParams& p, int row, int col,
             for (int e = 0; e < 8; ++e)
                 if (e < n_ok) dst[e] = src[e] + ((e & 1) ? bf16hi(t[e >> 1]) : bf16lo(t[e >> 1]));
         }
-    } else if constexpr (EPI == EPI_BIAS_RESID_BF16) {
+    } else if constexpr (EPI == EPI_BIAS_RESID_BF16 || EPI == EPI_BIAS_ADD_PER_IMAGE_BF16 || EPI == EPI_BIAS_RESID_CLAMP_BF16) {
         // out0(bf16) = bf16(float(bf16(acc + bias)) + float(aux(bf16)))     (aux may alias out0)
-        const __nv_bfloat16* src = reinterpret_cast<const __nv_bfloat16*>(p.aux) + off;
+        // per image: aux is a [B, ldo] table, one row per image of the convolution (a 128-row tile may hold two images)
+        const long long aux_off = EPI == EPI_BIAS_ADD_PER_IMAGE_BF16 ? static_cast<long long>(row / (p.conv_h * p.conv_w)) * p.ldo + col : off;
+        const __nv_bfloat16* src = reinterpret_cast<const __nv_bfloat16*>(p.aux) + aux_off;
         uint32_t rw[4] = {0u, 0u, 0u, 0u};
         if (n_ok == 8) {
             const uint4 r = *reinterpret_cast<const uint4*>(src);
@@ -175,6 +177,14 @@ __device__ __forceinline__ void epi_chunk(const GemmParams& p, int row, int col,
         }
 #pragma unroll
         for (int i = 0; i < 4; ++i) o[i] = pack_bf16x2(bf16lo(t[i]) + bf16lo(rw[i]), bf16hi(t[i]) + bf16hi(rw[i]));
+        if constexpr (EPI == EPI_BIAS_RESID_CLAMP_BF16) {
+            // torch.clamp to bf16's finite range on the rounded sum: +-inf (0x7f80 / 0xff80) -> +-max (0x7f7f / 0xff7f), NaN kept
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                if ((o[i] & 0x7fffu) == 0x7f80u) o[i] = (o[i] & 0xffff8000u) | 0x7f7fu;
+                if ((o[i] & 0x7fff0000u) == 0x7f800000u) o[i] = (o[i] & 0x8000ffffu) | 0x7f7f0000u;
+            }
+        }
     } else if constexpr (EPI == EPI_DGEGLU_BF16) {
         // t = bf16(da) at columns col.. of F; aux = hg [M, 2F]: h at col, gate at F + col.  out0 = dhg: dh at col, dgate at F + col.
         // (F % 8 == 0, so a chunk is either whole or outside: the caller only passes n_ok == 8.)
@@ -302,7 +312,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 const int col = n_t * BN + lane * 8;
                 const int n_ok = min(8, max(0, (EPI == EPI_DGEGLU_BF16 ? p.N >> 1 : p.N) - col));  // dGEGLU's GEMM is F wide
                 const int rows = min(BM, p.M - m_t * BM);
-                if constexpr (EPI == EPI_DGELU_BF16 || EPI == EPI_BIAS_RESID_F32 || EPI == EPI_BIAS_RESID_BF16) {
+                if constexpr (EPI == EPI_DGELU_BF16 || EPI == EPI_BIAS_RESID_F32 || EPI == EPI_BIAS_RESID_BF16 ||
+                              EPI == EPI_BIAS_RESID_CLAMP_BF16) {
                     // pull the tile's aux rows into L2 while its MMAs still run: three warps cannot hide HBM latency alone.
                     // Rows are 16-byte aligned and padded to ldo >= the 16-byte-rounded width, so no byte past a row is named.
                     constexpr int eb = EPI == EPI_BIAS_RESID_F32 ? 4 : 2;
@@ -311,6 +322,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                     const uint8_t* aux = reinterpret_cast<const uint8_t*>(p.aux);
                     for (int r = threadIdx.x - 9 * 32; r < rows; r += 32 * Cfg::EPI_WARPS)
                         bulk_prefetch_l2(aux + (static_cast<long long>(m_t * BM + r) * p.ldo + n0) * eb, bytes);
+                }
+                if constexpr (EPI == EPI_BIAS_ADD_PER_IMAGE_BF16) {  // the table has one row per image: prefetch the tile's images
+                    const int hw = p.conv_h * p.conv_w, n0 = n_t * BN;
+                    const int img0 = (m_t * BM) / hw, img1 = (m_t * BM + rows - 1) / hw;
+                    const uint32_t bytes = static_cast<uint32_t>((min(BN, p.N - n0) * 2 + 15) & ~15);
+                    const uint8_t* aux = reinterpret_cast<const uint8_t*>(p.aux);
+                    for (int b = img0 + threadIdx.x - 9 * 32; b <= img1; b += 32 * Cfg::EPI_WARPS)
+                        bulk_prefetch_l2(aux + (static_cast<long long>(b) * p.ldo + n0) * 2, bytes);
                 }
                 if constexpr (EPI == EPI_DGEGLU_BF16) {  // the same for both halves of hg: h at n0, the gate at F + n0
                     const int F = p.N >> 1, n0 = n_t * BN;
@@ -632,12 +651,13 @@ static int launch_gemm_impl(const CUtensorMap& tmA, const CUtensorMap& tmB, cons
 }
 
 // Operand majors each epilogue is compiled for: (0,0) forward and conv, (0,1) dgrad, (1,1) wgrad, conv wgrad and CLIP's db.
-// The plain bias epilogue takes all four (ops.gemm's general form).  GEGLU and the bf16 residual are forward epilogues (0,0),
-// dGEGLU a dgrad one (0,1).
+// The plain bias epilogue takes all four (ops.gemm's general form).  GEGLU, the bf16 residual and its two convolution variants
+// are forward epilogues (0,0), dGEGLU a dgrad one (0,1).
 template <int EPI, int TA, int TB>
 constexpr bool kHasMajors = EPI == EPI_BIAS_BF16 ||
                             (TA == 0 && TB == 0 && (EPI == EPI_BIAS_GELU_BF16 || EPI == EPI_BIAS_RESID_F32 ||
-                                                    EPI == EPI_BIAS_GEGLU_BF16 || EPI == EPI_BIAS_RESID_BF16)) ||
+                                                    EPI == EPI_BIAS_GEGLU_BF16 || EPI == EPI_BIAS_RESID_BF16 ||
+                                                    EPI == EPI_BIAS_ADD_PER_IMAGE_BF16 || EPI == EPI_BIAS_RESID_CLAMP_BF16)) ||
                             (TA == 0 && TB == 1 && (EPI == EPI_DGELU_BF16 || EPI == EPI_DGEGLU_BF16)) ||
                             (TA == 1 && TB == 1 && EPI == EPI_PARTIAL_F32);
 
@@ -727,6 +747,15 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
         if ((static_cast<unsigned long long>(ldo) * 2) % 16 != 0) return set_error(B200_ERR_ALIGN, "gemm: ldo rows must be 16-byte aligned");
         if (((reinterpret_cast<uintptr_t>(out0) | reinterpret_cast<uintptr_t>(out1) | reinterpret_cast<uintptr_t>(aux)) & 15u) != 0)
             return set_error(B200_ERR_ALIGN, "gemm: out0 / out1 / aux not 16-byte aligned");
+    }
+    if (epilogue == EPI_BIAS_ADD_PER_IMAGE_BF16 || epilogue == EPI_BIAS_RESID_CLAMP_BF16) {
+        // the ResBlock's convolution epilogues, checked before any tensor map is encoded
+        if (cg == nullptr || cg->mode != 1) return set_error(B200_ERR_ARG, "gemm: the per-image / clamped residual epilogues are for conv3x3 only");
+        if (aux == nullptr) return set_error(B200_ERR_ARG, "gemm: epilogue needs aux");
+        if (ldo < N) return set_error(B200_ERR_ARG, "gemm: ldo < N");
+        if ((static_cast<unsigned long long>(ldo) * 2) % 16 != 0) return set_error(B200_ERR_ALIGN, "gemm: ldo rows must be 16-byte aligned");
+        if (((reinterpret_cast<uintptr_t>(out0) | reinterpret_cast<uintptr_t>(aux)) & 15u) != 0)
+            return set_error(B200_ERR_ALIGN, "gemm: out0 / aux not 16-byte aligned");
     }
 
     CUtensorMap tmA, tmB;
@@ -818,6 +847,8 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
         case EPI_BIAS_GEGLU_BF16: return launch_gemm<EPI_BIAS_GEGLU_BF16>(tmA, tmB, p, a_mn, b_mn, grid, stream);
         case EPI_DGEGLU_BF16: return launch_gemm<EPI_DGEGLU_BF16>(tmA, tmB, p, a_mn, b_mn, grid, stream);
         case EPI_BIAS_RESID_BF16: return launch_gemm<EPI_BIAS_RESID_BF16>(tmA, tmB, p, a_mn, b_mn, grid, stream);
+        case EPI_BIAS_ADD_PER_IMAGE_BF16: return launch_gemm<EPI_BIAS_ADD_PER_IMAGE_BF16>(tmA, tmB, p, a_mn, b_mn, grid, stream);
+        case EPI_BIAS_RESID_CLAMP_BF16: return launch_gemm<EPI_BIAS_RESID_CLAMP_BF16>(tmA, tmB, p, a_mn, b_mn, grid, stream);
         default: return set_error(B200_ERR_ARG, "gemm: unknown epilogue");
     }
 }
@@ -844,7 +875,9 @@ extern "C" int b200_conv3x3_nhwc_bf16(const void* x, const void* w_packed, const
     if (W > BM || BM % W != 0) return set_error(B200_ERR_ARG, "conv3x3: the image width must divide 128");
     const int hb = H < BM / W ? H : BM / W;
     if (H % hb != 0 || BM % (W * hb) != 0) return set_error(B200_ERR_ARG, "conv3x3: H must be a multiple of 128 / W (or H * W must divide 128)");
-    if (epilogue != EPI_BIAS_BF16 && epilogue != EPI_BIAS_RESID_F32) return set_error(B200_ERR_ARG, "conv3x3: epilogue must be BIAS_BF16 or BIAS_RESID_F32");
+    if (epilogue != EPI_BIAS_BF16 && epilogue != EPI_BIAS_RESID_F32 && epilogue != EPI_BIAS_ADD_PER_IMAGE_BF16 &&
+        epilogue != EPI_BIAS_RESID_CLAMP_BF16)
+        return set_error(B200_ERR_ARG, "conv3x3: epilogue must be BIAS_BF16, BIAS_RESID_F32, BIAS_ADD_PER_IMAGE_BF16 or BIAS_RESID_CLAMP_BF16");
     ConvGeom cg{B, H, W, Cin, 1};
     const long long M = static_cast<long long>(B) * H * W;
     if (M > 0x7fffffffll) return set_error(B200_ERR_ARG, "conv3x3: too many pixels");

@@ -412,13 +412,11 @@ __global__ void __launch_bounds__(256) layernorm_bf16_bwd_kernel(const __nv_bflo
 // ------------------------------------------------------------------------------------------------
 // column sums of a bf16 matrix: grid (col chunks of 256, row slices); block (32, 8)
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) colsum_bf16_kernel(const __nv_bfloat16* __restrict__ x, long long ld, int rows,
-                                                          int cols, float* __restrict__ part) {
+// one block's share: part_row[c] = sum of x[r][c] over rows [r_begin, r_end), for the 256 columns of blockIdx.x
+__device__ __forceinline__ void colsum_slice(const __nv_bfloat16* __restrict__ x, long long ld, int r_begin, int r_end, int cols,
+                                             float* __restrict__ part_row) {
     __shared__ float sm[8][256 + 8];
     const int c0 = blockIdx.x * 256 + threadIdx.x * 8;
-    const int nslices = gridDim.y;
-    const int r_begin = static_cast<int>((static_cast<long long>(rows) * blockIdx.y) / nslices);
-    const int r_end = static_cast<int>((static_cast<long long>(rows) * (blockIdx.y + 1)) / nslices);
     float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     if (c0 < cols) {
         int r = r_begin + threadIdx.y;
@@ -447,8 +445,42 @@ __global__ void __launch_bounds__(256) colsum_bf16_kernel(const __nv_bfloat16* _
         float s = 0.f;
 #pragma unroll
         for (int w = 0; w < 8; ++w) s += sm[w][t];
-        part[static_cast<long long>(blockIdx.y) * cols + c] = s;
+        part_row[c] = s;
     }
+}
+
+__global__ void __launch_bounds__(256) colsum_bf16_kernel(const __nv_bfloat16* __restrict__ x, long long ld, int rows,
+                                                          int cols, float* __restrict__ part) {
+    const int nslices = gridDim.y;
+    const int r_begin = static_cast<int>((static_cast<long long>(rows) * blockIdx.y) / nslices);
+    const int r_end = static_cast<int>((static_cast<long long>(rows) * (blockIdx.y + 1)) / nslices);
+    colsum_slice(x, ld, r_begin, r_end, cols, part + static_cast<long long>(blockIdx.y) * cols);
+}
+
+// per-image column sums: grid (column chunks of 256, slices per image, images); x dense [B, hw, cols]; the partial row of
+// (image b, slice s) is b * gridDim.y + s
+__global__ void __launch_bounds__(256) colsum_per_image_kernel(const __nv_bfloat16* __restrict__ x, int hw, int cols,
+                                                               float* __restrict__ part) {
+    const int nslices = gridDim.y;
+    const int r_begin = static_cast<int>((static_cast<long long>(hw) * blockIdx.y) / nslices);
+    const int r_end = static_cast<int>((static_cast<long long>(hw) * (blockIdx.y + 1)) / nslices);
+    colsum_slice(x + static_cast<long long>(blockIdx.z) * hw * cols, cols, r_begin, r_end, cols,
+                 part + (static_cast<long long>(blockIdx.z) * nslices + blockIdx.y) * cols);
+}
+
+// per_image[b][c] = bf16(sum_s part[b][s][c]); total[c] = bf16_round(sum_b of those unrounded sums), all in a fixed order
+__global__ void __launch_bounds__(256) colsum_per_image_finish_kernel(const float* __restrict__ part, int B, int nslices, int cols,
+                                                                      __nv_bfloat16* __restrict__ per_image, float* __restrict__ total) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= cols) return;
+    float tot = 0.f;
+    for (int b = 0; b < B; ++b) {
+        float s = 0.f;
+        for (int j = 0; j < nslices; ++j) s += part[(static_cast<long long>(b) * nslices + j) * cols + c];
+        per_image[static_cast<long long>(b) * cols + c] = __float2bfloat16_rn(s);
+        tot += s;
+    }
+    total[c] = bf16_round(tot);
 }
 
 // out[c] (+)= sum_p part[p * part_ld + c]: block = 32 columns x 8 part lanes (a loop over up to 592 parts serially per
@@ -1080,6 +1112,36 @@ extern "C" int b200_colsum_finish2(const float* part, long long part_ld, int npa
     if (nparts <= 0 || cols0 <= 0 || cols1 <= 0 || part_ld < cols0 + cols1) return set_error(B200_ERR_ARG, "colsum_finish2: bad size");
     colsum_finish2_kernel<<<(cols0 + cols1 + 31) / 32, dim3(32, 8), 0, stream>>>(part, part_ld, nparts, cols0, out0, round0, cols1, out1, round1, accumulate);
     return check_launch("colsum_finish2");
+}
+
+// slices per image: about four blocks per SM of an H100 SXM over the whole grid, at most 32, at least 8 rows each
+static int colsum_per_image_slices(int B, int HW, int C) {
+    const int chunks = (C + 255) / 256;
+    int s = (132 * 4) / (chunks * B);
+    const int cap = (HW + 7) / 8 < 32 ? (HW + 7) / 8 : 32;
+    if (s > cap) s = cap;
+    return s < 1 ? 1 : s;
+}
+
+extern "C" long long b200_colsum_per_image_workspace_floats(int B, int HW, int C) {
+    if (B <= 0 || HW <= 0 || C <= 0) return 0;
+    return static_cast<long long>(B) * colsum_per_image_slices(B, HW, C) * C;
+}
+
+extern "C" int b200_colsum_per_image_bf16(const void* x_bf16, int B, int HW, int C, void* per_image_bf16, float* total, float* workspace,
+                                          cudaStream_t stream) {
+    if (B <= 0 || HW <= 0 || C <= 0 || C % 8 != 0) return set_error(B200_ERR_ARG, "colsum_per_image: need B, HW > 0 and C a positive multiple of 8");
+    if (static_cast<long long>(B) * HW > 0x7fffffffll) return set_error(B200_ERR_ARG, "colsum_per_image: too many rows");
+    if (x_bf16 == nullptr || per_image_bf16 == nullptr || total == nullptr || workspace == nullptr)
+        return set_error(B200_ERR_ARG, "colsum_per_image: null pointer");
+    if ((reinterpret_cast<uintptr_t>(x_bf16) & 15u) != 0) return set_error(B200_ERR_ALIGN, "colsum_per_image: x not 16-byte aligned");
+    const int slices = colsum_per_image_slices(B, HW, C);
+    colsum_per_image_kernel<<<dim3((C + 255) / 256, slices, B), dim3(32, 8), 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(x_bf16), HW, C,
+                                                                                         workspace);
+    if (const int rc = check_launch("colsum_per_image")) return rc;
+    colsum_per_image_finish_kernel<<<(C + 127) / 128, 128, 0, stream>>>(workspace, B, slices, C, reinterpret_cast<__nv_bfloat16*>(per_image_bf16),
+                                                                        total);
+    return check_launch("colsum_per_image_finish");
 }
 
 extern "C" int b200_splitk_reduce(const float* partial, int splits, long long n, float* out, int round_bf16,

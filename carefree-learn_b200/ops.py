@@ -25,6 +25,8 @@ EPI_DQGELU_BF16 = 6
 EPI_BIAS_GEGLU_BF16 = 7   # GEGLU: out0 = hg [M, 2F], out1 = a = h * gelu(gate) [M, F]  (b = W1 [2F, K])
 EPI_DGEGLU_BF16 = 8       # its backward through the FF2 dgrad: out0 = dhg [M, 2F] from aux = hg  (b = W2 MN-major [K, F])
 EPI_BIAS_RESID_BF16 = 9   # out0 = bf16(bf16(acc + bias) + aux), the bf16 residual stream (aux may alias out0)
+EPI_BIAS_ADD_PER_IMAGE_BF16 = 10  # conv3x3 only: out0 = bf16(bf16(acc + bias) + aux[image, c]), aux bf16 [B, Cout]
+EPI_BIAS_RESID_CLAMP_BF16 = 11    # conv3x3 only: 9, then +-inf -> +-bf16 max (NaN kept)
 
 _MAX_PARTS = 1024
 
@@ -171,6 +173,22 @@ def colsum(x: Tensor, out: Tensor, *, round_bf16: bool = True, accumulate: bool 
     call("b200_colsum_bf16", x.data_ptr(), x.stride(0), rows, cols, part.data_ptr(), _MAX_PARTS, ctypes.byref(nparts), _stream())
     call("b200_colsum_finish", part.data_ptr(), cols, nparts.value, cols, out.data_ptr(), int(round_bf16), int(accumulate), _stream())
     return out
+
+
+def colsum_per_image(x: Tensor) -> Tuple[Tensor, Tensor]:
+    """x: contiguous bf16 [B, ..., C] (the pixels of each image in between).  One pass over x returns (per_image bf16 [B, C] =
+    bf16(sum over image b's rows), total fp32 [C] = float(bf16(sum over all rows))): the gradients of a per-image [B, C] table
+    added to every pixel, and of the bias of the conv that wrote x."""
+    _need_cuda(x)
+    if x.dtype != torch.bfloat16 or x.dim() < 2 or not x.is_contiguous():
+        raise B200Error("colsum_per_image: need contiguous bf16 [B, ..., C]")
+    B, C = x.shape[0], x.shape[-1]
+    HW = x.numel() // max(B * C, 1)
+    per_image = torch.empty((B, C), dtype=torch.bfloat16, device=x.device)
+    total = torch.empty(C, dtype=torch.float32, device=x.device)
+    ws = WORKSPACE.get(x.device, int(_cabi.lib().b200_colsum_per_image_workspace_floats(B, HW, C)), "colsum_per_image")
+    call("b200_colsum_per_image_bf16", x.data_ptr(), B, HW, C, per_image.data_ptr(), total.data_ptr(), ws.data_ptr(), _stream())
+    return per_image, total
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -533,7 +551,9 @@ def unpack_conv3x3_weight(w_packed: Tensor, cin: int) -> Tensor:
 
 
 def conv3x3(x: Tensor, w_packed: Tensor, bias: Optional[Tensor] = None, *, epilogue: int = EPI_BIAS_BF16, aux: Optional[Tensor] = None) -> Tensor:
-    """x: bf16 [B, H, W, Cin] channels-last; w_packed: bf16 [Cout, 9 * Cin] -> bf16 (or fp32 with the residual epilogue) [B, H, W, Cout]."""
+    """x: bf16 [B, H, W, Cin] channels-last; w_packed: bf16 [Cout, 9 * Cin] -> bf16 (or fp32 with the residual epilogue) [B, H, W, Cout].
+    ``EPI_BIAS_ADD_PER_IMAGE_BF16``: aux = contiguous bf16 [B, Cout], added to every pixel of its image;
+    ``EPI_BIAS_RESID_CLAMP_BF16``: aux = contiguous bf16 [B, H, W, Cout] (or [B * H * W, Cout]), the sum clamped to bf16's finite range."""
     _need_cuda(x, w_packed, bias, aux)
     if x.dtype != torch.bfloat16 or x.dim() != 4 or not x.is_contiguous() or w_packed.dtype != torch.bfloat16 or not w_packed.is_contiguous():
         raise B200Error("conv3x3: need contiguous bf16 x [B, H, W, Cin] and w_packed [Cout, 9 * Cin]")
@@ -541,6 +561,10 @@ def conv3x3(x: Tensor, w_packed: Tensor, bias: Optional[Tensor] = None, *, epilo
     Cout = w_packed.shape[0]
     if w_packed.shape[1] != 9 * Cin or Cout % 8 != 0:
         raise B200Error("conv3x3: weight shape does not match (need [Cout, 9 * Cin], Cout % 8 == 0)")
+    if epilogue in (EPI_BIAS_ADD_PER_IMAGE_BF16, EPI_BIAS_RESID_CLAMP_BF16):
+        rows = B if epilogue == EPI_BIAS_ADD_PER_IMAGE_BF16 else B * H * W
+        if aux is None or aux.dtype != torch.bfloat16 or not aux.is_contiguous() or aux.numel() != rows * Cout or aux.shape[-1] != Cout:
+            raise B200Error(f"conv3x3: this epilogue needs a contiguous bf16 aux with {rows} rows of {Cout}")
     f32 = epilogue == EPI_BIAS_RESID_F32
     out = torch.empty((B, H, W, Cout), dtype=torch.float32 if f32 else torch.bfloat16, device=x.device)
     call("b200_conv3x3_nhwc_bf16", x.data_ptr(), w_packed.data_ptr(), _ptr(bias), out.data_ptr(), _ptr(aux), Cout, B, H, W, Cin, Cout, epilogue, _stream())

@@ -58,7 +58,15 @@ enum {
      * dgate = bf16(gelu_erf'(gate) * float(dg)), g = bf16(gelu_erf(gate)) -- eager's three roundings.  No bias. */
     B200_EPI_DGEGLU_BF16 = 8,
     /* out0[bf16] = bf16(float(bf16(acc + bias)) + float(aux[bf16]))   (aux may alias out0): the bf16 residual stream */
-    B200_EPI_BIAS_RESID_BF16 = 9
+    B200_EPI_BIAS_RESID_BF16 = 9,
+    /* The two 3x3-convolution epilogues of the UNet's ResBlock (b200_conv3x3_nhwc_bf16 only; b200_gemm_bf16 refuses them).
+     * Variants of 9, with eager's two bf16 roundings (cflearn/modules/core/convs/residual.py:232-249):
+     *   10: out0 = bf16(float(bf16(acc + bias)) + float(aux[row / (H * W), col])), aux = bf16 [B, ldo], one row per image:
+     *       conv1 plus the time embedding t[b, c].
+     *   11: as 9, then +-inf becomes +-bf16 max and NaN stays NaN (safe_clip_, toolkit.py:1236-1255): conv2 plus the shortcut.
+     * aux is required and 16-byte aligned. */
+    B200_EPI_BIAS_ADD_PER_IMAGE_BF16 = 10,
+    B200_EPI_BIAS_RESID_CLAMP_BF16 = 11
 };
 
 int b200_abi_version(void);
@@ -136,6 +144,14 @@ int b200_colsum_finish(const float* part, long long part_ld, int nparts, int col
 /* the same reduction with two destinations: columns [0, cols0) -> out0, [cols0, cols0 + cols1) -> out1 */
 int b200_colsum_finish2(const float* part, long long part_ld, int nparts, int cols0, float* out0, int round0, int cols1,
                         float* out1, int round1, int accumulate, cudaStream_t stream);
+/* Per-image column sums of x bf16 [B, HW, C] (dense, C % 8 == 0, x 16-byte aligned), one pass over x, no atomics:
+ *   per_image bf16 [B, C] = bf16(sum over the HW rows of image b)  (the gradient of a [B, C] table broadcast over the pixels:
+ *                           the ResBlock's time embedding, cflearn/modules/core/convs/residual.py:240-244)
+ *   total f32 [C] = float(bf16(sum over b of the unrounded per-image sums))  (the bias gradient of the conv that wrote x)
+ * workspace: b200_colsum_per_image_workspace_floats(B, HW, C) floats.  Deterministic. */
+long long b200_colsum_per_image_workspace_floats(int B, int HW, int C);
+int b200_colsum_per_image_bf16(const void* x_bf16, int B, int HW, int C, void* per_image_bf16, float* total, float* workspace,
+                               cudaStream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Fused multi-head self-attention on the PACKED qkv tensor, replaces the split/permute/contiguous copies at
@@ -277,7 +293,8 @@ int b200_fill_f32(float* dst, float value, long long n, cudaStream_t stream);
  * 3x3 convolution (stride 1, zero padding 1) on channels-last bf16 activations as an IMPLICIT GEMM on the wgmma main
  * loop: x [B, H, W, Cin], w_packed [Cout, 9 * Cin] (k = (ky * 3 + kx) * Cin + ci), bias bf16 [Cout] or NULL,
  * out0 / aux [B*H*W, ldo].  Cin % 64 == 0; W divides 128 and H is a multiple of 128 / W (or H * W divides 128).
- * epilogue: B200_EPI_BIAS_BF16 or B200_EPI_BIAS_RESID_F32.  No im2col matrix exists: each (tap, 64-channel) k-block is ONE
+ * epilogue: B200_EPI_BIAS_BF16, B200_EPI_BIAS_RESID_F32, B200_EPI_BIAS_RESID_CLAMP_BF16 (aux bf16 [B*H*W, ldo]) or
+ * B200_EPI_BIAS_ADD_PER_IMAGE_BF16 (aux bf16 [B, ldo]).  No im2col matrix exists: each (tap, 64-channel) k-block is ONE
  * TMA box of the activation shifted by the tap, its halo zero-filled by the TMA unit.
  * Replaces F.conv2d at cflearn/modules/core/convs/basic.py:155-174 for the UNet's 3x3 convolutions
  * (convs/residual.py:179-186,199-205; multimodal/diffusion/unet.py:213-217,269-272); the input gradient is the same
