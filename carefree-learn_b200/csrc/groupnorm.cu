@@ -33,13 +33,26 @@ __device__ __forceinline__ float silu_grad_f(float z) {
     return sg * (1.0f + z * (1.0f - sg));
 }
 
-// ---- pass 1 (forward): per-(image, slab, group) sum and sum of squares ------------------------------------------------
-// grid (nslab, B); part[((b * nslab + slab) * 32 + g) * 2 + {0,1}].  Thread -> (16-byte vector v of a pixel row, pixel lane pl):
-// consecutive threads read consecutive vectors; the per-lane, per-channel partials meet in dynamic shared memory
-// s[pl][2][C] and are added in a FIXED order.
+// ---- pass 1 (forward): per-(image, slab, group) count, mean and M2 (sum of squared deviations from that mean) -------------
+// The variance is never formed as E[x^2] - E[x]^2: in fp32 that loses (mean / std)^2 * eps_fp32 of it, i.e. every bit once a
+// group's mean is a few thousand of its standard deviations.  Each pixel lane sums (x - K) and (x - K)^2 about its own first
+// value K instead, which keeps the sums at the scale of the spread (K is one of the values, so it contributes to M2 whatever
+// it is); the lane partials then meet as (count, mean, M2) through Chan's pairwise update, in a FIXED order (no atomics).
+// grid (nslab, B); part[((b * nslab + slab) * 32 + g) * 3 + {n, mean, M2}].  Thread -> (16-byte vector v of a pixel row,
+// pixel lane pl): consecutive threads read consecutive vectors; the per-lane, per-channel mean and M2 meet in dynamic shared
+// memory s[pl][2][C].
 __device__ __forceinline__ int gn_lanes(int C) {  // pixel lanes a 256-thread block runs side by side
     const int cv = C / 8;
     return cv >= GN_THREADS ? 1 : GN_THREADS / cv;
+}
+// Fold the partial (nb, mb, m2b) into (n, m, m2) (Chan, Golub & LeVeque): exact algebra, no cancellation between large terms.
+__device__ __forceinline__ void gn_chan_merge(float& n, float& m, float& m2, float nb, float mb, float m2b) {
+    if (nb == 0.f) return;
+    if (n == 0.f) { n = nb; m = mb; m2 = m2b; return; }
+    const float nn = n + nb, d = mb - m, r = nb * fast_rcp(nn);
+    m = fmaf(d, r, m);
+    m2 += fmaf(d * d * n, r, m2b);
+    n = nn;
 }
 __global__ void __launch_bounds__(GN_THREADS) gn_stats_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ part, int HW, int C,
                                                               int pix_per_slab) {
@@ -48,52 +61,68 @@ __global__ void __launch_bounds__(GN_THREADS) gn_stats_kernel(const __nv_bfloat1
     const int cv = C / 8;
     const int lanes = gn_lanes(C);
     const int p0 = slab * pix_per_slab;
-    const int p1 = min(HW, p0 + pix_per_slab);
+    const int p1 = min(HW, p0 + pix_per_slab);  // p1 <= p0 for an empty trailing slab: every lane count is then 0
     const long long base = static_cast<long long>(b) * HW * C;
     for (int v0 = 0; v0 < cv; v0 += GN_THREADS) {  // (one pass unless a pixel row has more than 256 vectors: C > 2048)
         const int cvb = min(GN_THREADS, cv - v0);
         const int v = v0 + static_cast<int>(threadIdx.x) % cvb, pl = static_cast<int>(threadIdx.x) / cvb;
         if (pl < lanes) {
-            float a[8] = {0, 0, 0, 0, 0, 0, 0, 0}, q[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-            for (int pix = p0 + pl; pix < p1; pix += lanes) {
+            float K[8] = {0, 0, 0, 0, 0, 0, 0, 0}, a[8] = {0, 0, 0, 0, 0, 0, 0, 0}, q[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+            const int first = p0 + pl;
+            if (first < p1) {  // the lane's first pixel is its shift K (and contributes x - K = 0 to the sums)
+                const uint4 t = *reinterpret_cast<const uint4*>(x + base + static_cast<long long>(first) * C + v * 8);
+                K[0] = bf16lo(t.x); K[1] = bf16hi(t.x); K[2] = bf16lo(t.y); K[3] = bf16hi(t.y);
+                K[4] = bf16lo(t.z); K[5] = bf16hi(t.z); K[6] = bf16lo(t.w); K[7] = bf16hi(t.w);
+            }
+            for (int pix = first + lanes; pix < p1; pix += lanes) {
                 const uint4 t = *reinterpret_cast<const uint4*>(x + base + static_cast<long long>(pix) * C + v * 8);
                 const float f[8] = {bf16lo(t.x), bf16hi(t.x), bf16lo(t.y), bf16hi(t.y), bf16lo(t.z), bf16hi(t.z), bf16lo(t.w), bf16hi(t.w)};
 #pragma unroll
-                for (int k = 0; k < 8; ++k) { a[k] += f[k]; q[k] = fmaf(f[k], f[k], q[k]); }
+                for (int k = 0; k < 8; ++k) {
+                    const float d = f[k] - K[k];
+                    a[k] += d;
+                    q[k] = fmaf(d, d, q[k]);
+                }
             }
+            const float rn = first < p1 ? 1.0f / static_cast<float>((p1 - first + lanes - 1) / lanes) : 0.f;
             float* dst = gn_smem + static_cast<long long>(pl) * 2 * C + v * 8;
 #pragma unroll
-            for (int k = 0; k < 8; ++k) { dst[k] = a[k]; dst[C + k] = q[k]; }
+            for (int k = 0; k < 8; ++k) {
+                dst[k] = fmaf(a[k], rn, K[k]);                     // lane mean
+                dst[C + k] = fmaxf(fmaf(-a[k] * a[k], rn, q[k]), 0.f);  // lane M2 = sum (x - K)^2 - (sum (x - K))^2 / n
+            }
         }
     }
     __syncthreads();
     const int cpg = C / GN_GROUPS;
     if (threadIdx.x < GN_GROUPS) {
-        float a = 0.f, q = 0.f;
-        for (int pl = 0; pl < lanes; ++pl)
-            for (int c = threadIdx.x * cpg; c < (threadIdx.x + 1) * cpg; ++c) { a += gn_smem[pl * 2 * C + c]; q += gn_smem[pl * 2 * C + C + c]; }
-        float* o = part + ((static_cast<long long>(b) * nslab + slab) * GN_GROUPS + threadIdx.x) * 2;
-        o[0] = a;
-        o[1] = q;
+        float n = 0.f, m = 0.f, m2 = 0.f;
+        for (int pl = 0; pl < lanes; ++pl) {
+            const int first = p0 + pl;
+            const float nl = first < p1 ? static_cast<float>((p1 - first + lanes - 1) / lanes) : 0.f;
+            for (int c = threadIdx.x * cpg; c < (threadIdx.x + 1) * cpg; ++c)
+                gn_chan_merge(n, m, m2, nl, gn_smem[pl * 2 * C + c], gn_smem[pl * 2 * C + C + c]);
+        }
+        float* o = part + ((static_cast<long long>(b) * nslab + slab) * GN_GROUPS + threadIdx.x) * 3;
+        o[0] = n;
+        o[1] = m;
+        o[2] = m2;
     }
 }
 
-// ---- pass 1b: partials -> mean / rstd per (image, group) -----------------------------------------------------------
+// ---- pass 1b: slab partials -> mean / rstd per (image, group), merged in slab order -----------------------------------
 __global__ void gn_finish_stats_kernel(const float* __restrict__ part, int nslab, float inv_n, float eps, float* __restrict__ mean,
                                        float* __restrict__ rstd, int total) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;  // (b, g)
     if (i >= total) return;
     const int b = i / GN_GROUPS, g = i % GN_GROUPS;
-    float a = 0.f, q = 0.f;
+    float n = 0.f, m = 0.f, m2 = 0.f;
     for (int s = 0; s < nslab; ++s) {
-        const float* o = part + ((static_cast<long long>(b) * nslab + s) * GN_GROUPS + g) * 2;
-        a += o[0];
-        q += o[1];
+        const float* o = part + ((static_cast<long long>(b) * nslab + s) * GN_GROUPS + g) * 3;
+        gn_chan_merge(n, m, m2, o[0], o[1], o[2]);
     }
-    const float m = a * inv_n;
-    const float var = fmaxf(q * inv_n - m * m, 0.f);
     mean[i] = m;
-    rstd[i] = rsqrtf(var + eps);
+    rstd[i] = rsqrtf(m2 * inv_n + eps);
 }
 
 // ---- pass 2 (forward): y = bf16(act(x_hat * gamma + beta)) --------------------------------------------------------
@@ -277,7 +306,7 @@ using namespace b200;
 
 extern "C" long long b200_groupnorm_workspace_floats(int B, int HW, int C) {
     const int nslab = gn_slabs(B, HW);
-    // forward: B*nslab*32*2; backward: that + B*nslab*C*2 + 2*B*32
+    // backward: B*nslab*32*2 + B*nslab*C*2 + 2*B*32; the forward's B*nslab*32*3 fits in that because C >= 32
     return static_cast<long long>(B) * nslab * GN_GROUPS * 2 + static_cast<long long>(B) * nslab * C * 2 + 2ll * B * GN_GROUPS;
 }
 
