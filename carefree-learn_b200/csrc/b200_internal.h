@@ -26,7 +26,7 @@ void count_launch(int n = 1);
 int check_launch(const char* what);  // cudaGetLastError -> set_error
 
 int num_sms();
-int persistent_ctas();  // grid of the persistent kernels: num_sms() unless b200_set_persistent_ctas() lowered it (gemm_sm100.cu)
+int persistent_ctas();  // grid of the persistent kernels: num_sms() unless b200_set_persistent_ctas() lowered it (gemm_sm90.cu)
 int current_device_slot();  // cudaGetDevice() clamped to [0, 64): index of per-device caches
 int make_tmap(CUtensorMap* out, const void* base, int elem_bytes, int rank, const uint64_t* dims,
               const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes);

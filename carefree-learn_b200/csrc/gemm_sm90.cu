@@ -36,6 +36,9 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <array>
+#include <utility>
+
 #include "b200_internal.h"
 #include "ptx.cuh"
 
@@ -50,10 +53,52 @@ constexpr int MN_BOX_BYTES = 64 * BK * 2;   // one MN-major TMA box: 64 (MN) x 6
 constexpr int STAGING_ROW_BYTES = BN * 2;   // one bf16 row of the staging tile
 constexpr int STAGING_BYTES = BM * STAGING_ROW_BYTES;  // 64 KB
 
+// What each public epilogue of include/b200_cflearn.h is, in one place: the kernel, the argument check and the launcher table
+// read these fields instead of listing epilogues.  The arithmetic of an epilogue is its branch of epi_chunk / epi_geglu.
+enum EpiBias : int { BIAS_OPTIONAL, BIAS_PAIR, BIAS_IGNORED, BIAS_REFUSED };
+enum EpiAux : int { AUX_NONE, AUX_ROWS_BF16, AUX_ROWS_F32, AUX_IMAGE_BF16, AUX_HG_BF16 };
+enum EpiCols : int { COLS_N, COLS_F, COLS_F_PAIRED };
+enum : int { ENTRY_GEMM = 1, ENTRY_CONV3X3 = 2 };
+enum : int { MAJORS_00 = 1, MAJORS_01 = 2, MAJORS_11 = 8, MAJORS_ALL = 15 };
+
+struct EpiTraits {
+    int kernel;    // EPI of the kernel that runs it
+    bool quick;    // QuickGELU x * sigmoid(1.702 x) instead of the exact erf GELU
+    bool partial;  // split-K fp32 partials: no staging tile, the epilogue in the MMA warpgroups (288 threads, 4 stages)
+    bool out_f32;  // out0 is fp32, else bf16
+    int bias;      // OPTIONAL bf16 [N] or NULL; PAIR required [2F], 4-byte aligned, read as (h, gate) pairs; IGNORED; REFUSED: must be NULL
+    int aux;       // ROWS [M, ldo]; IMAGE bf16 [B, ldo], one row per image of the convolution; HG hg [M, ldo], h at c, the gate at F + c
+    bool out1;     // required: bf16 at ldo (GELU) or dense [M, F] (GEGLU)
+    int cols;      // N: the GEMM is N wide; F: N = 2F and the GEMM is F wide; F_PAIRED: N = 2F and a 256-column tile is 128 h
+                   // columns and their 128 gate columns (B behind a 3-D map)
+    int majors;    // (TA, TB) pairs compiled: bit 2 TA + TB
+    int entries;   // the entry points that accept it
+};
+
+// Indexed by the public enum value.  Operand majors: (0,0) forward and conv, (0,1) dgrad, (1,1) wgrad, conv wgrad and CLIP's
+// db; the plain bias epilogue takes all four (ops.gemm's general form).
+constexpr EpiTraits kEpi[] = {
+    // kernel                     quick  partial f32    bias           aux             out1   cols           majors      entries
+    {EPI_BIAS_BF16,               false, false,  false, BIAS_OPTIONAL, AUX_NONE,       false, COLS_N,        MAJORS_ALL, ENTRY_GEMM | ENTRY_CONV3X3},
+    {EPI_BIAS_GELU_BF16,          false, false,  false, BIAS_OPTIONAL, AUX_NONE,       true,  COLS_N,        MAJORS_00,  ENTRY_GEMM},
+    {EPI_BIAS_RESID_F32,          false, false,  true,  BIAS_OPTIONAL, AUX_ROWS_F32,   false, COLS_N,        MAJORS_00,  ENTRY_GEMM | ENTRY_CONV3X3},
+    {EPI_DGELU_BF16,              false, false,  false, BIAS_IGNORED,  AUX_ROWS_BF16,  false, COLS_N,        MAJORS_01,  ENTRY_GEMM},
+    {EPI_PARTIAL_F32,             false, true,   true,  BIAS_IGNORED,  AUX_NONE,       false, COLS_N,        MAJORS_11,  ENTRY_GEMM},
+    {EPI_BIAS_GELU_BF16,          true,  false,  false, BIAS_OPTIONAL, AUX_NONE,       true,  COLS_N,        MAJORS_00,  ENTRY_GEMM},
+    {EPI_DGELU_BF16,              true,  false,  false, BIAS_IGNORED,  AUX_ROWS_BF16,  false, COLS_N,        MAJORS_01,  ENTRY_GEMM},
+    {EPI_BIAS_GEGLU_BF16,         false, false,  false, BIAS_PAIR,     AUX_NONE,       true,  COLS_F_PAIRED, MAJORS_00,  ENTRY_GEMM},
+    {EPI_DGEGLU_BF16,             false, false,  false, BIAS_REFUSED,  AUX_HG_BF16,    false, COLS_F,        MAJORS_01,  ENTRY_GEMM},
+    {EPI_BIAS_RESID_BF16,         false, false,  false, BIAS_OPTIONAL, AUX_ROWS_BF16,  false, COLS_N,        MAJORS_00,  ENTRY_GEMM},
+    {EPI_BIAS_ADD_PER_IMAGE_BF16, false, false,  false, BIAS_OPTIONAL, AUX_IMAGE_BF16, false, COLS_N,        MAJORS_00,  ENTRY_CONV3X3},
+    {EPI_BIAS_RESID_CLAMP_BF16,   false, false,  false, BIAS_OPTIONAL, AUX_ROWS_BF16,  false, COLS_N,        MAJORS_00,  ENTRY_CONV3X3},
+};
+constexpr int kNumEpi = sizeof(kEpi) / sizeof(kEpi[0]);
+static_assert(kNumEpi == B200_EPI_BIAS_RESID_CLAMP_BF16 + 1, "one kEpi row per public epilogue");
+
 // Kernel layout by epilogue: OVERLAP = separate epilogue warpgroup (everything but the split-K partials).
 template <int EPI>
 struct GemmCfg {
-    static constexpr bool OVERLAP = EPI != EPI_PARTIAL_F32;
+    static constexpr bool OVERLAP = !kEpi[EPI].partial;
     static constexpr int STAGES = OVERLAP ? 3 : 4;
     static constexpr int THREADS = OVERLAP ? 384 : 288;
     static constexpr int EPI_WARPS = 3;  // warps 9-11
@@ -76,7 +121,6 @@ struct GemmParams {
     // an M tile is 128 consecutive pixels (whole image rows), k-block kb = (tap, 64-channel block), and the A tile of a tap is
     // the SAME box shifted by (kx - 1, ky - 1) -- TMA zero-fills what falls outside the image: the padding costs nothing
     int conv, conv_h, conv_w, conv_cin;
-    int act;  // GELU / dGELU epilogues: 0 = exact erf GELU (nn.GELU()), 1 = QuickGELU x * sigmoid(1.702 x) (activations.py:151-153)
 };
 
 // Work unit u -> (m tile, n tile, split, k-block range).  Consecutive units share the m tile (A stays in L2).
@@ -228,7 +272,7 @@ __device__ __forceinline__ void epi_chunk(const GemmParams& p, int row, int col,
             }
         }
     }
-    if constexpr (EPI != EPI_BIAS_RESID_F32) {
+    if constexpr (!kEpi[EPI].out_f32) {
         __nv_bfloat16* d0 = reinterpret_cast<__nv_bfloat16*>(p.out0) + off;
         if (n_ok == 8) {
             *reinterpret_cast<uint4*>(d0) = make_uint4(o[0], o[1], o[2], o[3]);
@@ -310,20 +354,19 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 int m_t, n_t, sp, kb0, kb1;
                 decode_unit(p, u, m_t, n_t, sp, kb0, kb1);
                 const int col = n_t * BN + lane * 8;
-                const int n_ok = min(8, max(0, (EPI == EPI_DGEGLU_BF16 ? p.N >> 1 : p.N) - col));  // dGEGLU's GEMM is F wide
+                const int n_ok = min(8, max(0, (kEpi[EPI].cols == COLS_F ? p.N >> 1 : p.N) - col));
                 const int rows = min(BM, p.M - m_t * BM);
-                if constexpr (EPI == EPI_DGELU_BF16 || EPI == EPI_BIAS_RESID_F32 || EPI == EPI_BIAS_RESID_BF16 ||
-                              EPI == EPI_BIAS_RESID_CLAMP_BF16) {
+                if constexpr (kEpi[EPI].aux == AUX_ROWS_BF16 || kEpi[EPI].aux == AUX_ROWS_F32) {
                     // pull the tile's aux rows into L2 while its MMAs still run: three warps cannot hide HBM latency alone.
                     // Rows are 16-byte aligned and padded to ldo >= the 16-byte-rounded width, so no byte past a row is named.
-                    constexpr int eb = EPI == EPI_BIAS_RESID_F32 ? 4 : 2;
+                    constexpr int eb = kEpi[EPI].aux == AUX_ROWS_F32 ? 4 : 2;
                     const int n0 = n_t * BN;
                     const uint32_t bytes = static_cast<uint32_t>((min(BN, p.N - n0) * eb + 15) & ~15);
                     const uint8_t* aux = reinterpret_cast<const uint8_t*>(p.aux);
                     for (int r = threadIdx.x - 9 * 32; r < rows; r += 32 * Cfg::EPI_WARPS)
                         bulk_prefetch_l2(aux + (static_cast<long long>(m_t * BM + r) * p.ldo + n0) * eb, bytes);
                 }
-                if constexpr (EPI == EPI_BIAS_ADD_PER_IMAGE_BF16) {  // the table has one row per image: prefetch the tile's images
+                if constexpr (kEpi[EPI].aux == AUX_IMAGE_BF16) {  // the table has one row per image: prefetch the tile's images
                     const int hw = p.conv_h * p.conv_w, n0 = n_t * BN;
                     const int img0 = (m_t * BM) / hw, img1 = (m_t * BM + rows - 1) / hw;
                     const uint32_t bytes = static_cast<uint32_t>((min(BN, p.N - n0) * 2 + 15) & ~15);
@@ -331,7 +374,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                     for (int b = img0 + threadIdx.x - 9 * 32; b <= img1; b += 32 * Cfg::EPI_WARPS)
                         bulk_prefetch_l2(aux + (static_cast<long long>(b) * p.ldo + n0) * 2, bytes);
                 }
-                if constexpr (EPI == EPI_DGEGLU_BF16) {  // the same for both halves of hg: h at n0, the gate at F + n0
+                if constexpr (kEpi[EPI].aux == AUX_HG_BF16) {  // the same for both halves of hg: h at n0, the gate at F + n0
                     const int F = p.N >> 1, n0 = n_t * BN;
                     const uint32_t bytes = static_cast<uint32_t>(min(BN, F - n0) * 2);
                     const __nv_bfloat16* aux = reinterpret_cast<const __nv_bfloat16*>(p.aux);
@@ -342,7 +385,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                     }
                 }
                 mbar_wait(staging_full, sphase);
-                if constexpr (EPI == EPI_BIAS_GEGLU_BF16) {
+                if constexpr (kEpi[EPI].cols == COLS_F_PAIRED) {
                     // the tile's 256 columns are 128 h columns and the matching 128 gate columns: a half-warp takes one row,
                     // lane l & 15 the h chunk l & 15 and the gate chunk 16 + (l & 15) -- one 8-column piece of out0's two
                     // halves and of out1 each
@@ -414,7 +457,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                             // (boxes past N = 9 Cin: tap >= 9 lands outside the image -> zero fill, bytes still credited)
                             tma_load_4d(b_dst + i * MN_BOX_BYTES, &tmB, &full_bar[stage], c0, kx - 1, tap < 9 ? y0 + ky - 1 : -65536, bimg);
                         }
-                    } else if constexpr (EPI == EPI_BIAS_GEGLU_BF16) {
+                    } else if constexpr (kEpi[EPI].cols == COLS_F_PAIRED) {
                         // W1 behind a 3-D map {K, F, 2}: one box = 128 h rows then the matching 128 gate rows (rows past F
                         // zero-filled), so the B tile holds [h | gate] of the same 128 columns
                         tma_load_3d(b_dst, &tmB, &full_bar[stage], kb * BK, n_t * (BN / 2), 0);
@@ -470,7 +513,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             for (int j = 0; j < 32; ++j) {
                 const int col = colq + j * 8;
                 float b0 = 0.f, b1 = 0.f;
-                if constexpr (EPI == EPI_BIAS_GEGLU_BF16) {
+                if constexpr (kEpi[EPI].bias == BIAS_PAIR) {
                     // tile column c < 128: h column n_t * 128 + c; c >= 128: gate column F + n_t * 128 + c - 128
                     // (the bias is required; f is even and F % 8 == 0, so f < F covers f + 1 too: one 4-byte load of the pair)
                     const int f = colq - n_t * (BN / 2) + (j & 15) * 8;  // colq = n_t * BN + (lane & 3) * 2
@@ -479,7 +522,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                         b0 = bf16lo(bp);
                         b1 = bf16hi(bp);
                     }
-                } else if constexpr (EPI != EPI_DGELU_BF16 && EPI != EPI_DGEGLU_BF16) {
+                } else if constexpr (kEpi[EPI].bias == BIAS_OPTIONAL) {
                     if (p.bias != nullptr) {
                         if (col < p.N) b0 = __bfloat162float(p.bias[col]);
                         if (col + 1 < p.N) b1 = __bfloat162float(p.bias[col + 1]);
@@ -650,38 +693,22 @@ static int launch_gemm_impl(const CUtensorMap& tmA, const CUtensorMap& tmB, cons
     return 0;
 }
 
-// Operand majors each epilogue is compiled for: (0,0) forward and conv, (0,1) dgrad, (1,1) wgrad, conv wgrad and CLIP's db.
-// The plain bias epilogue takes all four (ops.gemm's general form).  GEGLU, the bf16 residual and its two convolution variants
-// are forward epilogues (0,0), dGEGLU a dgrad one (0,1).
-template <int EPI, int TA, int TB>
-constexpr bool kHasMajors = EPI == EPI_BIAS_BF16 ||
-                            (TA == 0 && TB == 0 && (EPI == EPI_BIAS_GELU_BF16 || EPI == EPI_BIAS_RESID_F32 ||
-                                                    EPI == EPI_BIAS_GEGLU_BF16 || EPI == EPI_BIAS_RESID_BF16 ||
-                                                    EPI == EPI_BIAS_ADD_PER_IMAGE_BF16 || EPI == EPI_BIAS_RESID_CLAMP_BF16)) ||
-                            (TA == 0 && TB == 1 && (EPI == EPI_DGELU_BF16 || EPI == EPI_DGEGLU_BF16)) ||
-                            (TA == 1 && TB == 1 && EPI == EPI_PARTIAL_F32);
+typedef int (*GemmLauncher)(const CUtensorMap&, const CUtensorMap&, const GemmParams&, int, cudaStream_t);
 
-template <int EPI, bool QUICK, int TA, int TB>
-static int launch_majors(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int grid, cudaStream_t stream) {
-    if constexpr (kHasMajors<EPI, TA, TB>) return launch_gemm_impl<EPI, QUICK, TA, TB>(tmA, tmB, p, grid, stream);
-    else return set_error(B200_ERR_ARG, "gemm: operand majors not supported by this epilogue");
+// public epilogue P with majors (TA, TB): its kernel instance, or nullptr where kEpi[P] does not compile those majors
+template <int P, int TA, int TB>
+constexpr GemmLauncher launcher() {
+    if constexpr (((kEpi[P].majors >> (2 * TA + TB)) & 1) != 0) return &launch_gemm_impl<kEpi[P].kernel, kEpi[P].quick, TA, TB>;
+    else return nullptr;
 }
 
-template <int EPI, bool QUICK>
-static int launch_quick(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int a_mn, int b_mn, int grid,
-                        cudaStream_t stream) {
-    if (!a_mn) return b_mn ? launch_majors<EPI, QUICK, 0, 1>(tmA, tmB, p, grid, stream) : launch_majors<EPI, QUICK, 0, 0>(tmA, tmB, p, grid, stream);
-    return b_mn ? launch_majors<EPI, QUICK, 1, 1>(tmA, tmB, p, grid, stream) : launch_majors<EPI, QUICK, 1, 0>(tmA, tmB, p, grid, stream);
+template <int... P>
+constexpr std::array<std::array<GemmLauncher, 4>, sizeof...(P)> launcher_table(std::integer_sequence<int, P...>) {
+    return {{{launcher<P, 0, 0>(), launcher<P, 0, 1>(), launcher<P, 1, 0>(), launcher<P, 1, 1>()}...}};
 }
 
-template <int EPI>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int a_mn, int b_mn, int grid,
-                       cudaStream_t stream) {
-    if constexpr (EPI == EPI_BIAS_GELU_BF16 || EPI == EPI_DGELU_BF16) {
-        if (p.act != 0) return launch_quick<EPI, true>(tmA, tmB, p, a_mn, b_mn, grid, stream);
-    }
-    return launch_quick<EPI, false>(tmA, tmB, p, a_mn, b_mn, grid, stream);
-}
+// indexed by (public epilogue, 2 TA + TB)
+static constexpr auto kLaunch = launcher_table(std::make_integer_sequence<int, kNumEpi>{});
 
 }  // namespace b200
 
@@ -716,47 +743,46 @@ extern "C" int b200_gemm_pick_splits(int M, int N, int K) {
 
 struct ConvGeom { int B, H, W, Cin, mode; };  // mode 1: forward / input gradient (A behind the 4-D map); 2: weight gradient (B)
 
+// Every argument check of the GEMM entries, before any tensor map is encoded: a call is refused the same way with or without
+// a device.  conv_fwd: the call comes from b200_conv3x3_nhwc_bf16.
+static int check_gemm_args(const void* A, int a_mn, const void* B, int b_mn, int M, int N, int K, int epilogue, const void* bias,
+                           const void* out0, const void* out1, const void* aux, long long ldo, int splits, bool conv_fwd) {
+    if (epilogue < 0 || epilogue >= kNumEpi) return set_error(B200_ERR_ARG, "gemm: unknown epilogue");
+    const EpiTraits& e = kEpi[epilogue];
+    if (conv_fwd && !(e.entries & ENTRY_CONV3X3)) return set_error(B200_ERR_ARG, "conv3x3: epilogue not offered for convolutions");
+    if (!conv_fwd && !(e.entries & ENTRY_GEMM)) return set_error(B200_ERR_ARG, "gemm: epilogue offered by conv3x3 only");
+    if (M <= 0 || N <= 0 || K <= 0) return set_error(B200_ERR_ARG, "gemm: non-positive dimension");
+    // N need not be a multiple of 8: the bias is read in 16-byte groups (readable up to roundup(N, 8) elements) and the
+    // epilogue clips columns >= N
+    if (A == nullptr || B == nullptr || out0 == nullptr) return set_error(B200_ERR_ARG, "gemm: null pointer");
+    if (!e.partial && splits != 1) return set_error(B200_ERR_ARG, "gemm: split-K needs EPI_PARTIAL_F32");
+    if (kLaunch[epilogue][2 * a_mn + b_mn] == nullptr) return set_error(B200_ERR_ARG, "gemm: operand majors not supported by this epilogue");
+    if (e.cols != COLS_N && N % 16 != 0) return set_error(B200_ERR_ARG, "gemm: GEGLU epilogues need N = 2F with F % 8 == 0");
+    if (ldo < N) return set_error(B200_ERR_ARG, "gemm: ldo < N");
+    if (e.out1 && out1 == nullptr) return set_error(B200_ERR_ARG, "gemm: epilogue needs out1");
+    if (e.aux != AUX_NONE && aux == nullptr) return set_error(B200_ERR_ARG, "gemm: epilogue needs aux");
+    if (e.bias == BIAS_REFUSED && bias != nullptr) return set_error(B200_ERR_ARG, "gemm: epilogue takes no bias");
+    if (e.bias == BIAS_PAIR && (bias == nullptr || (reinterpret_cast<uintptr_t>(bias) & 3u) != 0))
+        return set_error(B200_ERR_ARG, "gemm: epilogue needs a 4-byte aligned bias [2F]");
+    // the epilogue writes and reads with plain 16-byte global accesses: rows must start 16-byte aligned
+    if ((static_cast<unsigned long long>(ldo) * (e.out_f32 ? 4 : 2)) % 16 != 0) return set_error(B200_ERR_ALIGN, "gemm: ldo rows must be 16-byte aligned");
+    if (((reinterpret_cast<uintptr_t>(out0) | reinterpret_cast<uintptr_t>(out1) | reinterpret_cast<uintptr_t>(aux)) & 15u) != 0)
+        return set_error(B200_ERR_ALIGN, "gemm: out0 / out1 / aux not 16-byte aligned");
+    return 0;
+}
+
 static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const void* B, long long ldb,
                          int b_mn_major, int M, int N, int K, int epilogue, const void* bias, void* out0,
                          void* out1, const void* aux, long long ldo, int splits, int max_ctas,
                          cudaStream_t stream, const ConvGeom* cg) {
-    int act = 0;  // the QuickGELU epilogues are the GELU / dGELU kernels with another activation
-    if (epilogue == B200_EPI_BIAS_QGELU_BF16) { epilogue = EPI_BIAS_GELU_BF16; act = 1; }
-    if (epilogue == B200_EPI_DQGELU_BF16) { epilogue = EPI_DGELU_BF16; act = 1; }
-    if (M <= 0 || N <= 0 || K <= 0) return set_error(B200_ERR_ARG, "gemm: non-positive dimension");
-    // N need not be a multiple of 8: the bias is read in 16-byte groups (readable up to roundup(N, 8) elements) and the
-    // TMA store clips columns >= N; the leading dimension must keep rows 16-byte aligned (checked in make_tmap).
-    if (A == nullptr || B == nullptr || out0 == nullptr) return set_error(B200_ERR_ARG, "gemm: null pointer");
+    const int a_mn = a_mn_major ? 1 : 0, b_mn = b_mn_major ? 1 : 0;
     if (splits < 1) splits = 1;
-    if (epilogue != EPI_PARTIAL_F32 && splits != 1) return set_error(B200_ERR_ARG, "gemm: split-K needs EPI_PARTIAL_F32");
+    if (const int rc = check_gemm_args(A, a_mn, B, b_mn, M, N, K, epilogue, bias, out0, out1, aux, ldo, splits, cg != nullptr && cg->mode == 1))
+        return rc;
+    const EpiTraits& e = kEpi[epilogue];
     const int num_kb = (K + BK - 1) / BK;
     if (splits > num_kb) splits = num_kb;
-    const bool geglu = epilogue == EPI_BIAS_GEGLU_BF16 || epilogue == EPI_DGEGLU_BF16;
-    if (geglu || epilogue == EPI_BIAS_RESID_BF16) {
-        // checked before any tensor map is encoded: these fail the same way with or without a device
-        if (cg != nullptr) return set_error(B200_ERR_ARG, "gemm: the GEGLU / bf16-residual epilogues are not offered for convolutions");
-        if (epilogue == EPI_DGEGLU_BF16 ? (a_mn_major || !b_mn_major) : (a_mn_major || b_mn_major))
-            return set_error(B200_ERR_ARG, "gemm: operand majors not supported by this epilogue");
-        if (geglu && N % 16 != 0) return set_error(B200_ERR_ARG, "gemm: GEGLU epilogues need N = 2F with F % 8 == 0");
-        if (ldo < N) return set_error(B200_ERR_ARG, "gemm: ldo < N");
-        if (epilogue == EPI_BIAS_GEGLU_BF16 && out1 == nullptr) return set_error(B200_ERR_ARG, "gemm: GEGLU epilogue needs out1 (a, [M, F])");
-        if (epilogue != EPI_BIAS_GEGLU_BF16 && aux == nullptr) return set_error(B200_ERR_ARG, "gemm: epilogue needs aux");
-        if (epilogue == EPI_DGEGLU_BF16 && bias != nullptr) return set_error(B200_ERR_ARG, "gemm: dGEGLU takes no bias");
-        if (epilogue == EPI_BIAS_GEGLU_BF16 && (bias == nullptr || (reinterpret_cast<uintptr_t>(bias) & 3u) != 0))
-            return set_error(B200_ERR_ARG, "gemm: GEGLU epilogue needs a 4-byte aligned bias [2F]");
-        if ((static_cast<unsigned long long>(ldo) * 2) % 16 != 0) return set_error(B200_ERR_ALIGN, "gemm: ldo rows must be 16-byte aligned");
-        if (((reinterpret_cast<uintptr_t>(out0) | reinterpret_cast<uintptr_t>(out1) | reinterpret_cast<uintptr_t>(aux)) & 15u) != 0)
-            return set_error(B200_ERR_ALIGN, "gemm: out0 / out1 / aux not 16-byte aligned");
-    }
-    if (epilogue == EPI_BIAS_ADD_PER_IMAGE_BF16 || epilogue == EPI_BIAS_RESID_CLAMP_BF16) {
-        // the ResBlock's convolution epilogues, checked before any tensor map is encoded
-        if (cg == nullptr || cg->mode != 1) return set_error(B200_ERR_ARG, "gemm: the per-image / clamped residual epilogues are for conv3x3 only");
-        if (aux == nullptr) return set_error(B200_ERR_ARG, "gemm: epilogue needs aux");
-        if (ldo < N) return set_error(B200_ERR_ARG, "gemm: ldo < N");
-        if ((static_cast<unsigned long long>(ldo) * 2) % 16 != 0) return set_error(B200_ERR_ALIGN, "gemm: ldo rows must be 16-byte aligned");
-        if (((reinterpret_cast<uintptr_t>(out0) | reinterpret_cast<uintptr_t>(aux)) & 15u) != 0)
-            return set_error(B200_ERR_ALIGN, "gemm: out0 / aux not 16-byte aligned");
-    }
+    const int n_cols = e.cols == COLS_N ? N : N / 2;  // the width of the GEMM itself
 
     CUtensorMap tmA, tmB;
     int rc;
@@ -774,8 +800,8 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
             uint32_t b4[4] = {BK, static_cast<uint32_t>(cg->W), static_cast<uint32_t>(hb), static_cast<uint32_t>(nb)};
             if ((rc = make_tmap(&tmA, A, 2, 4, d4, s4, b4, 128)) != 0) return rc;
         } else {
-        if (!a_mn_major) { d[0] = K; d[1] = M; bx[0] = BK; bx[1] = BM; }
-        else             { d[0] = M; d[1] = K; bx[0] = 64; bx[1] = BK; }
+        if (!a_mn) { d[0] = K; d[1] = M; bx[0] = BK; bx[1] = BM; }
+        else       { d[0] = M; d[1] = K; bx[0] = 64; bx[1] = BK; }
         s[0] = static_cast<uint64_t>(lda) * 2;
         if ((rc = make_tmap(&tmA, A, 2, 2, d, s, bx, 128)) != 0) return rc;
         }
@@ -787,44 +813,28 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
                               static_cast<uint64_t>(cg->H) * cg->W * cg->Cin * 2};
             uint32_t b4[4] = {64, static_cast<uint32_t>(cg->W), static_cast<uint32_t>(hb), 1};
             if ((rc = make_tmap(&tmB, B, 2, 4, d4, s4, b4, 128)) != 0) return rc;
-        } else if (epilogue == EPI_BIAS_GEGLU_BF16) {
+        } else if (e.cols == COLS_F_PAIRED) {
             // W1 [2F, ldb] as {K, F, 2}: one box is 128 rows of the h half and the same 128 rows of the gate half
-            const uint64_t F = static_cast<uint64_t>(N / 2);
+            const uint64_t F = static_cast<uint64_t>(n_cols);
             uint64_t d3[3] = {static_cast<uint64_t>(K), F, 2};
             uint64_t s3[2] = {static_cast<uint64_t>(ldb) * 2, F * static_cast<uint64_t>(ldb) * 2};
             uint32_t b3[3] = {BK, BN / 2, 2};
             if ((rc = make_tmap(&tmB, B, 2, 3, d3, s3, b3, 128)) != 0) return rc;
         } else {
-        const int nb = epilogue == EPI_DGEGLU_BF16 ? N / 2 : N;  // dGEGLU: the GEMM itself is F wide
-        if (!b_mn_major) { d[0] = K; d[1] = nb; bx[0] = BK; bx[1] = BN; }
-        else             { d[0] = nb; d[1] = K; bx[0] = 64; bx[1] = BK; }
+        if (!b_mn) { d[0] = K; d[1] = n_cols; bx[0] = BK; bx[1] = BN; }
+        else       { d[0] = n_cols; d[1] = K; bx[0] = 64; bx[1] = BK; }
         s[0] = static_cast<uint64_t>(ldb) * 2;
         if ((rc = make_tmap(&tmB, B, 2, 2, d, s, bx, 128)) != 0) return rc;
         }
     }
-    const bool out_f32 = (epilogue == EPI_BIAS_RESID_F32 || epilogue == EPI_PARTIAL_F32);
-    {
-        // The epilogue writes with plain 16-byte global stores: rows must start 16-byte aligned.
-        const int eb = out_f32 ? 4 : 2;
-        if ((static_cast<unsigned long long>(ldo) * eb) % 16 != 0) return set_error(B200_ERR_ALIGN, "gemm: ldo rows must be 16-byte aligned");
-        if ((reinterpret_cast<uintptr_t>(out0) & 15u) != 0) return set_error(B200_ERR_ALIGN, "gemm: out0 not 16-byte aligned");
-        if (epilogue == EPI_BIAS_GELU_BF16 && (out1 == nullptr || (reinterpret_cast<uintptr_t>(out1) & 15u) != 0))
-            return set_error(B200_ERR_ARG, "gemm: GELU epilogue needs a 16-byte aligned out1");
-        if ((epilogue == EPI_BIAS_RESID_F32 || epilogue == EPI_DGELU_BF16) &&
-            (aux == nullptr || (reinterpret_cast<uintptr_t>(aux) & 15u) != 0))
-            return set_error(B200_ERR_ARG, "gemm: epilogue needs a 16-byte aligned aux");
-    }
     GemmParams p;
-    p.act = act;
     p.conv = cg != nullptr ? cg->mode : 0;
     p.conv_h = cg != nullptr ? cg->H : 0;
     p.conv_w = cg != nullptr ? cg->W : 0;
     p.conv_cin = cg != nullptr ? cg->Cin : 0;
     p.M = M; p.N = N; p.K = K;
     p.num_m_tiles = (M + BM - 1) / BM;
-    // GEGLU's N tile holds 128 h columns and their 128 gate columns; dGEGLU's GEMM is F = N / 2 wide
-    const int tile_n = epilogue == EPI_BIAS_GEGLU_BF16 ? BN / 2 : BN;
-    const int n_cols = geglu ? N / 2 : N;
+    const int tile_n = e.cols == COLS_F_PAIRED ? BN / 2 : BN;
     p.num_n_tiles = (n_cols + tile_n - 1) / tile_n;
     p.splits = splits;
     p.num_kb = num_kb;
@@ -834,23 +844,10 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
     p.aux = aux;
     p.ldo = ldo;
     const long long units = static_cast<long long>(p.num_m_tiles) * p.num_n_tiles * splits;
-    const int a_mn = a_mn_major ? 1 : 0, b_mn = b_mn_major ? 1 : 0;
     int grid = persistent_ctas();
     if (max_ctas > 0 && max_ctas < grid) grid = max_ctas;
     if (units < grid) grid = static_cast<int>(units);
-    switch (epilogue) {
-        case EPI_BIAS_BF16: return launch_gemm<EPI_BIAS_BF16>(tmA, tmB, p, a_mn, b_mn, grid, stream);
-        case EPI_BIAS_GELU_BF16: return launch_gemm<EPI_BIAS_GELU_BF16>(tmA, tmB, p, a_mn, b_mn, grid, stream);
-        case EPI_BIAS_RESID_F32: return launch_gemm<EPI_BIAS_RESID_F32>(tmA, tmB, p, a_mn, b_mn, grid, stream);
-        case EPI_DGELU_BF16: return launch_gemm<EPI_DGELU_BF16>(tmA, tmB, p, a_mn, b_mn, grid, stream);
-        case EPI_PARTIAL_F32: return launch_gemm<EPI_PARTIAL_F32>(tmA, tmB, p, a_mn, b_mn, grid, stream);
-        case EPI_BIAS_GEGLU_BF16: return launch_gemm<EPI_BIAS_GEGLU_BF16>(tmA, tmB, p, a_mn, b_mn, grid, stream);
-        case EPI_DGEGLU_BF16: return launch_gemm<EPI_DGEGLU_BF16>(tmA, tmB, p, a_mn, b_mn, grid, stream);
-        case EPI_BIAS_RESID_BF16: return launch_gemm<EPI_BIAS_RESID_BF16>(tmA, tmB, p, a_mn, b_mn, grid, stream);
-        case EPI_BIAS_ADD_PER_IMAGE_BF16: return launch_gemm<EPI_BIAS_ADD_PER_IMAGE_BF16>(tmA, tmB, p, a_mn, b_mn, grid, stream);
-        case EPI_BIAS_RESID_CLAMP_BF16: return launch_gemm<EPI_BIAS_RESID_CLAMP_BF16>(tmA, tmB, p, a_mn, b_mn, grid, stream);
-        default: return set_error(B200_ERR_ARG, "gemm: unknown epilogue");
-    }
+    return kLaunch[epilogue][2 * a_mn + b_mn](tmA, tmB, p, grid, stream);
 }
 
 extern "C" int b200_gemm_bf16(const void* A, long long lda, int a_mn_major, const void* B, long long ldb,
@@ -875,9 +872,6 @@ extern "C" int b200_conv3x3_nhwc_bf16(const void* x, const void* w_packed, const
     if (W > BM || BM % W != 0) return set_error(B200_ERR_ARG, "conv3x3: the image width must divide 128");
     const int hb = H < BM / W ? H : BM / W;
     if (H % hb != 0 || BM % (W * hb) != 0) return set_error(B200_ERR_ARG, "conv3x3: H must be a multiple of 128 / W (or H * W must divide 128)");
-    if (epilogue != EPI_BIAS_BF16 && epilogue != EPI_BIAS_RESID_F32 && epilogue != EPI_BIAS_ADD_PER_IMAGE_BF16 &&
-        epilogue != EPI_BIAS_RESID_CLAMP_BF16)
-        return set_error(B200_ERR_ARG, "conv3x3: epilogue must be BIAS_BF16, BIAS_RESID_F32, BIAS_ADD_PER_IMAGE_BF16 or BIAS_RESID_CLAMP_BF16");
     ConvGeom cg{B, H, W, Cin, 1};
     const long long M = static_cast<long long>(B) * H * W;
     if (M > 0x7fffffffll) return set_error(B200_ERR_ARG, "conv3x3: too many pixels");

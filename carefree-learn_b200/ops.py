@@ -28,6 +28,25 @@ EPI_BIAS_RESID_BF16 = 9   # out0 = bf16(bf16(acc + bias) + aux), the bf16 residu
 EPI_BIAS_ADD_PER_IMAGE_BF16 = 10  # conv3x3 only: out0 = bf16(bf16(acc + bias) + aux[image, c]), aux bf16 [B, Cout]
 EPI_BIAS_RESID_CLAMP_BF16 = 11    # conv3x3 only: 9, then +-inf -> +-bf16 max (NaN kept)
 
+# What the torch-level checks need per epilogue (dtypes and shapes, which the C side cannot see): (out0 dtype, aux, out1).
+# aux has out0's dtype: "rows" = [M, N] with out0's leading dim (conv3x3: contiguous [B*H*W, Cout]), "image" = contiguous
+# [B, Cout], one row per image (conv3x3).  out1 is bf16: "rows" as for aux, "dense" = contiguous [M, N / 2] (GEGLU's a).
+_BF16, _F32 = torch.bfloat16, torch.float32
+EPILOGUES: Dict[int, Tuple[torch.dtype, Optional[str], Optional[str]]] = {
+    EPI_BIAS_BF16: (_BF16, None, None),
+    EPI_BIAS_GELU_BF16: (_BF16, None, "rows"),
+    EPI_BIAS_RESID_F32: (_F32, "rows", None),
+    EPI_DGELU_BF16: (_BF16, "rows", None),
+    EPI_PARTIAL_F32: (_F32, None, None),
+    EPI_BIAS_QGELU_BF16: (_BF16, None, "rows"),
+    EPI_DQGELU_BF16: (_BF16, "rows", None),
+    EPI_BIAS_GEGLU_BF16: (_BF16, None, "dense"),
+    EPI_DGEGLU_BF16: (_BF16, "rows", None),
+    EPI_BIAS_RESID_BF16: (_BF16, "rows", None),
+    EPI_BIAS_ADD_PER_IMAGE_BF16: (_BF16, "image", None),
+    EPI_BIAS_RESID_CLAMP_BF16: (_BF16, "rows", None),
+}
+
 _MAX_PARTS = 1024
 
 
@@ -96,28 +115,26 @@ def gemm(
         N, Kb = b.shape
     if K != Kb:
         raise B200Error(f"gemm reduction mismatch: {K} vs {Kb}")
+    dtype, aux_kind, out1_kind = EPILOGUES.get(epilogue, (_BF16, None, None))  # the C side refuses unknown epilogues
     # dGEGLU: the product da is F wide, its input hg and output dhg 2F wide -- the C-ABI's N is 2F for both GEGLU epilogues
     if epilogue == EPI_DGEGLU_BF16:
         N = 2 * N
-    f32_out = epilogue in (EPI_BIAS_RESID_F32, EPI_PARTIAL_F32)
     if out0 is None:
         if epilogue == EPI_PARTIAL_F32:
-            out0 = torch.empty((splits, M, N), dtype=torch.float32, device=a.device)
+            out0 = torch.empty((splits, M, N), dtype=dtype, device=a.device)
         else:  # rows stay 16-byte aligned for TMA: pad the leading dimension, hand back the [M, N] view
             npad = (N + 7) // 8 * 8
-            out0 = torch.empty((M, npad), dtype=torch.float32 if f32_out else torch.bfloat16, device=a.device)[:, :N]
-    if out0.dtype != (torch.float32 if f32_out else torch.bfloat16):
+            out0 = torch.empty((M, npad), dtype=dtype, device=a.device)[:, :N]
+    if out0.dtype != dtype:
         raise B200Error("gemm: out0 dtype does not match the epilogue")
     ldo = out0.stride(-2)
-    if epilogue in (EPI_BIAS_GEGLU_BF16, EPI_DGEGLU_BF16, EPI_BIAS_RESID_BF16):
-        if tuple(out0.shape) != (M, N) or out0.stride(1) != 1:
-            raise B200Error("gemm: out0 must be an [M, N] view with unit inner stride")
-        if epilogue == EPI_BIAS_GEGLU_BF16 and (out1 is None or out1.dtype != torch.bfloat16 or tuple(out1.shape) != (M, N // 2)
-                                                or not out1.is_contiguous()):
-            raise B200Error("gemm: the GEGLU epilogue needs out1 = contiguous bf16 [M, F]")
-        if epilogue != EPI_BIAS_GEGLU_BF16 and (aux is None or aux.dtype != torch.bfloat16 or tuple(aux.shape) != (M, N)
-                                                or aux.stride(0) != ldo or aux.stride(1) != 1):
-            raise B200Error("gemm: this epilogue needs a bf16 aux [M, N] with out0's leading dim")
+    if (aux_kind or out1_kind) and (tuple(out0.shape) != (M, N) or out0.stride(1) != 1):
+        raise B200Error("gemm: out0 must be an [M, N] view with unit inner stride")
+    for t, kind, dt, name in ((aux, aux_kind, dtype, "aux"), (out1, out1_kind, _BF16, "out1")):
+        if kind == "rows" and (t is None or t.dtype != dt or tuple(t.shape) != (M, N) or t.stride() != (ldo, 1)):
+            raise B200Error(f"gemm: this epilogue needs a {dt} {name} [M, N] with out0's leading dim")
+    if out1_kind == "dense" and (out1 is None or out1.dtype != _BF16 or tuple(out1.shape) != (M, N // 2) or not out1.is_contiguous()):
+        raise B200Error("gemm: the GEGLU epilogue needs out1 = contiguous bf16 [M, F]")
     call(
         "b200_gemm_bf16",
         a.data_ptr(), a.stride(0), int(a_mn_major),
@@ -561,11 +578,11 @@ def conv3x3(x: Tensor, w_packed: Tensor, bias: Optional[Tensor] = None, *, epilo
     Cout = w_packed.shape[0]
     if w_packed.shape[1] != 9 * Cin or Cout % 8 != 0:
         raise B200Error("conv3x3: weight shape does not match (need [Cout, 9 * Cin], Cout % 8 == 0)")
-    if epilogue in (EPI_BIAS_ADD_PER_IMAGE_BF16, EPI_BIAS_RESID_CLAMP_BF16):
-        rows = B if epilogue == EPI_BIAS_ADD_PER_IMAGE_BF16 else B * H * W
-        if aux is None or aux.dtype != torch.bfloat16 or not aux.is_contiguous() or aux.numel() != rows * Cout or aux.shape[-1] != Cout:
-            raise B200Error(f"conv3x3: this epilogue needs a contiguous bf16 aux with {rows} rows of {Cout}")
-    f32 = epilogue == EPI_BIAS_RESID_F32
-    out = torch.empty((B, H, W, Cout), dtype=torch.float32 if f32 else torch.bfloat16, device=x.device)
+    dtype, aux_kind, _ = EPILOGUES.get(epilogue, (_BF16, None, None))  # the C side refuses the others
+    if aux_kind:
+        rows = B if aux_kind == "image" else B * H * W
+        if aux is None or aux.dtype != dtype or not aux.is_contiguous() or aux.numel() != rows * Cout or aux.shape[-1] != Cout:
+            raise B200Error(f"conv3x3: this epilogue needs a contiguous {dtype} aux with {rows} rows of {Cout}")
+    out = torch.empty((B, H, W, Cout), dtype=dtype, device=x.device)
     call("b200_conv3x3_nhwc_bf16", x.data_ptr(), w_packed.data_ptr(), _ptr(bias), out.data_ptr(), _ptr(aux), Cout, B, H, W, Cin, Cout, epilogue, _stream())
     return out

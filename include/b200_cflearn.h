@@ -81,6 +81,9 @@ long long b200_launch_count(void);
  *   bias: bf16 [N] or NULL.  ldo: leading dimension (elements) of out0/out1/aux (but see the GEGLU epilogues: their
  *   out1 is dense).  N % 8 == 0.  out0 / out1 / aux 16-byte aligned.
  *   splits > 1 only with B200_EPI_PARTIAL_F32 (out0 is f32 [splits, M, ldo]).  max_ctas <= 0: all SMs.
+ *   ldo >= N.  out1 is required by the GELU epilogues (1, 5, 7), aux by 2, 3, 6, 8 and 9; bias is ignored by 3, 4 and 6.
+ *   Operand majors (a_mn_major, b_mn_major): any with BIAS_BF16, (0, 1) with 3, 6 and 8, (1, 1) with PARTIAL_F32, else (0, 0).
+ *   Every argument is checked before any tensor map is encoded.
  * Replaces F.linear at cflearn/modules/core/customs.py:85-89 (Linear.forward), the packed-QKV projection at
  * cflearn/modules/core/attentions.py:214, FeedForward's Linear->GELU->Linear at
  * cflearn/modules/core/mixed_stacks/channel_mixers.py:29-36, the k=s=16 patch-embed F.conv2d at

@@ -342,20 +342,6 @@ def test_new_entry_points_reject_bad_arguments():
     fake = ctypes.c_void_p(1 << 20)  # never dereferenced: every case fails its checks before any launch
     odd = ctypes.c_void_p((1 << 20) + 8)
 
-    def gemm(epi, N=2560, out1=fake, aux=fake, bias=fake, ldo=2560, out0=fake, a_mn=0, b_mn=0):
-        return lib.b200_gemm_bf16(fake, 320, a_mn, fake, 320, b_mn, 4096, N, 320, epi, bias, out0, out1, aux, ldo, 1, 0, null)
-
-    G, DG, R = ops.EPI_BIAS_GEGLU_BF16, ops.EPI_DGEGLU_BF16, ops.EPI_BIAS_RESID_BF16
-    assert gemm(G, out1=null) == -1 and "out1" in _cabi.last_error()
-    assert gemm(G, bias=null) == -1 and "bias" in _cabi.last_error()
-    assert gemm(G, N=2568) == -1 and gemm(DG, N=2568, b_mn=1, bias=null) == -1  # F = 1284 is not a multiple of 8
-    assert gemm(DG, aux=null, b_mn=1, bias=null) == -1 and gemm(R, aux=null) == -1
-    assert gemm(DG, b_mn=0, bias=null) == -1 and gemm(G, b_mn=1) == -1 and gemm(R, a_mn=1) == -1  # majors
-    assert gemm(DG, b_mn=1) == -1  # no bias in the backward
-    assert gemm(G, ldo=2552) == -1 and gemm(R, N=2556, ldo=2556) == -2
-    assert gemm(G, out1=odd) == -2 and gemm(DG, aux=odd, b_mn=1, bias=null) == -2 and gemm(R, out0=odd) == -2
-    assert "aligned" in _cabi.last_error()
-
     def ln_fwd(x=fake, y=fake, gamma=fake, rows=16, dim=320):
         return lib.b200_layernorm_bf16_fwd(x, gamma, fake, y, fake, fake, rows, dim, 1e-5, null)
 
