@@ -158,9 +158,10 @@ __device__ __forceinline__ void store_partial_pair(const GemmParams& p, int sp, 
 
 // Fused epilogue of 8 consecutive elements (row, col .. col + 7) of one output row; t = bf16(acc + bias) as 4 bf16 pairs.
 // n_ok: how many of the 8 columns are inside N (8 on every interior chunk).  Element for element the same arithmetic as
-// the per-pair epilogue it replaces, so results are bit-identical.
+// the per-pair epilogue it replaces, so results are bit-identical.  h8 (dGELU / dQuickGELU only): the chunk's h when n_ok == 8,
+// loaded by the caller rows ahead (see the epilogue loop).
 template <int EPI, bool QUICK>
-__device__ __forceinline__ void epi_chunk(const GemmParams& p, int row, int col, const uint32_t (&t)[4], int n_ok) {
+__device__ __forceinline__ void epi_chunk(const GemmParams& p, int row, int col, const uint32_t (&t)[4], int n_ok, const uint4& h8) {
     const long long off = static_cast<long long>(row) * p.ldo + col;
     uint32_t o[4];  // the bf16 output (out0) of the bf16 variants
     if constexpr (EPI == EPI_BIAS_BF16) {
@@ -254,8 +255,7 @@ __device__ __forceinline__ void epi_chunk(const GemmParams& p, int row, int col,
         const __nv_bfloat16* hsrc = reinterpret_cast<const __nv_bfloat16*>(p.aux) + off;
         uint32_t hw[4] = {0u, 0u, 0u, 0u};
         if (n_ok == 8) {
-            const uint4 h = *reinterpret_cast<const uint4*>(hsrc);
-            hw[0] = h.x; hw[1] = h.y; hw[2] = h.z; hw[3] = h.w;
+            hw[0] = h8.x; hw[1] = h8.y; hw[2] = h8.z; hw[3] = h8.w;
         } else {
 #pragma unroll
             for (int e = 0; e < 8; ++e)
@@ -398,13 +398,39 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                         const uint4 tg = *reinterpret_cast<const uint4*>(staging + staging_offset(r, 16 + hl));
                         if (ok) epi_geglu(p, m_t * BM + r, f, th, tg);
                     }
+                } else if constexpr (EPI == EPI_DGELU_BF16) {
+                    // as below, with the warp's h chunks loaded HQ rows ahead: the compiler cannot move a row's h load above
+                    // the previous row's store (they might alias), so loading it in place waits one L2 round trip per row
+                    constexpr int HQ = 4;
+                    const __nv_bfloat16* hrows = reinterpret_cast<const __nv_bfloat16*>(p.aux) + static_cast<long long>(m_t * BM) * p.ldo + col;
+                    const int r0 = warp - 9;
+                    uint4 hq[HQ] = {};
+#pragma unroll
+                    for (int i = 0; i < HQ; ++i) {
+                        const int r = r0 + i * Cfg::EPI_WARPS;
+                        if (n_ok == 8 && r < rows) hq[i] = *reinterpret_cast<const uint4*>(hrows + static_cast<long long>(r) * p.ldo);
+                    }
+                    for (int rb = r0; rb < rows; rb += HQ * Cfg::EPI_WARPS) {
+#pragma unroll
+                        for (int i = 0; i < HQ; ++i) {
+                            const int r = rb + i * Cfg::EPI_WARPS;
+                            if (r < rows) {
+                                const uint4 h8 = hq[i];
+                                const int rn = r + HQ * Cfg::EPI_WARPS;
+                                if (n_ok == 8 && rn < rows) hq[i] = *reinterpret_cast<const uint4*>(hrows + static_cast<long long>(rn) * p.ldo);
+                                const uint4 v = *reinterpret_cast<const uint4*>(staging + staging_offset(r, lane));
+                                const uint32_t t[4] = {v.x, v.y, v.z, v.w};
+                                if (n_ok > 0) epi_chunk<EPI, QUICK>(p, m_t * BM + r, col, t, n_ok, h8);
+                            }
+                        }
+                    }
                 } else {
                     // epilogue warp w takes rows w, w + 3, ...: one 512-byte row per warp access, 16 bytes per lane
 #pragma unroll 4
                     for (int r = warp - 9; r < rows; r += Cfg::EPI_WARPS) {
                         const uint4 v = *reinterpret_cast<const uint4*>(staging + staging_offset(r, lane));
                         const uint32_t t[4] = {v.x, v.y, v.z, v.w};
-                        if (n_ok > 0) epi_chunk<EPI, QUICK>(p, m_t * BM + r, col, t, n_ok);
+                        if (n_ok > 0) epi_chunk<EPI, QUICK>(p, m_t * BM + r, col, t, n_ok, make_uint4(0u, 0u, 0u, 0u));
                     }
                 }
                 mbar_arrive(staging_empty);
