@@ -27,6 +27,9 @@
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
+#include <stdio.h>
+
+#include <initializer_list>
 
 #include "b200_internal.h"
 #include "ptx.cuh"
@@ -1096,33 +1099,85 @@ static int g_attn_fwd_version = 0;
 static int g_attn_bwd_version = 0;
 static int g_attn_prefetch = 0;
 
-static int attn_check(int B, int T, int H, int Dh) {
-    if (B <= 0 || T <= 0 || H <= 0) return set_error(B200_ERR_ARG, "attention: non-positive size");
-    if (Dh != 64) return set_error(B200_ERR_ARG, "attention: head dim must be 64");
-    if (T > 256) return set_error(B200_ERR_ARG, "attention: T must be <= 256");
+// packed qkv with T <= 256 (resident kernels), packed qkv with T <= 16384 (streamed kernels), separate Q / K / V (streamed)
+enum AttnFamily { ATTN_RESIDENT, ATTN_LONG, ATTN_CROSS };
+
+// One call of an attention entry point, as check_attn_args sees it.  The packed entries pass qkv as q, k and v, dqkv as dq, dk
+// and dv, and the leading dims of their layout; the forward entries leave the backward's pointers null.
+struct AttnCall {
+    const char* entry;
+    AttnFamily family;
+    bool bwd;
+    int B, Tq, Tk, H, Dh, causal;
+    long long ldq, ldkv, ldo;
+    const void *q, *k, *v, *out, *lse;
+    const void *dout, *dq, *dk, *dv;  // required by the backward entries
+    const void* dbias_part;           // optional
+    const void* workspace;            // required by the streamed backward entries
+};
+
+static int attn_error(const AttnCall& c, int code, const char* what) {
+    char msg[160];
+    snprintf(msg, sizeof(msg), "%s: %s", c.entry, what);
+    return set_error(code, msg);
+}
+
+// Every argument check of the attention entries, before any tensor map is encoded: a call is refused the same way with or
+// without a device.
+static int check_attn_args(const AttnCall& c) {
+    const bool packed = c.family != ATTN_CROSS, resident = c.family == ATTN_RESIDENT;
+    if (c.B <= 0 || c.H <= 0 || c.Tq <= 0 || c.Tk <= 0) return attn_error(c, B200_ERR_ARG, "non-positive size");
+    const int max_t = resident ? 256 : LA_MAX_T;
+    if (c.Tq > max_t || c.Tk > max_t) return attn_error(c, B200_ERR_ARG, resident ? "T must be <= 256" : "T must be <= 16384");
+    if (packed && c.Dh != 64) return attn_error(c, B200_ERR_ARG, "head dim must be 64");
+    if (c.Dh < 8 || c.Dh > LA_MAX_DH || c.Dh % 8 != 0) return attn_error(c, B200_ERR_ARG, "head dim must be a multiple of 8 in [8, 160]");
+    if (c.causal && c.Tq != c.Tk) return attn_error(c, B200_ERR_ARG, "causal needs Tq == Tk");
+    const long long width = static_cast<long long>(c.H) * c.Dh;
+    if (c.ldq < width || c.ldkv < width || c.ldo < width) return attn_error(c, B200_ERR_ARG, "leading dim < H * Dh");
+    if (c.ldq % 8 != 0 || c.ldkv % 8 != 0 || c.ldo % 8 != 0) return attn_error(c, B200_ERR_ALIGN, "leading dims must be multiples of 8");
+    if (!(c.q && c.k && c.v && c.out && c.lse) || (c.bwd && !(c.dout && c.dq && c.dk && c.dv)))
+        return attn_error(c, B200_ERR_ARG, "null pointer");
+    if (c.bwd && !resident && c.workspace == nullptr) return attn_error(c, B200_ERR_ARG, "workspace is required");
+    // TMA bases, and the backward's 16-byte reads of out / dout
+    uintptr_t any = 0;
+    for (const void* p : {c.q, c.k, c.v, c.out, c.lse, c.dout, c.dq, c.dk, c.dv, c.dbias_part, c.workspace}) any |= reinterpret_cast<uintptr_t>(p);
+    if ((any & 15u) != 0) return attn_error(c, B200_ERR_ALIGN, "pointers must be 16-byte aligned");
     return 0;
+}
+
+// the dynamic shared-memory attribute belongs to the (function, device) pair
+template <typename Kernel>
+static int configure_smem(Kernel kernel, int smem, bool (&configured)[64]) {
+    const int dev = current_device_slot();
+    if (configured[dev]) return 0;
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) return set_error(B200_ERR_LAUNCH, cudaGetErrorString(e));
+    configured[dev] = true;
+    return 0;
+}
+
+// {width, T, B} over a packed [B, T, width] bf16 tensor; boxes of 64 columns x `rows` rows (128B-swizzled): rows >= T of an
+// image are zero-filled
+static int packed_tmap(CUtensorMap* tm, const void* base, int width, int T, int B, int rows) {
+    uint64_t dims[3] = {static_cast<uint64_t>(width), static_cast<uint64_t>(T), static_cast<uint64_t>(B)};
+    uint64_t strides[2] = {static_cast<uint64_t>(width) * 2, static_cast<uint64_t>(width) * 2 * static_cast<uint64_t>(T)};
+    uint32_t box[3] = {64, static_cast<uint32_t>(rows), 1};
+    return make_tmap(tm, base, 2, 3, dims, strides, box, 128);
 }
 
 extern "C" int b200_attention_fwd(const void* qkv_bf16, void* out_bf16, float* lse, int B, int T, int H, int Dh,
                                   float scale, int causal, cudaStream_t stream) {
-    int rc = attn_check(B, T, H, Dh);
+    const long long ld = 64ll * H;
+    int rc = check_attn_args({"attention_fwd", ATTN_RESIDENT, false, B, T, T, H, Dh, causal, 3 * ld, 3 * ld, ld, qkv_bf16, qkv_bf16,
+                              qkv_bf16, out_bf16, lse});
     if (rc) return rc;
     const int D = H * 64;
     const int tp = (T + 63) / 64 * 64;
     CUtensorMap tmQ, tmKV;
-    uint64_t dims[3] = {static_cast<uint64_t>(3 * D), static_cast<uint64_t>(T), static_cast<uint64_t>(B)};
-    uint64_t strides[2] = {static_cast<uint64_t>(3 * D) * 2, static_cast<uint64_t>(3 * D) * 2 * static_cast<uint64_t>(T)};
-    uint32_t boxq[3] = {64, 128, 1};
-    uint32_t boxkv[3] = {64, static_cast<uint32_t>(tp), 1};
-    if ((rc = make_tmap(&tmQ, qkv_bf16, 2, 3, dims, strides, boxq, 128)) != 0) return rc;
-    if ((rc = make_tmap(&tmKV, qkv_bf16, 2, 3, dims, strides, boxkv, 128)) != 0) return rc;
-    static bool configured[64] = {};  // per device: the attribute belongs to the (function, device) pair
-    const int dev = current_device_slot();
-    if (!configured[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AF_SMEM);
-        if (e != cudaSuccess) return set_error(B200_ERR_LAUNCH, cudaGetErrorString(e));
-        configured[dev] = true;
-    }
+    if ((rc = packed_tmap(&tmQ, qkv_bf16, 3 * D, T, B, 128)) != 0) return rc;
+    if ((rc = packed_tmap(&tmKV, qkv_bf16, 3 * D, T, B, tp)) != 0) return rc;
+    static bool configured[64] = {};
+    if ((rc = configure_smem(attn_fwd_kernel, AF_SMEM, configured)) != 0) return rc;
     AttnParams p;
     p.B = B; p.T = T; p.H = H; p.D = D; p.tp = tp; p.scale = scale; p.causal = causal;
     const int n_mt = (T + 127) / 128;
@@ -1139,30 +1194,17 @@ extern "C" int b200_set_attention_fwd_version(int version) {
 extern "C" int b200_attention_bwd(const void* qkv_bf16, const void* out_bf16, const void* dout_bf16, const float* lse,
                                   void* dqkv_bf16, int B, int T, int H, int Dh, float scale, int causal,
                                   float* dbias_part, cudaStream_t stream) {
-    int rc = attn_check(B, T, H, Dh);
+    const long long ld = 64ll * H;
+    int rc = check_attn_args({"attention_bwd", ATTN_RESIDENT, true, B, T, T, H, Dh, causal, 3 * ld, 3 * ld, ld, qkv_bf16, qkv_bf16,
+                              qkv_bf16, out_bf16, lse, dout_bf16, dqkv_bf16, dqkv_bf16, dqkv_bf16, dbias_part, nullptr});
     if (rc) return rc;
     const int D = H * 64;
     const int tp = (T + 63) / 64 * 64;
     CUtensorMap tmQKV, tmDO;
-    {
-        uint64_t dims[3] = {static_cast<uint64_t>(3 * D), static_cast<uint64_t>(T), static_cast<uint64_t>(B)};
-        uint64_t strides[2] = {static_cast<uint64_t>(3 * D) * 2, static_cast<uint64_t>(3 * D) * 2 * static_cast<uint64_t>(T)};
-        uint32_t box[3] = {64, static_cast<uint32_t>(tp), 1};
-        if ((rc = make_tmap(&tmQKV, qkv_bf16, 2, 3, dims, strides, box, 128)) != 0) return rc;
-    }
-    {
-        uint64_t dims[3] = {static_cast<uint64_t>(D), static_cast<uint64_t>(T), static_cast<uint64_t>(B)};
-        uint64_t strides[2] = {static_cast<uint64_t>(D) * 2, static_cast<uint64_t>(D) * 2 * static_cast<uint64_t>(T)};
-        uint32_t box[3] = {64, static_cast<uint32_t>(tp), 1};
-        if ((rc = make_tmap(&tmDO, dout_bf16, 2, 3, dims, strides, box, 128)) != 0) return rc;
-    }
+    if ((rc = packed_tmap(&tmQKV, qkv_bf16, 3 * D, T, B, tp)) != 0) return rc;
+    if ((rc = packed_tmap(&tmDO, dout_bf16, D, T, B, tp)) != 0) return rc;
     static bool configured[64] = {};
-    const int dev = current_device_slot();
-    if (!configured[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AB_SMEM);
-        if (e != cudaSuccess) return set_error(B200_ERR_LAUNCH, cudaGetErrorString(e));
-        configured[dev] = true;
-    }
+    if ((rc = configure_smem(attn_bwd_kernel, AB_SMEM, configured)) != 0) return rc;
     AttnParams p;
     p.B = B; p.T = T; p.H = H; p.D = D; p.tp = tp; p.scale = scale; p.causal = causal;
     attn_bwd_kernel<<<B * H, ATT_THREADS, AB_SMEM, stream>>>(tmQKV, tmDO, reinterpret_cast<const __nv_bfloat16*>(out_bf16),
@@ -1184,24 +1226,6 @@ extern "C" int b200_set_attention_bwd_version(int version) {
 }
 
 // ---- streamed kernels: any 1 <= Tq, Tk <= 16384, Dh <= 160 ----
-static int attn_long_check(int B, int T, int H, int Dh) {
-    if (B <= 0 || T <= 0 || H <= 0) return set_error(B200_ERR_ARG, "attention_long: non-positive size");
-    if (Dh != 64) return set_error(B200_ERR_ARG, "attention_long: head dim must be 64");
-    if (T > LA_MAX_T) return set_error(B200_ERR_ARG, "attention_long: T must be <= 16384");
-    return 0;
-}
-
-// the dynamic shared-memory attribute belongs to the (function, device) pair
-template <typename Kernel>
-static int attn_long_configure(Kernel kernel, int smem, bool (&configured)[64]) {
-    const int dev = current_device_slot();
-    if (configured[dev]) return 0;
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return set_error(B200_ERR_LAUNCH, cudaGetErrorString(e));
-    configured[dev] = true;
-    return 0;
-}
-
 // {Dh, H, T, B} over a [B, T, ld] bf16 tensor whose head h starts at column h * Dh; 64 x 64 boxes (128B-swizzled): columns
 // >= Dh and rows >= T of an image are zero-filled
 static int attn_long_tmap(CUtensorMap* tm, const void* base, long long ld, int Dh, int H, int T, int B) {
@@ -1241,7 +1265,7 @@ static int attn_long_fwd_launch(const CUtensorMap& tmQ, const CUtensorMap& tmK, 
                                 const LongParams& p, cudaStream_t stream) {
     constexpr int NB = (KS + 3) / 4;
     static bool configured[64] = {};
-    int rc = attn_long_configure(attn_long_fwd_kernel<KS>, LongCfg<NB>::F_SMEM, configured);
+    int rc = configure_smem(attn_long_fwd_kernel<KS>, LongCfg<NB>::F_SMEM, configured);
     if (rc) return rc;
     const int n_mt = (p.Tq + 127) / 128;
     attn_long_fwd_kernel<KS><<<p.B * p.H * n_mt, LA_THREADS, LongCfg<NB>::F_SMEM, stream>>>(tmQ, tmK, tmV, reinterpret_cast<__nv_bfloat16*>(out), lse, p);
@@ -1255,8 +1279,8 @@ static int attn_long_bwd_launch(const CUtensorMap& tmQ, const CUtensorMap& tmK, 
     using C = LongCfg<(KS + 3) / 4>;
     static bool configured_kv[64] = {}, configured_q[64] = {};
     int rc;
-    if ((rc = attn_long_configure(attn_long_dkdv_kernel<KS>, C::K_SMEM, configured_kv)) != 0) return rc;
-    if ((rc = attn_long_configure(attn_long_dq_kernel<KS>, C::Q_SMEM, configured_q)) != 0) return rc;
+    if ((rc = configure_smem(attn_long_dkdv_kernel<KS>, C::K_SMEM, configured_kv)) != 0) return rc;
+    if ((rc = configure_smem(attn_long_dq_kernel<KS>, C::Q_SMEM, configured_q)) != 0) return rc;
     const int n_kt = (p.Tk + C::K_ROWS - 1) / C::K_ROWS;
     attn_long_dkdv_kernel<KS><<<p.B * p.H * n_kt * p.nchunk, LA_THREADS, C::K_SMEM, stream>>>(
         tmQ, tmK, tmV, tmDO, lse, delta, reinterpret_cast<__nv_bfloat16*>(dk), reinterpret_cast<__nv_bfloat16*>(dv), part, csum_part, p);
@@ -1330,10 +1354,10 @@ static int attn_long_bwd_run(const void* q, long long ldq, const void* k, const 
 
 extern "C" int b200_attention_long_fwd(const void* qkv_bf16, void* out_bf16, float* lse, int B, int T, int H, int Dh,
                                        float scale, int causal, cudaStream_t stream) {
-    int rc = attn_long_check(B, T, H, Dh);
-    if (rc) return rc;
-    if (qkv_bf16 == nullptr || out_bf16 == nullptr || lse == nullptr) return set_error(B200_ERR_ARG, "attention_long_fwd: null pointer");
-    const int D = H * 64;
+    const long long D = 64ll * H;
+    if (const int rc = check_attn_args({"attention_long_fwd", ATTN_LONG, false, B, T, T, H, Dh, causal, 3 * D, 3 * D, D, qkv_bf16, qkv_bf16,
+                                        qkv_bf16, out_bf16, lse}))
+        return rc;
     const __nv_bfloat16* qkv = reinterpret_cast<const __nv_bfloat16*>(qkv_bf16);
     return attn_long_fwd_run(qkv, 3 * D, qkv + D, qkv + 2 * D, 3 * D, out_bf16, D, lse, B, T, T, H, 64, scale, causal, stream);
 }
@@ -1347,11 +1371,10 @@ extern "C" long long b200_attention_long_bwd_workspace_floats(int B, int T, int 
 extern "C" int b200_attention_long_bwd(const void* qkv_bf16, const void* out_bf16, const void* dout_bf16, const float* lse,
                                        void* dqkv_bf16, int B, int T, int H, int Dh, float scale, int causal,
                                        float* dbias_part, float* workspace, cudaStream_t stream) {
-    int rc = attn_long_check(B, T, H, Dh);
-    if (rc) return rc;
-    if (qkv_bf16 == nullptr || out_bf16 == nullptr || dout_bf16 == nullptr || lse == nullptr || dqkv_bf16 == nullptr || workspace == nullptr)
-        return set_error(B200_ERR_ARG, "attention_long_bwd: null pointer");
-    const int D = H * 64;
+    const long long D = 64ll * H;
+    if (const int rc = check_attn_args({"attention_long_bwd", ATTN_LONG, true, B, T, T, H, Dh, causal, 3 * D, 3 * D, D, qkv_bf16, qkv_bf16,
+                                        qkv_bf16, out_bf16, lse, dout_bf16, dqkv_bf16, dqkv_bf16, dqkv_bf16, dbias_part, workspace}))
+        return rc;
     const __nv_bfloat16* qkv = reinterpret_cast<const __nv_bfloat16*>(qkv_bf16);
     __nv_bfloat16* dqkv = reinterpret_cast<__nv_bfloat16*>(dqkv_bf16);
     return attn_long_bwd_run(qkv, 3 * D, qkv + D, qkv + 2 * D, 3 * D, out_bf16, D, dout_bf16, lse, dqkv, dqkv + D, dqkv + 2 * D, B, T, T, H, 64,
@@ -1359,27 +1382,10 @@ extern "C" int b200_attention_long_bwd(const void* qkv_bf16, const void* out_bf1
 }
 
 // ---- separate Q / K / V (cross-attention, head dims 8 ... 160) on the same streamed kernels ----
-static bool misaligned16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15u) != 0; }
-
-static int cross_check(int B, int Tq, int Tk, int H, int Dh, int causal, long long ldq, long long ldkv, long long ldo) {
-    if (B <= 0 || H <= 0) return set_error(B200_ERR_ARG, "cross_attention: non-positive size");
-    if (Tq < 1 || Tk < 1 || Tq > LA_MAX_T || Tk > LA_MAX_T) return set_error(B200_ERR_ARG, "cross_attention: Tq and Tk must be in [1, 16384]");
-    if (Dh < 8 || Dh > LA_MAX_DH || Dh % 8 != 0) return set_error(B200_ERR_ARG, "cross_attention: head dim must be a multiple of 8 in [8, 160]");
-    if (causal && Tq != Tk) return set_error(B200_ERR_ARG, "cross_attention: causal needs Tq == Tk");
-    const long long width = static_cast<long long>(H) * Dh;
-    if (ldq < width || ldkv < width || ldo < width) return set_error(B200_ERR_ARG, "cross_attention: leading dim < H * Dh");
-    if (ldq % 8 != 0 || ldkv % 8 != 0 || ldo % 8 != 0) return set_error(B200_ERR_ALIGN, "cross_attention: leading dims must be multiples of 8");
-    return 0;
-}
-
 extern "C" int b200_cross_attention_fwd(const void* q, long long ldq, const void* k, const void* v, long long ldkv, void* out, long long ldo,
                                         float* lse, int B, int Tq, int Tk, int H, int Dh, float scale, int causal, cudaStream_t stream) {
-    int rc = cross_check(B, Tq, Tk, H, Dh, causal, ldq, ldkv, ldo);
-    if (rc) return rc;
-    if (q == nullptr || k == nullptr || v == nullptr || out == nullptr || lse == nullptr)
-        return set_error(B200_ERR_ARG, "cross_attention_fwd: null pointer");
-    if (misaligned16(q) || misaligned16(k) || misaligned16(v) || misaligned16(out) || misaligned16(lse))
-        return set_error(B200_ERR_ALIGN, "cross_attention_fwd: pointers must be 16-byte aligned");
+    if (const int rc = check_attn_args({"cross_attention_fwd", ATTN_CROSS, false, B, Tq, Tk, H, Dh, causal, ldq, ldkv, ldo, q, k, v, out, lse}))
+        return rc;
     return attn_long_fwd_run(q, ldq, k, v, ldkv, out, ldo, lse, B, Tq, Tk, H, Dh, scale, causal, stream);
 }
 
@@ -1395,15 +1401,9 @@ extern "C" long long b200_cross_attention_bwd_workspace_floats(int B, int Tq, in
 extern "C" int b200_cross_attention_bwd(const void* q, long long ldq, const void* k, const void* v, long long ldkv, const void* out,
                                         long long ldo, const void* dout, const float* lse, void* dq, void* dk, void* dv, int B, int Tq, int Tk,
                                         int H, int Dh, float scale, int causal, float* workspace, cudaStream_t stream) {
-    int rc = cross_check(B, Tq, Tk, H, Dh, causal, ldq, ldkv, ldo);
-    if (rc) return rc;
-    if (q == nullptr || k == nullptr || v == nullptr || out == nullptr || dout == nullptr || lse == nullptr || dq == nullptr || dk == nullptr ||
-        dv == nullptr)
-        return set_error(B200_ERR_ARG, "cross_attention_bwd: null pointer");
-    if (workspace == nullptr) return set_error(B200_ERR_ARG, "cross_attention_bwd: workspace is required");
-    if (misaligned16(q) || misaligned16(k) || misaligned16(v) || misaligned16(out) || misaligned16(dout) || misaligned16(lse) ||
-        misaligned16(dq) || misaligned16(dk) || misaligned16(dv) || misaligned16(workspace))
-        return set_error(B200_ERR_ALIGN, "cross_attention_bwd: pointers must be 16-byte aligned");
+    if (const int rc = check_attn_args({"cross_attention_bwd", ATTN_CROSS, true, B, Tq, Tk, H, Dh, causal, ldq, ldkv, ldo, q, k, v, out, lse,
+                                        dout, dq, dk, dv, nullptr, workspace}))
+        return rc;
     return attn_long_bwd_run(q, ldq, k, v, ldkv, out, ldo, dout, lse, dq, dk, dv, B, Tq, Tk, H, Dh, scale, causal, nullptr, workspace, true,
                              stream);
 }

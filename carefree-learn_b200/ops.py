@@ -256,9 +256,9 @@ def _dense_bf16(t: Tensor, name: str) -> None:
         raise B200Error(f"layernorm_bf16: {name} must be a contiguous bf16 [rows, dim] tensor")
 
 
-def _dense_f32(t: Tensor, n: int, name: str) -> None:
+def _dense_f32(t: Tensor, n: int, name: str, what: str = "layernorm_bf16") -> None:
     if t.dtype != torch.float32 or tuple(t.shape) != (n,) or not t.is_contiguous():
-        raise B200Error(f"layernorm_bf16: {name} must be a contiguous fp32 [{n}] tensor")
+        raise B200Error(f"{what}: {name} must be a contiguous fp32 [{n}] tensor")
 
 
 def layernorm_bf16_fwd(x: Tensor, gamma: Tensor, beta: Tensor, eps: float) -> Tuple[Tensor, Tensor, Tensor]:
@@ -315,11 +315,21 @@ ATTENTION_MAX_T = 16384   # longest sequence the attention kernels accept
 ATTENTION_RESIDENT_MAX_T = 256  # up to here a whole head fits in shared memory; longer sequences use the streamed kernels
 
 
+def _packed_rows(t: Tensor, rows: int, width: int, msg: str) -> None:
+    """t: contiguous bf16 holding `rows` rows of `width` elements ([rows, width], or [B, T, width] with B * T = rows)."""
+    if t.dtype != torch.bfloat16 or not t.is_contiguous() or t.dim() < 2 or t.shape[-1] != width or t.numel() != rows * width:
+        raise B200Error(msg)
+
+
+def _lse(lse: Tensor, B: int, H: int, T: int, what: str) -> None:
+    if lse.dtype != torch.float32 or tuple(lse.shape) != (B, H, T) or not lse.is_contiguous():
+        raise B200Error(f"{what}: lse must be a contiguous fp32 [B, H, T] tensor")
+
+
 def attention_fwd(qkv: Tensor, B: int, T: int, H: int, *, scale: Optional[float] = None, causal: bool = False) -> Tuple[Tensor, Tensor]:
     _need_cuda(qkv)
     D = H * 64
-    if qkv.dtype != torch.bfloat16 or qkv.numel() != B * T * 3 * D or not qkv.is_contiguous():
-        raise B200Error("attention_fwd: qkv must be contiguous bf16 [B, T, 3*H*64]")
+    _packed_rows(qkv, B * T, 3 * D, "attention_fwd: qkv must be contiguous bf16 [B, T, 3*H*64]")
     out = torch.empty((B * T, D), dtype=torch.bfloat16, device=qkv.device)
     lse = torch.empty((B, H, T), dtype=torch.float32, device=qkv.device)
     sc = float(scale) if scale is not None else 0.125
@@ -332,10 +342,17 @@ def attention_bwd(qkv: Tensor, out: Tensor, dout: Tensor, lse: Tensor, B: int, T
                   dbias: Optional[Tensor] = None) -> Tensor:
     """dqkv (bf16 [B*T, 3*H*64]).  ``dbias`` (fp32 [3*H*64]): also receives the bf16-rounded column sums of dqkv -- the
     gradient of the packed qkv bias -- accumulated inside the kernel (no separate pass over dqkv)."""
-    _need_cuda(qkv, out, dout, lse)
+    _need_cuda(qkv, out, dout, lse, dqkv, dbias)
     D = H * 64
+    _packed_rows(qkv, B * T, 3 * D, "attention_bwd: qkv must be contiguous bf16 [B, T, 3*H*64]")
+    _packed_rows(out, B * T, D, "attention_bwd: out must be contiguous bf16 [B*T, H*64]")
+    _packed_rows(dout, B * T, D, "attention_bwd: dout must be contiguous bf16 [B*T, H*64]")
+    _lse(lse, B, H, T, "attention_bwd")
     if dqkv is None:
         dqkv = torch.empty((B * T, 3 * D), dtype=torch.bfloat16, device=qkv.device)
+    _packed_rows(dqkv, B * T, 3 * D, "attention_bwd: dqkv must be contiguous bf16 [B*T, 3*H*64]")
+    if dbias is not None:
+        _dense_f32(dbias, 3 * D, "dbias", "attention_bwd")
     sc = float(scale) if scale is not None else 0.125
     part = WORKSPACE.get(qkv.device, B * 3 * D, "attn_dbias") if dbias is not None else None
     if T <= ATTENTION_RESIDENT_MAX_T:
@@ -356,19 +373,24 @@ def _rows_view(t: Tensor, name: str) -> int:
     return t.stride(0)
 
 
-def cross_attention_fwd(q: Tensor, k: Tensor, v: Tensor, B: int, H: int, *, scale: Optional[float] = None,
-                        causal: bool = False) -> Tuple[Tensor, Tensor]:
-    """Attention with separate operands: q [B*Tq, >= H*Dh], k / v [B*Tk, >= H*Dh] (bf16 2-D views with unit inner stride, e.g.
-    column slices of one packed projection), head h at columns [h*Dh, (h+1)*Dh).  Returns (out bf16 [B*Tq, H*Dh], lse f32 [B, H, Tq])."""
-    _need_cuda(q, k, v)
+def _cross_operands(q: Tensor, k: Tensor, v: Tensor, B: int, H: int) -> Tuple[int, int, int, int, int]:
+    """(ldq, ldk, Tq, Tk, Dh) of the q / k / v views."""
     ldq, ldk, ldv = _rows_view(q, "q"), _rows_view(k, "k"), _rows_view(v, "v")
     if ldk != ldv or k.shape != v.shape:
         raise B200Error("cross_attention: k and v must share shape and leading dim")
     L = q.shape[1]
     if L % H != 0 or k.shape[1] != L or q.shape[0] % B != 0 or k.shape[0] % B != 0:
         raise B200Error("cross_attention: q / k / v widths must be H * Dh and rows a multiple of B")
-    Tq, Tk, Dh = q.shape[0] // B, k.shape[0] // B, L // H
-    out = torch.empty((B * Tq, L), dtype=torch.bfloat16, device=q.device)
+    return ldq, ldk, q.shape[0] // B, k.shape[0] // B, L // H
+
+
+def cross_attention_fwd(q: Tensor, k: Tensor, v: Tensor, B: int, H: int, *, scale: Optional[float] = None,
+                        causal: bool = False) -> Tuple[Tensor, Tensor]:
+    """Attention with separate operands: q [B*Tq, >= H*Dh], k / v [B*Tk, >= H*Dh] (bf16 2-D views with unit inner stride, e.g.
+    column slices of one packed projection), head h at columns [h*Dh, (h+1)*Dh).  Returns (out bf16 [B*Tq, H*Dh], lse f32 [B, H, Tq])."""
+    _need_cuda(q, k, v)
+    ldq, ldk, Tq, Tk, Dh = _cross_operands(q, k, v, B, H)
+    out = torch.empty((B * Tq, H * Dh), dtype=torch.bfloat16, device=q.device)
     lse = torch.empty((B, H, Tq), dtype=torch.float32, device=q.device)
     sc = float(scale) if scale is not None else Dh ** -0.5
     call("b200_cross_attention_fwd", q.data_ptr(), ldq, k.data_ptr(), v.data_ptr(), ldk, out.data_ptr(), out.stride(0), lse.data_ptr(),
@@ -381,18 +403,22 @@ def cross_attention_bwd(q: Tensor, k: Tensor, v: Tensor, out: Tensor, dout: Tens
                         dv: Optional[Tensor] = None) -> Tuple[Tensor, Tensor, Tensor]:
     """(dq, dk, dv) of ``cross_attention_fwd``.  dq / dk / dv may be given as views (dq with q's leading dim, dk / dv with k's), e.g.
     column slices of one packed [M, 3L] gradient for self-attention; otherwise they are allocated contiguous."""
-    _need_cuda(q, k, v, out, dout, lse)
-    ldq, ldk = _rows_view(q, "q"), _rows_view(k, "k")
+    _need_cuda(q, k, v, out, dout, lse, dq, dk, dv)
+    ldq, ldk, Tq, Tk, Dh = _cross_operands(q, k, v, B, H)
+    L = q.shape[1]
     if _rows_view(dout, "dout") != _rows_view(out, "out"):
         raise B200Error("cross_attention_bwd: dout must share out's leading dim")
-    L = q.shape[1]
-    Tq, Tk, Dh = q.shape[0] // B, k.shape[0] // B, L // H
+    if tuple(out.shape) != (B * Tq, L) or dout.shape != out.shape:
+        raise B200Error("cross_attention_bwd: out / dout must have q's rows and width")
+    _lse(lse, B, H, Tq, "cross_attention_bwd")
     if dq is None and dk is None and dv is None and ldq == L and ldk == L:
         dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
     if dq is None or dk is None or dv is None:
         raise B200Error("cross_attention_bwd: give all of dq, dk, dv or none (with contiguous q / k / v)")
     if _rows_view(dq, "dq") != ldq or _rows_view(dk, "dk") != ldk or _rows_view(dv, "dv") != ldk:
         raise B200Error("cross_attention_bwd: dq must share q's leading dim, dk / dv k's")
+    if dq.shape != q.shape or dk.shape != k.shape or dv.shape != k.shape:
+        raise B200Error("cross_attention_bwd: dq must have q's shape, dk / dv k's")
     sc = float(scale) if scale is not None else Dh ** -0.5
     ws = WORKSPACE.get(q.device, int(_cabi.lib().b200_cross_attention_bwd_workspace_floats(B, Tq, Tk, H, Dh)), "cross_attn")
     call("b200_cross_attention_bwd", q.data_ptr(), ldq, k.data_ptr(), v.data_ptr(), ldk, out.data_ptr(), out.stride(0), dout.data_ptr(),

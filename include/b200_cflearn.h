@@ -163,6 +163,11 @@ int b200_colsum_per_image_bf16(const void* x_bf16, int B, int HW, int C, void* p
  * inside each third (chunk(3, dim=-1) then view(B,T,H,Dh)).  out: bf16 [B, T, H*Dh].  lse: f32 [B, H, T]
  * (natural-log sum-exp of the scaled scores), saved for backward.  causal != 0 applies the lower-triangular
  * mask of cflearn/modules/nlp/encoder/transformer.py:42-48.  Dh must be 64, T <= 256.
+ * Pointers, for every attention entry point below: qkv (q, k, v), out, lse and, in the backward, dout and dqkv (dq, dk, dv)
+ * are required; dbias_part is optional; the streamed backward entries (long and cross) require their workspace.  Every
+ * non-NULL pointer is 16-byte aligned (TMA bases, and the backward reads out / dout in 16-byte groups).  All arguments are
+ * checked before any tensor map is encoded: a size outside the entry's range, a NULL required pointer or a missing workspace
+ * is B200_ERR_ARG, a misaligned pointer or leading dim B200_ERR_ALIGN.
  * --------------------------------------------------------------------------------------------------------- */
 int b200_attention_fwd(const void* qkv_bf16, void* out_bf16, float* lse, int B, int T, int H, int Dh, float scale,
                        int causal, cudaStream_t stream);
@@ -179,7 +184,7 @@ int b200_attention_bwd(const void* qkv_bf16, const void* out_bf16, const void* d
 /* The same attention for long sequences: 1 <= T <= 16384, Dh = 64, the same layouts, outputs and causal flag as
  * b200_attention_fwd / _bwd.  These kernels stream K / V (forward, dQ) or Q / dO (dK / dV) through shared memory in
  * 64-row blocks with an online softmax, so no head has to fit in shared memory at once.  Deterministic (no atomics).
- * workspace (backward, required): b200_attention_long_bwd_workspace_floats(B, T, H) floats of device scratch.
+ * workspace (backward): b200_attention_long_bwd_workspace_floats(B, T, H) floats of device scratch.
  * dbias_part (optional): the same per-image column sums as b200_attention_bwd writes. */
 int b200_attention_long_fwd(const void* qkv_bf16, void* out_bf16, float* lse, int B, int T, int H, int Dh, float scale,
                             int causal, cudaStream_t stream);
@@ -191,10 +196,10 @@ int b200_attention_long_bwd(const void* qkv_bf16, const void* out_bf16, const vo
  * CrossAttention, cflearn/modules/core/attentions.py:534-569 (heads folded into the batch, then sdp_attn ->
  * F.scaled_dot_product_attention at cflearn/toolkit.py:959-963).  q: bf16 [B, Tq, ldq], k / v: bf16 [B, Tk, ldkv], head h at
  * columns [h * Dh, h * Dh + Dh); out: bf16 [B, Tq, ldo]; lse: f32 [B, H, Tq].  1 <= Tq, Tk <= 16384; causal only with Tq == Tk.
- * Leading dims are multiples of 8 and >= H * Dh, pointers 16-byte aligned, so q / k / v may be column slices of one packed
+ * Leading dims are multiples of 8 and >= H * Dh, so q / k / v may be column slices of one packed
  * projection output (self-attention: q = qkv, k = qkv + H * Dh, v = qkv + 2 * H * Dh, ld = 3 * H * Dh).
  * Backward: dout uses ldo, dq uses ldq, dk / dv use ldkv (so dq / dk / dv may be views of one packed gradient buffer).
- * workspace (required): b200_cross_attention_bwd_workspace_floats(B, Tq, Tk, H, Dh) floats.  Deterministic (no atomics). */
+ * workspace (backward): b200_cross_attention_bwd_workspace_floats(B, Tq, Tk, H, Dh) floats.  Deterministic (no atomics). */
 int b200_cross_attention_fwd(const void* q, long long ldq, const void* k, const void* v, long long ldkv, void* out, long long ldo,
                              float* lse, int B, int Tq, int Tk, int H, int Dh, float scale, int causal, cudaStream_t stream);
 long long b200_cross_attention_bwd_workspace_floats(int B, int Tq, int Tk, int H, int Dh);

@@ -1,8 +1,8 @@
 """Attention with separate Q / K / V and head dims up to 160 (b200_cross_attention_*, ops.cross_attention_*, CrossAttentionB200):
 kernel parity against fp32 math and torch SDPA, determinism (including the query-split dK / dV grid), equality with the packed
 Dh-64 entry points, and module parity against oracle/unet_oracle.py::cross_attention at SD-v1.5 widths.  The CPU cases check the
-argument checks, the workspace formula, the module's parameters and its refusals; the others need an H100 (pytest -m gpu)."""
-import ctypes
+module's parameters and its refusals (the entry points' argument checks and workspace formula are in test_attention_contract.py);
+the others need an H100 (pytest -m gpu)."""
 import os
 import sys
 
@@ -213,56 +213,7 @@ def test_module_parity(query_dim, side, cross):
         assert _relerr(ours[k], eager[k]) <= 2.0 * floor + 1e-6, (k, _relerr(ours[k], eager[k]), floor)
 
 
-# ---- 5. CPU: argument checks, workspace formula, the module's parameters and refusals --------------------------------------
-def test_cross_entry_points_reject_bad_arguments():
-    lib = _cabi.lib()
-    null = ctypes.c_void_p(0)
-    fake = ctypes.c_void_p(1 << 20)  # never dereferenced: every case fails its checks before any launch
-    odd = ctypes.c_void_p((1 << 20) + 8)
-
-    def fwd(q=fake, ldq=512, k=fake, v=fake, ldkv=512, out=fake, ldo=512, lse=fake, B=1, Tq=4096, Tk=77, H=8, Dh=40, causal=0):
-        return lib.b200_cross_attention_fwd(q, ldq, k, v, ldkv, out, ldo, lse, B, Tq, Tk, H, Dh, 0.125, causal, null)
-
-    def bwd(ws=fake, dq=fake, Dh=40, Tq=4096, Tk=77, causal=0, ldq=512):
-        return lib.b200_cross_attention_bwd(fake, ldq, fake, fake, 512, fake, 512, fake, fake, dq, fake, fake, 1, Tq, Tk, 8, Dh, 0.125, causal,
-                                            ws, null)
-
-    for Dh in (0, 4, 12, 168, 192):
-        assert fwd(Dh=Dh) == -1 and bwd(Dh=Dh) == -1, Dh
-    for Tq, Tk in ((0, 77), (77, 0), (16385, 77), (77, 16385)):
-        assert fwd(Tq=Tq, Tk=Tk) == -1 and bwd(Tq=Tq, Tk=Tk) == -1
-    assert fwd(causal=1) == -1 and bwd(causal=1) == -1           # causal needs Tq == Tk
-    assert fwd(ldq=312) == -1 and fwd(ldkv=312) == -1 and fwd(ldo=312) == -1  # < H * Dh = 320
-    assert fwd(ldq=324) == -2 and fwd(ldkv=324) == -2 and bwd(ldq=324) == -2  # not a multiple of 8
-    assert fwd(q=null) == -1 and fwd(lse=null) == -1 and bwd(dq=null) == -1
-    assert "null" in _cabi.last_error()
-    assert bwd(ws=null) == -1 and "workspace" in _cabi.last_error()
-    assert fwd(k=odd) == -2 and bwd(dq=odd) == -2 and bwd(ws=odd) == -2
-    assert "aligned" in _cabi.last_error()
-
-
-def _chunks(B, Tq, Tk, H, Dh):
-    rows = 128 if Dh <= 64 else 64
-    ctas = B * H * -(-Tk // rows)
-    nqb = -(-Tq // 64)
-    want = min(nqb, 1 if ctas >= 132 else 132 // ctas)
-    per = -(-nqb // want)
-    return -(-nqb // per)
-
-
-@pytest.mark.parametrize("B,Tq,Tk,H,Dh", [(8, 4096, 77, 8, 40), (1, 4096, 77, 2, 40), (8, 1024, 77, 8, 80), (8, 256, 77, 8, 160),
-                                          (8, 64, 64, 8, 160), (2, 577, 577, 12, 64), (1, 1, 1, 1, 8)])
-def test_cross_workspace_formula(B, Tq, Tk, H, Dh):
-    n = _chunks(B, Tq, Tk, H, Dh)
-    delta = -(-(B * H * Tq) // 4) * 4
-    want = delta + (2 * n * B * H * Tk * Dh if n > 1 else 0)
-    assert _cabi.lib().b200_cross_attention_bwd_workspace_floats(B, Tq, Tk, H, Dh) == want
-    if (B, Tq, Tk, H) == (1, 4096, 77, 2):
-        assert n == 64  # the determinism test's split case really is split
-    if (B, Tq, Tk, H) == (8, 4096, 77, 8):
-        assert n == 2
-
-
+# ---- 5. CPU: the module's parameters and refusals ----------------------------------------------------------------------------
 def _reference_attn_shapes():
     fx = torch.load(os.path.join(ROOT, "tests", "golden", "unet_tiny_reference.pt"), weights_only=False)
     groups = {}
