@@ -78,9 +78,11 @@ long long b200_launch_count(void);
  * Dense layers: C[M,N] = A[M,K] . B[N,K]^T on the tensor cores (wgmma: bf16 in, fp32 accumulate in registers).
  *   a_mn_major = 0: A is row-major [M, lda] (K contiguous);  1: A is row-major [K, lda] (M contiguous).
  *   b_mn_major = 0: B is row-major [N, ldb] (K contiguous);  1: B is row-major [K, ldb] (N contiguous).
- *   bias: bf16 [N] or NULL.  ldo: leading dimension (elements) of out0/out1/aux (but see the GEGLU epilogues: their
- *   out1 is dense).  N % 8 == 0.  out0 / out1 / aux 16-byte aligned.
- *   splits > 1 only with B200_EPI_PARTIAL_F32 (out0 is f32 [splits, M, ldo]).  max_ctas <= 0: all SMs.
+ *   bias: bf16 [N] or NULL, read in 16-byte groups up to roundup(N, 8) elements (the values past N never reach an output).
+ *   ldo: leading dimension (elements) of out0/out1/aux (but see the GEGLU epilogues: their out1 is dense).  Any N >= 1;
+ *   columns >= N of out0 / out1 are never written.  out0 / out1 / aux 16-byte aligned.
+ *   splits > 1 only with B200_EPI_PARTIAL_F32 (out0 is f32 [s, M, ldo] with s = min(splits, ceil(K / 64)): one split per
+ *   64-deep k-block at most; planes s .. splits - 1 are not written).  max_ctas <= 0: all SMs.
  *   ldo >= N.  out1 is required by the GELU epilogues (1, 5, 7), aux by 2, 3, 6, 8 and 9; bias is ignored by 3, 4 and 6.
  *   Operand majors (a_mn_major, b_mn_major): any with BIAS_BF16, (0, 1) with 3, 6 and 8, (1, 1) with PARTIAL_F32, else (0, 0).
  *   Every argument is checked before any tensor map is encoded.
@@ -112,7 +114,8 @@ int b200_splitk_reduce(const float* partial, int splits, long long n, float* out
 int b200_layernorm_fwd(const float* x, long long ld_x, const float* gamma, const float* beta, void* y_bf16,
                        float* y_f32 /* optional [rows, dim]: the un-rounded fp32 result */, float* mean, float* rstd,
                        int rows, int dim, float eps, cudaStream_t stream);
-/* dx_out[f32] = (dres ? dres : 0) + LN'(dy); dx_out row stride ld_dx (so the head LN can scatter into token 0).
+/* dx_out[f32] = (dres ? dres : 0) + LN'(dy); dx_out and dres (f32, optional) both have row stride ld_dx (so the head LN
+ * can scatter into token 0).
  * dy: bf16 [rows, dim].  dx_bf16 (optional) receives bf16(dx_out) -- the gradient the preceding bf16 matmul
  * output sees under autocast.  dgb_part: f32 [nparts, 2*dim] workspace ([.., 0:dim] dgamma partials, [.., dim:2dim]
  * dbeta partials), reduced by b200_colsum_finish.  Returns nparts through *nparts_out (host int).
@@ -139,7 +142,9 @@ int b200_layernorm_bf16_bwd(const void* dy_bf16, const void* x_bf16, const float
                             cudaStream_t stream);
 
 /* column sums: part[p][c] = sum over a slice of rows of x[r][c]  (x bf16 or f32), then finish() reduces the
- * parts.  Bias gradients of every Linear (autograd of customs.py:89) and LN gamma/beta gradients. */
+ * parts.  Bias gradients of every Linear (autograd of customs.py:89) and LN gamma/beta gradients.
+ * b200_colsum_bf16: ld % 8 == 0 and ld >= roundup(cols, 8); each row is read in 16-byte groups up to roundup(cols, 8)
+ * elements (the values past cols never reach a part); part is [nparts, cols] dense, nparts <= max_parts. */
 int b200_colsum_bf16(const void* x_bf16, long long ld, int rows, int cols, float* part, int max_parts,
                      int* nparts_out, cudaStream_t stream);
 int b200_colsum_finish(const float* part, long long part_ld, int nparts, int cols, float* out, int round_bf16,
