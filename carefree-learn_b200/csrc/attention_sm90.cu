@@ -1116,43 +1116,25 @@ struct AttnCall {
     const void* workspace;            // required by the streamed backward entries
 };
 
-static int attn_error(const AttnCall& c, int code, const char* what) {
-    char msg[160];
-    snprintf(msg, sizeof(msg), "%s: %s", c.entry, what);
-    return set_error(code, msg);
-}
-
 // Every argument check of the attention entries, before any tensor map is encoded: a call is refused the same way with or
 // without a device.
 static int check_attn_args(const AttnCall& c) {
     const bool packed = c.family != ATTN_CROSS, resident = c.family == ATTN_RESIDENT;
-    if (c.B <= 0 || c.H <= 0 || c.Tq <= 0 || c.Tk <= 0) return attn_error(c, B200_ERR_ARG, "non-positive size");
+    if (c.B <= 0 || c.H <= 0 || c.Tq <= 0 || c.Tk <= 0) return refuse(B200_ERR_ARG, c.entry, "non-positive size");
     const int max_t = resident ? 256 : LA_MAX_T;
-    if (c.Tq > max_t || c.Tk > max_t) return attn_error(c, B200_ERR_ARG, resident ? "T must be <= 256" : "T must be <= 16384");
-    if (packed && c.Dh != 64) return attn_error(c, B200_ERR_ARG, "head dim must be 64");
-    if (c.Dh < 8 || c.Dh > LA_MAX_DH || c.Dh % 8 != 0) return attn_error(c, B200_ERR_ARG, "head dim must be a multiple of 8 in [8, 160]");
-    if (c.causal && c.Tq != c.Tk) return attn_error(c, B200_ERR_ARG, "causal needs Tq == Tk");
+    if (c.Tq > max_t || c.Tk > max_t) return refuse(B200_ERR_ARG, c.entry, resident ? "T must be <= 256" : "T must be <= 16384");
+    if (packed && c.Dh != 64) return refuse(B200_ERR_ARG, c.entry, "head dim must be 64");
+    if (c.Dh < 8 || c.Dh > LA_MAX_DH || c.Dh % 8 != 0) return refuse(B200_ERR_ARG, c.entry, "head dim must be a multiple of 8 in [8, 160]");
+    if (c.causal && c.Tq != c.Tk) return refuse(B200_ERR_ARG, c.entry, "causal needs Tq == Tk");
     const long long width = static_cast<long long>(c.H) * c.Dh;
-    if (c.ldq < width || c.ldkv < width || c.ldo < width) return attn_error(c, B200_ERR_ARG, "leading dim < H * Dh");
-    if (c.ldq % 8 != 0 || c.ldkv % 8 != 0 || c.ldo % 8 != 0) return attn_error(c, B200_ERR_ALIGN, "leading dims must be multiples of 8");
+    if (c.ldq < width || c.ldkv < width || c.ldo < width) return refuse(B200_ERR_ARG, c.entry, "leading dim < H * Dh");
+    if (c.ldq % 8 != 0 || c.ldkv % 8 != 0 || c.ldo % 8 != 0) return refuse(B200_ERR_ALIGN, c.entry, "leading dims must be multiples of 8");
     if (!(c.q && c.k && c.v && c.out && c.lse) || (c.bwd && !(c.dout && c.dq && c.dk && c.dv)))
-        return attn_error(c, B200_ERR_ARG, "null pointer");
-    if (c.bwd && !resident && c.workspace == nullptr) return attn_error(c, B200_ERR_ARG, "workspace is required");
+        return refuse(B200_ERR_ARG, c.entry, "null pointer");
+    if (c.bwd && !resident && c.workspace == nullptr) return refuse(B200_ERR_ARG, c.entry, "workspace is required");
     // TMA bases, and the backward's 16-byte reads of out / dout
-    uintptr_t any = 0;
-    for (const void* p : {c.q, c.k, c.v, c.out, c.lse, c.dout, c.dq, c.dk, c.dv, c.dbias_part, c.workspace}) any |= reinterpret_cast<uintptr_t>(p);
-    if ((any & 15u) != 0) return attn_error(c, B200_ERR_ALIGN, "pointers must be 16-byte aligned");
-    return 0;
-}
-
-// the dynamic shared-memory attribute belongs to the (function, device) pair
-template <typename Kernel>
-static int configure_smem(Kernel kernel, int smem, bool (&configured)[64]) {
-    const int dev = current_device_slot();
-    if (configured[dev]) return 0;
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return set_error(B200_ERR_LAUNCH, cudaGetErrorString(e));
-    configured[dev] = true;
+    if (!aligned(16, {c.q, c.k, c.v, c.out, c.lse, c.dout, c.dq, c.dk, c.dv, c.dbias_part, c.workspace}))
+        return refuse(B200_ERR_ALIGN, c.entry, "pointers must be 16-byte aligned");
     return 0;
 }
 

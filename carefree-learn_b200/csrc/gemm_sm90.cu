@@ -644,7 +644,7 @@ int make_tmap(CUtensorMap* out, const void* base, int elem_bytes, int rank, cons
         es[i] = 1;
     }
     for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_bytes[i];
-    if ((reinterpret_cast<uintptr_t>(base) & 15u) != 0) return set_error(B200_ERR_ALIGN, "tensor base not 16 B aligned");
+    if (!aligned(16, {base})) return set_error(B200_ERR_ALIGN, "tensor base not 16 B aligned");
     for (int i = 0; i + 1 < rank; ++i)
         if (gstr[i] % 16 != 0) return set_error(B200_ERR_ALIGN, "tensor stride not a multiple of 16 B");
     if (const int rc = ensure_current_context()) return rc;
@@ -704,16 +704,10 @@ static int g_gemm_multicast = 0;
 template <int EPI, bool QUICK, int TA, int TB>
 static int launch_gemm_impl(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int grid, cudaStream_t stream) {
     using Cfg = GemmCfg<EPI>;
-    static bool configured[64] = {};  // the opt-in to > 48 KB of dynamic shared memory is per function AND per device
-    cudaError_t e;
-    const int dev = current_device_slot();
-    if (!configured[dev]) {
-        e = cudaFuncSetAttribute(gemm_bf16_kernel<EPI, QUICK, TA, TB>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
-        if (e != cudaSuccess) return set_error(B200_ERR_LAUNCH, cudaGetErrorString(e));
-        configured[dev] = true;
-    }
+    static bool configured[64] = {};
+    if (const int rc = configure_smem(gemm_bf16_kernel<EPI, QUICK, TA, TB>, Cfg::SMEM_BYTES, configured)) return rc;
     gemm_bf16_kernel<EPI, QUICK, TA, TB><<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
-    e = cudaGetLastError();
+    const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(B200_ERR_LAUNCH, cudaGetErrorString(e));
     count_launch(1);
     return 0;
@@ -773,27 +767,26 @@ struct ConvGeom { int B, H, W, Cin, mode; };  // mode 1: forward / input gradien
 // a device.  conv_fwd: the call comes from b200_conv3x3_nhwc_bf16.
 static int check_gemm_args(const void* A, int a_mn, const void* B, int b_mn, int M, int N, int K, int epilogue, const void* bias,
                            const void* out0, const void* out1, const void* aux, long long ldo, int splits, bool conv_fwd) {
-    if (epilogue < 0 || epilogue >= kNumEpi) return set_error(B200_ERR_ARG, "gemm: unknown epilogue");
+    if (epilogue < 0 || epilogue >= kNumEpi) return refuse(B200_ERR_ARG, "gemm", "unknown epilogue");
     const EpiTraits& e = kEpi[epilogue];
-    if (conv_fwd && !(e.entries & ENTRY_CONV3X3)) return set_error(B200_ERR_ARG, "conv3x3: epilogue not offered for convolutions");
-    if (!conv_fwd && !(e.entries & ENTRY_GEMM)) return set_error(B200_ERR_ARG, "gemm: epilogue offered by conv3x3 only");
-    if (M <= 0 || N <= 0 || K <= 0) return set_error(B200_ERR_ARG, "gemm: non-positive dimension");
+    if (conv_fwd && !(e.entries & ENTRY_CONV3X3)) return refuse(B200_ERR_ARG, "conv3x3", "epilogue not offered for convolutions");
+    if (!conv_fwd && !(e.entries & ENTRY_GEMM)) return refuse(B200_ERR_ARG, "gemm", "epilogue offered by conv3x3 only");
+    if (M <= 0 || N <= 0 || K <= 0) return refuse(B200_ERR_ARG, "gemm", "non-positive dimension");
     // N need not be a multiple of 8: the bias is read in 16-byte groups (readable up to roundup(N, 8) elements) and the
     // epilogue clips columns >= N
-    if (A == nullptr || B == nullptr || out0 == nullptr) return set_error(B200_ERR_ARG, "gemm: null pointer");
-    if (!e.partial && splits != 1) return set_error(B200_ERR_ARG, "gemm: split-K needs EPI_PARTIAL_F32");
-    if (kLaunch[epilogue][2 * a_mn + b_mn] == nullptr) return set_error(B200_ERR_ARG, "gemm: operand majors not supported by this epilogue");
-    if (e.cols != COLS_N && N % 16 != 0) return set_error(B200_ERR_ARG, "gemm: GEGLU epilogues need N = 2F with F % 8 == 0");
-    if (ldo < N) return set_error(B200_ERR_ARG, "gemm: ldo < N");
-    if (e.out1 && out1 == nullptr) return set_error(B200_ERR_ARG, "gemm: epilogue needs out1");
-    if (e.aux != AUX_NONE && aux == nullptr) return set_error(B200_ERR_ARG, "gemm: epilogue needs aux");
-    if (e.bias == BIAS_REFUSED && bias != nullptr) return set_error(B200_ERR_ARG, "gemm: epilogue takes no bias");
-    if (e.bias == BIAS_PAIR && (bias == nullptr || (reinterpret_cast<uintptr_t>(bias) & 3u) != 0))
-        return set_error(B200_ERR_ARG, "gemm: epilogue needs a 4-byte aligned bias [2F]");
+    if (A == nullptr || B == nullptr || out0 == nullptr) return refuse(B200_ERR_ARG, "gemm", "null pointer");
+    if (!e.partial && splits != 1) return refuse(B200_ERR_ARG, "gemm", "split-K needs EPI_PARTIAL_F32");
+    if (kLaunch[epilogue][2 * a_mn + b_mn] == nullptr) return refuse(B200_ERR_ARG, "gemm", "operand majors not supported by this epilogue");
+    if (e.cols != COLS_N && N % 16 != 0) return refuse(B200_ERR_ARG, "gemm", "GEGLU epilogues need N = 2F with F % 8 == 0");
+    if (ldo < N) return refuse(B200_ERR_ARG, "gemm", "ldo < N");
+    if (e.out1 && out1 == nullptr) return refuse(B200_ERR_ARG, "gemm", "epilogue needs out1");
+    if (e.aux != AUX_NONE && aux == nullptr) return refuse(B200_ERR_ARG, "gemm", "epilogue needs aux");
+    if (e.bias == BIAS_REFUSED && bias != nullptr) return refuse(B200_ERR_ARG, "gemm", "epilogue takes no bias");
+    if (e.bias == BIAS_PAIR && (bias == nullptr || !aligned(4, {bias})))
+        return refuse(B200_ERR_ARG, "gemm", "epilogue needs a 4-byte aligned bias [2F]");
     // the epilogue writes and reads with plain 16-byte global accesses: rows must start 16-byte aligned
-    if ((static_cast<unsigned long long>(ldo) * (e.out_f32 ? 4 : 2)) % 16 != 0) return set_error(B200_ERR_ALIGN, "gemm: ldo rows must be 16-byte aligned");
-    if (((reinterpret_cast<uintptr_t>(out0) | reinterpret_cast<uintptr_t>(out1) | reinterpret_cast<uintptr_t>(aux)) & 15u) != 0)
-        return set_error(B200_ERR_ALIGN, "gemm: out0 / out1 / aux not 16-byte aligned");
+    if ((static_cast<unsigned long long>(ldo) * (e.out_f32 ? 4 : 2)) % 16 != 0) return refuse(B200_ERR_ALIGN, "gemm", "ldo rows must be 16-byte aligned");
+    if (!aligned(16, {out0, out1, aux})) return refuse(B200_ERR_ALIGN, "gemm", "out0 / out1 / aux not 16-byte aligned");
     return 0;
 }
 
@@ -893,14 +886,14 @@ extern "C" int b200_gemm_bf16(const void* A, long long lda, int a_mn_major, cons
 // same call with the weights flipped and transposed ([Cin, 9 * Cout], tap (2-ky, 2-kx)).
 extern "C" int b200_conv3x3_nhwc_bf16(const void* x, const void* w_packed, const void* bias, void* out0, const void* aux, long long ldo,
                                       int B, int H, int W, int Cin, int Cout, int epilogue, cudaStream_t stream) {
-    if (B <= 0 || H <= 0 || W <= 0 || Cin <= 0 || Cout <= 0) return set_error(B200_ERR_ARG, "conv3x3: non-positive size");
-    if (Cin % BK != 0) return set_error(B200_ERR_ARG, "conv3x3: Cin must be a multiple of 64");
-    if (W > BM || BM % W != 0) return set_error(B200_ERR_ARG, "conv3x3: the image width must divide 128");
+    if (B <= 0 || H <= 0 || W <= 0 || Cin <= 0 || Cout <= 0) return refuse(B200_ERR_ARG, "conv3x3", "non-positive size");
+    if (Cin % BK != 0) return refuse(B200_ERR_ARG, "conv3x3", "Cin must be a multiple of 64");
+    if (W > BM || BM % W != 0) return refuse(B200_ERR_ARG, "conv3x3", "the image width must divide 128");
     const int hb = H < BM / W ? H : BM / W;
-    if (H % hb != 0 || BM % (W * hb) != 0) return set_error(B200_ERR_ARG, "conv3x3: H must be a multiple of 128 / W (or H * W must divide 128)");
+    if (H % hb != 0 || BM % (W * hb) != 0) return refuse(B200_ERR_ARG, "conv3x3", "H must be a multiple of 128 / W (or H * W must divide 128)");
     ConvGeom cg{B, H, W, Cin, 1};
     const long long M = static_cast<long long>(B) * H * W;
-    if (M > 0x7fffffffll) return set_error(B200_ERR_ARG, "conv3x3: too many pixels");
+    if (M > 0x7fffffffll) return refuse(B200_ERR_ARG, "conv3x3", "too many pixels");
     return gemm_dispatch(x, Cin, 0, w_packed, 9ll * Cin, 0, static_cast<int>(M), Cout, 9 * Cin, epilogue, bias, out0, nullptr, aux, ldo, 1, 0,
                          stream, &cg);
 }
@@ -912,12 +905,12 @@ extern "C" int b200_conv3x3_nhwc_bf16(const void* x, const void* w_packed, const
 // Replaces the weight half of torch's conv2d backward for convs/basic.py:155-174 under the UNet blocks (convs/residual.py:179-205).
 extern "C" int b200_conv3x3_wgrad_nhwc_bf16(const void* dy, long long ld_dy, const void* x, void* partials, int B, int H, int W, int Cin,
                                             int Cout, int splits, cudaStream_t stream) {
-    if (B <= 0 || H <= 0 || W <= 0 || Cin <= 0 || Cout <= 0) return set_error(B200_ERR_ARG, "conv3x3 wgrad: non-positive size");
-    if (Cin % 64 != 0) return set_error(B200_ERR_ARG, "conv3x3 wgrad: Cin must be a multiple of 64");
-    if (W > BK || BK % W != 0) return set_error(B200_ERR_ARG, "conv3x3 wgrad: the image width must divide 64");
-    if ((static_cast<long long>(H) * W) % BK != 0) return set_error(B200_ERR_ARG, "conv3x3 wgrad: H * W must be a multiple of 64");
+    if (B <= 0 || H <= 0 || W <= 0 || Cin <= 0 || Cout <= 0) return refuse(B200_ERR_ARG, "conv3x3 wgrad", "non-positive size");
+    if (Cin % 64 != 0) return refuse(B200_ERR_ARG, "conv3x3 wgrad", "Cin must be a multiple of 64");
+    if (W > BK || BK % W != 0) return refuse(B200_ERR_ARG, "conv3x3 wgrad", "the image width must divide 64");
+    if ((static_cast<long long>(H) * W) % BK != 0) return refuse(B200_ERR_ARG, "conv3x3 wgrad", "H * W must be a multiple of 64");
     const long long K = static_cast<long long>(B) * H * W;
-    if (K > 0x7fffffffll) return set_error(B200_ERR_ARG, "conv3x3 wgrad: too many pixels");
+    if (K > 0x7fffffffll) return refuse(B200_ERR_ARG, "conv3x3 wgrad", "too many pixels");
     ConvGeom cg{B, H, W, Cin, 2};
     return gemm_dispatch(dy, ld_dy, 1, x, Cin, 1, Cout, 9 * Cin, static_cast<int>(K), EPI_PARTIAL_F32, nullptr, partials, nullptr, nullptr,
                          9ll * Cin, splits, 0, stream, &cg);

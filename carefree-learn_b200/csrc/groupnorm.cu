@@ -279,9 +279,9 @@ __global__ void __launch_bounds__(GN_THREADS) gn_bwd_apply_kernel(const __nv_bfl
     *reinterpret_cast<uint4*>(dx + i * 8) = w;
 }
 
-static int gn_check(int B, int HW, int C) {
-    if (B <= 0 || HW <= 0 || C <= 0) return set_error(B200_ERR_ARG, "groupnorm: non-positive size");
-    if (C % 8 != 0 || C % GN_GROUPS != 0 || C > GN_MAX_C) return set_error(B200_ERR_ARG, "groupnorm: need C % 32 == 0 and C <= 2560");
+static int gn_check(const char* entry, int B, int HW, int C) {
+    if (B <= 0 || HW <= 0 || C <= 0) return refuse(B200_ERR_ARG, entry, "non-positive size");
+    if (C % 8 != 0 || C % GN_GROUPS != 0 || C > GN_MAX_C) return refuse(B200_ERR_ARG, entry, "need C % 32 == 0 and C <= 2560");
     return 0;
 }
 
@@ -312,10 +312,12 @@ extern "C" long long b200_groupnorm_workspace_floats(int B, int HW, int C) {
 
 extern "C" int b200_groupnorm_silu_fwd(const void* x_bf16, const float* gamma, const float* beta, void* y_bf16, float* mean, float* rstd,
                                        float* workspace, int B, int HW, int C, float eps, int silu, cudaStream_t stream) {
-    int rc = gn_check(B, HW, C);
+    const char* E = "groupnorm_fwd";
+    int rc = gn_check(E, B, HW, C);
     if (rc) return rc;
-    if (x_bf16 == nullptr || y_bf16 == nullptr || mean == nullptr || rstd == nullptr || workspace == nullptr)
-        return set_error(B200_ERR_ARG, "groupnorm_fwd: null pointer");
+    if (!x_bf16 || !gamma || !beta || !y_bf16 || !mean || !rstd || !workspace) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(16, {x_bf16, y_bf16})) return refuse(B200_ERR_ALIGN, E, "x / y not 16-byte aligned");
+    if (!aligned(4, {gamma, beta, mean, rstd, workspace})) return refuse(B200_ERR_ALIGN, E, "gamma / beta / mean / rstd / workspace not 4-byte aligned");
     const int nslab = gn_slabs(B, HW);
     const int pps = (HW + nslab - 1) / nslab;
     const __nv_bfloat16* x = reinterpret_cast<const __nv_bfloat16*>(x_bf16);
@@ -333,10 +335,14 @@ extern "C" int b200_groupnorm_silu_fwd(const void* x_bf16, const float* gamma, c
 extern "C" int b200_groupnorm_silu_bwd(const void* x_bf16, const void* dy_bf16, const float* gamma, const float* beta, const float* mean,
                                        const float* rstd, void* dx_bf16, float* dgamma, float* dbeta, float* workspace, int B, int HW, int C,
                                        int silu, int accumulate, cudaStream_t stream) {
-    int rc = gn_check(B, HW, C);
+    const char* E = "groupnorm_bwd";
+    int rc = gn_check(E, B, HW, C);
     if (rc) return rc;
-    if (x_bf16 == nullptr || dy_bf16 == nullptr || dx_bf16 == nullptr || dgamma == nullptr || dbeta == nullptr || workspace == nullptr)
-        return set_error(B200_ERR_ARG, "groupnorm_bwd: null pointer");
+    if (!x_bf16 || !dy_bf16 || !gamma || !beta || !mean || !rstd || !dx_bf16 || !dgamma || !dbeta || !workspace)
+        return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(16, {x_bf16, dy_bf16, dx_bf16})) return refuse(B200_ERR_ALIGN, E, "x / dy / dx not 16-byte aligned");
+    if (!aligned(4, {gamma, beta, mean, rstd, dgamma, dbeta, workspace}))
+        return refuse(B200_ERR_ALIGN, E, "gamma / beta / mean / rstd / dgamma / dbeta / workspace not 4-byte aligned");
     const int nslab = gn_slabs(B, HW);
     const int pps = (HW + nslab - 1) / nslab;
     float* part_g = workspace;

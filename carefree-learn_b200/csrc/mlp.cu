@@ -134,14 +134,17 @@ extern "C" int b200_fcnn_step(const float* x, const float* y, const float* dpred
                               float* part, int M, int n_layers, const int* dims, const int* w_offsets,
                               const int* b_offsets, int arena_len, int loss_mode, float w_mae, float w_mse,
                               int* nblocks_out, cudaStream_t stream) {
-    if (M <= 0 || n_layers < 1 || n_layers > MLP_MAX_L || arena_len <= 0) return set_error(B200_ERR_ARG, "fcnn_step: need 1 <= layers <= 8 and M > 0");
-    if (part != nullptr && loss_mode == 0 && dpred == nullptr) return set_error(B200_ERR_ARG, "fcnn_step: backward without a loss needs dpred");
-    if (part != nullptr && loss_mode == 1 && y == nullptr) return set_error(B200_ERR_ARG, "fcnn_step: the fused loss needs labels");
+    const char* E = "fcnn_step";
+    if (M <= 0 || n_layers < 1 || n_layers > MLP_MAX_L || arena_len <= 0) return refuse(B200_ERR_ARG, E, "need 1 <= layers <= 8 and M > 0");
+    if (!x || !params || !dims || !w_offsets || !b_offsets) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (part != nullptr && loss_mode == 0 && dpred == nullptr) return refuse(B200_ERR_ARG, E, "backward without a loss needs dpred (null pointer)");
+    if (part != nullptr && loss_mode == 1 && y == nullptr) return refuse(B200_ERR_ARG, E, "the fused loss needs labels (null pointer)");
+    if (!aligned(4, {x, y, dpred, params, pred, part})) return refuse(B200_ERR_ALIGN, E, "pointers not 4-byte aligned");
     MlpParams p;
     p.M = M; p.L = n_layers; p.P = arena_len; p.loss_mode = loss_mode; p.w_mae = w_mae; p.w_mse = w_mse;
     int aoff = 0;
     for (int l = 0; l <= n_layers; ++l) {
-        if (dims[l] <= 0) return set_error(B200_ERR_ARG, "fcnn_step: non-positive layer width");
+        if (dims[l] <= 0) return refuse(B200_ERR_ARG, E, "non-positive layer width");
         p.dims[l] = dims[l];
         p.aoff[l] = aoff;
         aoff += dims[l] * MLP_LD;
@@ -150,10 +153,10 @@ extern "C" int b200_fcnn_step(const float* x, const float* y, const float* dpred
         p.woff[l] = w_offsets[l];
         p.boff[l] = b_offsets[l];
         if (p.woff[l] < 0 || p.woff[l] + dims[l] * dims[l + 1] > arena_len || (p.boff[l] >= 0 && p.boff[l] + dims[l + 1] > arena_len))
-            return set_error(B200_ERR_ARG, "fcnn_step: parameter offsets outside the arena");
+            return refuse(B200_ERR_ARG, E, "parameter offsets outside the arena");
     }
     const size_t smem = (static_cast<size_t>(arena_len) + aoff) * sizeof(float);
-    if (smem > 220 * 1024) return set_error(B200_ERR_ARG, "fcnn_step: network too wide for the fused shared-memory kernel (parameters + activations > 220 KB)");
+    if (smem > 220 * 1024) return refuse(B200_ERR_ARG, E, "network too wide for the fused shared-memory kernel (parameters + activations > 220 KB)");
     if (smem > 48 * 1024) {
         cudaError_t e = cudaFuncSetAttribute(mlp_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
         if (e != cudaSuccess) return set_error(B200_ERR_LAUNCH, cudaGetErrorString(e));

@@ -9,6 +9,7 @@
 #include <string.h>
 
 #include <atomic>
+#include <type_traits>
 
 #include "b200_internal.h"
 #include "ptx.cuh"
@@ -24,6 +25,11 @@ static std::atomic<long long> g_launches{0};
 int set_error(int code, const char* msg) {
     snprintf(g_err, sizeof(g_err), "%s", msg ? msg : "");
     return code;
+}
+int refuse(int code, const char* entry, const char* rule) {
+    char msg[256];
+    snprintf(msg, sizeof(msg), "%s: %s", entry, rule);
+    return set_error(code, msg);
 }
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 int check_launch(const char* what) {
@@ -960,136 +966,141 @@ __global__ void adam_dev_kernel(float* __restrict__ p, const float* __restrict__
     reinterpret_cast<float4*>(v)[i] = vv;
 }
 
-template <int NV>
-static int ln_fwd_launch(const float* x, long long ld_x, const float* gamma, const float* beta, void* y, float* y32,
-                         float* mean, float* rstd, int rows, int dim, float eps, cudaStream_t st) {
-    const int blocks = (rows + 7) / 8;
-    layernorm_fwd_kernel<NV><<<blocks, 256, 0, st>>>(x, ld_x, gamma, beta, reinterpret_cast<__nv_bfloat16*>(y), y32,
-                                                     mean, rstd, rows, dim, eps);
-    return check_launch("layernorm_fwd");
+// The row-width ladders of the two LayerNorm families: launch(std::integral_constant<int, NV>) with the fewest 16-byte chunks per
+// lane that hold a row (fp32 rows: dim <= 128 * NV; bf16 rows: dim <= 256 * NV)
+template <typename Launch>
+static int ln_dispatch(int dim, Launch launch) {
+    const int nv = (dim + 127) / 128;
+    if (nv <= 4) return launch(std::integral_constant<int, 4>());
+    if (nv <= 6) return launch(std::integral_constant<int, 6>());
+    return launch(std::integral_constant<int, 8>());
 }
+template <typename Launch>
+static int lnb_dispatch(int dim, Launch launch) {
+    const int nv = (dim + 255) / 256;
+    if (nv <= 2) return launch(std::integral_constant<int, 2>());
+    if (nv <= 4) return launch(std::integral_constant<int, 4>());
+    if (nv <= 5) return launch(std::integral_constant<int, 5>());
+    return launch(std::integral_constant<int, 8>());
+}
+
+// grid of the LayerNorm backwards (= partial rows written): two resident 256-thread blocks per SM (one wave), at most one block per
+// 8 rows and at most max_parts
+static int ln_bwd_parts(int rows, int max_parts) {
+    int nparts = num_sms() * 2;
+    if (nparts > (rows + 7) / 8) nparts = (rows + 7) / 8;
+    return nparts < max_parts ? nparts : max_parts;
+}
+
 template <int NV, bool DXSUM, bool DYF32>
-static int ln_bwd_launch2(const void* dy, const float* x, long long ld_x, const float* gamma, const float* mean,
-                          const float* rstd, const float* dres, float* dx_out, long long ld_dx, void* dx_bf16,
-                          float* part, int nparts, int rows, int dim, cudaStream_t st) {
-    const size_t smem = static_cast<size_t>(8) * (DXSUM ? 3 : 2) * dim * sizeof(float);
-    if (smem > 48 * 1024) {
-        cudaFuncSetAttribute(layernorm_bwd_kernel<NV, DXSUM, DYF32>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    }
-    layernorm_bwd_kernel<NV, DXSUM, DYF32><<<nparts, 256, smem, st>>>(dy, x, ld_x, gamma, mean,
-                                                               rstd, dres, dx_out, ld_dx,
-                                                               reinterpret_cast<__nv_bfloat16*>(dx_bf16), part, rows, dim);
+static int ln_bwd_launch(const void* dy, const float* x, long long ld_x, const float* gamma, const float* mean, const float* rstd,
+                         const float* dres, float* dx_out, long long ld_dx, void* dx_bf16, float* part, int nparts, int rows, int dim,
+                         cudaStream_t st) {
+    constexpr int NP = DXSUM ? 3 : 2;
+    static bool configured[64] = {};
+    if (const int rc = configure_smem(layernorm_bwd_kernel<NV, DXSUM, DYF32>, 8 * NP * 128 * NV * 4, configured)) return rc;
+    layernorm_bwd_kernel<NV, DXSUM, DYF32><<<nparts, 256, static_cast<size_t>(8) * NP * dim * sizeof(float), st>>>(
+        dy, x, ld_x, gamma, mean, rstd, dres, dx_out, ld_dx, reinterpret_cast<__nv_bfloat16*>(dx_bf16), part, rows, dim);
     return check_launch("layernorm_bwd");
 }
-template <int NV>
-static int ln_bwd_launch(const void* dy, const float* x, long long ld_x, const float* gamma, const float* mean,
-                         const float* rstd, const float* dres, float* dx_out, long long ld_dx, void* dx_bf16,
-                         float* part, int nparts, int rows, int dim, bool dxsum, bool dyf32, cudaStream_t st) {
-    if (dyf32) return ln_bwd_launch2<NV, false, true>(dy, x, ld_x, gamma, mean, rstd, dres, dx_out, ld_dx, dx_bf16, part, nparts, rows, dim, st);
-    if (dxsum) return ln_bwd_launch2<NV, true, false>(dy, x, ld_x, gamma, mean, rstd, dres, dx_out, ld_dx, dx_bf16, part, nparts, rows, dim, st);
-    return ln_bwd_launch2<NV, false, false>(dy, x, ld_x, gamma, mean, rstd, dres, dx_out, ld_dx, dx_bf16, part, nparts, rows, dim, st);
-}
 
-template <int NV>
-static int lnb_fwd_launch(const void* x, const float* gamma, const float* beta, void* y, float* mean, float* rstd, int rows, int dim,
-                          float eps, cudaStream_t st) {
-    layernorm_bf16_fwd_kernel<NV><<<(rows + 7) / 8, 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(x), gamma, beta,
-                                                                   reinterpret_cast<__nv_bfloat16*>(y), mean, rstd, rows, dim, eps);
-    return check_launch("layernorm_bf16_fwd");
-}
-template <int NV>
-static int lnb_bwd_launch(const void* dy, const void* x, const float* gamma, const float* mean, const float* rstd, const void* dres,
-                          void* dx, float* part, int nparts, int rows, int dim, cudaStream_t st) {
-    const size_t smem = static_cast<size_t>(8) * 2 * dim * sizeof(float);
-    if (smem > 48 * 1024) cudaFuncSetAttribute(layernorm_bf16_bwd_kernel<NV>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    layernorm_bf16_bwd_kernel<NV><<<nparts, 256, smem, st>>>(
-        reinterpret_cast<const __nv_bfloat16*>(dy), reinterpret_cast<const __nv_bfloat16*>(x), gamma, mean, rstd,
-        reinterpret_cast<const __nv_bfloat16*>(dres), reinterpret_cast<__nv_bfloat16*>(dx), part, rows, dim);
-    return check_launch("layernorm_bf16_bwd");
-}
-
-static bool misaligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) != 0; }
+// products of sizes that a kernel indexes in 32-bit int
+static bool int_overflow(long long a, long long b) { return a * b > 0x7fffffffll; }
 
 }  // namespace b200
 
 using namespace b200;
 
 extern "C" int b200_abi_version(void) { return B200_ABI_VERSION; }
+extern "C" const char* b200_last_error(void) { return g_err; }
+extern "C" long long b200_launch_count(void) { return g_launches.load(); }
 
 extern "C" int b200_layernorm_bf16_fwd(const void* x, const float* gamma, const float* beta, void* y, float* mean, float* rstd, int rows,
                                        int dim, float eps, cudaStream_t stream) {
-    if (rows <= 0 || dim <= 0 || dim % 8 != 0 || dim > 256 * LNB_MAX_V8)
-        return set_error(B200_ERR_ARG, "layernorm_bf16_fwd: need rows > 0, 0 < dim <= 2048, dim % 8 == 0");
-    if (!x || !gamma || !beta || !y || !mean || !rstd) return set_error(B200_ERR_ARG, "layernorm_bf16_fwd: null pointer");
-    if (misaligned16(x) || misaligned16(gamma) || misaligned16(beta) || misaligned16(y))
-        return set_error(B200_ERR_ALIGN, "layernorm_bf16_fwd: x / gamma / beta / y not 16-byte aligned");
-    const int nv = (dim + 255) / 256;
-    if (nv <= 2) return lnb_fwd_launch<2>(x, gamma, beta, y, mean, rstd, rows, dim, eps, stream);
-    if (nv <= 4) return lnb_fwd_launch<4>(x, gamma, beta, y, mean, rstd, rows, dim, eps, stream);
-    if (nv <= 5) return lnb_fwd_launch<5>(x, gamma, beta, y, mean, rstd, rows, dim, eps, stream);
-    return lnb_fwd_launch<8>(x, gamma, beta, y, mean, rstd, rows, dim, eps, stream);
+    const char* E = "layernorm_bf16_fwd";
+    if (rows <= 0 || dim <= 0 || dim % 8 != 0 || dim > 256 * LNB_MAX_V8) return refuse(B200_ERR_ARG, E, "need rows > 0, 0 < dim <= 2048, dim % 8 == 0");
+    if (!x || !gamma || !beta || !y || !mean || !rstd) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(16, {x, gamma, beta, y})) return refuse(B200_ERR_ALIGN, E, "x / gamma / beta / y not 16-byte aligned");
+    if (!aligned(4, {mean, rstd})) return refuse(B200_ERR_ALIGN, E, "mean / rstd not 4-byte aligned");
+    return lnb_dispatch(dim, [&](auto nv) {
+        layernorm_bf16_fwd_kernel<decltype(nv)::value><<<(rows + 7) / 8, 256, 0, stream>>>(
+            reinterpret_cast<const __nv_bfloat16*>(x), gamma, beta, reinterpret_cast<__nv_bfloat16*>(y), mean, rstd, rows, dim, eps);
+        return check_launch("layernorm_bf16_fwd");
+    });
 }
 
 extern "C" int b200_layernorm_bf16_bwd(const void* dy, const void* x, const float* gamma, const float* mean, const float* rstd,
                                        const void* dres, void* dx, float* dgb_part, int max_parts, int* nparts_out, int rows, int dim,
                                        cudaStream_t stream) {
-    if (rows <= 0 || dim <= 0 || dim % 8 != 0 || dim > 256 * LNB_MAX_V8)
-        return set_error(B200_ERR_ARG, "layernorm_bf16_bwd: need rows > 0, 0 < dim <= 2048, dim % 8 == 0");
-    if (!dy || !x || !gamma || !mean || !rstd || !dx || !dgb_part) return set_error(B200_ERR_ARG, "layernorm_bf16_bwd: null pointer");
-    if (max_parts < 1) return set_error(B200_ERR_ARG, "layernorm_bf16_bwd: max_parts < 1");
-    if (misaligned16(dy) || misaligned16(x) || misaligned16(gamma) || misaligned16(dx) || (dres != nullptr && misaligned16(dres)))
-        return set_error(B200_ERR_ALIGN, "layernorm_bf16_bwd: dy / x / gamma / dres / dx not 16-byte aligned");
-    int nparts = num_sms() * 2;
-    const int need = (rows + 7) / 8;
-    if (nparts > need) nparts = need;
-    if (nparts > max_parts) nparts = max_parts;
+    const char* E = "layernorm_bf16_bwd";
+    if (rows <= 0 || dim <= 0 || dim % 8 != 0 || dim > 256 * LNB_MAX_V8) return refuse(B200_ERR_ARG, E, "need rows > 0, 0 < dim <= 2048, dim % 8 == 0");
+    if (max_parts < 1) return refuse(B200_ERR_ARG, E, "max_parts < 1");
+    if (!dy || !x || !gamma || !mean || !rstd || !dx || !dgb_part) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(16, {dy, x, gamma, dres, dx})) return refuse(B200_ERR_ALIGN, E, "dy / x / gamma / dres / dx not 16-byte aligned");
+    if (!aligned(4, {mean, rstd, dgb_part})) return refuse(B200_ERR_ALIGN, E, "mean / rstd / dgb_part not 4-byte aligned");
+    const int nparts = ln_bwd_parts(rows, max_parts);
     if (nparts_out) *nparts_out = nparts;
-    const int nv = (dim + 255) / 256;
-    if (nv <= 2) return lnb_bwd_launch<2>(dy, x, gamma, mean, rstd, dres, dx, dgb_part, nparts, rows, dim, stream);
-    if (nv <= 4) return lnb_bwd_launch<4>(dy, x, gamma, mean, rstd, dres, dx, dgb_part, nparts, rows, dim, stream);
-    if (nv <= 5) return lnb_bwd_launch<5>(dy, x, gamma, mean, rstd, dres, dx, dgb_part, nparts, rows, dim, stream);
-    return lnb_bwd_launch<8>(dy, x, gamma, mean, rstd, dres, dx, dgb_part, nparts, rows, dim, stream);
+    return lnb_dispatch(dim, [&](auto nv) {
+        constexpr int NV = decltype(nv)::value;
+        static bool configured[64] = {};
+        if (const int rc = configure_smem(layernorm_bf16_bwd_kernel<NV>, 8 * 2 * 256 * NV * 4, configured)) return rc;
+        layernorm_bf16_bwd_kernel<NV><<<nparts, 256, static_cast<size_t>(8) * 2 * dim * sizeof(float), stream>>>(
+            reinterpret_cast<const __nv_bfloat16*>(dy), reinterpret_cast<const __nv_bfloat16*>(x), gamma, mean, rstd,
+            reinterpret_cast<const __nv_bfloat16*>(dres), reinterpret_cast<__nv_bfloat16*>(dx), dgb_part, rows, dim);
+        return check_launch("layernorm_bf16_bwd");
+    });
 }
-extern "C" const char* b200_last_error(void) { return g_err; }
-extern "C" long long b200_launch_count(void) { return g_launches.load(); }
 
 extern "C" int b200_layernorm_fwd(const float* x, long long ld_x, const float* gamma, const float* beta, void* y_bf16,
                                   float* y_f32, float* mean, float* rstd, int rows, int dim, float eps,
                                   cudaStream_t stream) {
-    if (rows <= 0 || dim <= 0 || dim % 4 != 0 || dim > 128 * LN_MAX_V4) return set_error(B200_ERR_ARG, "layernorm_fwd: need 0 < dim <= 1024, dim % 4 == 0");
-    if (ld_x % 4 != 0) return set_error(B200_ERR_ALIGN, "layernorm_fwd: ld_x % 4 != 0");
-    const int nv = (dim + 127) / 128;
-    if (nv <= 4) return ln_fwd_launch<4>(x, ld_x, gamma, beta, y_bf16, y_f32, mean, rstd, rows, dim, eps, stream);
-    if (nv <= 6) return ln_fwd_launch<6>(x, ld_x, gamma, beta, y_bf16, y_f32, mean, rstd, rows, dim, eps, stream);
-    return ln_fwd_launch<8>(x, ld_x, gamma, beta, y_bf16, y_f32, mean, rstd, rows, dim, eps, stream);
+    const char* E = "layernorm_fwd";
+    if (rows <= 0 || dim <= 0 || dim % 4 != 0 || dim > 128 * LN_MAX_V4) return refuse(B200_ERR_ARG, E, "need rows > 0, 0 < dim <= 1024, dim % 4 == 0");
+    if (!x || !gamma || !beta || !y_bf16 || !mean || !rstd) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (ld_x < dim) return refuse(B200_ERR_ARG, E, "ld_x < dim");
+    if (ld_x % 4 != 0) return refuse(B200_ERR_ALIGN, E, "ld_x % 4 != 0");
+    if (!aligned(16, {x, gamma, beta, y_bf16, y_f32})) return refuse(B200_ERR_ALIGN, E, "x / gamma / beta / y_bf16 / y_f32 not 16-byte aligned");
+    if (!aligned(4, {mean, rstd})) return refuse(B200_ERR_ALIGN, E, "mean / rstd not 4-byte aligned");
+    return ln_dispatch(dim, [&](auto nv) {
+        layernorm_fwd_kernel<decltype(nv)::value><<<(rows + 7) / 8, 256, 0, stream>>>(
+            x, ld_x, gamma, beta, reinterpret_cast<__nv_bfloat16*>(y_bf16), y_f32, mean, rstd, rows, dim, eps);
+        return check_launch("layernorm_fwd");
+    });
 }
 
 extern "C" int b200_layernorm_bwd(const void* dy, int dy_is_f32, const float* x, long long ld_x, const float* gamma,
                                   const float* mean, const float* rstd, const float* dres, float* dx_out,
                                   long long ld_dx, void* dx_bf16, float* dgb_part, int max_parts, int* nparts_out,
                                   int rows, int dim, int dx_colsum, cudaStream_t stream) {
-    if (rows <= 0 || dim <= 0 || dim % 4 != 0 || dim > 128 * LN_MAX_V4) return set_error(B200_ERR_ARG, "layernorm_bwd: need 0 < dim <= 1024, dim % 4 == 0");
-    if (ld_x % 4 != 0 || ld_dx % 4 != 0) return set_error(B200_ERR_ALIGN, "layernorm_bwd: ld % 4 != 0");
-    if (max_parts < 1) return set_error(B200_ERR_ARG, "layernorm_bwd: max_parts < 1");
-    if (dx_colsum && dx_bf16 == nullptr) return set_error(B200_ERR_ARG, "layernorm_bwd: dx_colsum needs dx_bf16");
-    if (dx_colsum && dy_is_f32) return set_error(B200_ERR_ARG, "layernorm_bwd: dx_colsum is not offered with an fp32 dy");
-    const bool dyf = dy_is_f32 != 0;
-    const bool dxs = dx_colsum != 0;
-    int nparts = num_sms() * 2  /* two resident 256-thread blocks per SM: one wave */;
-    const int need = (rows + 7) / 8;
-    if (nparts > need) nparts = need;
-    if (nparts > max_parts) nparts = max_parts;
+    const char* E = "layernorm_bwd";
+    if (rows <= 0 || dim <= 0 || dim % 4 != 0 || dim > 128 * LN_MAX_V4) return refuse(B200_ERR_ARG, E, "need rows > 0, 0 < dim <= 1024, dim % 4 == 0");
+    if (max_parts < 1) return refuse(B200_ERR_ARG, E, "max_parts < 1");
+    if (dx_colsum && dy_is_f32) return refuse(B200_ERR_ARG, E, "dx_colsum is not offered with an fp32 dy");
+    if (!dy || !x || !gamma || !mean || !rstd || !dx_out || !dgb_part) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (dx_colsum && dx_bf16 == nullptr) return refuse(B200_ERR_ARG, E, "dx_colsum needs dx_bf16 (null pointer)");
+    if (ld_x < dim || ld_dx < dim) return refuse(B200_ERR_ARG, E, "ld_x / ld_dx < dim");
+    if (ld_x % 4 != 0 || ld_dx % 4 != 0) return refuse(B200_ERR_ALIGN, E, "ld % 4 != 0");
+    if (!aligned(16, {dy, x, gamma, dres, dx_out, dx_bf16})) return refuse(B200_ERR_ALIGN, E, "dy / x / gamma / dres / dx_out / dx_bf16 not 16-byte aligned");
+    if (!aligned(4, {mean, rstd, dgb_part})) return refuse(B200_ERR_ALIGN, E, "mean / rstd / dgb_part not 4-byte aligned");
+    const int nparts = ln_bwd_parts(rows, max_parts);
     if (nparts_out) *nparts_out = nparts;
-    const int nv = (dim + 127) / 128;
-    if (nv <= 4) return ln_bwd_launch<4>(dy, x, ld_x, gamma, mean, rstd, dres, dx_out, ld_dx, dx_bf16, dgb_part, nparts, rows, dim, dxs, dyf, stream);
-    if (nv <= 6) return ln_bwd_launch<6>(dy, x, ld_x, gamma, mean, rstd, dres, dx_out, ld_dx, dx_bf16, dgb_part, nparts, rows, dim, dxs, dyf, stream);
-    return ln_bwd_launch<8>(dy, x, ld_x, gamma, mean, rstd, dres, dx_out, ld_dx, dx_bf16, dgb_part, nparts, rows, dim, dxs, dyf, stream);
+    return ln_dispatch(dim, [&](auto nv) {
+        constexpr int NV = decltype(nv)::value;
+        if (dy_is_f32) return ln_bwd_launch<NV, false, true>(dy, x, ld_x, gamma, mean, rstd, dres, dx_out, ld_dx, dx_bf16, dgb_part, nparts, rows, dim, stream);
+        if (dx_colsum) return ln_bwd_launch<NV, true, false>(dy, x, ld_x, gamma, mean, rstd, dres, dx_out, ld_dx, dx_bf16, dgb_part, nparts, rows, dim, stream);
+        return ln_bwd_launch<NV, false, false>(dy, x, ld_x, gamma, mean, rstd, dres, dx_out, ld_dx, dx_bf16, dgb_part, nparts, rows, dim, stream);
+    });
 }
 
 extern "C" int b200_colsum_bf16(const void* x_bf16, long long ld, int rows, int cols, float* part, int max_parts,
                                 int* nparts_out, cudaStream_t stream) {
-    if (rows <= 0 || cols <= 0 || ld % 8 != 0 || ld < (cols + 7) / 8 * 8) return set_error(B200_ERR_ARG, "colsum: ld must be a multiple of 8 and >= roundup(cols, 8)");
-    if (max_parts < 1) return set_error(B200_ERR_ARG, "colsum: max_parts < 1");
+    const char* E = "colsum";
+    if (rows <= 0 || cols <= 0 || max_parts < 1) return refuse(B200_ERR_ARG, E, "need rows, cols > 0 and max_parts >= 1");
+    if (!x_bf16 || !part) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (ld < (cols + 7) / 8 * 8) return refuse(B200_ERR_ARG, E, "ld must be >= roundup(cols, 8)");
+    if (ld % 8 != 0) return refuse(B200_ERR_ALIGN, E, "ld must be a multiple of 8");
+    if (!aligned(16, {x_bf16})) return refuse(B200_ERR_ALIGN, E, "x not 16-byte aligned");
+    if (!aligned(4, {part})) return refuse(B200_ERR_ALIGN, E, "part not 4-byte aligned");
     const int chunks = (cols + 255) / 256;
     int slices = (num_sms() * 4) / chunks;
     if (slices < 1) slices = 1;
@@ -1102,14 +1113,22 @@ extern "C" int b200_colsum_bf16(const void* x_bf16, long long ld, int rows, int 
 
 extern "C" int b200_colsum_finish(const float* part, long long part_ld, int nparts, int cols, float* out, int round_bf16,
                                   int accumulate, cudaStream_t stream) {
-    if (nparts <= 0 || cols <= 0 || part_ld < cols) return set_error(B200_ERR_ARG, "colsum_finish: bad size");
+    const char* E = "colsum_finish";
+    if (nparts <= 0 || cols <= 0) return refuse(B200_ERR_ARG, E, "bad size");
+    if (!part || !out) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (part_ld < cols) return refuse(B200_ERR_ARG, E, "part_ld < cols");
+    if (!aligned(4, {part, out})) return refuse(B200_ERR_ALIGN, E, "part / out not 4-byte aligned");
     colsum_finish_kernel<<<(cols + 31) / 32, dim3(32, 8), 0, stream>>>(part, part_ld, nparts, cols, out, round_bf16, accumulate);
     return check_launch("colsum_finish");
 }
 
 extern "C" int b200_colsum_finish2(const float* part, long long part_ld, int nparts, int cols0, float* out0, int round0,
                                    int cols1, float* out1, int round1, int accumulate, cudaStream_t stream) {
-    if (nparts <= 0 || cols0 <= 0 || cols1 <= 0 || part_ld < cols0 + cols1) return set_error(B200_ERR_ARG, "colsum_finish2: bad size");
+    const char* E = "colsum_finish2";
+    if (nparts <= 0 || cols0 <= 0 || cols1 <= 0) return refuse(B200_ERR_ARG, E, "bad size");
+    if (!part || !out0 || !out1) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (part_ld < static_cast<long long>(cols0) + cols1) return refuse(B200_ERR_ARG, E, "part_ld < cols0 + cols1");
+    if (!aligned(4, {part, out0, out1})) return refuse(B200_ERR_ALIGN, E, "part / out0 / out1 not 4-byte aligned");
     colsum_finish2_kernel<<<(cols0 + cols1 + 31) / 32, dim3(32, 8), 0, stream>>>(part, part_ld, nparts, cols0, out0, round0, cols1, out1, round1, accumulate);
     return check_launch("colsum_finish2");
 }
@@ -1130,11 +1149,12 @@ extern "C" long long b200_colsum_per_image_workspace_floats(int B, int HW, int C
 
 extern "C" int b200_colsum_per_image_bf16(const void* x_bf16, int B, int HW, int C, void* per_image_bf16, float* total, float* workspace,
                                           cudaStream_t stream) {
-    if (B <= 0 || HW <= 0 || C <= 0 || C % 8 != 0) return set_error(B200_ERR_ARG, "colsum_per_image: need B, HW > 0 and C a positive multiple of 8");
-    if (static_cast<long long>(B) * HW > 0x7fffffffll) return set_error(B200_ERR_ARG, "colsum_per_image: too many rows");
-    if (x_bf16 == nullptr || per_image_bf16 == nullptr || total == nullptr || workspace == nullptr)
-        return set_error(B200_ERR_ARG, "colsum_per_image: null pointer");
-    if ((reinterpret_cast<uintptr_t>(x_bf16) & 15u) != 0) return set_error(B200_ERR_ALIGN, "colsum_per_image: x not 16-byte aligned");
+    const char* E = "colsum_per_image";
+    if (B <= 0 || HW <= 0 || C <= 0 || C % 8 != 0) return refuse(B200_ERR_ARG, E, "need B, HW > 0 and C a positive multiple of 8");
+    if (int_overflow(B, HW)) return refuse(B200_ERR_ARG, E, "too many rows");
+    if (!x_bf16 || !per_image_bf16 || !total || !workspace) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(16, {x_bf16})) return refuse(B200_ERR_ALIGN, E, "x not 16-byte aligned");
+    if (!aligned(4, {per_image_bf16, total, workspace})) return refuse(B200_ERR_ALIGN, E, "per_image / total / workspace not 4-byte aligned");
     const int slices = colsum_per_image_slices(B, HW, C);
     colsum_per_image_kernel<<<dim3((C + 255) / 256, slices, B), dim3(32, 8), 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(x_bf16), HW, C,
                                                                                          workspace);
@@ -1146,14 +1166,20 @@ extern "C" int b200_colsum_per_image_bf16(const void* x_bf16, int B, int HW, int
 
 extern "C" int b200_splitk_reduce(const float* partial, int splits, long long n, float* out, int round_bf16,
                                   int accumulate, cudaStream_t stream) {
-    if (splits < 1 || n <= 0 || n % 4 != 0) return set_error(B200_ERR_ARG, "splitk_reduce: n must be a positive multiple of 4");
+    const char* E = "splitk_reduce";
+    if (splits < 1 || n <= 0 || n % 4 != 0) return refuse(B200_ERR_ARG, E, "need splits >= 1 and n a positive multiple of 4");
+    if (!partial || !out) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(16, {partial, out})) return refuse(B200_ERR_ALIGN, E, "partial / out not 16-byte aligned");
     const long long n4 = n / 4;
     splitk_reduce_kernel<<<static_cast<unsigned>((n4 + 255) / 256), 256, 0, stream>>>(partial, splits, n4, out, round_bf16, accumulate);
     return check_launch("splitk_reduce");
 }
 
 extern "C" int b200_patch_im2col(const float* x, void* cols_bf16, int B, int C, int img, int patch, cudaStream_t stream) {
-    if (B <= 0 || C <= 0 || img <= 0 || patch <= 0 || patch % 16 != 0 || img % patch != 0) return set_error(B200_ERR_ARG, "patch_im2col: need patch % 16 == 0 and img % patch == 0");
+    const char* E = "patch_im2col";
+    if (B <= 0 || C <= 0 || img <= 0 || patch <= 0 || patch % 16 != 0 || img % patch != 0) return refuse(B200_ERR_ARG, E, "need patch % 16 == 0 and img % patch == 0");
+    if (!x || !cols_bf16) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(16, {x, cols_bf16})) return refuse(B200_ERR_ALIGN, E, "x / cols not 16-byte aligned");
     const long long total = static_cast<long long>(B) * C * img * (img / 16);
     patch_im2col_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(x, reinterpret_cast<__nv_bfloat16*>(cols_bf16), B, C, img, patch);
     return check_launch("patch_im2col");
@@ -1161,17 +1187,19 @@ extern "C" int b200_patch_im2col(const float* x, void* cols_bf16, int B, int C, 
 
 extern "C" int b200_patch_im2col_u8(const void* x_u8_hwc, void* cols_bf16, int B, int C, int img, int patch, double division,
                                     const double* mean_host, const double* std_host, cudaStream_t stream) {
-    if (B <= 0 || img <= 0 || patch <= 0 || patch % 16 != 0 || img % patch != 0) return set_error(B200_ERR_ARG, "patch_im2col_u8: need patch % 16 == 0 and img % patch == 0");
-    if (C < 1 || C > 4) return set_error(B200_ERR_ARG, "patch_im2col_u8: 1 <= channels <= 4");
-    if (division == 0.0) return set_error(B200_ERR_ARG, "patch_im2col_u8: division == 0");
-    if ((reinterpret_cast<uintptr_t>(x_u8_hwc) & 15u) != 0) return set_error(B200_ERR_ALIGN, "patch_im2col_u8: input not 16-byte aligned");
+    const char* E = "patch_im2col_u8";
+    if (B <= 0 || img <= 0 || patch <= 0 || patch % 16 != 0 || img % patch != 0) return refuse(B200_ERR_ARG, E, "need patch % 16 == 0 and img % patch == 0");
+    if (C < 1 || C > 4) return refuse(B200_ERR_ARG, E, "1 <= channels <= 4");
+    if (division == 0.0) return refuse(B200_ERR_ARG, E, "division == 0");
     NormParams np_;
     np_.division = division;
     for (int c = 0; c < 4; ++c) {
         np_.mean[c] = (mean_host != nullptr && c < C) ? mean_host[c] : 0.0;
         np_.stdv[c] = (std_host != nullptr && c < C) ? std_host[c] : 1.0;
-        if (np_.stdv[c] == 0.0) return set_error(B200_ERR_ARG, "patch_im2col_u8: std == 0");
+        if (np_.stdv[c] == 0.0) return refuse(B200_ERR_ARG, E, "std == 0");
     }
+    if (!x_u8_hwc || !cols_bf16) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(16, {x_u8_hwc, cols_bf16})) return refuse(B200_ERR_ALIGN, E, "input / cols not 16-byte aligned");
     const long long total = static_cast<long long>(B) * img * (img / 16);
     const unsigned blocks = static_cast<unsigned>((total + 255) / 256);
     const uint8_t* x = reinterpret_cast<const uint8_t*>(x_u8_hwc);
@@ -1187,7 +1215,10 @@ extern "C" int b200_patch_im2col_u8(const void* x_u8_hwc, void* cols_bf16, int B
 
 extern "C" int b200_assemble_tokens(const void* patch_bf16, const float* cls, const float* pos, float* net, int B, int np,
                                     int D, const void* conv_bias_bf16, cudaStream_t stream) {
-    if (B <= 0 || np <= 0 || D <= 0 || D % 8 != 0) return set_error(B200_ERR_ARG, "assemble_tokens: D % 8 != 0");
+    const char* E = "assemble_tokens";
+    if (B <= 0 || np <= 0 || D <= 0 || D % 8 != 0) return refuse(B200_ERR_ARG, E, "need B, np > 0 and D a positive multiple of 8");
+    if (!patch_bf16 || !cls || !pos || !net) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(16, {patch_bf16, cls, pos, net, conv_bias_bf16})) return refuse(B200_ERR_ALIGN, E, "pointers must be 16-byte aligned");
     const long long total = static_cast<long long>(B) * (np + 1) * (D / 8);
     assemble_tokens_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(patch_bf16), cls, pos, net, B, np, D,
                                                                                        reinterpret_cast<const __nv_bfloat16*>(conv_bias_bf16));
@@ -1196,7 +1227,11 @@ extern "C" int b200_assemble_tokens(const void* patch_bf16, const float* cls, co
 
 extern "C" int b200_assemble_tokens_bwd(const float* dnet, void* dpatch_bf16, float* dpos, float* dcls, int B, int np,
                                         int D, int accumulate, cudaStream_t stream) {
-    if (B <= 0 || np <= 0 || D <= 0 || D % 4 != 0) return set_error(B200_ERR_ARG, "assemble_tokens_bwd: D % 4 != 0");
+    const char* E = "assemble_tokens_bwd";
+    if (B <= 0 || np <= 0 || D <= 0 || D % 4 != 0) return refuse(B200_ERR_ARG, E, "need B, np > 0 and D a positive multiple of 4");
+    if (int_overflow(np + 1ll, D / 4)) return refuse(B200_ERR_ARG, E, "(np + 1) * D / 4 overflows int");
+    if (!dnet || !dpatch_bf16 || !dpos || !dcls) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(16, {dnet, dpatch_bf16, dpos, dcls})) return refuse(B200_ERR_ALIGN, E, "pointers must be 16-byte aligned");
     const int total = (np + 1) * (D / 4);
     assemble_tokens_bwd_kernel<<<(total + 127) / 128, 128, 0, stream>>>(dnet, reinterpret_cast<__nv_bfloat16*>(dpatch_bf16), dpos, dcls, B, np, D, accumulate);
     return check_launch("assemble_tokens_bwd");
@@ -1204,7 +1239,11 @@ extern "C" int b200_assemble_tokens_bwd(const float* dnet, void* dpatch_bf16, fl
 
 extern "C" int b200_embedding_fwd(const long long* ids, const float* weight, float* out, long long n, int D, int V,
                                   int* bad_index_flag, cudaStream_t stream) {
-    if (n <= 0 || D <= 0 || D % 4 != 0 || V <= 0 || bad_index_flag == nullptr) return set_error(B200_ERR_ARG, "embedding_fwd: need D % 4 == 0 and a flag");
+    const char* E = "embedding_fwd";
+    if (n <= 0 || D <= 0 || D % 4 != 0 || V <= 0) return refuse(B200_ERR_ARG, E, "need n, V > 0 and D a positive multiple of 4");
+    if (!ids || !weight || !out || !bad_index_flag) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(16, {weight, out})) return refuse(B200_ERR_ALIGN, E, "weight / out not 16-byte aligned");
+    if (!aligned(8, {ids}) || !aligned(4, {bad_index_flag})) return refuse(B200_ERR_ALIGN, E, "ids / flag not naturally aligned");
     const long long total = n * (D / 4);
     embedding_fwd_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(ids, weight, out, total, D / 4, V, bad_index_flag);
     return check_launch("embedding_fwd");
@@ -1212,7 +1251,10 @@ extern "C" int b200_embedding_fwd(const long long* ids, const float* weight, flo
 
 extern "C" int b200_embedding_bwd(const long long* ids, const float* dnet, float* dweight, long long n, int D, int V,
                                   int padding_idx, cudaStream_t stream) {
-    if (n <= 0 || D <= 0 || V <= 0) return set_error(B200_ERR_ARG, "embedding_bwd: bad size");
+    const char* E = "embedding_bwd";
+    if (n <= 0 || D <= 0 || V <= 0) return refuse(B200_ERR_ARG, E, "bad size");
+    if (!ids || !dnet || !dweight) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(8, {ids}) || !aligned(4, {dnet, dweight})) return refuse(B200_ERR_ALIGN, E, "pointers not naturally aligned");
     const long long total = n * D;
     embedding_bwd_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(ids, dnet, dweight, total, D, V, padding_idx);
     return check_launch("embedding_bwd");
@@ -1220,26 +1262,40 @@ extern "C" int b200_embedding_bwd(const long long* ids, const float* dnet, float
 
 extern "C" int b200_argmax_gather_rows(const long long* ids, const float* x, float* out, int* pos, int B, int T, int D,
                                        cudaStream_t stream) {
-    if (B <= 0 || T <= 0 || D <= 0) return set_error(B200_ERR_ARG, "argmax_gather_rows: bad size");
+    const char* E = "argmax_gather_rows";
+    if (B <= 0 || T <= 0 || D <= 0) return refuse(B200_ERR_ARG, E, "bad size");
+    if (!ids || !x || !out || !pos) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(8, {ids}) || !aligned(4, {x, out, pos})) return refuse(B200_ERR_ALIGN, E, "pointers not naturally aligned");
     argmax_gather_kernel<<<B, 128, 0, stream>>>(ids, x, out, pos, T, D);
     return check_launch("argmax_gather_rows");
 }
 
 extern "C" int b200_scatter_rows(const float* dout, const int* pos, float* dx, int B, int T, int D, cudaStream_t stream) {
-    if (B <= 0 || T <= 0 || D <= 0) return set_error(B200_ERR_ARG, "scatter_rows: bad size");
+    const char* E = "scatter_rows";
+    if (B <= 0 || T <= 0 || D <= 0) return refuse(B200_ERR_ARG, E, "bad size");
+    if (!dout || !pos || !dx) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(4, {dout, pos, dx})) return refuse(B200_ERR_ALIGN, E, "pointers not 4-byte aligned");
     scatter_rows_kernel<<<B, 128, 0, stream>>>(dout, pos, dx, T, D);
     return check_launch("scatter_rows");
 }
 
 extern "C" int b200_add_pos(const float* x, const float* pos, float* net, int B, int T, int D, cudaStream_t stream) {
-    if (B <= 0 || T <= 0 || D <= 0 || D % 4 != 0) return set_error(B200_ERR_ARG, "add_pos: D % 4 != 0");
+    const char* E = "add_pos";
+    if (B <= 0 || T <= 0 || D <= 0 || D % 4 != 0) return refuse(B200_ERR_ARG, E, "need B, T > 0 and D a positive multiple of 4");
+    if (int_overflow(T, D / 4)) return refuse(B200_ERR_ARG, E, "T * D / 4 overflows int");
+    if (!x || !pos || !net) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(16, {x, pos, net})) return refuse(B200_ERR_ALIGN, E, "pointers must be 16-byte aligned");
     const long long n4 = static_cast<long long>(B) * T * (D / 4);
     add_pos_kernel<<<static_cast<unsigned>((n4 + 255) / 256), 256, 0, stream>>>(x, pos, net, n4, T * (D / 4));
     return check_launch("add_pos");
 }
 
 extern "C" int b200_add_pos_bwd(const float* dnet, float* dpos, int B, int T, int D, int accumulate, cudaStream_t stream) {
-    if (B <= 0 || T <= 0 || D <= 0 || D % 4 != 0) return set_error(B200_ERR_ARG, "add_pos_bwd: D % 4 != 0");
+    const char* E = "add_pos_bwd";
+    if (B <= 0 || T <= 0 || D <= 0 || D % 4 != 0) return refuse(B200_ERR_ARG, E, "need B, T > 0 and D a positive multiple of 4");
+    if (int_overflow(T, D / 4)) return refuse(B200_ERR_ARG, E, "T * D / 4 overflows int");
+    if (!dnet || !dpos) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(16, {dnet, dpos})) return refuse(B200_ERR_ALIGN, E, "pointers must be 16-byte aligned");
     const int td4 = T * (D / 4);
     add_pos_bwd_kernel<<<(td4 + 127) / 128, 128, 0, stream>>>(dnet, dpos, B, td4, accumulate);
     return check_launch("add_pos_bwd");
@@ -1249,8 +1305,12 @@ extern "C" int b200_softmax_xent_fwd_bwd(const void* logits_bf16, long long ldl,
                                          float* loss_rows, float* loss_mean, void* dlogits_bf16, int* bad_label_flag,
                                          int B, int C, float grad_scale, const float* grad_scale_dev,
                                          cudaStream_t stream) {
-    if (B <= 0 || C <= 0) return set_error(B200_ERR_ARG, "softmax_xent: bad size");
-    if (bad_label_flag == nullptr || loss_rows == nullptr) return set_error(B200_ERR_ARG, "softmax_xent: null output");
+    const char* E = "softmax_xent";
+    if (B <= 0 || C <= 0) return refuse(B200_ERR_ARG, E, "bad size");
+    if (!logits_bf16 || !labels || !loss_rows || !bad_label_flag) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (ldl < C) return refuse(B200_ERR_ARG, E, "ldl < C");
+    if (!aligned(2, {logits_bf16, dlogits_bf16}) || !aligned(8, {labels}) || !aligned(4, {loss_rows, loss_mean, bad_label_flag, grad_scale_dev}))
+        return refuse(B200_ERR_ALIGN, E, "pointers not naturally aligned");
     softmax_xent_kernel<<<B, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(logits_bf16), ldl, labels, loss_rows,
                                                reinterpret_cast<__nv_bfloat16*>(dlogits_bf16), bad_label_flag, B, C, grad_scale, grad_scale_dev);
     int rc = check_launch("softmax_xent");
@@ -1264,7 +1324,12 @@ extern "C" int b200_softmax_xent_fwd_bwd(const void* logits_bf16, long long ldl,
 
 extern "C" int b200_symmetric_xent_fwd_bwd(const void* logits_bf16, long long ldl, float* loss, void* dlogits_bf16, float* lse_ws, int B,
                                            float grad_scale, const float* grad_scale_dev, cudaStream_t stream) {
-    if (B <= 0 || logits_bf16 == nullptr || loss == nullptr || lse_ws == nullptr) return set_error(B200_ERR_ARG, "symmetric_xent: bad arguments");
+    const char* E = "symmetric_xent";
+    if (B <= 0) return refuse(B200_ERR_ARG, E, "bad size");
+    if (!logits_bf16 || !loss || !lse_ws) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (ldl < B) return refuse(B200_ERR_ARG, E, "ldl < B");
+    if (!aligned(2, {logits_bf16, dlogits_bf16}) || !aligned(4, {loss, lse_ws, grad_scale_dev}))
+        return refuse(B200_ERR_ALIGN, E, "pointers not naturally aligned");
     const __nv_bfloat16* lg = reinterpret_cast<const __nv_bfloat16*>(logits_bf16);
     sym_xent_stats_kernel<<<(2 * B + 7) / 8, 256, 0, stream>>>(lg, ldl, B, lse_ws);
     int rc = check_launch("symmetric_xent_stats");
@@ -1281,7 +1346,10 @@ extern "C" int b200_symmetric_xent_fwd_bwd(const void* logits_bf16, long long ld
 }
 
 extern "C" int b200_cast_f32_to_bf16(const float* src, void* dst_bf16, long long n, cudaStream_t stream) {
-    if (n <= 0) return set_error(B200_ERR_ARG, "cast: n <= 0");
+    const char* E = "cast";
+    if (n <= 0) return refuse(B200_ERR_ARG, E, "n <= 0");
+    if (!src || !dst_bf16) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(16, {src, dst_bf16})) return refuse(B200_ERR_ALIGN, E, "src / dst not 16-byte aligned");
     const long long thr = (n + 7) / 8;
     cast_f32_bf16_kernel<<<static_cast<unsigned>((thr + 255) / 256), 256, 0, stream>>>(src, reinterpret_cast<__nv_bfloat16*>(dst_bf16), n);
     return check_launch("cast_f32_bf16");
@@ -1289,8 +1357,12 @@ extern "C" int b200_cast_f32_to_bf16(const float* src, void* dst_bf16, long long
 extern "C" int b200_adam_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n,
                               float lr, float beta1, float beta2, float eps, float weight_decay, int step,
                               int* step_dev, cudaStream_t stream) {
-    if (n <= 0 || n % 4 != 0) return set_error(B200_ERR_ARG, "adam_step: n must be a positive multiple of 4");
-    if (step_dev == nullptr && step < 1) return set_error(B200_ERR_ARG, "adam_step: step >= 1 (or pass step_dev)");
+    const char* E = "adam_step";
+    if (n <= 0 || n % 4 != 0) return refuse(B200_ERR_ARG, E, "n must be a positive multiple of 4");
+    if (step_dev == nullptr && step < 1) return refuse(B200_ERR_ARG, E, "step >= 1 (or pass step_dev)");
+    if (!params || !grads || !exp_avg || !exp_avg_sq) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(16, {params, grads, exp_avg, exp_avg_sq})) return refuse(B200_ERR_ALIGN, E, "arenas not 16-byte aligned");
+    if (!aligned(4, {step_dev})) return refuse(B200_ERR_ALIGN, E, "step_dev not 4-byte aligned");
     if (step_dev != nullptr) {
         increment_kernel<<<1, 1, 0, stream>>>(step_dev);
         int rc = check_launch("adam_step_increment");
@@ -1306,8 +1378,11 @@ extern "C" int b200_adam_step(float* params, const float* grads, float* exp_avg,
 }
 extern "C" int b200_adam_step_dev(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n,
                                   const float* hyper_dev, int* step_dev, int increment, cudaStream_t stream) {
-    if (n <= 0 || n % 4 != 0) return set_error(B200_ERR_ARG, "adam_step_dev: n must be a positive multiple of 4");
-    if (hyper_dev == nullptr || step_dev == nullptr) return set_error(B200_ERR_ARG, "adam_step_dev: hyper_dev and step_dev are required");
+    const char* E = "adam_step_dev";
+    if (n <= 0 || n % 4 != 0) return refuse(B200_ERR_ARG, E, "n must be a positive multiple of 4");
+    if (!params || !grads || !exp_avg || !exp_avg_sq || !hyper_dev || !step_dev) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(16, {params, grads, exp_avg, exp_avg_sq})) return refuse(B200_ERR_ALIGN, E, "arenas not 16-byte aligned");
+    if (!aligned(4, {hyper_dev, step_dev})) return refuse(B200_ERR_ALIGN, E, "hyper_dev / step_dev not 4-byte aligned");
     if (increment) {
         increment_kernel<<<1, 1, 0, stream>>>(step_dev);
         int rc = check_launch("adam_step_increment");
@@ -1318,7 +1393,10 @@ extern "C" int b200_adam_step_dev(float* params, const float* grads, float* exp_
     return check_launch("adam_step_dev");
 }
 extern "C" int b200_fill_f32(float* dst, float value, long long n, cudaStream_t stream) {
-    if (n <= 0) return set_error(B200_ERR_ARG, "fill: n <= 0");
+    const char* E = "fill";
+    if (n <= 0) return refuse(B200_ERR_ARG, E, "n <= 0");
+    if (!dst) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(16, {dst})) return refuse(B200_ERR_ALIGN, E, "dst not 16-byte aligned");
     const long long thr = (n + 3) / 4;
     fill_f32_kernel<<<static_cast<unsigned>((thr + 255) / 256), 256, 0, stream>>>(dst, value, n);
     return check_launch("fill_f32");

@@ -172,7 +172,12 @@ def pick_splits(M: int, N: int, K: int) -> int:
 
 def wgrad(dy: Tensor, x: Tensor, out: Tensor, *, round_bf16: bool = True, accumulate: bool = False) -> Tensor:
     """out[N_out, K_in] (fp32) (+)= dy[M, N_out]^T . x[M, K_in]   (split-K over the M tokens, then reduce)."""
+    _need_cuda(dy, x, out)
+    if dy.dtype != _BF16 or x.dtype != _BF16 or dy.dim() != 2 or x.dim() != 2 or dy.shape[0] != x.shape[0]:
+        raise B200Error("wgrad: need bf16 dy [M, N_out] and x [M, K_in]")
     M, n_out = dy.shape
+    if out.dtype != _F32 or tuple(out.shape) != (n_out, x.shape[1]) or not out.is_contiguous():
+        raise B200Error("wgrad: out must be a contiguous fp32 [N_out, K_in] tensor")
     k_in = x.shape[1]
     splits = pick_splits(n_out, k_in, M)
     part = WORKSPACE.get(dy.device, splits * n_out * k_in, "splitk")[: splits * n_out * k_in].view(splits, n_out, k_in)
@@ -184,7 +189,10 @@ def wgrad(dy: Tensor, x: Tensor, out: Tensor, *, round_bf16: bool = True, accumu
 def colsum(x: Tensor, out: Tensor, *, round_bf16: bool = True, accumulate: bool = False) -> Tensor:
     """out[cols] (fp32) (+)= sum over rows of x[rows, cols] (bf16): bias gradients."""
     _need_cuda(x, out)
+    if x.dtype != _BF16 or x.dim() != 2 or x.stride(1) != 1:
+        raise B200Error("colsum: x must be a 2-D bf16 view with unit inner stride")
     rows, cols = x.shape
+    _dense_f32(out, cols, "out", "colsum")
     part = WORKSPACE.get(x.device, _MAX_PARTS * cols, "colsum")
     nparts = ctypes.c_int(0)
     call("b200_colsum_bf16", x.data_ptr(), x.stride(0), rows, cols, part.data_ptr(), _MAX_PARTS, ctypes.byref(nparts), _stream())
@@ -211,9 +219,20 @@ def colsum_per_image(x: Tensor) -> Tuple[Tensor, Tensor]:
 # ----------------------------------------------------------------------------------------------------------------
 # LayerNorm
 # ----------------------------------------------------------------------------------------------------------------
+def _strided_f32(t: Tensor, rows: int, dim: int, ld: int, msg: str) -> None:
+    """t: contiguous fp32 holding `rows` rows of `dim` elements `ld` apart (ld > dim: e.g. token 0 of each image)."""
+    if t.dtype != _F32 or not t.is_contiguous() or ld < dim or t.numel() < (rows - 1) * ld + dim:
+        raise B200Error(msg)
+
+
 def layernorm_fwd(x: Tensor, gamma: Tensor, beta: Tensor, eps: float, *, rows: int, dim: int, ld_x: int,
                   y_f32: Optional[Tensor] = None) -> Tuple[Tensor, Tensor, Tensor]:
-    _need_cuda(x, gamma, beta)
+    _need_cuda(x, gamma, beta, y_f32)
+    _strided_f32(x, rows, dim, ld_x, "layernorm_fwd: x must be contiguous fp32 holding rows of dim elements ld_x apart")
+    _dense_f32(gamma, dim, "gamma", "layernorm_fwd")
+    _dense_f32(beta, dim, "beta", "layernorm_fwd")
+    if y_f32 is not None:
+        _packed_rows(y_f32, rows, dim, "layernorm_fwd: y_f32 must be contiguous fp32 [rows, dim]", _F32)
     y = torch.empty((rows, dim), dtype=torch.bfloat16, device=x.device)
     mean = torch.empty(rows, dtype=torch.float32, device=x.device)
     rstd = torch.empty(rows, dtype=torch.float32, device=x.device)
@@ -229,6 +248,20 @@ def layernorm_bwd(
 ) -> None:
     """LayerNorm backward.  ``dx_colsum`` (fp32 [dim]): also receives the bf16-rounded column sums of ``dx_bf16``,
     i.e. the bias gradient of the Linear layer whose dY this dx is -- fused, no extra pass over dx."""
+    _need_cuda(dy, x, gamma, mean, rstd, dres, dx_out, dx_bf16, dgamma, dbeta, dx_colsum)
+    if dy.dtype not in (_BF16, _F32):
+        raise B200Error("layernorm_bwd: dy must be bf16 or fp32")
+    _packed_rows(dy, rows, dim, "layernorm_bwd: dy must be contiguous [rows, dim]", dy.dtype)
+    _strided_f32(x, rows, dim, ld_x, "layernorm_bwd: x must be contiguous fp32 holding rows of dim elements ld_x apart")
+    _strided_f32(dx_out, rows, dim, ld_dx, "layernorm_bwd: dx_out must be contiguous fp32 holding rows of dim elements ld_dx apart")
+    if dres is not None:
+        _strided_f32(dres, rows, dim, ld_dx, "layernorm_bwd: dres must be contiguous fp32 holding rows of dim elements ld_dx apart")
+    if dx_bf16 is not None:
+        _packed_rows(dx_bf16, rows, dim, "layernorm_bwd: dx_bf16 must be contiguous bf16 [rows, dim]")
+    for t, n, name in ((gamma, dim, "gamma"), (mean, rows, "mean"), (rstd, rows, "rstd"), (dgamma, dim, "dgamma"), (dbeta, dim, "dbeta")):
+        _dense_f32(t, n, name, "layernorm_bwd")
+    if dx_colsum is not None:
+        _dense_f32(dx_colsum, dim, "dx_colsum", "layernorm_bwd")
     nw = 3 if dx_colsum is not None else 2
     part = WORKSPACE.get(x.device, 3 * _MAX_PARTS * dim, "lnbwd")
     nparts = ctypes.c_int(0)
@@ -315,9 +348,9 @@ ATTENTION_MAX_T = 16384   # longest sequence the attention kernels accept
 ATTENTION_RESIDENT_MAX_T = 256  # up to here a whole head fits in shared memory; longer sequences use the streamed kernels
 
 
-def _packed_rows(t: Tensor, rows: int, width: int, msg: str) -> None:
-    """t: contiguous bf16 holding `rows` rows of `width` elements ([rows, width], or [B, T, width] with B * T = rows)."""
-    if t.dtype != torch.bfloat16 or not t.is_contiguous() or t.dim() < 2 or t.shape[-1] != width or t.numel() != rows * width:
+def _packed_rows(t: Tensor, rows: int, width: int, msg: str, dtype: torch.dtype = _BF16) -> None:
+    """t: contiguous `dtype` holding `rows` rows of `width` elements ([rows, width], or [B, T, width] with B * T = rows)."""
+    if t.dtype != dtype or not t.is_contiguous() or t.dim() < 2 or t.shape[-1] != width or t.numel() != rows * width:
         raise B200Error(msg)
 
 
@@ -458,24 +491,41 @@ def patch_im2col_u8(x: Tensor, patch: int, division: float = 255.0, mean=None, s
 def add_pos(x: Tensor, pos: Tensor, B: int, T: int, D: int) -> Tensor:
     """net[b, t, :] = x[b, t, :] + pos[t, :] (fp32): the text tower's input stage."""
     _need_cuda(x, pos)
+    _packed_rows(x, B * T, D, "add_pos: x must be contiguous fp32 [B, T, D]", _F32)
+    _packed_rows(pos, T, D, "add_pos: pos must be contiguous fp32 [T, D]", _F32)
     net = torch.empty((B, T, D), dtype=torch.float32, device=x.device)
     call("b200_add_pos", x.data_ptr(), pos.data_ptr(), net.data_ptr(), B, T, D, _stream())
     return net
 
 
 def add_pos_bwd(dnet: Tensor, dpos: Tensor, B: int, T: int, D: int, accumulate: bool = False) -> None:
+    _need_cuda(dnet, dpos)
+    _packed_rows(dnet, B * T, D, "add_pos_bwd: dnet must be contiguous fp32 [B, T, D]", _F32)
+    _packed_rows(dpos, T, D, "add_pos_bwd: dpos must be contiguous fp32 [T, D]", _F32)
     call("b200_add_pos_bwd", dnet.data_ptr(), dpos.data_ptr(), B, T, D, int(accumulate), _stream())
 
 
 def assemble_tokens(patch: Tensor, cls: Tensor, pos: Tensor, B: int, np_: int, D: int, conv_bias: Optional[Tensor] = None) -> Tensor:
     """net[b, 0] = cls + pos[0]; net[b, t] = float(patch[b, t-1]) + pos[t].  ``conv_bias`` (bf16 [D]): the patch rows first become
     bf16(patch + bias) -- the separate bf16 bias add eager's convolution performs."""
+    _need_cuda(patch, cls, pos, conv_bias)
+    _packed_rows(patch, B * np_, D, "assemble_tokens: patch must be contiguous bf16 [B * np, D]")
+    _packed_rows(pos, np_ + 1, D, "assemble_tokens: pos must be contiguous fp32 [np + 1, D]", _F32)
+    if cls.dtype != _F32 or not cls.is_contiguous() or cls.numel() != D:
+        raise B200Error("assemble_tokens: cls must be contiguous fp32 with D elements")
+    if conv_bias is not None and (conv_bias.dtype != _BF16 or not conv_bias.is_contiguous() or conv_bias.numel() != D):
+        raise B200Error("assemble_tokens: conv_bias must be contiguous bf16 with D elements")
     net = torch.empty((B, np_ + 1, D), dtype=torch.float32, device=patch.device)
     call("b200_assemble_tokens", patch.data_ptr(), cls.data_ptr(), pos.data_ptr(), net.data_ptr(), B, np_, D, _ptr(conv_bias), _stream())
     return net
 
 
 def assemble_tokens_bwd(dnet: Tensor, dpos: Tensor, dcls: Tensor, B: int, np_: int, D: int, accumulate: bool = False) -> Tensor:
+    _need_cuda(dnet, dpos, dcls)
+    _packed_rows(dnet, B * (np_ + 1), D, "assemble_tokens_bwd: dnet must be contiguous fp32 [B, np + 1, D]", _F32)
+    _packed_rows(dpos, np_ + 1, D, "assemble_tokens_bwd: dpos must be contiguous fp32 [np + 1, D]", _F32)
+    if dcls.dtype != _F32 or not dcls.is_contiguous() or dcls.numel() != D:
+        raise B200Error("assemble_tokens_bwd: dcls must be contiguous fp32 with D elements")
     dpatch = torch.empty((B * np_, D), dtype=torch.bfloat16, device=dnet.device)
     call("b200_assemble_tokens_bwd", dnet.data_ptr(), dpatch.data_ptr(), dpos.data_ptr(), dcls.data_ptr(), B, np_, D, int(accumulate), _stream())
     return dpatch
@@ -513,6 +563,9 @@ def cast_bf16(src: Tensor, dst: Optional[Tensor] = None) -> Tensor:
 
 
 def fill_f32(dst: Tensor, value: float) -> Tensor:
+    _need_cuda(dst)
+    if dst.dtype != _F32 or not dst.is_contiguous():
+        raise B200Error("fill_f32: need contiguous fp32")
     call("b200_fill_f32", dst.data_ptr(), float(value), dst.numel(), _stream())
     return dst
 
@@ -526,6 +579,8 @@ def groupnorm_silu_fwd(x: Tensor, gamma: Tensor, beta: Tensor, eps: float, *, si
     if x.dtype != torch.bfloat16 or x.dim() != 3 or not x.is_contiguous():
         raise B200Error("groupnorm_silu_fwd: need contiguous bf16 [B, HW, C]")
     B, HW, C = x.shape
+    _dense_f32(gamma, C, "gamma", "groupnorm_silu_fwd")
+    _dense_f32(beta, C, "beta", "groupnorm_silu_fwd")
     y = torch.empty_like(x)
     mean = torch.empty((B, 32), dtype=torch.float32, device=x.device)
     rstd = torch.empty((B, 32), dtype=torch.float32, device=x.device)
@@ -537,8 +592,15 @@ def groupnorm_silu_fwd(x: Tensor, gamma: Tensor, beta: Tensor, eps: float, *, si
 
 def groupnorm_silu_bwd(x: Tensor, dy: Tensor, gamma: Tensor, beta: Tensor, mean: Tensor, rstd: Tensor, *, silu: bool = True,
                        dgamma: Optional[Tensor] = None, dbeta: Optional[Tensor] = None, accumulate: bool = False) -> Tuple[Tensor, Tensor, Tensor]:
-    _need_cuda(x, dy, gamma, beta, mean, rstd)
+    _need_cuda(x, dy, gamma, beta, mean, rstd, dgamma, dbeta)
+    if x.dtype != torch.bfloat16 or x.dim() != 3 or not x.is_contiguous():
+        raise B200Error("groupnorm_silu_bwd: need contiguous bf16 x [B, HW, C]")
     B, HW, C = x.shape
+    for t, name in ((mean, "mean"), (rstd, "rstd")):
+        if t.dtype != _F32 or tuple(t.shape) != (B, 32) or not t.is_contiguous():
+            raise B200Error(f"groupnorm_silu_bwd: {name} must be a contiguous fp32 [B, 32] tensor")
+    _dense_f32(gamma, C, "gamma", "groupnorm_silu_bwd")
+    _dense_f32(beta, C, "beta", "groupnorm_silu_bwd")
     if dy.dtype != torch.bfloat16 or dy.shape != x.shape or not dy.is_contiguous():
         raise B200Error("groupnorm_silu_bwd: dy must be contiguous bf16 with x's shape")
     dx = torch.empty_like(x)
@@ -546,6 +608,8 @@ def groupnorm_silu_bwd(x: Tensor, dy: Tensor, gamma: Tensor, beta: Tensor, mean:
         dgamma = torch.empty(C, dtype=torch.float32, device=x.device)
         dbeta = torch.empty(C, dtype=torch.float32, device=x.device)
         accumulate = False
+    _dense_f32(dgamma, C, "dgamma", "groupnorm_silu_bwd")
+    _dense_f32(dbeta, C, "dbeta", "groupnorm_silu_bwd")
     ws = WORKSPACE.get(x.device, int(_cabi.lib().b200_groupnorm_workspace_floats(B, HW, C)), "groupnorm")
     call("b200_groupnorm_silu_bwd", x.data_ptr(), dy.data_ptr(), gamma.data_ptr(), beta.data_ptr(), mean.data_ptr(), rstd.data_ptr(),
          dx.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), ws.data_ptr(), B, HW, C, int(silu), int(accumulate), _stream())

@@ -11,7 +11,14 @@
  *   - asynchronous on `stream`; never allocates, never synchronises, never falls back to the CPU;
  *   - returns 0 on success or a negative B200_ERR_* code; b200_last_error() describes the last failure
  *     on the calling thread;
- *   - bf16 = IEEE bfloat16 (round-to-nearest-even), f32 = IEEE binary32.
+ *   - bf16 = IEEE bfloat16 (round-to-nearest-even), f32 = IEEE binary32;
+ *   - every argument is checked before anything is launched.  A refused call returns B200_ERR_ARG for a size outside the
+ *     entry's range, a NULL required pointer or a leading dimension smaller than the row width, and B200_ERR_ALIGN for a
+ *     misaligned pointer or a leading dimension that is not a multiple of the kernel's vector width;
+ *   - every non-NULL device pointer is 16-byte aligned, except the ones an entry's comment names as ELEMENT-WISE: its
+ *     kernels access them one element at a time, so they need only their natural alignment (2 bytes for bf16, 4 for f32
+ *     and int32, 8 for int64);
+ *   - sizes whose products a kernel indexes in 32-bit int are refused when the product would overflow.
  */
 #ifndef B200_CFLEARN_H_
 #define B200_CFLEARN_H_
@@ -100,7 +107,8 @@ int b200_gemm_pick_splits(int M, int N, int K);
  * mode, so the setting is only recorded.  Returns the previous setting. */
 int b200_set_gemm_multicast(int enable);
 /* out[f32][n] (+)= round( sum_s partial[s][n] ); round_bf16 mirrors autocast (the weight grad of a bf16 matmul
- * is produced in bf16, cf. cflearn/schema.py:1266-1276 autocast + :980 backward). accumulate: 0 overwrite. */
+ * is produced in bf16, cf. cflearn/schema.py:1266-1276 autocast + :980 backward). accumulate: 0 overwrite.
+ * n % 4 == 0; partial and out required. */
 int b200_splitk_reduce(const float* partial, int splits, long long n, float* out, int round_bf16, int accumulate,
                        cudaStream_t stream);
 
@@ -109,7 +117,8 @@ int b200_splitk_reduce(const float* partial, int splits, long long n, float* out
  * (cflearn/modules/core/norms.py:88-89,118-124; used at mixed_stacks/api.py:141,155,397-402).
  *   x: f32 [rows, ld_x] (first `dim` columns are normalised; ld_x lets the head LN read only token 0 of each
  *   image -- api.py:365).  y: bf16 [rows, dim] (the value autocast hands to the next F.linear).
- *   mean, rstd: f32 [rows], saved for backward.
+ *   mean, rstd: f32 [rows], saved for backward.  Required: x, gamma, beta, y_bf16, mean, rstd; ld_x >= dim, ld_x % 4 == 0.
+ *   Element-wise: mean, rstd.
  * --------------------------------------------------------------------------------------------------------- */
 int b200_layernorm_fwd(const float* x, long long ld_x, const float* gamma, const float* beta, void* y_bf16,
                        float* y_f32 /* optional [rows, dim]: the un-rounded fp32 result */, float* mean, float* rstd,
@@ -122,7 +131,9 @@ int b200_layernorm_fwd(const float* x, long long ld_x, const float* gamma, const
  * dy is bf16 [rows, dim], or fp32 when dy_is_f32 != 0 (a LayerNorm whose output is the fp32 residual stream itself:
  * CLIP's embedding_norm, mixed_stacks/api.py:433-434).  dx_colsum != 0 (needs dx_bf16, bf16 dy): the part rows are 3*dim wide and columns [2*dim, 3*dim) hold the column sums of
  * the bf16-rounded dx rows, i.e. the bias gradient of the Linear layer whose output gradient this dx is (the
- * separate b200_colsum_bf16 pass over dx_bf16 is then not needed). */
+ * separate b200_colsum_bf16 pass over dx_bf16 is then not needed).  Required: dy, x, gamma, mean, rstd, dx_out, dgb_part;
+ * optional: dres, dx_bf16, nparts_out; ld_x, ld_dx >= dim and multiples of 4; max_parts >= 1.  Element-wise: mean, rstd,
+ * dgb_part. */
 int b200_layernorm_bwd(const void* dy, int dy_is_f32, const float* x, long long ld_x, const float* gamma, const float* mean,
                        const float* rstd, const float* dres, float* dx_out, long long ld_dx, void* dx_bf16,
                        float* dgb_part, int max_parts, int* nparts_out, int rows, int dim, int dx_colsum,
@@ -130,7 +141,7 @@ int b200_layernorm_bwd(const void* dy, int dy_is_f32, const float* x, long long 
 
 /* LayerNorm over BF16 rows: the SD-v1.5 UNet's SpatialTransformerBlock norms (mixed_stacks/api.py:800-812), whose residual
  * stream is bf16 under autocast.  x, y, dy, dres, dx: bf16 [rows, dim] dense; gamma, beta f32 [dim]; 0 < dim <= 2048,
- * dim % 8 == 0; x / y / dy / dres / dx / gamma / beta 16-byte aligned.
+ * dim % 8 == 0; dres is optional, every other pointer required.  Element-wise: mean, rstd, dgb_part.
  *   forward : y = bf16(LN_fp32(x)); mean, rstd f32 [rows].
  *   backward: dx = bf16(float(dres) + float(bf16(LN'(dy))))  (dres NULL: dx = bf16(LN'(dy))) -- eager's cast back to the bf16
  *             input followed by the bf16 accumulation of the residual branch.  dgb_part: f32 [nparts, 2 * dim] ([.., 0:dim]
@@ -144,7 +155,10 @@ int b200_layernorm_bf16_bwd(const void* dy_bf16, const void* x_bf16, const float
 /* column sums: part[p][c] = sum over a slice of rows of x[r][c]  (x bf16 or f32), then finish() reduces the
  * parts.  Bias gradients of every Linear (autograd of customs.py:89) and LN gamma/beta gradients.
  * b200_colsum_bf16: ld % 8 == 0 and ld >= roundup(cols, 8); each row is read in 16-byte groups up to roundup(cols, 8)
- * elements (the values past cols never reach a part); part is [nparts, cols] dense, nparts <= max_parts. */
+ * elements (the values past cols never reach a part); part is [nparts, cols] dense, nparts <= max_parts.  x and part are
+ * required, nparts_out optional; part is element-wise.
+ * b200_colsum_finish / _finish2: part_ld >= cols (cols0 + cols1); part and out (out0, out1) required and element-wise, so
+ * part may point into a row (e.g. at a column offset). */
 int b200_colsum_bf16(const void* x_bf16, long long ld, int rows, int cols, float* part, int max_parts,
                      int* nparts_out, cudaStream_t stream);
 int b200_colsum_finish(const float* part, long long part_ld, int nparts, int cols, float* out, int round_bf16,
@@ -156,7 +170,8 @@ int b200_colsum_finish2(const float* part, long long part_ld, int nparts, int co
  *   per_image bf16 [B, C] = bf16(sum over the HW rows of image b)  (the gradient of a [B, C] table broadcast over the pixels:
  *                           the ResBlock's time embedding, cflearn/modules/core/convs/residual.py:240-244)
  *   total f32 [C] = float(bf16(sum over b of the unrounded per-image sums))  (the bias gradient of the conv that wrote x)
- * workspace: b200_colsum_per_image_workspace_floats(B, HW, C) floats.  Deterministic. */
+ * workspace: b200_colsum_per_image_workspace_floats(B, HW, C) floats.  Deterministic.  All pointers required;
+ * element-wise: per_image, total, workspace. */
 long long b200_colsum_per_image_workspace_floats(int B, int HW, int C);
 int b200_colsum_per_image_bf16(const void* x_bf16, int B, int HW, int C, void* per_image_bf16, float* total, float* workspace,
                                cudaStream_t stream);
@@ -221,7 +236,9 @@ int b200_cross_attention_bwd(const void* q, long long ldq, const void* k, const 
  * part[nblocks, arena_len + 1] receives per-128-sample gradient partials in arena layout (b200_colsum_finish sums
  * them) and, in column arena_len, the loss partial.  loss_mode 1: w_mae * mean|p - y| + w_mse * mean (p - y)^2
  * ("multi_task" of "mae" + "mse", losses/basic.py:45-61, losses/common.py:72-88); loss_mode 0: dpred [M, dims[n]] is
- * the gradient of the output (autograd's backward).  *nblocks_out (host int) = number of partial rows written. */
+ * the gradient of the output (autograd's backward).  *nblocks_out (host int) = number of partial rows written.
+ * Required: x, params and the host arrays dims, w_offsets, b_offsets (and y with loss_mode 1, dpred with loss_mode 0 when
+ * part != NULL); optional: y, dpred, pred, part, nblocks_out.  Element-wise: every device pointer. */
 int b200_fcnn_step(const float* x, const float* y, const float* dpred, const float* params, float* pred, float* part,
                    int M, int n_layers, const int* dims, const int* w_offsets, const int* b_offsets, int arena_len,
                    int loss_mode, float w_mae, float w_mse, int* nblocks_out, cudaStream_t stream);
@@ -231,6 +248,7 @@ int b200_fcnn_step(const float* x, const float* y, const float* dpred, const flo
  *   im2col : x f32 [B, C, IMG, IMG] (NCHW) -> cols bf16 [B*(IMG/P)^2, C*P*P]  (k index = (c, ky, kx))
  *   assemble: net f32 [B, 1+np, D] = cat(cls, float(patch bf16 [B*np, D])) + pos[1+np, D]
  *   assemble_bwd: dpatch bf16 [B*np, D] = bf16(dnet[:,1:,:]); dpos f32 [1+np, D] = sum_b dnet; dcls f32 [D]
+ * Every device pointer is required (conv_bias_bf16 optional); assemble_bwd needs (np + 1) * D / 4 to fit in int.
  * --------------------------------------------------------------------------------------------------------- */
 int b200_patch_im2col(const float* x, void* cols_bf16, int B, int C, int img, int patch, cudaStream_t stream);
 /* The same matrix straight from the RAW batch: x = uint8 [B, img, img, C] (HWC, C <= 4), value = ((x / division) - mean[c])
@@ -247,7 +265,8 @@ int b200_assemble_tokens(const void* patch_bf16, const float* cls, const float* 
 int b200_assemble_tokens_bwd(const float* dnet, void* dpatch_bf16, float* dpos, float* dcls, int B, int np, int D,
                              int accumulate, cudaStream_t stream);
 /* Text-tower input stage (TeTEncoder, cflearn/modules/nlp/encoder/transformer.py:92 -> mixed_stacks/api.py:419-438 without
- * a head token): net f32 [B, T, D] = x f32 [B, T, D] + pos f32 [T, D];  backward: dpos = sum over the batch of dnet. */
+ * a head token): net f32 [B, T, D] = x f32 [B, T, D] + pos f32 [T, D];  backward: dpos = sum over the batch of dnet.
+ * D % 4 == 0, T * D / 4 fits in int; every pointer required. */
 int b200_add_pos(const float* x, const float* pos, float* net, int B, int T, int D, cudaStream_t stream);
 int b200_add_pos_bwd(const float* dnet, float* dpos, int B, int T, int D, int accumulate, cudaStream_t stream);
 
@@ -255,7 +274,9 @@ int b200_add_pos_bwd(const float* dnet, float* dpos, int B, int T, int D, int ac
  *   embedding_fwd : out f32 [n, D] = weight f32 [V, D][ids[n]]; ids outside [0, V) set *bad_index_flag (device int)
  *   embedding_bwd : dweight[ids[n]] += dnet[n] for ids[n] != padding_idx (dweight zeroed by the caller; fp32 atomics)
  *   argmax_gather : pos[b] = first arg-max of ids[b, :]; out f32 [B, D] = x f32 [B, T, D][b, pos[b]]
- *   scatter_rows  : dx[b, pos[b], :] = dout[b, :]   (dx zero-filled by the caller) */
+ *   scatter_rows  : dx[b, pos[b], :] = dout[b, :]   (dx zero-filled by the caller)
+ * Every pointer is required.  Element-wise: ids and bad_index_flag of embedding_fwd (weight and out are read in 16-byte
+ * groups, D % 4 == 0), every pointer of the other three. */
 int b200_embedding_fwd(const long long* ids, const float* weight, float* out, long long n, int D, int V, int* bad_index_flag,
                        cudaStream_t stream);
 int b200_embedding_bwd(const long long* ids, const float* dnet, float* dweight, long long n, int D, int V, int padding_idx,
@@ -270,6 +291,8 @@ int b200_scatter_rows(const float* dout, const int* pos, float* dx, int B, int T
  * grad_scale * (grad_scale_dev ? *grad_scale_dev : 1) / B) -- grad_scale_dev is the upstream gradient of the mean
  * loss living on the device (autograd's grad_output), so backward needs no host synchronisation.
  * The label gather is integer-exact; out-of-range labels set *bad_label_flag (device int).
+ * Required: logits, labels, loss_rows, bad_label_flag; optional: loss_mean, dlogits, grad_scale_dev; ldl >= C.
+ * Element-wise: every pointer of both cross entropies.
  * --------------------------------------------------------------------------------------------------------- */
 int b200_softmax_xent_fwd_bwd(const void* logits_bf16, long long ldl, const long long* labels, float* loss_rows,
                               float* loss_mean, void* dlogits_bf16, int* bad_label_flag, int B, int C,
@@ -277,7 +300,8 @@ int b200_softmax_xent_fwd_bwd(const void* logits_bf16, long long ldl, const long
 /* Symmetric (contrastive) cross entropy of a square bf16 logits matrix L [B, B] (leading dimension ldl) with targets
  * arange(B): loss[0] = (CE(L) + CE(L^T)) / 2, dlogits = bf16 of the fp32 gradient scaled by grad_scale (* grad_scale_dev[0]).
  * The training objective of CLIP (cflearn/modules/multimodal/clip.py:209-256 produce L; the reference ships no loss for
- * it, SURVEY.md 8d -- the definition is oracle/clip_oracle.py::symmetric_cross_entropy).  lse_ws: 2*B floats of scratch. */
+ * it, SURVEY.md 8d -- the definition is oracle/clip_oracle.py::symmetric_cross_entropy).  lse_ws: 2*B floats of scratch.
+ * Required: logits, loss, lse_ws; optional: dlogits, grad_scale_dev; ldl >= B. */
 int b200_symmetric_xent_fwd_bwd(const void* logits_bf16, long long ldl, float* loss, void* dlogits_bf16, float* lse_ws, int B,
                                 float grad_scale, const float* grad_scale_dev, cudaStream_t stream);
 
@@ -286,6 +310,7 @@ int b200_symmetric_xent_fwd_bwd(const void* logits_bf16, long long ldl, float* l
  * optimizer "adam", cflearn/optimizers.py:29-32, stepped at cflearn/schema.py:983).  n % 4 == 0.
  * step_dev == NULL: `step` (>= 1) is the host-side step count.  step_dev != NULL: a device int that is incremented
  * (on the stream) and then used as the step count, so the call can be replayed from a CUDA graph.
+ * The four arenas are required; element-wise: step_dev (and hyper_dev below).
  * --------------------------------------------------------------------------------------------------------- */
 int b200_adam_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n, float lr,
                    float beta1, float beta2, float eps, float weight_decay, int step, int* step_dev,
@@ -294,11 +319,12 @@ int b200_adam_step(float* params, const float* grads, float* exp_avg, float* exp
  * grad_scale} (6 floats; grad_scale multiplies the gradient first: 1/world after a SUM all-reduce, or the clip
  * coefficient of cflearn/schema.py:981-982).  A captured CUDA graph therefore follows an LR scheduler
  * (cflearn/pipeline/blocks/basic.py:334-352 "warmup" is the reference's default) without being re-captured.
- * increment != 0: *step_dev += 1 first (pass 0 for all but the first slice when one step updates several slices). */
+ * increment != 0: *step_dev += 1 first (pass 0 for all but the first slice when one step updates several slices).
+ * hyper_dev and step_dev are required. */
 int b200_adam_step_dev(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n,
                        const float* hyper_dev, int* step_dev, int increment, cudaStream_t stream);
 
-/* element-wise helpers */
+/* element-wise helpers (every pointer required and 16-byte aligned) */
 int b200_cast_f32_to_bf16(const float* src, void* dst_bf16, long long n, cudaStream_t stream);
 int b200_fill_f32(float* dst, float value, long long n, cudaStream_t stream);
 
@@ -339,7 +365,8 @@ int b200_set_persistent_ctas(int n, int launches);
  * (cflearn/modules/core/convs/residual.py:176-178,197-198,221,241; multimodal/diffusion/unet.py:264-268;
  * SpatialTransformer.norm without activation, mixed_stacks/api.py:866-870).  mean / rstd: f32 [B, 32], kept for backward.
  * Backward: dx = bf16 of the fp32 GroupNorm (o SiLU) gradient, dgamma / dbeta f32 [C] (accumulate != 0: added).
- * workspace: b200_groupnorm_workspace_floats(B, HW, C) floats.  Deterministic (no atomics).
+ * workspace: b200_groupnorm_workspace_floats(B, HW, C) floats.  Deterministic (no atomics).  Every pointer is required,
+ * gamma and beta included.  Element-wise: every pointer but x, y, dy and dx.
  * --------------------------------------------------------------------------------------------------------- */
 long long b200_groupnorm_workspace_floats(int B, int HW, int C);
 int b200_groupnorm_silu_fwd(const void* x_bf16, const float* gamma, const float* beta, void* y_bf16, float* mean, float* rstd,
