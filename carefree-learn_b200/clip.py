@@ -19,7 +19,7 @@ import torch.nn as nn
 from torch import Tensor
 
 from . import ops
-from ._cabi import B200Error, call
+from ._cabi import B200Error
 from .vit import ParamArena, TeTEncoderB200, ViTEncoderB200
 
 
@@ -35,26 +35,16 @@ class _EmbeddingFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx: Any, ids: Tensor, weight: Tensor, padding_idx: int) -> Tensor:
-        if not weight.is_cuda or ids.dtype != torch.int64:
-            raise B200Error("token embedding needs CUDA tensors and int64 indices (there is no CPU fallback)")
         ids = ids.contiguous()
-        n, (V, D) = ids.numel(), weight.shape
-        out = torch.empty(ids.shape + (D,), dtype=torch.float32, device=weight.device)
-        bad = torch.zeros(1, dtype=torch.int32, device=weight.device)
-        call("b200_embedding_fwd", ids.data_ptr(), weight.data_ptr(), out.data_ptr(), n, D, V, bad.data_ptr(), ops._stream())
+        out, _ = ops.embedding_fwd(ids, weight)
         ctx.save_for_backward(ids)
-        ctx.shape, ctx.padding_idx, ctx.bad = (V, D), padding_idx, bad
+        ctx.shape, ctx.padding_idx = weight.shape, padding_idx
         return out
 
     @staticmethod
     def backward(ctx: Any, dnet: Tensor) -> Tuple[Any, ...]:
         (ids,) = ctx.saved_tensors
-        V, D = ctx.shape
-        dw = torch.empty((V, D), dtype=torch.float32, device=dnet.device)
-        ops.fill_f32(dw, 0.0)
-        dnet = dnet.contiguous().float()
-        call("b200_embedding_bwd", ids.data_ptr(), dnet.data_ptr(), dw.data_ptr(), ids.numel(), D, V, int(ctx.padding_idx), ops._stream())
-        return None, dw, None
+        return None, ops.embedding_bwd(ids, dnet.contiguous().float(), *ctx.shape, ctx.padding_idx), None
 
 
 class _ArgmaxPoolFn(torch.autograd.Function):
@@ -62,24 +52,15 @@ class _ArgmaxPoolFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx: Any, net: Tensor, ids: Tensor) -> Tensor:
-        B, T, D = net.shape
-        net = net.contiguous().float()
-        out = torch.empty((B, D), dtype=torch.float32, device=net.device)
-        pos = torch.empty(B, dtype=torch.int32, device=net.device)
-        call("b200_argmax_gather_rows", ids.contiguous().data_ptr(), net.data_ptr(), out.data_ptr(), pos.data_ptr(), B, T, D, ops._stream())
+        out, pos = ops.argmax_gather_rows(net.contiguous().float(), ids.contiguous())
         ctx.save_for_backward(pos)
-        ctx.shape = (B, T, D)
+        ctx.T = net.shape[1]
         return out
 
     @staticmethod
     def backward(ctx: Any, dout: Tensor) -> Tuple[Any, ...]:
         (pos,) = ctx.saved_tensors
-        B, T, D = ctx.shape
-        dx = torch.empty((B, T, D), dtype=torch.float32, device=dout.device)
-        ops.fill_f32(dx, 0.0)
-        dout = dout.contiguous().float()
-        call("b200_scatter_rows", dout.data_ptr(), pos.data_ptr(), dx.data_ptr(), B, T, D, ops._stream())
-        return dx, None
+        return ops.scatter_rows(dout.contiguous().float(), pos, ctx.T), None
 
 
 class _LinearBf16Fn(torch.autograd.Function):
@@ -99,12 +80,7 @@ class _LinearBf16Fn(torch.autograd.Function):
     def backward(ctx: Any, dy: Tensor) -> Tuple[Any, ...]:
         xb, wb = ctx.saved_tensors
         dy = dy.contiguous()
-        if dy.dtype != torch.bfloat16:
-            dy = ops.cast_bf16(dy.float())
-        if dy.stride(0) % 8 != 0:  # TMA rows must be 16-byte aligned
-            pad = torch.zeros((dy.shape[0], (dy.shape[1] + 7) // 8 * 8), dtype=torch.bfloat16, device=dy.device)
-            pad[:, : dy.shape[1]].copy_(dy)
-            dy = pad[:, : dy.shape[1]]
+        dy = ops.tma_aligned(dy if dy.dtype == torch.bfloat16 else ops.cast_bf16(dy.float()))
         dx = ops.gemm(dy, wb, b_mn_major=True)                       # [B, out] . [out, in] -> bf16 [B, in]
         dw = torch.empty(wb.shape, dtype=torch.float32, device=dy.device)
         ops.wgrad(dy, xb, dw)                                        # dy^T . x -> [out, in]
@@ -132,12 +108,7 @@ class _MatmulNTFn(torch.autograd.Function):
     def backward(ctx: Any, dy: Tensor) -> Tuple[Any, ...]:
         a, b = ctx.saved_tensors
         dy = dy.contiguous()
-        if dy.dtype != torch.bfloat16:
-            dy = ops.cast_bf16(dy.float())
-        if dy.stride(0) % 8 != 0:
-            pad = torch.zeros((dy.shape[0], (dy.shape[1] + 7) // 8 * 8), dtype=torch.bfloat16, device=dy.device)
-            pad[:, : dy.shape[1]].copy_(dy)
-            dy = pad[:, : dy.shape[1]]
+        dy = ops.tma_aligned(dy if dy.dtype == torch.bfloat16 else ops.cast_bf16(dy.float()))
         da = ops.gemm(dy, b, b_mn_major=True)                        # dy . b        -> [Ba, L]
         db = ops.gemm(dy, a, a_mn_major=True, b_mn_major=True)       # dy^T . a      -> [Bb, L]
         return (da if ctx.dtypes[0] == torch.bfloat16 else da.float()), (db if ctx.dtypes[1] == torch.bfloat16 else db.float())
@@ -148,24 +119,15 @@ class _SymmetricXentFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx: Any, logits: Tensor) -> Tensor:
-        if not logits.is_cuda or logits.dtype != torch.bfloat16 or logits.dim() != 2 or logits.shape[0] != logits.shape[1] or logits.stride(1) != 1:
-            raise B200Error("symmetric_cross_entropy expects the square bf16 logits CLIPB200.forward returns (CUDA; no CPU fallback)")
-        Bn = logits.shape[0]
-        loss = torch.empty(1, dtype=torch.float32, device=logits.device)
-        ws = torch.empty(2 * Bn, dtype=torch.float32, device=logits.device)
-        call("b200_symmetric_xent_fwd_bwd", logits.data_ptr(), logits.stride(0), loss.data_ptr(), None, ws.data_ptr(), Bn, 1.0, None, ops._stream())
-        ctx.save_for_backward(logits, ws)
+        loss = ops.symmetric_xent(logits)
+        ctx.save_for_backward(logits)
         return loss.reshape(())
 
     @staticmethod
     def backward(ctx: Any, grad_out: Tensor) -> Tuple[Any, ...]:
-        logits, ws = ctx.saved_tensors
-        Bn = logits.shape[0]
-        go = grad_out.reshape(1).contiguous().float()
-        loss = torch.empty(1, dtype=torch.float32, device=logits.device)
+        (logits,) = ctx.saved_tensors
         dlogits = torch.empty_strided(logits.shape, logits.stride(), dtype=torch.bfloat16, device=logits.device)
-        call("b200_symmetric_xent_fwd_bwd", logits.data_ptr(), logits.stride(0), loss.data_ptr(), dlogits.data_ptr(), ws.data_ptr(), Bn, 1.0,
-             go.data_ptr(), ops._stream())
+        ops.symmetric_xent(logits, dlogits=dlogits, grad_scale_dev=grad_out.reshape(1).contiguous().float())
         return (dlogits,)
 
 

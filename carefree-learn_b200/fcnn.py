@@ -10,7 +10,6 @@ silently differing.  Initialisation follows the reference: xavier_normal weights
 """
 from __future__ import annotations
 
-import ctypes
 import math
 from typing import Any, List, Optional, Tuple
 
@@ -19,7 +18,6 @@ import torch.nn as nn
 from torch import Tensor
 
 from . import ops
-from ._cabi import B200Error, call
 from .vit import ParamArena, _register_dotted
 
 
@@ -45,14 +43,14 @@ class _FCNNFn(torch.autograd.Function):
     def forward(ctx: Any, module: "FCNNB200", x: Tensor, *params: Tensor) -> Tensor:
         ctx.module = module
         ctx.save_for_backward(x)
-        return module._launch(x, None, None, want_grads=False)[0]
+        return module._launch(x)[0]
 
     @staticmethod
     def backward(ctx: Any, dpred: Tensor) -> Tuple[Any, ...]:
         module = ctx.module
         (x,) = ctx.saved_tensors
         G = torch.empty_like(module.arena.flat)
-        module._launch(x, None, dpred.contiguous().float(), want_grads=True, grad_out=G)
+        module._launch(x, dpred=dpred.contiguous().float(), grads=G)
         grads = tuple(module.arena.view(G, k) for k, _ in module.arena.spec)
         return (None, None) + grads
 
@@ -91,49 +89,31 @@ class FCNNB200(nn.Module):
             _register_dotted(self, key, p)
             params[key] = p
         self.arena.attach(params)
-        self._woff = (ctypes.c_int * (n + 1))(*[self.arena.offsets[k] for k, _ in spec if k.endswith("weight")])
-        self._boff = (ctypes.c_int * (n + 1))(*([self.arena.offsets[k] for k, _ in spec if k.endswith("bias")] if bias else [-1] * (n + 1)))
-        self._dims = (ctypes.c_int * (n + 2))(*self.dims)
+        self._woff = [self.arena.offsets[k] for k, _ in spec if k.endswith("weight")]
+        self._boff = [self.arena.offsets[k] for k, _ in spec if k.endswith("bias")] if bias else [-1] * (n + 1)
 
     # ---- kernel launch ------------------------------------------------------------------------------------------
-    def _launch(self, x: Tensor, y: Optional[Tensor], dpred: Optional[Tensor], *, want_grads: bool,
-                grad_out: Optional[Tensor] = None, loss_weights: Tuple[float, float] = (1.0, 1.0)) -> Tuple[Tensor, Optional[Tensor]]:
-        if not x.is_cuda:
-            raise B200Error("FCNNB200 runs on CUDA only: there is no CPU fallback")
+    def _launch(self, x: Tensor, *, y: Optional[Tensor] = None, dpred: Optional[Tensor] = None, grads: Optional[Tensor] = None,
+                loss_weights: Tuple[float, float] = (1.0, 1.0)) -> Tuple[Tensor, Optional[Tensor]]:
         if x.dim() != 2 or x.shape[1] != self.input_dim:
             raise ValueError(f"expected input [B, {self.input_dim}], got {tuple(x.shape)}")
         self.arena.ensure()
-        x = x.contiguous().float()
-        M, P = x.shape[0], self.arena.total
-        pred = torch.empty((M, self.output_dim), dtype=torch.float32, device=x.device)
-        nblk = ctypes.c_int(0)
-        part = None
-        if want_grads:
-            part = ops.WORKSPACE.get(x.device, ((M + 127) // 128) * (P + 1), "fcnn")
-            if y is not None:
-                y = y.reshape(M, self.output_dim).contiguous().float()
-        call("b200_fcnn_step", x.data_ptr(), ops._ptr(y), ops._ptr(dpred), self.arena.flat.data_ptr(), pred.data_ptr(), ops._ptr(part),
-             M, len(self.dims) - 1, self._dims, self._woff, self._boff, P, int(y is not None), float(loss_weights[0]),
-             float(loss_weights[1]), ctypes.byref(nblk), ops._stream())
-        loss = None
-        if want_grads:
-            G = grad_out if grad_out is not None else self.arena.grad
-            call("b200_colsum_finish", part.data_ptr(), P + 1, nblk.value, P, G.data_ptr(), 0, 0, ops._stream())
-            if y is not None:
-                loss = torch.empty((), dtype=torch.float32, device=x.device)
-                call("b200_colsum_finish", part.data_ptr() + 4 * P, P + 1, nblk.value, 1, loss.data_ptr(), 0, 0, ops._stream())
-        return pred, loss
+        if y is not None:
+            y = y.reshape(x.shape[0], self.output_dim).contiguous().float()
+        return ops.fcnn_step(x.contiguous().float(), self.arena.flat, self.dims, self._woff, self._boff, y=y, dpred=dpred, grads=grads,
+                             loss_weights=loss_weights)
 
     # ---- reference surface --------------------------------------------------------------------------------------
     def forward(self, net: Tensor) -> Tensor:  # fcnn.py:58-59
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             return _FCNNFn.apply(self, net, *[self.arena.params[k] for k, _ in self.arena.spec])
-        return self._launch(net, None, None, want_grads=False)[0]
+        return self._launch(net)[0]
 
     def train_step(self, x: Tensor, y: Tensor, *, loss_weights: Tuple[float, float] = (1.0, 1.0)) -> Tuple[Tensor, Tensor]:
         """Forward + ``multi_task[mae, mse]`` loss + backward in one launch; sets ``.grad`` of every parameter (views of
         the gradient arena, overwritten every call) and returns (loss, predictions)."""
-        pred, loss = self._launch(x, y, None, want_grads=True, loss_weights=loss_weights)
+        self.arena.ensure()  # may re-create the gradient arena
+        pred, loss = self._launch(x, y=y, grads=self.arena.grad, loss_weights=loss_weights)
         for key, p in self.arena.params.items():
             p.grad = self.arena.g(key)
         return loss, pred

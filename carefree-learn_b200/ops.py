@@ -7,7 +7,7 @@ ATen fallback.
 from __future__ import annotations
 
 import ctypes
-from typing import Dict, Optional, Tuple
+from typing import Dict, Optional, Sequence, Tuple
 
 import torch
 from torch import Tensor
@@ -58,10 +58,48 @@ def _stream() -> int:
     return torch.cuda.current_stream().cuda_stream
 
 
-def _need_cuda(*ts: Optional[Tensor]) -> None:
-    for t in ts:
-        if t is not None and not t.is_cuda:
-            raise B200Error("b200 kernels need CUDA tensors (there is no CPU fallback)")
+def _check(what: str, name: str, t: Optional[Tensor], dtype: Optional[torch.dtype], shape: Optional[Tuple[Optional[int], ...]] = None,
+           *, numel: Optional[int] = None, rows: Optional[int] = None, width: int = 0, ld: Optional[int] = None, view: bool = False,
+           contiguous: bool = True, optional: bool = False) -> int:
+    """Refuses, with ``B200Error("<what>: <name> must be ...")``, a tensor the library cannot take as ``name``.  ``t`` must be a
+    CUDA tensor of ``dtype`` (None: any), contiguous unless ``contiguous=False``, and where given
+      - ``shape``: exactly this shape (None entries: any size); ``numel``: this many elements;
+      - ``rows`` / ``width``: ``rows`` rows of ``width`` elements, [rows, width] or any [..., width] whose leading sizes multiply
+        to ``rows``; with ``ld``, rows ``ld >= width`` elements apart inside ``t`` (e.g. token 0 of each image);
+      - ``view``: instead of contiguous, 2-D with unit inner stride; the row stride is returned (the leading dim the library takes).
+    ``optional``: None passes."""
+    if t is None and optional:
+        return 0
+    ok = t is not None and t.is_cuda and (dtype is None or t.dtype == dtype)
+    if ok and view:
+        ok = t.dim() == 2 and t.stride(1) == 1
+    elif ok and contiguous:
+        ok = t.is_contiguous()
+    if ok and shape is not None:
+        ok = t.dim() == len(shape) and all(s is None or s == n for s, n in zip(shape, t.shape))
+    if ok and numel is not None:
+        ok = t.numel() == numel
+    if ok and rows is not None and ld is not None:
+        ok = width <= ld and t.numel() >= (rows - 1) * ld + width
+    elif ok and rows is not None:
+        ok = t.dim() >= 2 and t.shape[-1] == width and t.numel() == rows * width
+    if not ok:
+        need = ["a 2-D view with unit inner stride" if view else "contiguous" if contiguous else "",
+                "[" + ", ".join("*" if s is None else str(s) for s in shape) + "]" if shape is not None else "",
+                f"{numel} elements" if numel is not None else "",
+                f"{rows} rows of {width}" + (f" elements {ld} apart" if ld is not None else "") if rows is not None else ""]
+        got = "None" if t is None else f"{t.dtype} {list(t.shape)} with strides {list(t.stride())} on {t.device}"
+        kind = f"a CUDA {dtype} tensor" if dtype is not None else "a CUDA tensor"
+        raise B200Error(f"{what}: {name} must be {kind}: " + ", ".join(n for n in need if n) + f" (got {got})")
+    return t.stride(0) if view else 0
+
+
+def _colsum_finish(part: Tensor, part_ld: int, nparts: int, col0: int, cols: int, out: Tensor, *, round_bf16: bool = False,
+                   accumulate: bool = False) -> None:
+    """out[:cols] (+)= the column sums of part[:nparts, col0 : col0 + cols] (fp32 partials, rows part_ld apart): the second pass
+    of every split reduction (bias, LayerNorm and FCNN parameter gradients)."""
+    call("b200_colsum_finish", part.data_ptr() + 4 * col0, part_ld, nparts, cols, out.data_ptr(), int(round_bf16), int(accumulate),
+         _stream())
 
 
 class Workspace:
@@ -100,11 +138,9 @@ def gemm(
     max_ctas: int = 0,
 ) -> Tensor:
     """C[M,N] = A . B^T on wgmma (sm_90a).  ``a``: [M,K] (or [K,M] if a_mn_major); ``b``: [N,K] (or [K,N])."""
-    _need_cuda(a, b, bias, out0, out1, aux)
-    if a.dtype != torch.bfloat16 or b.dtype != torch.bfloat16:
-        raise B200Error("gemm operands must be bf16")
-    if a.dim() != 2 or b.dim() != 2 or a.stride(1) != 1 or b.stride(1) != 1:
-        raise B200Error("gemm operands must be 2-D with unit inner stride")
+    _check("gemm", "a", a, _BF16, view=True)
+    _check("gemm", "b", b, _BF16, view=True)
+    _check("gemm", "bias", bias, None, contiguous=False, optional=True)
     if a_mn_major:
         K, M = a.shape
     else:
@@ -125,16 +161,18 @@ def gemm(
         else:  # rows stay 16-byte aligned for TMA: pad the leading dimension, hand back the [M, N] view
             npad = (N + 7) // 8 * 8
             out0 = torch.empty((M, npad), dtype=dtype, device=a.device)[:, :N]
-    if out0.dtype != dtype:
-        raise B200Error("gemm: out0 dtype does not match the epilogue")
+    if aux_kind or out1_kind:
+        _check("gemm", "out0", out0, dtype, (M, N), view=True)
+    else:
+        _check("gemm", "out0", out0, dtype, contiguous=False)
     ldo = out0.stride(-2)
-    if (aux_kind or out1_kind) and (tuple(out0.shape) != (M, N) or out0.stride(1) != 1):
-        raise B200Error("gemm: out0 must be an [M, N] view with unit inner stride")
     for t, kind, dt, name in ((aux, aux_kind, dtype, "aux"), (out1, out1_kind, _BF16, "out1")):
-        if kind == "rows" and (t is None or t.dtype != dt or tuple(t.shape) != (M, N) or t.stride() != (ldo, 1)):
-            raise B200Error(f"gemm: this epilogue needs a {dt} {name} [M, N] with out0's leading dim")
-    if out1_kind == "dense" and (out1 is None or out1.dtype != _BF16 or tuple(out1.shape) != (M, N // 2) or not out1.is_contiguous()):
-        raise B200Error("gemm: the GEGLU epilogue needs out1 = contiguous bf16 [M, F]")
+        if kind == "rows" and _check("gemm", name, t, dt, (M, N), view=True) != ldo:
+            raise B200Error(f"gemm: {name} must have out0's leading dim {ldo}")
+        if kind == "dense":
+            _check("gemm", name, t, _BF16, (M, N // 2))
+        if kind is None:
+            _check("gemm", name, t, None, contiguous=False, optional=True)
     call(
         "b200_gemm_bf16",
         a.data_ptr(), a.stride(0), int(a_mn_major),
@@ -147,13 +185,22 @@ def gemm(
 def geglu(x: Tensor, w1: Tensor, b1: Tensor, *, max_ctas: int = 0) -> Tuple[Tensor, Tensor]:
     """GEGLU's projection and gate in one GEMM: x [M, K] bf16, w1 [2F, K] bf16 (h rows, then gate rows), b1 [2F] bf16.
     Returns (hg [M, 2F] = bf16(x w1^T + b1), a [M, F] = bf16(h * bf16(gelu(gate))))."""
-    _need_cuda(x, w1, b1)
     F2 = w1.shape[0]
     if F2 % 16 != 0:
         raise B200Error("geglu: need F % 8 == 0")
     a = torch.empty((x.shape[0], F2 // 2), dtype=torch.bfloat16, device=x.device)
     hg = gemm(x, w1, bias=b1, epilogue=EPI_BIAS_GEGLU_BF16, out1=a, max_ctas=max_ctas)
     return hg, a
+
+
+def tma_aligned(t: Tensor) -> Tensor:
+    """``t`` (bf16 [rows, cols]) with rows TMA can load: itself if its inner stride is 1 and its row stride a multiple of 8
+    elements (16 bytes), else a copy in zero-padded rows (e.g. a gradient produced by a foreign loss)."""
+    if t.stride(1) == 1 and t.stride(0) % 8 == 0:
+        return t
+    padded = torch.zeros((t.shape[0], (t.shape[1] + 7) // 8 * 8), dtype=torch.bfloat16, device=t.device)
+    padded[:, : t.shape[1]].copy_(t)
+    return padded[:, : t.shape[1]]
 
 
 _NUM_SMS: Dict[int, int] = {}
@@ -172,13 +219,11 @@ def pick_splits(M: int, N: int, K: int) -> int:
 
 def wgrad(dy: Tensor, x: Tensor, out: Tensor, *, round_bf16: bool = True, accumulate: bool = False) -> Tensor:
     """out[N_out, K_in] (fp32) (+)= dy[M, N_out]^T . x[M, K_in]   (split-K over the M tokens, then reduce)."""
-    _need_cuda(dy, x, out)
-    if dy.dtype != _BF16 or x.dtype != _BF16 or dy.dim() != 2 or x.dim() != 2 or dy.shape[0] != x.shape[0]:
-        raise B200Error("wgrad: need bf16 dy [M, N_out] and x [M, K_in]")
+    _check("wgrad", "dy", dy, _BF16, view=True)
     M, n_out = dy.shape
-    if out.dtype != _F32 or tuple(out.shape) != (n_out, x.shape[1]) or not out.is_contiguous():
-        raise B200Error("wgrad: out must be a contiguous fp32 [N_out, K_in] tensor")
+    _check("wgrad", "x", x, _BF16, (M, None), view=True)
     k_in = x.shape[1]
+    _check("wgrad", "out", out, _F32, (n_out, k_in))
     splits = pick_splits(n_out, k_in, M)
     part = WORKSPACE.get(dy.device, splits * n_out * k_in, "splitk")[: splits * n_out * k_in].view(splits, n_out, k_in)
     gemm(dy, x, a_mn_major=True, b_mn_major=True, epilogue=EPI_PARTIAL_F32, out0=part, splits=splits)
@@ -188,15 +233,13 @@ def wgrad(dy: Tensor, x: Tensor, out: Tensor, *, round_bf16: bool = True, accumu
 
 def colsum(x: Tensor, out: Tensor, *, round_bf16: bool = True, accumulate: bool = False) -> Tensor:
     """out[cols] (fp32) (+)= sum over rows of x[rows, cols] (bf16): bias gradients."""
-    _need_cuda(x, out)
-    if x.dtype != _BF16 or x.dim() != 2 or x.stride(1) != 1:
-        raise B200Error("colsum: x must be a 2-D bf16 view with unit inner stride")
+    ldx = _check("colsum", "x", x, _BF16, view=True)
     rows, cols = x.shape
-    _dense_f32(out, cols, "out", "colsum")
+    _check("colsum", "out", out, _F32, (cols,))
     part = WORKSPACE.get(x.device, _MAX_PARTS * cols, "colsum")
     nparts = ctypes.c_int(0)
-    call("b200_colsum_bf16", x.data_ptr(), x.stride(0), rows, cols, part.data_ptr(), _MAX_PARTS, ctypes.byref(nparts), _stream())
-    call("b200_colsum_finish", part.data_ptr(), cols, nparts.value, cols, out.data_ptr(), int(round_bf16), int(accumulate), _stream())
+    call("b200_colsum_bf16", x.data_ptr(), ldx, rows, cols, part.data_ptr(), _MAX_PARTS, ctypes.byref(nparts), _stream())
+    _colsum_finish(part, cols, nparts.value, 0, cols, out, round_bf16=round_bf16, accumulate=accumulate)
     return out
 
 
@@ -204,10 +247,9 @@ def colsum_per_image(x: Tensor) -> Tuple[Tensor, Tensor]:
     """x: contiguous bf16 [B, ..., C] (the pixels of each image in between).  One pass over x returns (per_image bf16 [B, C] =
     bf16(sum over image b's rows), total fp32 [C] = float(bf16(sum over all rows))): the gradients of a per-image [B, C] table
     added to every pixel, and of the bias of the conv that wrote x."""
-    _need_cuda(x)
-    if x.dtype != torch.bfloat16 or x.dim() < 2 or not x.is_contiguous():
-        raise B200Error("colsum_per_image: need contiguous bf16 [B, ..., C]")
-    B, C = x.shape[0], x.shape[-1]
+    C = x.shape[-1]
+    _check("colsum_per_image", "x", x, _BF16, rows=x.numel() // max(C, 1), width=C)
+    B = x.shape[0]
     HW = x.numel() // max(B * C, 1)
     per_image = torch.empty((B, C), dtype=torch.bfloat16, device=x.device)
     total = torch.empty(C, dtype=torch.float32, device=x.device)
@@ -219,20 +261,12 @@ def colsum_per_image(x: Tensor) -> Tuple[Tensor, Tensor]:
 # ----------------------------------------------------------------------------------------------------------------
 # LayerNorm
 # ----------------------------------------------------------------------------------------------------------------
-def _strided_f32(t: Tensor, rows: int, dim: int, ld: int, msg: str) -> None:
-    """t: contiguous fp32 holding `rows` rows of `dim` elements `ld` apart (ld > dim: e.g. token 0 of each image)."""
-    if t.dtype != _F32 or not t.is_contiguous() or ld < dim or t.numel() < (rows - 1) * ld + dim:
-        raise B200Error(msg)
-
-
 def layernorm_fwd(x: Tensor, gamma: Tensor, beta: Tensor, eps: float, *, rows: int, dim: int, ld_x: int,
                   y_f32: Optional[Tensor] = None) -> Tuple[Tensor, Tensor, Tensor]:
-    _need_cuda(x, gamma, beta, y_f32)
-    _strided_f32(x, rows, dim, ld_x, "layernorm_fwd: x must be contiguous fp32 holding rows of dim elements ld_x apart")
-    _dense_f32(gamma, dim, "gamma", "layernorm_fwd")
-    _dense_f32(beta, dim, "beta", "layernorm_fwd")
-    if y_f32 is not None:
-        _packed_rows(y_f32, rows, dim, "layernorm_fwd: y_f32 must be contiguous fp32 [rows, dim]", _F32)
+    _check("layernorm_fwd", "x", x, _F32, rows=rows, width=dim, ld=ld_x)
+    _check("layernorm_fwd", "gamma", gamma, _F32, (dim,))
+    _check("layernorm_fwd", "beta", beta, _F32, (dim,))
+    _check("layernorm_fwd", "y_f32", y_f32, _F32, rows=rows, width=dim, optional=True)
     y = torch.empty((rows, dim), dtype=torch.bfloat16, device=x.device)
     mean = torch.empty(rows, dtype=torch.float32, device=x.device)
     rstd = torch.empty(rows, dtype=torch.float32, device=x.device)
@@ -248,20 +282,15 @@ def layernorm_bwd(
 ) -> None:
     """LayerNorm backward.  ``dx_colsum`` (fp32 [dim]): also receives the bf16-rounded column sums of ``dx_bf16``,
     i.e. the bias gradient of the Linear layer whose dY this dx is -- fused, no extra pass over dx."""
-    _need_cuda(dy, x, gamma, mean, rstd, dres, dx_out, dx_bf16, dgamma, dbeta, dx_colsum)
-    if dy.dtype not in (_BF16, _F32):
-        raise B200Error("layernorm_bwd: dy must be bf16 or fp32")
-    _packed_rows(dy, rows, dim, "layernorm_bwd: dy must be contiguous [rows, dim]", dy.dtype)
-    _strided_f32(x, rows, dim, ld_x, "layernorm_bwd: x must be contiguous fp32 holding rows of dim elements ld_x apart")
-    _strided_f32(dx_out, rows, dim, ld_dx, "layernorm_bwd: dx_out must be contiguous fp32 holding rows of dim elements ld_dx apart")
-    if dres is not None:
-        _strided_f32(dres, rows, dim, ld_dx, "layernorm_bwd: dres must be contiguous fp32 holding rows of dim elements ld_dx apart")
-    if dx_bf16 is not None:
-        _packed_rows(dx_bf16, rows, dim, "layernorm_bwd: dx_bf16 must be contiguous bf16 [rows, dim]")
+    what = "layernorm_bwd"
+    _check(what, "dy", dy, _F32 if dy.dtype == _F32 else _BF16, rows=rows, width=dim)  # bf16, or fp32 (an fp32 residual stream)
+    _check(what, "x", x, _F32, rows=rows, width=dim, ld=ld_x)
+    _check(what, "dx_out", dx_out, _F32, rows=rows, width=dim, ld=ld_dx)
+    _check(what, "dres", dres, _F32, rows=rows, width=dim, ld=ld_dx, optional=True)
+    _check(what, "dx_bf16", dx_bf16, _BF16, rows=rows, width=dim, optional=True)
     for t, n, name in ((gamma, dim, "gamma"), (mean, rows, "mean"), (rstd, rows, "rstd"), (dgamma, dim, "dgamma"), (dbeta, dim, "dbeta")):
-        _dense_f32(t, n, name, "layernorm_bwd")
-    if dx_colsum is not None:
-        _dense_f32(dx_colsum, dim, "dx_colsum", "layernorm_bwd")
+        _check(what, name, t, _F32, (n,))
+    _check(what, "dx_colsum", dx_colsum, _F32, (dim,), optional=True)
     nw = 3 if dx_colsum is not None else 2
     part = WORKSPACE.get(x.device, 3 * _MAX_PARTS * dim, "lnbwd")
     nparts = ctypes.c_int(0)
@@ -276,32 +305,21 @@ def layernorm_bwd(
              dim, dx_colsum.data_ptr(), 1, int(accumulate), _stream())
         return
     if adjacent:
-        call("b200_colsum_finish", part.data_ptr(), nw * dim, nparts.value, 2 * dim, dgamma.data_ptr(), 0, int(accumulate), _stream())
+        _colsum_finish(part, nw * dim, nparts.value, 0, 2 * dim, dgamma, accumulate=accumulate)
     else:
-        call("b200_colsum_finish", part.data_ptr(), nw * dim, nparts.value, dim, dgamma.data_ptr(), 0, int(accumulate), _stream())
-        call("b200_colsum_finish", part.data_ptr() + 4 * dim, nw * dim, nparts.value, dim, dbeta.data_ptr(), 0, int(accumulate), _stream())
+        _colsum_finish(part, nw * dim, nparts.value, 0, dim, dgamma, accumulate=accumulate)
+        _colsum_finish(part, nw * dim, nparts.value, dim, dim, dbeta, accumulate=accumulate)
     if dx_colsum is not None:
-        call("b200_colsum_finish", part.data_ptr() + 8 * dim, nw * dim, nparts.value, dim, dx_colsum.data_ptr(), 1, int(accumulate), _stream())
-
-
-def _dense_bf16(t: Tensor, name: str) -> None:
-    if t.dtype != torch.bfloat16 or t.dim() != 2 or not t.is_contiguous():
-        raise B200Error(f"layernorm_bf16: {name} must be a contiguous bf16 [rows, dim] tensor")
-
-
-def _dense_f32(t: Tensor, n: int, name: str, what: str = "layernorm_bf16") -> None:
-    if t.dtype != torch.float32 or tuple(t.shape) != (n,) or not t.is_contiguous():
-        raise B200Error(f"{what}: {name} must be a contiguous fp32 [{n}] tensor")
+        _colsum_finish(part, nw * dim, nparts.value, 2 * dim, dim, dx_colsum, round_bf16=True, accumulate=accumulate)
 
 
 def layernorm_bf16_fwd(x: Tensor, gamma: Tensor, beta: Tensor, eps: float) -> Tuple[Tensor, Tensor, Tensor]:
     """LayerNorm of bf16 rows x [rows, dim] with fp32 statistics: (y = bf16(LN(x)), mean f32 [rows], rstd f32 [rows]).
     gamma / beta: contiguous fp32 [dim]."""
-    _need_cuda(x, gamma, beta)
-    _dense_bf16(x, "x")
+    _check("layernorm_bf16_fwd", "x", x, _BF16, (None, None))
     rows, dim = x.shape
-    _dense_f32(gamma, dim, "gamma")
-    _dense_f32(beta, dim, "beta")
+    _check("layernorm_bf16_fwd", "gamma", gamma, _F32, (dim,))
+    _check("layernorm_bf16_fwd", "beta", beta, _F32, (dim,))
     y = torch.empty_like(x)
     mean = torch.empty(rows, dtype=torch.float32, device=x.device)
     rstd = torch.empty(rows, dtype=torch.float32, device=x.device)
@@ -313,31 +331,26 @@ def layernorm_bf16_fwd(x: Tensor, gamma: Tensor, beta: Tensor, eps: float) -> Tu
 def layernorm_bf16_bwd(dy: Tensor, x: Tensor, gamma: Tensor, mean: Tensor, rstd: Tensor, *, dres: Optional[Tensor] = None,
                        dgamma: Optional[Tensor] = None, dbeta: Optional[Tensor] = None, accumulate: bool = False) -> Tuple[Tensor, Tensor, Tensor]:
     """(dx, dgamma, dbeta): dx = bf16(dres + bf16(LN'(dy))) bf16 [rows, dim]; dgamma / dbeta fp32 [dim] (``accumulate``: added)."""
-    _need_cuda(dy, x, gamma, mean, rstd, dres)
-    _dense_bf16(dy, "dy")
-    _dense_bf16(x, "x")
-    if dres is not None:
-        _dense_bf16(dres, "dres")
+    what = "layernorm_bf16_bwd"
+    _check(what, "x", x, _BF16, (None, None))
     rows, dim = x.shape
-    if dy.shape != x.shape or (dres is not None and dres.shape != x.shape):
-        raise B200Error("layernorm_bf16_bwd: dy / dres must have x's shape")
-    _dense_f32(gamma, dim, "gamma")
-    _dense_f32(mean, rows, "mean")
-    _dense_f32(rstd, rows, "rstd")
+    _check(what, "dy", dy, _BF16, (rows, dim))
+    _check(what, "dres", dres, _BF16, (rows, dim), optional=True)
+    for t, n, name in ((gamma, dim, "gamma"), (mean, rows, "mean"), (rstd, rows, "rstd")):
+        _check(what, name, t, _F32, (n,))
     dx = torch.empty_like(x)
     if dgamma is None:
         dgamma = torch.empty(dim, dtype=torch.float32, device=x.device)
         dbeta = torch.empty(dim, dtype=torch.float32, device=x.device)
         accumulate = False
-    _need_cuda(dgamma, dbeta)
-    _dense_f32(dgamma, dim, "dgamma")
-    _dense_f32(dbeta, dim, "dbeta")
+    _check(what, "dgamma", dgamma, _F32, (dim,))
+    _check(what, "dbeta", dbeta, _F32, (dim,))
     part = WORKSPACE.get(x.device, 2 * _MAX_PARTS * dim, "lnbwd")
     nparts = ctypes.c_int(0)
     call("b200_layernorm_bf16_bwd", dy.data_ptr(), x.data_ptr(), gamma.data_ptr(), mean.data_ptr(), rstd.data_ptr(), _ptr(dres),
          dx.data_ptr(), part.data_ptr(), _MAX_PARTS, ctypes.byref(nparts), rows, dim, _stream())
-    call("b200_colsum_finish", part.data_ptr(), 2 * dim, nparts.value, dim, dgamma.data_ptr(), 0, int(accumulate), _stream())
-    call("b200_colsum_finish", part.data_ptr() + 4 * dim, 2 * dim, nparts.value, dim, dbeta.data_ptr(), 0, int(accumulate), _stream())
+    _colsum_finish(part, 2 * dim, nparts.value, 0, dim, dgamma, accumulate=accumulate)
+    _colsum_finish(part, 2 * dim, nparts.value, dim, dim, dbeta, accumulate=accumulate)
     return dx, dgamma, dbeta
 
 
@@ -348,21 +361,9 @@ ATTENTION_MAX_T = 16384   # longest sequence the attention kernels accept
 ATTENTION_RESIDENT_MAX_T = 256  # up to here a whole head fits in shared memory; longer sequences use the streamed kernels
 
 
-def _packed_rows(t: Tensor, rows: int, width: int, msg: str, dtype: torch.dtype = _BF16) -> None:
-    """t: contiguous `dtype` holding `rows` rows of `width` elements ([rows, width], or [B, T, width] with B * T = rows)."""
-    if t.dtype != dtype or not t.is_contiguous() or t.dim() < 2 or t.shape[-1] != width or t.numel() != rows * width:
-        raise B200Error(msg)
-
-
-def _lse(lse: Tensor, B: int, H: int, T: int, what: str) -> None:
-    if lse.dtype != torch.float32 or tuple(lse.shape) != (B, H, T) or not lse.is_contiguous():
-        raise B200Error(f"{what}: lse must be a contiguous fp32 [B, H, T] tensor")
-
-
 def attention_fwd(qkv: Tensor, B: int, T: int, H: int, *, scale: Optional[float] = None, causal: bool = False) -> Tuple[Tensor, Tensor]:
-    _need_cuda(qkv)
     D = H * 64
-    _packed_rows(qkv, B * T, 3 * D, "attention_fwd: qkv must be contiguous bf16 [B, T, 3*H*64]")
+    _check("attention_fwd", "qkv", qkv, _BF16, rows=B * T, width=3 * D)
     out = torch.empty((B * T, D), dtype=torch.bfloat16, device=qkv.device)
     lse = torch.empty((B, H, T), dtype=torch.float32, device=qkv.device)
     sc = float(scale) if scale is not None else 0.125
@@ -375,17 +376,15 @@ def attention_bwd(qkv: Tensor, out: Tensor, dout: Tensor, lse: Tensor, B: int, T
                   dbias: Optional[Tensor] = None) -> Tensor:
     """dqkv (bf16 [B*T, 3*H*64]).  ``dbias`` (fp32 [3*H*64]): also receives the bf16-rounded column sums of dqkv -- the
     gradient of the packed qkv bias -- accumulated inside the kernel (no separate pass over dqkv)."""
-    _need_cuda(qkv, out, dout, lse, dqkv, dbias)
-    D = H * 64
-    _packed_rows(qkv, B * T, 3 * D, "attention_bwd: qkv must be contiguous bf16 [B, T, 3*H*64]")
-    _packed_rows(out, B * T, D, "attention_bwd: out must be contiguous bf16 [B*T, H*64]")
-    _packed_rows(dout, B * T, D, "attention_bwd: dout must be contiguous bf16 [B*T, H*64]")
-    _lse(lse, B, H, T, "attention_bwd")
+    what, D = "attention_bwd", H * 64
+    _check(what, "qkv", qkv, _BF16, rows=B * T, width=3 * D)
+    _check(what, "out", out, _BF16, rows=B * T, width=D)
+    _check(what, "dout", dout, _BF16, rows=B * T, width=D)
+    _check(what, "lse", lse, _F32, (B, H, T))
     if dqkv is None:
         dqkv = torch.empty((B * T, 3 * D), dtype=torch.bfloat16, device=qkv.device)
-    _packed_rows(dqkv, B * T, 3 * D, "attention_bwd: dqkv must be contiguous bf16 [B*T, 3*H*64]")
-    if dbias is not None:
-        _dense_f32(dbias, 3 * D, "dbias", "attention_bwd")
+    _check(what, "dqkv", dqkv, _BF16, rows=B * T, width=3 * D)
+    _check(what, "dbias", dbias, _F32, (3 * D,), optional=True)
     sc = float(scale) if scale is not None else 0.125
     part = WORKSPACE.get(qkv.device, B * 3 * D, "attn_dbias") if dbias is not None else None
     if T <= ATTENTION_RESIDENT_MAX_T:
@@ -396,19 +395,13 @@ def attention_bwd(qkv: Tensor, out: Tensor, dout: Tensor, lse: Tensor, B: int, T
         call("b200_attention_long_bwd", qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr(), dqkv.data_ptr(), B, T, H, 64, sc,
              int(causal), _ptr(part), ws.data_ptr(), _stream())
     if dbias is not None:
-        call("b200_colsum_finish", part.data_ptr(), 3 * D, B, 3 * D, dbias.data_ptr(), 1, 0, _stream())
+        _colsum_finish(part, 3 * D, B, 0, 3 * D, dbias, round_bf16=True)
     return dqkv
-
-
-def _rows_view(t: Tensor, name: str) -> int:
-    if t.dtype != torch.bfloat16 or t.dim() != 2 or t.stride(1) != 1:
-        raise B200Error(f"cross_attention: {name} must be a 2-D bf16 view with unit inner stride")
-    return t.stride(0)
 
 
 def _cross_operands(q: Tensor, k: Tensor, v: Tensor, B: int, H: int) -> Tuple[int, int, int, int, int]:
     """(ldq, ldk, Tq, Tk, Dh) of the q / k / v views."""
-    ldq, ldk, ldv = _rows_view(q, "q"), _rows_view(k, "k"), _rows_view(v, "v")
+    ldq, ldk, ldv = (_check("cross_attention", name, t, _BF16, view=True) for name, t in (("q", q), ("k", k), ("v", v)))
     if ldk != ldv or k.shape != v.shape:
         raise B200Error("cross_attention: k and v must share shape and leading dim")
     L = q.shape[1]
@@ -421,7 +414,6 @@ def cross_attention_fwd(q: Tensor, k: Tensor, v: Tensor, B: int, H: int, *, scal
                         causal: bool = False) -> Tuple[Tensor, Tensor]:
     """Attention with separate operands: q [B*Tq, >= H*Dh], k / v [B*Tk, >= H*Dh] (bf16 2-D views with unit inner stride, e.g.
     column slices of one packed projection), head h at columns [h*Dh, (h+1)*Dh).  Returns (out bf16 [B*Tq, H*Dh], lse f32 [B, H, Tq])."""
-    _need_cuda(q, k, v)
     ldq, ldk, Tq, Tk, Dh = _cross_operands(q, k, v, B, H)
     out = torch.empty((B * Tq, H * Dh), dtype=torch.bfloat16, device=q.device)
     lse = torch.empty((B, H, Tq), dtype=torch.float32, device=q.device)
@@ -436,37 +428,35 @@ def cross_attention_bwd(q: Tensor, k: Tensor, v: Tensor, out: Tensor, dout: Tens
                         dv: Optional[Tensor] = None) -> Tuple[Tensor, Tensor, Tensor]:
     """(dq, dk, dv) of ``cross_attention_fwd``.  dq / dk / dv may be given as views (dq with q's leading dim, dk / dv with k's), e.g.
     column slices of one packed [M, 3L] gradient for self-attention; otherwise they are allocated contiguous."""
-    _need_cuda(q, k, v, out, dout, lse, dq, dk, dv)
+    what = "cross_attention_bwd"
     ldq, ldk, Tq, Tk, Dh = _cross_operands(q, k, v, B, H)
     L = q.shape[1]
-    if _rows_view(dout, "dout") != _rows_view(out, "out"):
-        raise B200Error("cross_attention_bwd: dout must share out's leading dim")
-    if tuple(out.shape) != (B * Tq, L) or dout.shape != out.shape:
-        raise B200Error("cross_attention_bwd: out / dout must have q's rows and width")
-    _lse(lse, B, H, Tq, "cross_attention_bwd")
+    ldo = _check(what, "out", out, _BF16, (B * Tq, L), view=True)
+    if _check(what, "dout", dout, _BF16, (B * Tq, L), view=True) != ldo:
+        raise B200Error(f"{what}: dout must share out's leading dim")
+    _check(what, "lse", lse, _F32, (B, H, Tq))
     if dq is None and dk is None and dv is None and ldq == L and ldk == L:
         dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
     if dq is None or dk is None or dv is None:
-        raise B200Error("cross_attention_bwd: give all of dq, dk, dv or none (with contiguous q / k / v)")
-    if _rows_view(dq, "dq") != ldq or _rows_view(dk, "dk") != ldk or _rows_view(dv, "dv") != ldk:
-        raise B200Error("cross_attention_bwd: dq must share q's leading dim, dk / dv k's")
-    if dq.shape != q.shape or dk.shape != k.shape or dv.shape != k.shape:
-        raise B200Error("cross_attention_bwd: dq must have q's shape, dk / dv k's")
+        raise B200Error(f"{what}: give all of dq, dk, dv or none (with contiguous q / k / v)")
+    for name, t, like, ld in (("dq", dq, q, ldq), ("dk", dk, k, ldk), ("dv", dv, k, ldk)):
+        if _check(what, name, t, _BF16, tuple(like.shape), view=True) != ld:
+            raise B200Error(f"{what}: dq must share q's leading dim, dk / dv k's")
     sc = float(scale) if scale is not None else Dh ** -0.5
     ws = WORKSPACE.get(q.device, int(_cabi.lib().b200_cross_attention_bwd_workspace_floats(B, Tq, Tk, H, Dh)), "cross_attn")
-    call("b200_cross_attention_bwd", q.data_ptr(), ldq, k.data_ptr(), v.data_ptr(), ldk, out.data_ptr(), out.stride(0), dout.data_ptr(),
+    call("b200_cross_attention_bwd", q.data_ptr(), ldq, k.data_ptr(), v.data_ptr(), ldk, out.data_ptr(), ldo, dout.data_ptr(),
          lse.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), B, Tq, Tk, H, Dh, sc, int(causal), ws.data_ptr(), _stream())
     return dq, dk, dv
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# patch embedding glue, loss, casts
+# glue (patch embedding, CLIP text: integer-indexed row moves, bit-exact), losses, casts
 # ----------------------------------------------------------------------------------------------------------------
 def patch_im2col(x: Tensor, patch: int) -> Tensor:
-    _need_cuda(x)
+    _check("patch_im2col", "x", x, _F32, (None, None, None, None))
     B, C, Hh, Ww = x.shape
-    if Hh != Ww or x.dtype != torch.float32 or not x.is_contiguous():
-        raise B200Error("patch_im2col: need contiguous fp32 [B, C, S, S]")
+    if Hh != Ww:
+        raise B200Error("patch_im2col: x must be square images [B, C, S, S]")
     side = Hh // patch
     cols = torch.empty((B * side * side, C * patch * patch), dtype=torch.bfloat16, device=x.device)
     call("b200_patch_im2col", x.data_ptr(), cols.data_ptr(), B, C, Hh, patch, _stream())
@@ -475,10 +465,10 @@ def patch_im2col(x: Tensor, patch: int) -> Tensor:
 
 def patch_im2col_u8(x: Tensor, patch: int, division: float = 255.0, mean=None, std=None) -> Tensor:
     """uint8 [B, S, S, C] (HWC) -> normalised bf16 im2col matrix: the reference's host-side input pipeline fused into the stem."""
-    _need_cuda(x)
-    if x.dtype != torch.uint8 or x.dim() != 4 or not x.is_contiguous() or x.shape[1] != x.shape[2]:
-        raise B200Error("patch_im2col_u8: need contiguous uint8 [B, S, S, C]")
-    B, S, _, C = x.shape
+    _check("patch_im2col_u8", "x", x, torch.uint8, (None, None, None, None))
+    B, S, Ww, C = x.shape
+    if S != Ww:
+        raise B200Error("patch_im2col_u8: x must be square images [B, S, S, C]")
     side = S // patch
     cols = torch.empty((B * side * side, C * patch * patch), dtype=torch.bfloat16, device=x.device)
     dbl = ctypes.c_double * C
@@ -490,42 +480,35 @@ def patch_im2col_u8(x: Tensor, patch: int, division: float = 255.0, mean=None, s
 
 def add_pos(x: Tensor, pos: Tensor, B: int, T: int, D: int) -> Tensor:
     """net[b, t, :] = x[b, t, :] + pos[t, :] (fp32): the text tower's input stage."""
-    _need_cuda(x, pos)
-    _packed_rows(x, B * T, D, "add_pos: x must be contiguous fp32 [B, T, D]", _F32)
-    _packed_rows(pos, T, D, "add_pos: pos must be contiguous fp32 [T, D]", _F32)
+    _check("add_pos", "x", x, _F32, rows=B * T, width=D)
+    _check("add_pos", "pos", pos, _F32, rows=T, width=D)
     net = torch.empty((B, T, D), dtype=torch.float32, device=x.device)
     call("b200_add_pos", x.data_ptr(), pos.data_ptr(), net.data_ptr(), B, T, D, _stream())
     return net
 
 
 def add_pos_bwd(dnet: Tensor, dpos: Tensor, B: int, T: int, D: int, accumulate: bool = False) -> None:
-    _need_cuda(dnet, dpos)
-    _packed_rows(dnet, B * T, D, "add_pos_bwd: dnet must be contiguous fp32 [B, T, D]", _F32)
-    _packed_rows(dpos, T, D, "add_pos_bwd: dpos must be contiguous fp32 [T, D]", _F32)
+    _check("add_pos_bwd", "dnet", dnet, _F32, rows=B * T, width=D)
+    _check("add_pos_bwd", "dpos", dpos, _F32, rows=T, width=D)
     call("b200_add_pos_bwd", dnet.data_ptr(), dpos.data_ptr(), B, T, D, int(accumulate), _stream())
 
 
 def assemble_tokens(patch: Tensor, cls: Tensor, pos: Tensor, B: int, np_: int, D: int, conv_bias: Optional[Tensor] = None) -> Tensor:
     """net[b, 0] = cls + pos[0]; net[b, t] = float(patch[b, t-1]) + pos[t].  ``conv_bias`` (bf16 [D]): the patch rows first become
     bf16(patch + bias) -- the separate bf16 bias add eager's convolution performs."""
-    _need_cuda(patch, cls, pos, conv_bias)
-    _packed_rows(patch, B * np_, D, "assemble_tokens: patch must be contiguous bf16 [B * np, D]")
-    _packed_rows(pos, np_ + 1, D, "assemble_tokens: pos must be contiguous fp32 [np + 1, D]", _F32)
-    if cls.dtype != _F32 or not cls.is_contiguous() or cls.numel() != D:
-        raise B200Error("assemble_tokens: cls must be contiguous fp32 with D elements")
-    if conv_bias is not None and (conv_bias.dtype != _BF16 or not conv_bias.is_contiguous() or conv_bias.numel() != D):
-        raise B200Error("assemble_tokens: conv_bias must be contiguous bf16 with D elements")
+    _check("assemble_tokens", "patch", patch, _BF16, rows=B * np_, width=D)
+    _check("assemble_tokens", "pos", pos, _F32, rows=np_ + 1, width=D)
+    _check("assemble_tokens", "cls", cls, _F32, numel=D)
+    _check("assemble_tokens", "conv_bias", conv_bias, _BF16, numel=D, optional=True)
     net = torch.empty((B, np_ + 1, D), dtype=torch.float32, device=patch.device)
     call("b200_assemble_tokens", patch.data_ptr(), cls.data_ptr(), pos.data_ptr(), net.data_ptr(), B, np_, D, _ptr(conv_bias), _stream())
     return net
 
 
 def assemble_tokens_bwd(dnet: Tensor, dpos: Tensor, dcls: Tensor, B: int, np_: int, D: int, accumulate: bool = False) -> Tensor:
-    _need_cuda(dnet, dpos, dcls)
-    _packed_rows(dnet, B * (np_ + 1), D, "assemble_tokens_bwd: dnet must be contiguous fp32 [B, np + 1, D]", _F32)
-    _packed_rows(dpos, np_ + 1, D, "assemble_tokens_bwd: dpos must be contiguous fp32 [np + 1, D]", _F32)
-    if dcls.dtype != _F32 or not dcls.is_contiguous() or dcls.numel() != D:
-        raise B200Error("assemble_tokens_bwd: dcls must be contiguous fp32 with D elements")
+    _check("assemble_tokens_bwd", "dnet", dnet, _F32, rows=B * (np_ + 1), width=D)
+    _check("assemble_tokens_bwd", "dpos", dpos, _F32, rows=np_ + 1, width=D)
+    _check("assemble_tokens_bwd", "dcls", dcls, _F32, numel=D)
     dpatch = torch.empty((B * np_, D), dtype=torch.bfloat16, device=dnet.device)
     call("b200_assemble_tokens_bwd", dnet.data_ptr(), dpatch.data_ptr(), dpos.data_ptr(), dcls.data_ptr(), B, np_, D, int(accumulate), _stream())
     return dpatch
@@ -534,28 +517,43 @@ def assemble_tokens_bwd(dnet: Tensor, dpos: Tensor, dcls: Tensor, B: int, np_: i
 def softmax_xent(logits: Tensor, labels: Tensor, *, grad_scale: float = 1.0, need_grad: bool = True,
                  grad_scale_dev: Optional[Tensor] = None) -> Tuple[Tensor, Tensor, Optional[Tensor], Tensor]:
     """Returns (loss_mean[1], loss_rows[B], dlogits bf16 [B,C] or None, bad_label_flag int32[1])."""
-    _need_cuda(logits, labels)
+    ldl = _check("softmax_xent", "logits", logits, _BF16, view=True)
     Bn, C = logits.shape
-    if logits.dtype != torch.bfloat16 or logits.stride(1) != 1:
-        raise B200Error("softmax_xent: logits must be bf16 with unit inner stride")
-    if labels.dtype != torch.int64 or labels.numel() != Bn or not labels.is_contiguous():
-        raise B200Error("softmax_xent: labels must be contiguous int64 with one entry per row")
+    _check("softmax_xent", "labels", labels, torch.int64, numel=Bn)
     loss_rows = torch.empty(Bn, dtype=torch.float32, device=logits.device)
     loss_mean = torch.empty(1, dtype=torch.float32, device=logits.device)
     # dlogits shares the logits' row stride (a multiple of 8 elements so the head dgrad / wgrad can TMA it)
-    dlogits = torch.empty_strided((Bn, C), (logits.stride(0), 1), dtype=torch.bfloat16, device=logits.device) if need_grad else None
+    dlogits = torch.empty_strided((Bn, C), (ldl, 1), dtype=torch.bfloat16, device=logits.device) if need_grad else None
     bad = torch.zeros(1, dtype=torch.int32, device=logits.device)
     call(
-        "b200_softmax_xent_fwd_bwd", logits.data_ptr(), logits.stride(0), labels.data_ptr(), loss_rows.data_ptr(),
+        "b200_softmax_xent_fwd_bwd", logits.data_ptr(), ldl, labels.data_ptr(), loss_rows.data_ptr(),
         loss_mean.data_ptr(), _ptr(dlogits), bad.data_ptr(), Bn, C, float(grad_scale), _ptr(grad_scale_dev), _stream(),
     )
     return loss_mean, loss_rows, dlogits, bad
 
 
+def symmetric_xent(logits: Tensor, *, dlogits: Optional[Tensor] = None, grad_scale: float = 1.0,
+                   grad_scale_dev: Optional[Tensor] = None) -> Tensor:
+    """CLIP's contrastive loss (CE(L, arange) + CE(L^T, arange)) / 2 of the square bf16 logits L [B, B] (unit inner stride), fp32
+    [1].  ``dlogits`` (a bf16 [B, B] view with L's row stride) also receives the gradient, scaled by ``grad_scale`` (and by the
+    device fp32 [1] ``grad_scale_dev``)."""
+    what = "symmetric_xent"
+    ldl = _check(what, "logits", logits, _BF16, view=True)
+    Bn = logits.shape[0]
+    if logits.shape[1] != Bn:
+        raise B200Error(f"{what}: logits must be square, got {list(logits.shape)}")
+    if dlogits is not None and _check(what, "dlogits", dlogits, _BF16, (Bn, Bn), view=True) != ldl:
+        raise B200Error(f"{what}: dlogits must share logits' row stride")
+    _check(what, "grad_scale_dev", grad_scale_dev, _F32, (1,), optional=True)
+    loss = torch.empty(1, dtype=torch.float32, device=logits.device)
+    ws = torch.empty(2 * Bn, dtype=torch.float32, device=logits.device)
+    call("b200_symmetric_xent_fwd_bwd", logits.data_ptr(), ldl, loss.data_ptr(), _ptr(dlogits), ws.data_ptr(), Bn, float(grad_scale),
+         _ptr(grad_scale_dev), _stream())
+    return loss
+
+
 def cast_bf16(src: Tensor, dst: Optional[Tensor] = None) -> Tensor:
-    _need_cuda(src)
-    if src.dtype != torch.float32 or not src.is_contiguous():
-        raise B200Error("cast_bf16: need contiguous fp32")
+    _check("cast_bf16", "src", src, _F32)
     if dst is None:
         dst = torch.empty(src.shape, dtype=torch.bfloat16, device=src.device)
     call("b200_cast_f32_to_bf16", src.data_ptr(), dst.data_ptr(), src.numel(), _stream())
@@ -563,11 +561,107 @@ def cast_bf16(src: Tensor, dst: Optional[Tensor] = None) -> Tensor:
 
 
 def fill_f32(dst: Tensor, value: float) -> Tensor:
-    _need_cuda(dst)
-    if dst.dtype != _F32 or not dst.is_contiguous():
-        raise B200Error("fill_f32: need contiguous fp32")
+    _check("fill_f32", "dst", dst, _F32)
     call("b200_fill_f32", dst.data_ptr(), float(value), dst.numel(), _stream())
     return dst
+
+
+def embedding_fwd(ids: Tensor, weight: Tensor) -> Tuple[Tensor, Tensor]:
+    """(out fp32 [*ids.shape, D] = weight[ids], bad int32 [1]: non-zero if an id was outside [0, V)).  ids: contiguous int64;
+    weight: contiguous fp32 [V, D]."""
+    _check("embedding_fwd", "ids", ids, torch.int64)
+    _check("embedding_fwd", "weight", weight, _F32, (None, None))
+    V, D = weight.shape
+    out = torch.empty(ids.shape + (D,), dtype=torch.float32, device=weight.device)
+    bad = torch.zeros(1, dtype=torch.int32, device=weight.device)
+    call("b200_embedding_fwd", ids.data_ptr(), weight.data_ptr(), out.data_ptr(), ids.numel(), D, V, bad.data_ptr(), _stream())
+    return out, bad
+
+
+def embedding_bwd(ids: Tensor, dnet: Tensor, V: int, D: int, padding_idx: int) -> Tensor:
+    """dweight fp32 [V, D]: the rows of dnet (contiguous fp32, one row of D per id) summed into the rows their ids name, except
+    ``padding_idx``'s."""
+    _check("embedding_bwd", "ids", ids, torch.int64)
+    _check("embedding_bwd", "dnet", dnet, _F32, numel=ids.numel() * D)
+    dw = fill_f32(torch.empty((V, D), dtype=torch.float32, device=dnet.device), 0.0)
+    call("b200_embedding_bwd", ids.data_ptr(), dnet.data_ptr(), dw.data_ptr(), ids.numel(), D, V, int(padding_idx), _stream())
+    return dw
+
+
+def argmax_gather_rows(net: Tensor, ids: Tensor) -> Tuple[Tensor, Tensor]:
+    """(out fp32 [B, D] = net[b, pos[b]], pos int32 [B] = the first arg-max of ids[b]).  net: contiguous fp32 [B, T, D]; ids:
+    contiguous int64 [B, T]."""
+    _check("argmax_gather_rows", "net", net, _F32, (None, None, None))
+    B, T, D = net.shape
+    _check("argmax_gather_rows", "ids", ids, torch.int64, (B, T))
+    out = torch.empty((B, D), dtype=torch.float32, device=net.device)
+    pos = torch.empty(B, dtype=torch.int32, device=net.device)
+    call("b200_argmax_gather_rows", ids.data_ptr(), net.data_ptr(), out.data_ptr(), pos.data_ptr(), B, T, D, _stream())
+    return out, pos
+
+
+def scatter_rows(dout: Tensor, pos: Tensor, T: int) -> Tensor:
+    """The backward of ``argmax_gather_rows``: dx fp32 [B, T, D], zero but for dx[b, pos[b]] = dout[b].  dout: contiguous fp32
+    [B, D]; pos: contiguous int32 [B]."""
+    _check("scatter_rows", "dout", dout, _F32, (None, None))
+    B, D = dout.shape
+    _check("scatter_rows", "pos", pos, torch.int32, (B,))
+    dx = fill_f32(torch.empty((B, T, D), dtype=torch.float32, device=dout.device), 0.0)
+    call("b200_scatter_rows", dout.data_ptr(), pos.data_ptr(), dx.data_ptr(), B, T, D, _stream())
+    return dx
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# optimizer, fused FCNN
+# ----------------------------------------------------------------------------------------------------------------
+def adam_step(params: Tensor, grads: Tensor, exp_avg: Tensor, exp_avg_sq: Tensor, *, hyper: Sequence[float] = (), step: int = 0,
+              hyper_dev: Optional[Tensor] = None, step_dev: Optional[Tensor] = None, increment: bool = True) -> None:
+    """One Adam update (torch.optim.Adam without amsgrad) of contiguous fp32 tensors of equal numel, in place.  Either with host
+    ``hyper`` = (lr, beta1, beta2, eps, weight_decay) at step count ``step`` >= 1, or with every hyper-parameter on the device:
+    ``hyper_dev`` fp32 [6] = (lr, beta1, beta2, eps, weight_decay, grad_scale) and the step counter ``step_dev`` int32 [1],
+    incremented first when ``increment`` (so the update can be replayed from a CUDA graph)."""
+    what = "adam_step"
+    _check(what, "params", params, _F32)
+    n = params.numel()
+    for name, t in (("grads", grads), ("exp_avg", exp_avg), ("exp_avg_sq", exp_avg_sq)):
+        _check(what, name, t, _F32, numel=n)
+    if hyper_dev is None:
+        call("b200_adam_step", params.data_ptr(), grads.data_ptr(), exp_avg.data_ptr(), exp_avg_sq.data_ptr(), n, *hyper, step, None,
+             _stream())
+        return
+    _check(what, "hyper_dev", hyper_dev, _F32, (6,))
+    _check(what, "step_dev", step_dev, torch.int32, (1,))
+    call("b200_adam_step_dev", params.data_ptr(), grads.data_ptr(), exp_avg.data_ptr(), exp_avg_sq.data_ptr(), n, hyper_dev.data_ptr(),
+         step_dev.data_ptr(), int(increment), _stream())
+
+
+def fcnn_step(x: Tensor, params: Tensor, dims: Sequence[int], w_offsets: Sequence[int], b_offsets: Sequence[int], *,
+              y: Optional[Tensor] = None, dpred: Optional[Tensor] = None, grads: Optional[Tensor] = None,
+              loss_weights: Tuple[float, float] = (1.0, 1.0)) -> Tuple[Tensor, Optional[Tensor]]:
+    """The fused ReLU MLP dims[0] -> ... -> dims[-1] (csrc/mlp.cu) on x fp32 [M, dims[0]], its weights and biases in the flat fp32
+    arena ``params`` at ``w_offsets`` / ``b_offsets`` (-1: no bias).  Returns (pred fp32 [M, dims[-1]], loss).  With ``grads`` (an
+    arena like ``params``) it also writes the parameter gradients of either the multi_task[mae, mse] loss against ``y``
+    (weighted ``loss_weights``; ``loss`` is its fp32 scalar) or of ``dpred`` = d(pred), with ``loss`` None."""
+    what = "fcnn_step"
+    _check(what, "x", x, _F32, (None, dims[0]))
+    _check(what, "params", params, _F32, (None,))
+    M, P = x.shape[0], params.numel()
+    _check(what, "y", y, _F32, (M, dims[-1]), optional=True)
+    _check(what, "dpred", dpred, _F32, (M, dims[-1]), optional=True)
+    _check(what, "grads", grads, _F32, (P,), optional=True)
+    pred = torch.empty((M, dims[-1]), dtype=torch.float32, device=x.device)
+    part = WORKSPACE.get(x.device, ((M + 127) // 128) * (P + 1), "fcnn") if grads is not None else None
+    nblk = ctypes.c_int(0)
+    host_arrays = ((ctypes.c_int * len(v))(*v) for v in (dims, w_offsets, b_offsets))
+    call("b200_fcnn_step", x.data_ptr(), _ptr(y), _ptr(dpred), params.data_ptr(), pred.data_ptr(), _ptr(part), M, len(dims) - 1,
+         *host_arrays, P, int(y is not None), float(loss_weights[0]), float(loss_weights[1]), ctypes.byref(nblk), _stream())
+    loss = None
+    if grads is not None:
+        _colsum_finish(part, P + 1, nblk.value, 0, P, grads)
+        if y is not None:  # column P of the partials: the loss
+            loss = torch.empty((), dtype=torch.float32, device=x.device)
+            _colsum_finish(part, P + 1, nblk.value, P, 1, loss)
+    return pred, loss
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -575,12 +669,10 @@ def fill_f32(dst: Tensor, value: float) -> Tensor:
 # ----------------------------------------------------------------------------------------------------------------
 def groupnorm_silu_fwd(x: Tensor, gamma: Tensor, beta: Tensor, eps: float, *, silu: bool = True) -> Tuple[Tensor, Tensor, Tensor]:
     """x: bf16 [B, HW, C] (channels last).  Returns (y bf16 [B, HW, C], mean f32 [B, 32], rstd f32 [B, 32])."""
-    _need_cuda(x, gamma, beta)
-    if x.dtype != torch.bfloat16 or x.dim() != 3 or not x.is_contiguous():
-        raise B200Error("groupnorm_silu_fwd: need contiguous bf16 [B, HW, C]")
+    _check("groupnorm_silu_fwd", "x", x, _BF16, (None, None, None))
     B, HW, C = x.shape
-    _dense_f32(gamma, C, "gamma", "groupnorm_silu_fwd")
-    _dense_f32(beta, C, "beta", "groupnorm_silu_fwd")
+    _check("groupnorm_silu_fwd", "gamma", gamma, _F32, (C,))
+    _check("groupnorm_silu_fwd", "beta", beta, _F32, (C,))
     y = torch.empty_like(x)
     mean = torch.empty((B, 32), dtype=torch.float32, device=x.device)
     rstd = torch.empty((B, 32), dtype=torch.float32, device=x.device)
@@ -592,24 +684,19 @@ def groupnorm_silu_fwd(x: Tensor, gamma: Tensor, beta: Tensor, eps: float, *, si
 
 def groupnorm_silu_bwd(x: Tensor, dy: Tensor, gamma: Tensor, beta: Tensor, mean: Tensor, rstd: Tensor, *, silu: bool = True,
                        dgamma: Optional[Tensor] = None, dbeta: Optional[Tensor] = None, accumulate: bool = False) -> Tuple[Tensor, Tensor, Tensor]:
-    _need_cuda(x, dy, gamma, beta, mean, rstd, dgamma, dbeta)
-    if x.dtype != torch.bfloat16 or x.dim() != 3 or not x.is_contiguous():
-        raise B200Error("groupnorm_silu_bwd: need contiguous bf16 x [B, HW, C]")
+    what = "groupnorm_silu_bwd"
+    _check(what, "x", x, _BF16, (None, None, None))
     B, HW, C = x.shape
-    for t, name in ((mean, "mean"), (rstd, "rstd")):
-        if t.dtype != _F32 or tuple(t.shape) != (B, 32) or not t.is_contiguous():
-            raise B200Error(f"groupnorm_silu_bwd: {name} must be a contiguous fp32 [B, 32] tensor")
-    _dense_f32(gamma, C, "gamma", "groupnorm_silu_bwd")
-    _dense_f32(beta, C, "beta", "groupnorm_silu_bwd")
-    if dy.dtype != torch.bfloat16 or dy.shape != x.shape or not dy.is_contiguous():
-        raise B200Error("groupnorm_silu_bwd: dy must be contiguous bf16 with x's shape")
+    _check(what, "dy", dy, _BF16, (B, HW, C))
+    _check(what, "mean", mean, _F32, (B, 32))
+    _check(what, "rstd", rstd, _F32, (B, 32))
     dx = torch.empty_like(x)
     if dgamma is None:
         dgamma = torch.empty(C, dtype=torch.float32, device=x.device)
         dbeta = torch.empty(C, dtype=torch.float32, device=x.device)
         accumulate = False
-    _dense_f32(dgamma, C, "dgamma", "groupnorm_silu_bwd")
-    _dense_f32(dbeta, C, "dbeta", "groupnorm_silu_bwd")
+    for t, name in ((gamma, "gamma"), (beta, "beta"), (dgamma, "dgamma"), (dbeta, "dbeta")):
+        _check(what, name, t, _F32, (C,))
     ws = WORKSPACE.get(x.device, int(_cabi.lib().b200_groupnorm_workspace_floats(B, HW, C)), "groupnorm")
     call("b200_groupnorm_silu_bwd", x.data_ptr(), dy.data_ptr(), gamma.data_ptr(), beta.data_ptr(), mean.data_ptr(), rstd.data_ptr(),
          dx.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), ws.data_ptr(), B, HW, C, int(silu), int(accumulate), _stream())
@@ -633,13 +720,11 @@ def conv3x3_wgrad(dy: Tensor, x: Tensor, out: Optional[Tensor] = None, *, round_
     """Weight gradient of ``conv3x3``: dy bf16 [B, H, W, Cout], x bf16 [B, H, W, Cin] -> fp32 [Cout, 9 * Cin] in the PACKED layout
     of ``pack_conv3x3_weight`` (``unpack_conv3x3_weight`` gives the reference's [Cout, Cin, 3, 3]).  One split-K implicit GEMM over
     the B * H * W pixels plus the split-K reduction; ``round_bf16`` rounds like eager's bf16 conv backward does."""
-    _need_cuda(dy, x, out)
-    if dy.dtype != torch.bfloat16 or x.dtype != torch.bfloat16 or dy.dim() != 4 or x.dim() != 4 or not dy.is_contiguous() or not x.is_contiguous():
-        raise B200Error("conv3x3_wgrad: need contiguous bf16 dy [B, H, W, Cout] and x [B, H, W, Cin]")
+    _check("conv3x3_wgrad", "x", x, _BF16, (None, None, None, None))
     B, H, W, Cin = x.shape
+    _check("conv3x3_wgrad", "dy", dy, _BF16, (B, H, W, None))
     Cout = dy.shape[3]
-    if tuple(dy.shape[:3]) != (B, H, W):
-        raise B200Error("conv3x3_wgrad: dy and x disagree on [B, H, W]")
+    _check("conv3x3_wgrad", "out", out, None, contiguous=False, optional=True)  # any CUDA tensor, as before
     if out is None:
         out = torch.empty((Cout, 9 * Cin), dtype=torch.float32, device=x.device)
         accumulate = False
@@ -661,18 +746,18 @@ def conv3x3(x: Tensor, w_packed: Tensor, bias: Optional[Tensor] = None, *, epilo
     """x: bf16 [B, H, W, Cin] channels-last; w_packed: bf16 [Cout, 9 * Cin] -> bf16 (or fp32 with the residual epilogue) [B, H, W, Cout].
     ``EPI_BIAS_ADD_PER_IMAGE_BF16``: aux = contiguous bf16 [B, Cout], added to every pixel of its image;
     ``EPI_BIAS_RESID_CLAMP_BF16``: aux = contiguous bf16 [B, H, W, Cout] (or [B * H * W, Cout]), the sum clamped to bf16's finite range."""
-    _need_cuda(x, w_packed, bias, aux)
-    if x.dtype != torch.bfloat16 or x.dim() != 4 or not x.is_contiguous() or w_packed.dtype != torch.bfloat16 or not w_packed.is_contiguous():
-        raise B200Error("conv3x3: need contiguous bf16 x [B, H, W, Cin] and w_packed [Cout, 9 * Cin]")
+    _check("conv3x3", "x", x, _BF16, (None, None, None, None))
     B, H, W, Cin = x.shape
+    _check("conv3x3", "w_packed", w_packed, _BF16, (None, 9 * Cin))
     Cout = w_packed.shape[0]
-    if w_packed.shape[1] != 9 * Cin or Cout % 8 != 0:
-        raise B200Error("conv3x3: weight shape does not match (need [Cout, 9 * Cin], Cout % 8 == 0)")
+    if Cout % 8 != 0:
+        raise B200Error(f"conv3x3: need Cout % 8 == 0, got {Cout}")
+    _check("conv3x3", "bias", bias, None, contiguous=False, optional=True)
     dtype, aux_kind, _ = EPILOGUES.get(epilogue, (_BF16, None, None))  # the C side refuses the others
     if aux_kind:
-        rows = B if aux_kind == "image" else B * H * W
-        if aux is None or aux.dtype != dtype or not aux.is_contiguous() or aux.numel() != rows * Cout or aux.shape[-1] != Cout:
-            raise B200Error(f"conv3x3: this epilogue needs a contiguous {dtype} aux with {rows} rows of {Cout}")
+        _check("conv3x3", "aux", aux, dtype, rows=B if aux_kind == "image" else B * H * W, width=Cout)
+    else:
+        _check("conv3x3", "aux", aux, None, contiguous=False, optional=True)
     out = torch.empty((B, H, W, Cout), dtype=dtype, device=x.device)
     call("b200_conv3x3_nhwc_bf16", x.data_ptr(), w_packed.data_ptr(), _ptr(bias), out.data_ptr(), _ptr(aux), Cout, B, H, W, Cin, Cout, epilogue, _stream())
     return out

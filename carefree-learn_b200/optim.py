@@ -21,7 +21,6 @@ import torch
 from torch import Tensor
 
 from . import ops
-from ._cabi import call
 
 
 class ArenaAdam(torch.optim.Optimizer):
@@ -150,11 +149,10 @@ class ArenaAdam(torch.optim.Optimizer):
                 raise ValueError("grad_scale needs ArenaAdam(capturable=True)")
         for idx, a in enumerate(self.arenas()):
             if self.capturable:
-                call("b200_adam_step_dev", a.flat.data_ptr(), a.grad.data_ptr(), self.exp_avgs[idx].data_ptr(), self.exp_avg_sqs[idx].data_ptr(),
-                     a.total, self.hyper_dev.data_ptr(), self.step_dev.data_ptr(), int(idx == 0), ops._stream())
+                ops.adam_step(a.flat, a.grad, self.exp_avgs[idx], self.exp_avg_sqs[idx], hyper_dev=self.hyper_dev, step_dev=self.step_dev,
+                              increment=idx == 0)
             else:
-                call("b200_adam_step", a.flat.data_ptr(), a.grad.data_ptr(), self.exp_avgs[idx].data_ptr(), self.exp_avg_sqs[idx].data_ptr(),
-                     a.total, lr, b1, b2, eps, wd, self.step_count, None, ops._stream())
+                ops.adam_step(a.flat, a.grad, self.exp_avgs[idx], self.exp_avg_sqs[idx], hyper=(lr, b1, b2, eps, wd), step=self.step_count)
 
     def zero_grad(self, set_to_none: bool = True) -> None:
         if set_to_none:

@@ -541,11 +541,7 @@ class _ClassifierFn(torch.autograd.Function):
         G = _pick_grad_arena(arena, keys)
         if dlogits.dtype != torch.bfloat16:
             raise B200Error("classifier backward expects a bf16 gradient for the bf16 logits")
-        if dlogits.stride(1) != 1 or dlogits.stride(0) % 8 != 0:  # e.g. produced by a foreign loss: re-pad the rows
-            padded = torch.zeros((dlogits.shape[0], (dlogits.shape[1] + 7) // 8 * 8), dtype=torch.bfloat16, device=dlogits.device)
-            padded[:, : dlogits.shape[1]].copy_(dlogits)
-            dlogits = padded[:, : dlogits.shape[1]]
-        d_enc = eng.head_backward(sv, dlogits, G)
+        d_enc = eng.head_backward(sv, ops.tma_aligned(dlogits), G)
         eng.encoder_backward(sv, d_enc, G)
         if eng.reducer is not None:
             eng.reducer.finish()

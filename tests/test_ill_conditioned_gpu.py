@@ -417,8 +417,6 @@ def test_softmax_xent(case):
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", XENT_CASES)
 def test_symmetric_xent(case):
-    from cflearn_b200._cabi import call
-
     x, _ = xent_input(case, seed=10 + XENT_CASES.index(case))
     B = min(x.shape)
     x = x[:B, :B].clone()
@@ -433,11 +431,8 @@ def test_symmetric_xent(case):
     ld = (B + 15) // 8 * 8
     logits = _padded(x, ld)
     gs, gsd = (0.5, torch.tensor([3.0], device=DEV)) if case == "scale_dev" else (1.0, None)
-    loss = torch.empty(1, device=DEV)
-    ws = torch.empty(2 * B, device=DEV)
     dl = torch.zeros(B, ld, dtype=torch.bfloat16, device=DEV)[:, :B]
-    call("b200_symmetric_xent_fwd_bwd", logits.data_ptr(), logits.stride(0), loss.data_ptr(), dl.data_ptr(), ws.data_ptr(), B, gs,
-         None if gsd is None else gsd.data_ptr(), ops._stream())
+    loss = ops.symmetric_xent(logits, dlogits=dl, grad_scale=gs, grad_scale_dev=gsd)
     torch.cuda.synchronize()
     sc = gs * (gsd.item() if gsd is not None else 1.0)
     ld64 = logits.to(F64).requires_grad_(True)

@@ -5,6 +5,7 @@ Every refusal of the C-ABI happens before anything is launched, so it is the sam
 are fake and never dereferenced: refused calls stop at the argument checks.  A call that passes them fails its first launch with
 B200_ERR_LAUNCH on a machine without a GPU; the matrices that make such calls run only there, so no kernel ever sees a fake
 pointer.  Host arrays (nparts_out, fcnn_step's dims and offsets) are real."""
+import ast
 import ctypes
 import itertools
 import os
@@ -250,22 +251,43 @@ def test_refusals_name_the_rule():
     assert call("b200_fcnn_step", dims=None) == ARG and "null" in _cabi.last_error()
 
 
+NO_CONTRACT = {
+    "b200_abi_version", "b200_last_error", "b200_launch_count", "b200_gemm_pick_splits", "b200_set_gemm_multicast",
+    "b200_set_attention_fwd_version", "b200_set_attention_bwd_version", "b200_set_attention_prefetch", "b200_set_persistent_ctas",
+    "b200_colsum_per_image_workspace_floats", "b200_attention_long_bwd_workspace_floats", "b200_cross_attention_bwd_workspace_floats",
+    "b200_groupnorm_workspace_floats",
+} | {n for n in _cabi.SIGNATURES if n.startswith("b200_comm_")}
+
+
 def test_every_entry_point_has_a_contract():
     """Each name of the C-ABI is covered exactly once: by the GEMM contract (check_gemm_args), the attention contract, this
     file, or the list of entries that take no device pointers or talk to NCCL."""
     import test_attention_contract
     gemm = {"b200_gemm_bf16", "b200_conv3x3_nhwc_bf16", "b200_conv3x3_wgrad_nhwc_bf16"}
     attention = set(test_attention_contract.ENTRIES)
-    no_contract = {
-        "b200_abi_version", "b200_last_error", "b200_launch_count", "b200_gemm_pick_splits", "b200_set_gemm_multicast",
-        "b200_set_attention_fwd_version", "b200_set_attention_bwd_version", "b200_set_attention_prefetch", "b200_set_persistent_ctas",
-        "b200_colsum_per_image_workspace_floats", "b200_attention_long_bwd_workspace_floats", "b200_cross_attention_bwd_workspace_floats",
-        "b200_groupnorm_workspace_floats",
-    } | {n for n in _cabi.SIGNATURES if n.startswith("b200_comm_")}
-    groups = [gemm, attention, set(ENTRIES), no_contract]
+    groups = [gemm, attention, set(ENTRIES), NO_CONTRACT]
     for name in _cabi.SIGNATURES:
         assert sum(name in g for g in groups) == 1, name
     assert set().union(*groups) == set(_cabi.SIGNATURES)
+
+
+def _names_in_code(path):
+    """Identifiers, attribute names and whole string constants of a module: names in comments or docstrings do not count."""
+    with open(path) as f:
+        tree = ast.parse(f.read())
+    return {n.id if isinstance(n, ast.Name) else n.attr if isinstance(n, ast.Attribute) else n.value for n in ast.walk(tree)
+            if isinstance(n, (ast.Name, ast.Attribute)) or (isinstance(n, ast.Constant) and isinstance(n.value, str))}
+
+
+def test_only_ops_calls_the_compute_entry_points():
+    """ops.py is the one module that knows the compute entry points' arguments (and checks every tensor it hands them): each is
+    named there and in no other module of the package but the ctypes binding."""
+    compute = set(_cabi.SIGNATURES) - NO_CONTRACT
+    pkg = os.path.join(ROOT, "carefree-learn_b200")
+    assert not compute - _names_in_code(os.path.join(pkg, "ops.py"))
+    for name in sorted(os.listdir(pkg)):
+        if name.endswith(".py") and name not in ("ops.py", "_cabi.py"):
+            assert not compute & _names_in_code(os.path.join(pkg, name)), name
 
 
 # ---- moved unchanged from the ResBlock and SpatialTransformer test files ----------------------------------------------------
@@ -430,4 +452,102 @@ def test_ops_groupnorm_refuses_bad_tensors():
     _refused(bwd, mean=_f32(32, B).t())
     _refused(bwd, dgamma=_f32(C + 1), dbeta=_f32(C))
     _refused(bwd, dgamma=_f32(C), dbeta=_f32(C, 2)[:, 0])
+    torch.cuda.synchronize()
+
+
+@pytest.mark.gpu
+def test_ops_text_glue_refuses_bad_tensors():
+    V, D, B, T = 50, 64, 2, 7
+    w, ids = _f32(V, D), torch.randint(0, V, (B, T), device="cuda")
+    ops.embedding_fwd(ids, w)
+    _refused(ops.embedding_fwd, ids.int(), w)                  # dtype
+    _refused(ops.embedding_fwd, ids.t(), w)                    # not contiguous
+    _refused(ops.embedding_fwd, ids, w.to(torch.bfloat16))     # e.g. the weight of CLIPB200.bfloat16()
+    _refused(ops.embedding_fwd, ids, w.reshape(-1))            # shape
+    _refused(ops.embedding_fwd, ids, _f32(D, V).t())
+    dnet = _f32(B, T, D)
+    ops.embedding_bwd(ids, dnet, V, D, 0)
+    _refused(ops.embedding_bwd, ids.int(), dnet, V, D, 0)
+    _refused(ops.embedding_bwd, ids.t(), dnet, V, D, 0)
+    _refused(ops.embedding_bwd, ids, dnet.half(), V, D, 0)
+    _refused(ops.embedding_bwd, ids, dnet[:-1], V, D, 0)
+    _refused(ops.embedding_bwd, ids, dnet.transpose(0, 1), V, D, 0)
+    net = _f32(B, T, D)
+    _, pos = ops.argmax_gather_rows(net, ids)
+    _refused(ops.argmax_gather_rows, net.half(), ids)
+    _refused(ops.argmax_gather_rows, net.reshape(B * T, D), ids)
+    _refused(ops.argmax_gather_rows, _f32(B, D, T).transpose(1, 2), ids)
+    _refused(ops.argmax_gather_rows, net, ids.int())
+    _refused(ops.argmax_gather_rows, net, ids[:, :-1])         # ids do not match net's [B, T]
+    _refused(ops.argmax_gather_rows, _f32(B, T + 1, D), ids)
+    _refused(ops.argmax_gather_rows, net, ids.t().contiguous().t())
+    dout = _f32(B, D)
+    ops.scatter_rows(dout, pos, T)
+    _refused(ops.scatter_rows, dout.double(), pos, T)
+    _refused(ops.scatter_rows, dout[:-1], pos, T)
+    _refused(ops.scatter_rows, _f32(D, B).t(), pos, T)
+    _refused(ops.scatter_rows, dout, pos.long(), T)
+    _refused(ops.scatter_rows, dout, pos[:-1], T)
+    torch.cuda.synchronize()
+
+
+@pytest.mark.gpu
+def test_ops_symmetric_xent_refuses_bad_tensors():
+    B = 16
+    logits, dl = _bf16(B, B), torch.empty(B, B, dtype=torch.bfloat16, device="cuda")
+    ops.symmetric_xent(logits)
+    ops.symmetric_xent(logits, dlogits=dl, grad_scale_dev=_f32(1))
+    _refused(ops.symmetric_xent, logits.float())
+    _refused(ops.symmetric_xent, logits[:, :-1])               # not square
+    _refused(ops.symmetric_xent, _bf16(B, B).t())              # inner stride
+    _refused(ops.symmetric_xent, logits, dlogits=dl.float())
+    _refused(ops.symmetric_xent, logits, dlogits=dl[:-1])
+    _refused(ops.symmetric_xent, logits, dlogits=_bf16(B, 2 * B)[:, :B])  # another row stride than the logits'
+    _refused(ops.symmetric_xent, logits, grad_scale_dev=_f32(2))
+    _refused(ops.symmetric_xent, logits, grad_scale_dev=_f32(1).half())
+    torch.cuda.synchronize()
+
+
+@pytest.mark.gpu
+def test_ops_adam_step_refuses_bad_tensors():
+    n = 1024
+    p, g, m, v = _f32(n), _f32(n), torch.zeros(n, device="cuda"), torch.zeros(n, device="cuda")
+    hyper, step = torch.tensor([1e-3, 0.9, 0.999, 1e-8, 0.0, 1.0], device="cuda"), torch.zeros(1, dtype=torch.int32, device="cuda")
+    host = lambda **kw: ops.adam_step(**dict(dict(params=p, grads=g, exp_avg=m, exp_avg_sq=v, hyper=(1e-3, 0.9, 0.999, 1e-8, 0.0),  # noqa: E731
+                                                  step=1), **kw))
+    dev = lambda **kw: ops.adam_step(**dict(dict(params=p, grads=g, exp_avg=m, exp_avg_sq=v, hyper_dev=hyper, step_dev=step), **kw))  # noqa: E731
+    host()
+    dev()
+    _refused(host, params=p.double())
+    _refused(host, params=_f32(2 * n)[::2])
+    _refused(host, grads=g[:-4])
+    _refused(host, exp_avg=_f32(2 * n)[::2])
+    _refused(host, exp_avg_sq=v.to(torch.bfloat16))
+    _refused(dev, hyper_dev=hyper[:5])
+    _refused(dev, hyper_dev=hyper.double())
+    _refused(dev, step_dev=step.long())
+    _refused(dev, step_dev=None)
+    torch.cuda.synchronize()
+
+
+@pytest.mark.gpu
+def test_ops_fcnn_step_refuses_bad_tensors():
+    dims, woff, boff, P = [10, 32, 1], [0, 352], [320, 384], 388  # the arena of DIMS / WOFF / BOFF above
+    M = 128
+    params, x, y, grads = _f32(P) * 0.1, _f32(M, 10), _f32(M, 1), torch.empty(P, device="cuda")
+    step = lambda **kw: ops.fcnn_step(**dict(dict(x=x, params=params, dims=dims, w_offsets=woff, b_offsets=boff, y=y,  # noqa: E731
+                                                  grads=grads), **kw))
+    step()
+    step(y=None, dpred=_f32(M, 1))
+    step(y=None, grads=None)
+    _refused(step, x=x.double())
+    _refused(step, x=_f32(M, 11))
+    _refused(step, x=_f32(10, M).t())
+    _refused(step, params=params.half())
+    _refused(step, params=_f32(2 * P)[::2])
+    _refused(step, y=y[:-1])
+    _refused(step, y=y.half())
+    _refused(step, y=None, dpred=_f32(M, 2))
+    _refused(step, grads=grads[:-1])
+    _refused(step, grads=_f32(P, 2)[:, 0])
     torch.cuda.synchronize()
