@@ -38,34 +38,18 @@ def shard_indices(n: int, rank: int, world: int) -> range:
 
 
 class GradBucketReducer:
-    def __init__(self, arena, num_layers: int, process_group=None):
+    """Bucketed gradient averaging over ``torch.distributed``.  ``buckets`` (``ViTGeometry.buckets()``): for each point
+    of the engine's backward that calls ``ready``, the parameter keys of each arena span complete there."""
+
+    def __init__(self, arena, buckets: Dict[BucketKey, List[List[str]]], process_group=None):
         self.arena = arena
         self.group = process_group
         self.world = dist.get_world_size(process_group) if dist.is_initialized() else 1
-        self.buckets: Dict[BucketKey, Tuple[int, int]] = {}
-        keys = [k for k, _ in arena.spec]
-        offs = arena.offsets
-
-        def span(pred) -> Tuple[int, int]:
-            ks = [k for k in keys if pred(k)]
-            lo = offs[ks[0]]
-            last = ks[-1]
-            hi = offs[last]
-            n = 1
-            for s in arena.shapes[last]:
-                n *= s
-            return lo, hi + (n + 63) // 64 * 64
-
-        self.buckets["stem"] = span(lambda k: k.startswith("to_patches") or k.startswith("encoder.embedding_norm.")
-                                    or k in ("encoder.head_token", "encoder.pos_encoding.pos_encoding"))
-        for i in range(num_layers):
-            self.buckets[i] = span(lambda k, i=i: k.startswith(f"encoder.mixing_blocks.{i}."))
-        self.buckets["tail"] = span(lambda k: k.startswith("encoder.head.") or k.startswith("encoder.head_norm.") or k.startswith("head.linear"))
-        if "output_projection" in offs:  # a parameter of the encoder itself: first in state_dict order, written with the tail
-            self.buckets["proj"] = span(lambda k: k == "output_projection")
+        self.buckets: Dict[BucketKey, List[Tuple[int, int]]] = {
+            point: [arena.span(keys) for keys in runs] for point, runs in buckets.items()}
         self.comm_stream: Optional[torch.cuda.Stream] = None
         self._pending: List = []
-        self.use_backend_avg = True
+        self._forked = False
 
     def _stream(self) -> torch.cuda.Stream:
         if self.comm_stream is None:
@@ -73,38 +57,39 @@ class GradBucketReducer:
         return self.comm_stream
 
     def ready(self, key: BucketKey, grad: Optional[torch.Tensor] = None) -> None:
-        """Bucket ``key`` of the gradient arena ``grad`` is complete on the current stream: start reducing it."""
+        """Bucket ``key`` of the gradient arena ``grad`` (default: the arena's own) is complete on the current stream:
+        start reducing it."""
         if self.world == 1:
             return
-        if key == "tail" and "proj" in self.buckets:
-            self.ready("proj", grad)
-        lo, hi = self.buckets[key]
         if grad is None:
             grad = self.arena.grad
+        views = [grad[lo:hi] for lo, hi in self.buckets[key]]
         if not grad.is_cuda:  # gloo path (host-side logic tests): same protocol, SUM then divide in finish()
-            work = dist.all_reduce(grad[lo:hi], op=dist.ReduceOp.SUM, group=self.group, async_op=True)
-            self._pending.append((work, grad[lo:hi], True))
+            for v in views:
+                self._pending.append((dist.all_reduce(v, op=dist.ReduceOp.SUM, group=self.group, async_op=True), v))
             return
-        ev = torch.cuda.Event()
-        ev.record(torch.cuda.current_stream())
         cs = self._stream()
-        cs.wait_event(ev)
+        cs.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(cs):
-            work = dist.all_reduce(grad[lo:hi], op=dist.ReduceOp.AVG, group=self.group, async_op=True)
-            self._pending.append((work, None, False))
+            for v in views:
+                self._allreduce(v)
+        self._forked = True
+
+    def _allreduce(self, view: torch.Tensor) -> None:
+        """In-place average of ``view`` over the ranks, enqueued on the communication stream."""
+        work = dist.all_reduce(view, op=dist.ReduceOp.AVG, group=self.group, async_op=True)
+        self._pending.append((work, None))
 
     def finish(self) -> None:
-        if self.world == 1:
-            return
-        on_host = False
-        for work, view, host in self._pending:
+        """The compute stream waits for every bucket started since the last ``finish`` (gloo: the host waits, then averages)."""
+        for work, host_view in self._pending:
             work.wait()  # on CUDA this only orders streams, it does not block the host
-            if host:
-                view.div_(self.world)
-                on_host = True
+            if host_view is not None:
+                host_view.div_(self.world)
         self._pending.clear()
-        if not on_host:
+        if self._forked:
             torch.cuda.current_stream().wait_stream(self._stream())
+            self._forked = False
 
 
 class NativeComm:
@@ -181,61 +166,24 @@ class TorchComm:
 class NativeBucketReducer(GradBucketReducer):
     """Same bucket protocol as ``GradBucketReducer`` over a ``NativeComm``: works eagerly AND under stream capture.
 
-    ``ready(key)`` forks the communication stream off the compute stream (event) and enqueues the bucket's all-reduce
-    there; ``finish()`` joins.  The persistent kernels assign their tiles to CTAs statically, so a CTA that cannot start
-    because NCCL holds its SM stretches its kernel by the whole duration of the all-reduce: the GEMM launched right behind a
-    bucket runs on ``SMs - comm.ctas`` CTAs (``engine.shrink_next``).  ``B200_DP_SHRINK=all`` shrinks EVERY persistent kernel
-    from the first bucket to the join instead (``b200_set_persistent_ctas``) -- the smaller grids cost a wave on every backward
-    GEMM; kept for A/B timing."""
+    ``ready(key)`` forks the communication stream off the compute stream and enqueues the bucket's all-reduce there;
+    ``finish()`` joins.  The persistent kernels assign their tiles to CTAs statically, so a CTA that cannot start because
+    NCCL holds its SM stretches its kernel by the whole duration of the all-reduce: the GEMM launched right behind a
+    bucket runs on ``SMs - comm.ctas`` CTAs (``engine.shrink_next``)."""
 
-    def __init__(self, arena, num_layers: int, comm: NativeComm, engine: Any = None):
-        super().__init__(arena, num_layers, process_group=None)
+    def __init__(self, arena, buckets: Dict[BucketKey, List[List[str]]], comm: NativeComm, engine: Any = None):
+        super().__init__(arena, buckets, process_group=None)
         self.comm = comm
         self.world = comm.world
         self.engine = engine
-        self._launched = False
-        self._prev_limit: Optional[int] = None
+
+    def _allreduce(self, view: torch.Tensor) -> None:
+        self.comm.allreduce_(view, average=True)
 
     def ready(self, key: BucketKey, grad: Optional[torch.Tensor] = None) -> None:
-        if self.world == 1:
-            return
-        if key == "tail" and "proj" in self.buckets:
-            self.ready("proj", grad)
-        lo, hi = self.buckets[key]
-        if grad is None:
-            grad = self.arena.grad
-        cur = torch.cuda.current_stream()
-        ev = torch.cuda.Event()
-        ev.record(cur)
-        cs = self._stream()
-        cs.wait_event(ev)
-        with torch.cuda.stream(cs):
-            self.comm.allreduce_(grad[lo:hi], average=True)
-        mode = os.environ.get("B200_DP_SHRINK", "next")
-        if mode == "next":  # the ONE GEMM launched right behind the bucket (the next block's FF2 input gradient)
-            if self.engine is not None and key != "stem":
-                self.engine.shrink_next = self.comm.ctas
-        elif self.comm.ctas > 0:
-            from . import ops
-
-            limit = max(2, (ops.num_sms() - self.comm.ctas) // 2 * 2)
-            if mode.startswith("next") and mode[4:].isdigit():  # "next3": the next three persistent launches
-                if key != "stem":
-                    _cabi.lib().b200_set_persistent_ctas(limit, int(mode[4:]))
-            elif not self._launched:                             # "all": from the first bucket to the join
-                self._prev_limit = _cabi.lib().b200_set_persistent_ctas(limit, 0)
-        self._launched = True
-
-    def finish(self) -> None:
-        if self.world == 1 or not self._launched:
-            return
-        torch.cuda.current_stream().wait_stream(self._stream())
-        self._launched = False
-        if os.environ.get("B200_DP_SHRINK", "next") not in ("next", "all"):
-            _cabi.lib().b200_set_persistent_ctas(0, 0)
-        if self._prev_limit is not None:
-            _cabi.lib().b200_set_persistent_ctas(self._prev_limit, 0)
-            self._prev_limit = None
+        super().ready(key, grad)
+        if self.world > 1 and self.engine is not None and key != "stem":
+            self.engine.shrink_next = self.comm.ctas  # the next block's FF2 input-gradient GEMM
 
     def _stream(self) -> torch.cuda.Stream:
         if self.comm_stream is None:
@@ -247,7 +195,7 @@ class NativeBucketReducer(GradBucketReducer):
 def attach_native_reducer(module, comm: NativeComm) -> NativeBucketReducer:
     """Overlapped, capturable gradient averaging for a ViTEncoderB200 / VanillaClassifierB200."""
     module.arena.ensure()
-    red = NativeBucketReducer(module.arena, module.geo.L, comm, module.engine)
+    red = NativeBucketReducer(module.arena, module.geo.buckets(), comm, module.engine)
     module.engine.reducer = red
     return red
 
@@ -278,19 +226,10 @@ def detach_reducers(module) -> None:
         t.engine.reducer = None
 
 
-def allreduce_flat_cpu(grad: torch.Tensor, buckets: List[Tuple[int, int]], group=None) -> None:
-    """Host-side (gloo) version of the bucket protocol, used by the world_size=2 CPU tests."""
-    world = dist.get_world_size(group)
-    works = [dist.all_reduce(grad[lo:hi], op=dist.ReduceOp.SUM, group=group, async_op=True) for lo, hi in buckets]
-    for w in works:
-        w.wait()
-    grad.div_(world)
-
-
 def attach_reducer(module, process_group=None) -> GradBucketReducer:
     """Enable overlapped gradient averaging for a ViTEncoderB200 / VanillaClassifierB200."""
     module.arena.ensure()
-    red = GradBucketReducer(module.arena, module.geo.L, process_group)
+    red = GradBucketReducer(module.arena, module.geo.buckets(), process_group)
     module.engine.reducer = red
     return red
 

@@ -17,8 +17,7 @@ backward is still running.
 from __future__ import annotations
 
 import math
-import os
-from typing import Any, Dict, List, Optional, Tuple
+from typing import Any, Dict, List, Optional, Tuple, Union
 
 import torch
 import torch.nn as nn
@@ -31,23 +30,10 @@ PREDICTIONS_KEY = "predictions"  # cflearn/constants.py:6
 LATENT_KEY = "latent"
 
 _ALIGN = 64  # elements; keeps every view 16-byte aligned in both the fp32 and the bf16 arena
-_NVTX = os.environ.get("B200_NVTX", "0") == "1"
-_STEM_BIAS_SPLIT = os.environ.get("B200_STEM_BIAS", "split") != "fused"
 
 
-class _nvtx:
-    """NVTX range per stage (B200_NVTX=1; off by default: a push / pop pair per stage costs host time on the eager path)."""
-
-    def __init__(self, name: str):
-        self.name = name
-
-    def __enter__(self) -> None:
-        if _NVTX:
-            torch.cuda.nvtx.range_push(self.name)
-
-    def __exit__(self, *exc: Any) -> None:
-        if _NVTX:
-            torch.cuda.nvtx.range_pop()
+def _padded(shape: Tuple[int, ...]) -> int:
+    return (math.prod(shape) + _ALIGN - 1) // _ALIGN * _ALIGN
 
 
 # -----------------------------------------------------------------------------------------------------------------
@@ -62,7 +48,7 @@ class ParamArena:
         off = 0
         for key, shape in self.spec:
             self.offsets[key] = off
-            off += (math.prod(shape) + _ALIGN - 1) // _ALIGN * _ALIGN
+            off += _padded(shape)
         self.total = off
         self.shapes = dict(self.spec)
         self.flat: Optional[Tensor] = None
@@ -123,6 +109,35 @@ class ParamArena:
     def g(self, key: str, arena: Optional[Tensor] = None) -> Tensor:  # fp32 grad view
         return self.view(self.grad if arena is None else arena, key)
 
+    def span(self, keys: List[str]) -> Tuple[int, int]:
+        """[lo, hi) of the arena holding ``keys``, which are consecutive in the layout (one all-reduce bucket)."""
+        return self.offsets[keys[0]], self.offsets[keys[-1]] + _padded(self.shapes[keys[-1]])
+
+    def grad_arena(self, keys: List[str]) -> Tensor:
+        """Where a backward writes: the main gradient arena (overwrite), unless some parameter already holds a gradient
+        (gradient accumulation): then the scratch arena, added on by ``publish_grads``."""
+        if not any(self.params[k].grad is not None for k in keys):
+            return self.grad
+        if self.grad_scratch is None:
+            self.grad_scratch = torch.zeros_like(self.grad)
+        return self.grad_scratch
+
+    def publish_grads(self, G: Tensor, keys: List[str]) -> None:
+        """Make ``p.grad`` views of the gradient arena (no copies), after a backward wrote ``G`` (see ``grad_arena``)."""
+        with torch.no_grad():
+            for key in keys:
+                p = self.params[key]
+                v = self.view(self.grad, key)
+                if G is self.grad:
+                    if p.grad is None or p.grad.data_ptr() != v.data_ptr():
+                        p.grad = v
+                else:  # accumulation step: G is the scratch arena
+                    if p.grad is None:
+                        v.copy_(self.view(G, key))
+                        p.grad = v
+                    else:
+                        p.grad.add_(self.view(G, key))
+
 
 def _register_dotted(root: nn.Module, key: str, param: nn.Parameter) -> None:
     parts = key.split(".")
@@ -177,34 +192,48 @@ class ViTGeometry:
     def head_norm_key(self) -> str:  # mixed_stacks/api.py:383-395: PreNorm(head) vs head then head_norm
         return "encoder.head_norm." if self.norm_after_head else "encoder.head.norms.0."
 
-    def spec(self, with_head: bool) -> List[Tuple[str, Tuple[int, ...]]]:
+    def _groups(self) -> List[Tuple[Union[int, str], List[Tuple[str, Tuple[int, ...]]]]]:
+        """The parameters in the reference's state_dict order (a module's own parameters precede its sub-modules'),
+        in runs labelled with the point of ``ViTEngine.encoder_backward`` after which their gradients are complete."""
         d, p, c, ff = self.D, self.patch, self.cin, self.FF
-        # (key order = the reference's state_dict order: a module's own parameters precede its sub-modules')
-        out: List[Tuple[str, Tuple[int, ...]]] = []
-        if self.out_dim is not None:
-            out.append(("output_projection", (d, self.out_dim)))
+        out: List[Tuple[Union[int, str], List[Tuple[str, Tuple[int, ...]]]]] = []
+        if self.out_dim is not None:  # a parameter of the encoder itself: first in state_dict order, written with the tail
+            out.append(("tail", [("output_projection", (d, self.out_dim))]))
         if self.tokens:
-            out.append(("encoder.pos_encoding.pos_encoding", (1, self.T, d)))
+            stem = [("encoder.pos_encoding.pos_encoding", (1, self.T, d))]
         else:
-            out.append(("to_patches.projection.weight", (d, c, p, p)))
+            stem = [("to_patches.projection.weight", (d, c, p, p))]
             if self.conv_bias:
-                out.append(("to_patches.projection.bias", (d,)))
-            out += [("encoder.head_token", (1, 1, d)), ("encoder.pos_encoding.pos_encoding", (1, self.T, d))]
+                stem.append(("to_patches.projection.bias", (d,)))
+            stem += [("encoder.head_token", (1, 1, d)), ("encoder.pos_encoding.pos_encoding", (1, self.T, d))]
         if self.emb_eps is not None:
-            out += [("encoder.embedding_norm.weight", (d,)), ("encoder.embedding_norm.bias", (d,))]
+            stem += [("encoder.embedding_norm.weight", (d,)), ("encoder.embedding_norm.bias", (d,))]
+        out.append(("stem", stem))
         for i in range(self.L):
             b = f"encoder.mixing_blocks.{i}."
-            out += [
+            out.append((i, [
                 (b + "token_norm.weight", (d,)), (b + "token_norm.bias", (d,)),
                 (b + "token_mixing.net.in_w", (3 * d, d)), (b + "token_mixing.net.qkv_bias", (3 * d,)),
                 (b + "token_mixing.net.out_linear.linear.weight", (d, d)), (b + "token_mixing.net.out_linear.linear.bias", (d,)),
                 (b + "channel_norm.weight", (d,)), (b + "channel_norm.bias", (d,)),
                 (b + "channel_mixing.net.0.linear.weight", (ff, d)), (b + "channel_mixing.net.0.linear.bias", (ff,)),
                 (b + "channel_mixing.net.3.linear.weight", (d, ff)), (b + "channel_mixing.net.3.linear.bias", (d,)),
-            ]
-        out += [(self.head_norm_key + "weight", (d,)), (self.head_norm_key + "bias", (d,))]
-        if with_head:
-            out += [("head.linear.weight", (self.C, d)), ("head.linear.bias", (self.C,))]
+            ]))
+        tail = [(self.head_norm_key + "weight", (d,)), (self.head_norm_key + "bias", (d,))]
+        if self.C is not None:
+            tail += [("head.linear.weight", (self.C, d)), ("head.linear.bias", (self.C,))]
+        out.append(("tail", tail))
+        return out
+
+    def spec(self) -> List[Tuple[str, Tuple[int, ...]]]:
+        return [kv for _, run in self._groups() for kv in run]
+
+    def buckets(self) -> Dict[Union[int, str], List[List[str]]]:
+        """Gradient all-reduce buckets: for each point where ``encoder_backward`` calls ``reducer.ready``, the keys of
+        each contiguous run of the arena that is complete there."""
+        out: Dict[Union[int, str], List[List[str]]] = {}
+        for point, run in self._groups():
+            out.setdefault(point, []).append([k for k, _ in run])
         return out
 
 
@@ -241,27 +270,6 @@ class ViTEngine:
         # imagenet / affine normalisation blocks (data/blocks/cv/normalize.py); None: division by 255 only
         self.input_pipeline: Optional[Dict[str, Any]] = None
         self.shrink_next = 0  # SMs to leave free for an in-flight bucket all-reduce when launching the next GEMM (dp.py)
-        self.d_input: Optional[Tensor] = None  # token mode: gradient w.r.t. the embedded input of the last backward
-        # B200_SIDE_COLSUM=1 puts the HBM-bound bias-gradient column sums on a side stream (a parallel branch of the
-        # captured graph).  Off by default: the persistent GEMM holds ~193 KB of shared memory on every SM, so no other
-        # CTA can become resident next to it.
-        self.side_colsum = os.environ.get("B200_SIDE_COLSUM", "0") == "1"
-        self._side: Optional[torch.cuda.Stream] = None
-
-    def _bias_grad(self, dy: Tensor, out: Tensor) -> None:
-        """out = column sums of dy; on the side stream when enabled (the caller joins with ``_join_side``)."""
-        if not self.side_colsum:
-            ops.colsum(dy, out)
-            return
-        if self._side is None or self._side.device != dy.device:
-            self._side = torch.cuda.Stream(device=dy.device)
-        self._side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(self._side):
-            ops.colsum(dy, out)
-
-    def _join_side(self) -> None:
-        if self.side_colsum and self._side is not None:
-            torch.cuda.current_stream().wait_stream(self._side)
 
     # ---- stages (also the units of the teacher-forced parity tests, tests/test_taps_gpu.py) --------------------
     def stem_forward(self, x: Tensor) -> Tuple[Optional[Tensor], Tensor]:
@@ -277,12 +285,10 @@ class ViTEngine:
             cols = ops.patch_im2col(x, g.patch)
         # F.conv2d with a bias on CUDA is TWO roundings in eager: ATen's cuDNN path produces the bf16 convolution output and
         # then runs `output.add_(bias)` on the bf16 tensor (aten/native/Convolution.cpp) -- unlike F.linear, whose bias is
-        # fused before the single rounding.  B200_STEM_BIAS=fused restores the single rounding (A/B; tools/probe_conv_bias.py).
-        split = g.conv_bias and _STEM_BIAS_SPLIT
-        patch = ops.gemm(cols, A.w("to_patches.projection.weight").view(D, -1),
-                         bias=A.w("to_patches.projection.bias") if (g.conv_bias and not split) else None)
+        # fused before the single rounding (tools/probe_conv_bias.py).  So the bias is added after the GEMM's rounding.
+        patch = ops.gemm(cols, A.w("to_patches.projection.weight").view(D, -1))
         net = ops.assemble_tokens(patch, A.p("encoder.head_token"), A.p("encoder.pos_encoding.pos_encoding"), B, g.np, D,
-                                  conv_bias=A.w("to_patches.projection.bias") if split else None).view(B * T, D)
+                                  conv_bias=A.w("to_patches.projection.bias") if g.conv_bias else None).view(B * T, D)
         return cols, net
 
     def block_forward(self, i: int, net: Tensor, B: int) -> Tuple[Tensor, Tuple[Tensor, ...]]:
@@ -316,7 +322,7 @@ class ViTEngine:
         b = f"encoder.mixing_blocks.{i}."
         net, mean1, rstd1, ln1, qkv, attn, lse, mid, mean2, rstd2, ln2, h, act = saved
         if not ff2_bias_done:
-            self._bias_grad(dnet_bf, A.g(b + "channel_mixing.net.3.linear.bias", G))
+            ops.colsum(dnet_bf, A.g(b + "channel_mixing.net.3.linear.bias", G))
         # FeedForward: net_out = mid + W2 gelu(W1 ln2 + b1) + b2
         ff1_bias = A.g(b + "channel_mixing.net.0.linear.bias", G)
         shrink, self.shrink_next = self.shrink_next, 0  # the previous block's bucket is being all-reduced right now
@@ -326,7 +332,7 @@ class ViTEngine:
         ops.wgrad(dnet_bf, act, A.g(b + "channel_mixing.net.3.linear.weight", G))
         dln2 = ops.gemm(dh, A.w(b + "channel_mixing.net.0.linear.weight"), b_mn_major=True)
         ops.wgrad(dh, ln2, A.g(b + "channel_mixing.net.0.linear.weight", G))
-        self._bias_grad(dh, ff1_bias)
+        ops.colsum(dh, ff1_bias)
         dmid = torch.empty((M, D), dtype=torch.float32, device=dev)
         dmid_bf = torch.empty((M, D), dtype=torch.bfloat16, device=dev)
         ops.layernorm_bwd(dln2, mid, A.p(b + "channel_norm.weight"), mean2, rstd2, rows=M, dim=D, ld_x=D, dres=dnet,
@@ -339,7 +345,6 @@ class ViTEngine:
         dqkv = ops.attention_bwd(qkv, attn, dattn, lse, B, T, g.H, causal=g.causal, dbias=A.g(b + "token_mixing.net.qkv_bias", G))
         dln1 = ops.gemm(dqkv, A.w(b + "token_mixing.net.in_w"), b_mn_major=True)
         ops.wgrad(dqkv, ln1, A.g(b + "token_mixing.net.in_w", G))
-        self._join_side()  # dnet_bf is overwritten below, and this block's bias gradients must be complete
         ops.layernorm_bwd(dln1, net, A.p(b + "token_norm.weight"), mean1, rstd1, rows=M, dim=D, ld_x=D, dres=dmid,
                           dx_out=dnet, ld_dx=D, dx_bf16=dnet_bf,
                           dgamma=A.g(b + "token_norm.weight", G), dbeta=A.g(b + "token_norm.bias", G),
@@ -351,8 +356,7 @@ class ViTEngine:
         dpatch = ops.assemble_tokens_bwd(dnet, A.g("encoder.pos_encoding.pos_encoding", G), A.g("encoder.head_token", G), sv.B, g.np, g.D)
         ops.wgrad(dpatch, sv.cols, A.g("to_patches.projection.weight", G).view(g.D, -1))
         if g.conv_bias:
-            self._bias_grad(dpatch, A.g("to_patches.projection.bias", G))
-        self._join_side()
+            ops.colsum(dpatch, A.g("to_patches.projection.bias", G))
 
     # ---- forward ------------------------------------------------------------------------------------------
     def encoder_forward(self, x: Tensor, want_f32: bool) -> Tuple[Tensor, Optional[Tensor], _Saved]:
@@ -372,8 +376,7 @@ class ViTEngine:
         B, T, D, M = x.shape[0], g.T, g.D, x.shape[0] * g.T
         sv = _Saved()
         sv.B = B
-        with _nvtx("b200.stem.fwd"):
-            cols, net = self.stem_forward(x)
+        cols, net = self.stem_forward(x)
         sv.emb_in = None
         if g.emb_eps is not None:  # embedding_norm (api.py:433-434): its fp32 output IS the residual stream
             normed = torch.empty_like(net)
@@ -383,8 +386,7 @@ class ViTEngine:
         sv.cols = cols
         sv.blocks = []
         for i in range(g.L):
-            with _nvtx(f"b200.block{i}.fwd"):
-                net, saved = self.block_forward(i, net, B)
+            net, saved = self.block_forward(i, net, B)
             sv.blocks.append(saved)
         hrows, hld = (M, D) if g.tokens else (B, T * D)
         enc_f32 = torch.empty((hrows, D), dtype=torch.float32, device=x.device) if want_f32 else None
@@ -417,10 +419,11 @@ class ViTEngine:
         ops.colsum(dlogits, A.g("head.linear.bias", G))
         return d_enc
 
-    def encoder_backward(self, sv: _Saved, d_enc_bf16: Tensor, G: Tensor) -> None:
+    def encoder_backward(self, sv: _Saved, d_enc_bf16: Tensor, G: Tensor) -> Optional[Tensor]:
         """Writes every encoder parameter gradient into the flat arena ``G`` (overwrite semantics).  ``d_enc_bf16``: the
         gradient of the head LayerNorm's output -- bf16 [B, D] (vision: it feeds a bf16 matmul) or, in token mode,
-        fp32 [B*T, D] (the LayerNorm output itself is what the module returns)."""
+        fp32 [B*T, D] (the LayerNorm output itself is what the module returns).  Token mode returns the gradient of the
+        embedded input [B, T, D]."""
         g, A = self.geo, self.arena
         B, T, D, M = sv.B, g.T, g.D, sv.B * g.T
         dev = d_enc_bf16.device
@@ -439,12 +442,11 @@ class ViTEngine:
             dnet_bf = ops.cast_bf16(dnet)
         # bias gradient of the last block's FF2 (dY = dnet_bf); every other Linear whose dY comes out of a LayerNorm
         # backward gets its bias gradient from that kernel (dx_colsum)
-        self._bias_grad(dnet_bf, A.g(f"encoder.mixing_blocks.{g.L - 1}.channel_mixing.net.3.linear.bias", G))
+        ops.colsum(dnet_bf, A.g(f"encoder.mixing_blocks.{g.L - 1}.channel_mixing.net.3.linear.bias", G))
         if red is not None:
             red.ready("tail", G)
         for i in reversed(range(g.L)):
-            with _nvtx(f"b200.block{i}.bwd"):
-                self.block_backward(i, sv.blocks[i], dnet, dnet_bf, G, B)
+            self.block_backward(i, sv.blocks[i], dnet, dnet_bf, G, B)
             sv.blocks[i] = None  # release this block's activations
             if red is not None:
                 red.ready(i, G)
@@ -456,98 +458,65 @@ class ViTEngine:
             dnet = dpre
         if g.tokens:  # net = x + pos: the input gradient is dnet itself
             ops.add_pos_bwd(dnet, A.g("encoder.pos_encoding.pos_encoding", G), B, T, D)
-            self.d_input = dnet.view(B, T, D)
-            if red is not None:
-                red.ready("stem", G)
-            return
-        with _nvtx("b200.stem.bwd"):
+        else:
             self.stem_backward(sv, dnet, G)
         if red is not None:
             red.ready("stem", G)
+        return dnet.view(B, T, D) if g.tokens else None
+
+    # ---- the whole stack: the encoder, then what the geometry puts after it ----------------------------------------
+    def stack_forward(self, x: Tensor, head: bool) -> Tuple[Tensor, _Saved]:
+        """The module output: the classifier's bf16 logits (``head``), the bf16 ``net @ output_projection``, or the fp32
+        head LayerNorm output (vision: [B, D] of the cls token; token mode: [B, T, D])."""
+        g = self.geo
+        bf16_tail = head or g.out_dim is not None
+        enc_bf16, enc_f32, sv = self.encoder_forward(x, want_f32=not bf16_tail)
+        if head:
+            return self.head_forward(enc_bf16), sv
+        if g.out_dim is not None:
+            return self.projection_forward(enc_bf16), sv
+        return (enc_f32.view(sv.B, g.T, g.D) if g.tokens else enc_f32), sv
+
+    def stack_backward(self, sv: _Saved, d_out: Tensor, G: Tensor, head: bool) -> Optional[Tensor]:
+        """Backward of ``stack_forward`` from the gradient of its output; returns the input gradient in token mode."""
+        g = self.geo
+        if head:
+            if d_out.dtype != torch.bfloat16:
+                raise B200Error("classifier backward expects a bf16 gradient for the bf16 logits")
+            d_enc = self.head_backward(sv, ops.tma_aligned(d_out), G)
+        elif g.tokens:  # fp32: the LayerNorm output is the module output
+            d_enc = d_out.contiguous().float().view(-1, g.D)
+        else:  # under autocast the encoder output feeds a bf16 matmul, so its gradient is bf16-representable
+            d_enc = d_out.contiguous() if d_out.dtype == torch.bfloat16 else ops.cast_bf16(d_out.contiguous().float())
+            if g.out_dim is not None:
+                d_enc = self.projection_backward(sv, d_enc, G)
+        return self.encoder_backward(sv, d_enc, G)
 
 
 # -----------------------------------------------------------------------------------------------------------------
 # autograd glue
 # -----------------------------------------------------------------------------------------------------------------
-def _publish_grads(arena: ParamArena, G: Tensor, keys: List[str]) -> None:
-    """Make ``p.grad`` views of the gradient arena (no copies).  Called at the end of backward."""
-    with torch.no_grad():
-        for key in keys:
-            p = arena.params[key]
-            v = arena.view(arena.grad, key)
-            if G is arena.grad:
-                if p.grad is None or p.grad.data_ptr() != v.data_ptr():
-                    p.grad = v
-            else:  # accumulation step: G is the scratch arena
-                if p.grad is None:
-                    v.copy_(arena.view(G, key))
-                    p.grad = v
-                else:
-                    p.grad.add_(arena.view(G, key))
-
-
-def _pick_grad_arena(arena: ParamArena, keys: List[str]) -> Tensor:
-    """Overwrite the main arena unless some parameter already holds a gradient (gradient accumulation)."""
-    accumulating = any(arena.params[k].grad is not None for k in keys)
-    if not accumulating:
-        return arena.grad
-    if arena.grad_scratch is None:
-        arena.grad_scratch = torch.zeros_like(arena.grad)
-    return arena.grad_scratch
-
-
-class _EncoderFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx: Any, module: "ViTEncoderB200", x: Tensor, *params: Tensor) -> Tensor:
-        proj = module.geo.out_dim is not None
-        enc_bf16, enc_f32, sv = module.engine.encoder_forward(x, want_f32=not proj)
-        ctx.module, ctx.sv = module, sv
-        if proj:  # `net @ output_projection` is a bf16 matmul under autocast: the encoder returns bf16 [B, output_dim]
-            return module.engine.projection_forward(enc_bf16)
-        return enc_f32
+class _StackFn(torch.autograd.Function):
+    """The whole native stack of one module as ONE autograd node (``ViTEngine.stack_forward``).  Its backward writes every
+    parameter gradient into the gradient arena and publishes them as ``p.grad`` views, so autograd receives ``None`` for
+    the parameters; only token mode returns an input gradient."""
 
     @staticmethod
-    def backward(ctx: Any, d_enc: Tensor) -> Tuple[Any, ...]:
-        module, sv = ctx.module, ctx.sv
-        arena, eng = module.arena, module.engine
-        keys = module.encoder_keys
-        G = _pick_grad_arena(arena, keys)
-        # under autocast the encoder output feeds a bf16 matmul, so its gradient is bf16-representable
-        d_bf = d_enc.contiguous() if d_enc.dtype == torch.bfloat16 else ops.cast_bf16(d_enc.contiguous().float())
-        if module.geo.out_dim is not None:
-            d_bf = eng.projection_backward(sv, d_bf, G)
-        eng.encoder_backward(sv, d_bf, G)
+    def forward(ctx: Any, engine: ViTEngine, keys: List[str], head: bool, x: Tensor, *params: Tensor) -> Tensor:
+        out, sv = engine.stack_forward(x, head)
+        ctx.engine, ctx.keys, ctx.head, ctx.sv = engine, keys, head, sv
+        return out
+
+    @staticmethod
+    def backward(ctx: Any, d_out: Tensor) -> Tuple[Any, ...]:
+        eng, keys = ctx.engine, ctx.keys
+        G = eng.arena.grad_arena(keys)
+        d_in = eng.stack_backward(ctx.sv, d_out, G, ctx.head)
         if eng.reducer is not None:
             eng.reducer.finish()
-        _publish_grads(arena, G, keys)
+        eng.arena.publish_grads(G, keys)
         ctx.sv = None
-        return (None, None) + (None,) * len(keys)
-
-
-class _ClassifierFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx: Any, module: "VanillaClassifierB200", x: Tensor, *params: Tensor) -> Tensor:
-        eng = module.engine
-        enc_bf16, _, sv = eng.encoder_forward(x, want_f32=False)
-        logits = eng.head_forward(enc_bf16)
-        ctx.module, ctx.sv = module, sv
-        return logits
-
-    @staticmethod
-    def backward(ctx: Any, dlogits: Tensor) -> Tuple[Any, ...]:
-        module, sv = ctx.module, ctx.sv
-        arena, eng = module.arena, module.engine
-        keys = module.all_keys
-        G = _pick_grad_arena(arena, keys)
-        if dlogits.dtype != torch.bfloat16:
-            raise B200Error("classifier backward expects a bf16 gradient for the bf16 logits")
-        d_enc = eng.head_backward(sv, ops.tma_aligned(dlogits), G)
-        eng.encoder_backward(sv, d_enc, G)
-        if eng.reducer is not None:
-            eng.reducer.finish()
-        _publish_grads(arena, G, keys)
-        ctx.sv = None
-        return (None, None) + (None,) * len(keys)
+        return (None, None, None, d_in) + (None,) * len(keys)
 
 
 class _SoftmaxXentFn(torch.autograd.Function):
@@ -598,7 +567,58 @@ def _check_supported(**kw: Any) -> None:
             )
 
 
-class ViTEncoderB200(nn.Module):
+def _check_common(name: str, latent_dim: int, *, default_heads: int, norm_kwargs: Optional[Dict[str, Any]],
+                  embedding_norm: Optional[nn.Module], attention_kwargs: Optional[Dict[str, Any]],
+                  feedforward_kwargs: Optional[Dict[str, Any]]) -> Dict[str, Any]:
+    """The keywords both encoders read alike; returns the ``ViTGeometry`` keywords they determine."""
+    fk = dict(feedforward_kwargs or {})
+    if set(fk) - {"activation"}:
+        raise NotImplementedError(f"unsupported feedforward_kwargs: {sorted(set(fk) - {'activation'})}")
+    emb_eps: Optional[float] = None
+    if embedding_norm is not None:  # clip.py:131: nn.LayerNorm(latent_dim, eps)
+        if not isinstance(embedding_norm, nn.LayerNorm) or tuple(embedding_norm.normalized_shape) != (latent_dim,) \
+                or not embedding_norm.elementwise_affine or embedding_norm.bias is None:
+            raise NotImplementedError("embedding_norm must be an affine nn.LayerNorm(latent_dim)")
+        emb_eps = float(embedding_norm.eps)
+    ak = dict(attention_kwargs or {})
+    if ak.get("num_heads", default_heads) != latent_dim // 64 or not ak.get("bias", True) or set(ak) - {"num_heads", "bias"}:
+        raise NotImplementedError(f"{name} needs attention_kwargs num_heads = latent_dim // 64 (head dim 64) and bias=True, "
+                                  f"got {ak}")
+    eps = float((norm_kwargs or {}).get("eps", 1e-6))  # norms.py:118-119 default, clip.py:128 overrides to 1e-5
+    return dict(eps=eps, embedding_norm_eps=emb_eps, activation=fk.get("activation", "GELU"))
+
+
+class _FusedStack(nn.Module):
+    """What ``ViTEncoderB200`` and ``TeTEncoderB200`` share: parameters in one arena, one engine, one autograd node."""
+
+    def _build(self, geo: ViTGeometry, embedding_norm: Optional[nn.Module], defer_head: bool = False) -> None:
+        """Parameters with the reference initialisation (an ``embedding_norm`` instance handed in is adopted), registered
+        under the reference's names, then the arena and the engine.  ``defer_head``: the classifier registers
+        ``head.linear.*`` itself, after its ``encoder`` sub-module (the reference's key order)."""
+        spec = geo.spec()
+        params: Dict[str, nn.Parameter] = {}
+        for key, shape in spec:
+            p = nn.Parameter(_init_param(key, shape))
+            if embedding_norm is not None and key.startswith("encoder.embedding_norm."):
+                p.data.copy_(getattr(embedding_norm, key.rsplit(".", 1)[1]).data)
+            params[key] = p
+            if not (defer_head and key.startswith("head.linear")):
+                _register_dotted(self, key, p)
+        self.geo = geo
+        self.arena = ParamArena(spec)
+        self.arena.attach(params)
+        self.engine = ViTEngine(geo, self.arena)
+        self.all_keys = [k for k, _ in spec]
+        self.encoder_keys = [k for k in self.all_keys if not k.startswith("head.linear")]
+
+    def _run(self, net: Tensor, head: bool = False) -> Tensor:
+        """The stack on ``net`` as one autograd node; ``head``: through the classifier head."""
+        keys = self.all_keys if head else self.encoder_keys
+        self.arena.ensure()
+        return _StackFn.apply(self.engine, keys, head, net, *[self.arena.params[k] for k in keys])
+
+
+class ViTEncoderB200(_FusedStack):
     """Drop-in for ``ViTEncoder`` (registered as ``encoders.vit`` in the reference, transformer.py:16-17)."""
 
     def __init__(
@@ -632,56 +652,27 @@ class ViTEncoderB200(nn.Module):
         _check_supported(to_patches_type=to_patches_type, dropout=dropout, drop_path_rate=drop_path_rate, norm_type=norm_type,
                          residual_after_norm=residual_after_norm, use_head_token=use_head_token,
                          use_positional_encoding=use_positional_encoding)
-        fk = dict(feedforward_kwargs or {})
-        if set(fk) - {"activation"}:
-            raise NotImplementedError(f"unsupported feedforward_kwargs: {sorted(set(fk) - {'activation'})}")
-        emb_eps: Optional[float] = None
-        if embedding_norm is not None:  # clip.py:131: nn.LayerNorm(latent_dim, eps)
-            if not isinstance(embedding_norm, nn.LayerNorm) or tuple(embedding_norm.normalized_shape) != (latent_dim,) \
-                    or not embedding_norm.elementwise_affine or embedding_norm.bias is None:
-                raise NotImplementedError("embedding_norm must be an affine nn.LayerNorm(latent_dim)")
-            emb_eps = float(embedding_norm.eps)
+        common = _check_common("ViTEncoderB200", latent_dim, default_heads=latent_dim // 64, norm_kwargs=norm_kwargs,
+                               embedding_norm=embedding_norm, attention_kwargs=attention_kwargs,
+                               feedforward_kwargs=feedforward_kwargs)
         tpc = dict(to_patches_config or {})
         if set(tpc) - {"bias"}:
             raise NotImplementedError(f"unsupported to_patches_config: {sorted(set(tpc) - {'bias'})}")
-        ak = dict(attention_kwargs or {})
-        if ak.get("num_heads", latent_dim // 64) != latent_dim // 64 or not ak.get("bias", True):
-            raise NotImplementedError("ViTEncoderB200 supports the default attention_kwargs only (bias=True, head dim 64)")
-        if set(ak) - {"num_heads", "bias"}:
-            raise NotImplementedError(f"unsupported attention_kwargs: {sorted(set(ak) - {'num_heads', 'bias'})}")
-        eps = float((norm_kwargs or {}).get("eps", 1e-6))  # norms.py:118-119 default, clip.py:128 overrides to 1e-5
-        self.geo = ViTGeometry(img_size=img_size, patch_size=patch_size, in_channels=in_channels, latent_dim=latent_dim,
-                               num_layers=num_layers, ff_ratio=feedforward_dim_ratio, eps=eps, num_classes=_num_classes,
-                               conv_bias=bool(tpc.get("bias", True)), embedding_norm_eps=emb_eps, norm_after_head=bool(norm_after_head),
-                               output_dim=output_dim, activation=fk.get("activation", "GELU"))
-        spec = self.geo.spec(with_head=_num_classes is not None)
-        self.arena = ParamArena(spec)
-        params: Dict[str, nn.Parameter] = {}
-        for key, shape in spec:
-            p = nn.Parameter(_init_param(key, shape))
-            if embedding_norm is not None and key.startswith("encoder.embedding_norm."):
-                p.data.copy_(getattr(embedding_norm, key.rsplit(".", 1)[1]).data)  # the instance handed in is adopted
-            params[key] = p
-            if not (_defer_head and key.startswith("head.linear")):  # the classifier registers its head itself
-                _register_dotted(self, key, p)
-        self.arena.attach(params)
-        self.engine = ViTEngine(self.geo, self.arena)
-        self.all_keys = [k for k, _ in spec]
-        self.encoder_keys = [k for k in self.all_keys if not k.startswith("head.linear")]
+        self._build(ViTGeometry(img_size=img_size, patch_size=patch_size, in_channels=in_channels, latent_dim=latent_dim,
+                                num_layers=num_layers, ff_ratio=feedforward_dim_ratio, num_classes=_num_classes,
+                                conv_bias=bool(tpc.get("bias", True)), norm_after_head=bool(norm_after_head),
+                                output_dim=output_dim, **common),
+                    embedding_norm, defer_head=_defer_head)
         self.latent_dim = latent_dim
 
     def named_arena_parameters(self):
         """(arena key, parameter) pairs: the reference ``ViTEncoder`` state_dict names (+ ``head.linear.*``)."""
         return [(k, self.arena.params[k]) for k in self.all_keys]
 
-    def _param_list(self, keys: List[str]) -> List[nn.Parameter]:
-        return [self.arena.params[k] for k in keys]
-
     def forward(self, net: Tensor, *, hw: Any = None, hwp: Any = None, deterministic: bool = False) -> Tensor:
         if hwp is not None:
             raise NotImplementedError("positional-encoding interpolation (hwp) is outside the fused path")
-        self.arena.ensure()
-        return _EncoderFn.apply(self, net, *self._param_list(self.encoder_keys))
+        return self._run(net)
 
     def encode(self, net: Tensor) -> Tensor:  # IEncoder.encode, cv/common.py:42-50
         return self.forward(net)
@@ -694,29 +685,7 @@ class ViTEncoderB200(nn.Module):
                                           std=None if std is None else [float(v) for v in std])
 
 
-class _TokenEncoderFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx: Any, module: "TeTEncoderB200", x: Tensor, *params: Tensor) -> Tensor:
-        _, enc_f32, sv = module.engine.encoder_forward(x, want_f32=True)
-        ctx.module, ctx.sv = module, sv
-        return enc_f32.view(x.shape[0], module.geo.T, module.geo.D)
-
-    @staticmethod
-    def backward(ctx: Any, d_out: Tensor) -> Tuple[Any, ...]:
-        module, sv = ctx.module, ctx.sv
-        arena, eng = module.arena, module.engine
-        keys = module.all_keys
-        G = _pick_grad_arena(arena, keys)
-        eng.encoder_backward(sv, d_out.contiguous().float().view(-1, module.geo.D), G)  # fp32: the LN output is the module output
-        if eng.reducer is not None:
-            eng.reducer.finish()
-        _publish_grads(arena, G, keys)
-        ctx.sv = None
-        d_in, eng.d_input = eng.d_input, None
-        return (None, d_in) + (None,) * len(keys)
-
-
-class TeTEncoderB200(nn.Module):
+class TeTEncoderB200(_FusedStack):
     """Drop-in for ``TeTEncoder`` (registered as ``tet``, cflearn/modules/nlp/encoder/transformer.py:16-99): the text
     tower's transformer stack on an already embedded sequence [B, T, D] -> LayerNorm-ed tokens [B, T, D] (fp32).
     Same kernels as the ViT blocks with the causal flag of the attention kernels (``use_triu_attn_mask``); the
@@ -736,45 +705,23 @@ class TeTEncoderB200(nn.Module):
                 or no_head_norm not in (None, False) or norm_after_head:
             raise NotImplementedError("TeTEncoderB200 implements the configuration CLIP's text tower uses (pre-norm LayerNorm, "
                                       "no dropout / drop-path, learned positions, head_pooler=None)")
-        ak = dict(attention_kwargs or {})
-        if ak.get("num_heads", 6) != latent_dim // 64 or not ak.get("bias", True) or set(ak) - {"num_heads", "bias"}:
-            raise NotImplementedError("TeTEncoderB200 needs attention_kwargs num_heads = latent_dim // 64 (head dim 64) and bias=True")
-        fk = dict(feedforward_kwargs or {})
-        if set(fk) - {"activation"}:
-            raise NotImplementedError(f"unsupported feedforward_kwargs: {sorted(set(fk) - {'activation'})}")
-        emb_eps: Optional[float] = None
-        if embedding_norm is not None:
-            if not isinstance(embedding_norm, nn.LayerNorm) or tuple(embedding_norm.normalized_shape) != (latent_dim,) \
-                    or not embedding_norm.elementwise_affine or embedding_norm.bias is None:
-                raise NotImplementedError("embedding_norm must be an affine nn.LayerNorm(latent_dim)")
-            emb_eps = float(embedding_norm.eps)
+        # the reference TeTEncoder's num_heads defaults to 6, whatever latent_dim is
+        common = _check_common("TeTEncoderB200", latent_dim, default_heads=6, norm_kwargs=norm_kwargs, embedding_norm=embedding_norm,
+                               attention_kwargs=attention_kwargs, feedforward_kwargs=feedforward_kwargs)
         if use_triu_attn_mask:  # transformer.py:42-48
             self.register_buffer("attention_mask", torch.ones(context_length, context_length, dtype=torch.bool).triu_(1))
         else:
             self.attention_mask = None
-        eps = float((norm_kwargs or {}).get("eps", 1e-6))
-        self.geo = ViTGeometry(img_size=0, patch_size=16, in_channels=0, latent_dim=latent_dim, num_layers=num_layers,
-                               ff_ratio=feedforward_dim_ratio, eps=eps, num_classes=None, embedding_norm_eps=emb_eps,
-                               activation=fk.get("activation", "GELU"), context_length=context_length, causal=bool(use_triu_attn_mask))
-        spec = self.geo.spec(with_head=False)
-        self.arena = ParamArena(spec)
-        params: Dict[str, nn.Parameter] = {}
-        for key, shape in spec:
-            p = nn.Parameter(_init_param(key, shape))
-            if embedding_norm is not None and key.startswith("encoder.embedding_norm."):
-                p.data.copy_(getattr(embedding_norm, key.rsplit(".", 1)[1]).data)
-            params[key] = p
-            _register_dotted(self, key, p)
-        self.arena.attach(params)
-        self.engine = ViTEngine(self.geo, self.arena)
-        self.all_keys = [k for k, _ in spec]
+        self._build(ViTGeometry(img_size=0, patch_size=16, in_channels=0, latent_dim=latent_dim, num_layers=num_layers,
+                                ff_ratio=feedforward_dim_ratio, num_classes=None, context_length=context_length,
+                                causal=bool(use_triu_attn_mask), **common),
+                    embedding_norm)
         self.latent_dim = latent_dim
 
     def forward(self, net: Tensor, mask: Optional[Tensor] = None, *, apply_head: bool = True, clip_skip: int = 0, **kwargs: Any) -> Tensor:
         if mask is not None or not apply_head or clip_skip != 0:
             raise NotImplementedError("TeTEncoderB200: custom masks, apply_head=False and clip_skip are outside the fused path")
-        self.arena.ensure()
-        return _TokenEncoderFn.apply(self, net, *[self.arena.params[k] for k in self.all_keys])
+        return self._run(net)
 
 
 class VanillaClassifierB200(nn.Module):
@@ -845,11 +792,9 @@ class VanillaClassifierB200(nn.Module):
 
     def forward(self, net: Tensor, *, return_latent: bool = False) -> Dict[str, Tensor]:
         self.check_labels()
-        self.arena.ensure()
         if return_latent:
-            return {LATENT_KEY: _EncoderFn.apply(self.encoder, net, *self.encoder._param_list(self.encoder_keys))}
-        logits = _ClassifierFn.apply(self, net, *self.encoder._param_list(self.all_keys))
-        return {PREDICTIONS_KEY: logits}
+            return {LATENT_KEY: self.encoder._run(net)}
+        return {PREDICTIONS_KEY: self.encoder._run(net, head=True)}
 
     def train_step(self, net: Tensor, labels: Tensor) -> Tensor:
         """forward + CrossEntropyLoss + backward (IDLModel.train, schema.py:1266-1276,:980); returns the loss.

@@ -350,9 +350,8 @@ int b200_conv3x3_wgrad_nhwc_bf16(const void* dy, long long ld_dy, const void* x,
 
 /* Upper bound on the grid of every persistent kernel of this library (the GEMMs); 0 = all SMs (default);
  * launches > 0: the bound lapses by itself after that many persistent launches.  Returns the previous value.  For co-scheduling with other kernels that must hold SMs (an NCCL all-reduce in flight): tiles are
- * assigned to CTAs statically, so a CTA that has to wait for an SM stretches its kernel.  The data-parallel step's default
- * shrinks only the GEMM launched right behind a bucket (max_ctas of b200_gemm_bf16); B200_DP_SHRINK=all uses this knob for the
- * whole bucket window (an alternative schedule for A/B timing).  (DistributedDataParallel's overlap,
+ * assigned to CTAs statically, so a CTA that has to wait for an SM stretches its kernel.  The package's data-parallel step
+ * does not use this bound: it shrinks only the GEMM launched right behind a bucket (max_ctas of b200_gemm_bf16).  (DistributedDataParallel's overlap,
  * accelerate.prepare, cflearn/schema.py:1174-1180, has no such knob: eager kernels are not persistent.) */
 int b200_set_persistent_ctas(int n, int launches);
 

@@ -168,13 +168,23 @@ def test_param_arena_views_and_state_dict_roundtrip():
 
 
 def test_bucket_layout_covers_arena_without_overlap():
-    m = registry.build_module("cv_clf", config=dict(in_channels=3, num_classes=16, img_size=32, latent_dim=128, encoder="vit",
-                                                    encoder_config=dict(patch_size=16, num_layers=3)))
-    red = dp.GradBucketReducer(m.arena, 3)
-    spans = sorted(red.buckets.values())
-    assert spans[0][0] == 0 and spans[-1][1] == m.arena.total
-    for (lo0, hi0), (lo1, hi1) in zip(spans, spans[1:]):
-        assert hi0 == lo1
+    clf = registry.build_module("cv_clf", config=dict(in_channels=3, num_classes=16, img_size=32, latent_dim=128, encoder="vit",
+                                                      encoder_config=dict(patch_size=16, num_layers=3)))
+    # CLIP's vision tower: output_projection and embedding_norm, so the "tail" point holds two spans
+    clip_vision = registry.build_module("encoders.vit", config=dict(
+        img_size=64, patch_size=32, in_channels=3, latent_dim=128, to_patches_config={"bias": False}, num_layers=3,
+        norm_kwargs={"eps": 1e-5}, embedding_norm=torch.nn.LayerNorm(128, 1e-5), attention_kwargs={"num_heads": 2},
+        feedforward_kwargs={"activation": "quick_gelu"}, norm_after_head=True, output_dim=64))
+    # token mode: no patch stem
+    text = registry.build_module("tet", config=dict(latent_dim=128, context_length=12, use_triu_attn_mask=True, num_layers=3,
+                                                    attention_kwargs={"num_heads": 2}))
+    for m in (clf, clip_vision, text):
+        red = dp.GradBucketReducer(m.arena, m.geo.buckets())
+        spans = sorted(s for runs in red.buckets.values() for s in runs)
+        assert spans[0][0] == 0 and spans[-1][1] == m.arena.total
+        for (lo0, hi0), (lo1, hi1) in zip(spans, spans[1:]):
+            assert hi0 == lo1
+    assert len(clip_vision.geo.buckets()["tail"]) == 2
     assert list(dp.shard_indices(10, 1, 4)) == [1, 5, 9]
 
 
