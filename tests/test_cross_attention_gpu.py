@@ -1,5 +1,5 @@
 """Attention with separate Q / K / V and head dims up to 160 (b200_cross_attention_*, ops.cross_attention_*, CrossAttentionB200):
-kernel parity against fp32 math and torch SDPA, determinism (including the query-split dK / dV grid), equality with the packed
+kernel parity against float64 math and torch SDPA, determinism (including the query-split dK / dV grid), equality with the packed
 Dh-64 entry points, and module parity against oracle/unet_oracle.py::cross_attention at SD-v1.5 widths.  The CPU cases check the
 module's parameters and its refusals (the entry points' argument checks and workspace formula are in test_attention_contract.py);
 the others need an H100 (pytest -m gpu)."""
@@ -17,18 +17,9 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 import cflearn_b200  # noqa: F401,E402
 from cflearn_b200 import _cabi, ops  # noqa: E402
 from cflearn_b200.attention import CrossAttentionB200  # noqa: E402
+from _refs import attention_rows, rand_bf16, relerr, with_grads  # noqa: E402
 
 DEV = "cuda"
-
-
-def _rand_bf16(*shape, seed=0):
-    g = torch.Generator(device="cpu").manual_seed(seed)
-    return torch.randn(*shape, generator=g).to(torch.bfloat16).to(DEV)
-
-
-def _relerr(a, b):
-    a, b = a.float(), b.float()
-    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
 
 
 def _heads(x, B, H):  # [B*T, >= H*Dh] view -> [B, H, T, Dh]
@@ -36,27 +27,17 @@ def _heads(x, B, H):  # [B*T, >= H*Dh] view -> [B, H, T, Dh]
     return x.reshape(B, -1, H, Dh).permute(0, 2, 1, 3)
 
 
-def _ref(q, k, v, B, H, causal):
-    qf, kf, vf = (_heads(t.float(), B, H) for t in (q, k, v))
-    s = (qf @ kf.transpose(-1, -2)) * qf.shape[-1] ** -0.5
-    if causal:
-        T = s.shape[-1]
-        s = s.masked_fill(torch.ones(T, T, device=s.device, dtype=torch.bool).triu(1), float("-inf"))
-    o = torch.softmax(s, -1) @ vf
-    return o.permute(0, 2, 1, 3).reshape(q.shape[0], -1), torch.logsumexp(s, -1)
-
-
 def _operands(B, Tq, Tk, H, Dh, packed, seed):
     """q / k / v as column views of packed projection outputs (self: one [M, 3L] buffer; cross: q [M, L] + kv [Mc, 2L]) or as
     separate contiguous tensors."""
     L = H * Dh
     if packed and Tq == Tk:
-        qkv = _rand_bf16(B * Tq, 3 * L, seed=seed)
+        qkv = rand_bf16(B * Tq, 3 * L, seed=seed)
         return qkv[:, :L], qkv[:, L:2 * L], qkv[:, 2 * L:]
     if packed:
-        kv = _rand_bf16(B * Tk, 2 * L, seed=seed + 1)
-        return _rand_bf16(B * Tq, L, seed=seed), kv[:, :L], kv[:, L:]
-    return _rand_bf16(B * Tq, L, seed=seed), _rand_bf16(B * Tk, L, seed=seed + 1), _rand_bf16(B * Tk, L, seed=seed + 2)
+        kv = rand_bf16(B * Tk, 2 * L, seed=seed + 1)
+        return rand_bf16(B * Tq, L, seed=seed), kv[:, :L], kv[:, L:]
+    return rand_bf16(B * Tq, L, seed=seed), rand_bf16(B * Tk, L, seed=seed + 1), rand_bf16(B * Tk, L, seed=seed + 2)
 
 
 def _bwd(q, k, v, out, dout, lse, B, H, causal, packed):
@@ -74,22 +55,21 @@ def _run_case(B, Tq, Tk, H, Dh, causal, packed, seed=0):
     q, k, v = _operands(B, Tq, Tk, H, Dh, packed, seed)
     out, lse = ops.cross_attention_fwd(q, k, v, B, H, causal=causal)
     torch.cuda.synchronize()
-    ref_o, ref_lse = _ref(q, k, v, B, H, causal)
-    assert _relerr(out, ref_o) < 5e-3, _relerr(out, ref_o)
-    assert torch.allclose(lse, ref_lse, rtol=1e-4, atol=1e-4), (lse - ref_lse).abs().max().item()
+    scale = Dh ** -0.5
+    ref_o, ref_lse = attention_rows(q, k, v, B, H, scale, causal)
+    assert relerr(out, ref_o) < 5e-3, relerr(out, ref_o)
+    assert torch.allclose(lse.double(), ref_lse, rtol=1e-4, atol=1e-4), (lse.double() - ref_lse).abs().max().item()
     sdpa = F.scaled_dot_product_attention(*(_heads(t, B, H) for t in (q, k, v)), is_causal=causal)
-    assert _relerr(out, sdpa.permute(0, 2, 1, 3).reshape(B * Tq, H * Dh)) < 5e-3
-    dout = _rand_bf16(B * Tq, H * Dh, seed=seed + 7)
+    assert relerr(out, sdpa.permute(0, 2, 1, 3).reshape(B * Tq, H * Dh)) < 5e-3
+    dout = rand_bf16(B * Tq, H * Dh, seed=seed + 7)
     dq, dk, dv = _bwd(q, k, v, out, dout, lse, B, H, causal, packed)
     torch.cuda.synchronize()
-    qf, kf, vf = (t.float().requires_grad_(True) for t in (q, k, v))
-    ro, _ = _ref(qf, kf, vf, B, H, causal)
-    ro.backward(dout.float())
-    for name, ours, ref in (("dq", dq, qf.grad), ("dk", dk, kf.grad), ("dv", dv, vf.grad)):
+    _, (dq64, dk64, dv64) = with_grads(attention_rows, (q, k, v), dout, B, H, scale, causal)
+    for name, ours, ref in (("dq", dq, dq64), ("dk", dk, dk64), ("dv", dv, dv64)):
         if name != "dv" and Tk == 1:  # one key: P = 1 and dS = 0, so dQ / dK are 0 up to rounding and a relative error means nothing
-            assert ours.float().norm() <= 1e-2 * vf.grad.norm(), ours.float().norm().item()
+            assert ours.double().norm() <= 1e-2 * dv64.norm(), ours.float().norm().item()
             continue
-        e = _relerr(ours, ref)
+        e = relerr(ours, ref)
         assert e < 1e-2, f"{name}: {e}"
     return q, k, v, out, dout, lse, (dq, dk, dv)
 
@@ -135,8 +115,8 @@ def test_backward_is_deterministic(B, H, Tq, Tk, Dh):
 def test_matches_long_entry_points(B, T, H, causal):
     """Grids of >= 132 dK / dV CTAs: the new entry does not split the queries, so it must equal b200_attention_long_* bit for bit."""
     D = H * 64
-    qkv = _rand_bf16(B * T, 3 * D, seed=T)
-    dout = _rand_bf16(B * T, D, seed=T + 1)
+    qkv = rand_bf16(B * T, 3 * D, seed=T)
+    dout = rand_bf16(B * T, D, seed=T + 1)
     stream = torch.cuda.current_stream().cuda_stream
     out_l = torch.empty((B * T, D), dtype=torch.bfloat16, device=DEV)
     lse_l = torch.empty((B, H, T), dtype=torch.float32, device=DEV)
@@ -208,9 +188,9 @@ def test_module_parity(query_dim, side, cross):
         refs.append(r)
     eager, fp32 = refs
     for k in ours:
-        floor = _relerr(eager[k], fp32[k])
-        assert _relerr(ours[k], fp32[k]) <= 1.5 * floor + 1e-6, (k, _relerr(ours[k], fp32[k]), floor)
-        assert _relerr(ours[k], eager[k]) <= 2.0 * floor + 1e-6, (k, _relerr(ours[k], eager[k]), floor)
+        floor = relerr(eager[k], fp32[k])
+        assert relerr(ours[k], fp32[k]) <= 1.5 * floor + 1e-6, (k, relerr(ours[k], fp32[k]), floor)
+        assert relerr(ours[k], eager[k]) <= 2.0 * floor + 1e-6, (k, relerr(ours[k], eager[k]), floor)
 
 
 # ---- 5. CPU: the module's parameters and refusals ----------------------------------------------------------------------------

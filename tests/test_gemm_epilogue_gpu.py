@@ -8,14 +8,10 @@ import torch.nn.functional as F
 
 import cflearn_b200  # noqa: F401  (registers the package)
 from cflearn_b200 import ops
+from _refs import rand_bf16
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-
-
-def _rand_bf16(*shape, scale=1.0, seed=0):
-    g = torch.Generator(device="cpu").manual_seed(seed)
-    return (torch.randn(*shape, generator=g) * scale).to(torch.bfloat16).to(DEV)
 
 
 def _padded(M, N, dtype):
@@ -34,7 +30,7 @@ def _gelu_pair(a, b, bias, M, N, max_ctas=0, epilogue=ops.EPI_BIAS_GELU_BF16):
 def test_result_independent_of_cta_count(epilogue):
     # 4096 x 2048: 256 tiles; one CTA runs all of them, so the staging tile's full / empty phases wrap 256 times
     M, N, K = 4096, 2048, 256
-    a, b, bias = _rand_bf16(M, K, seed=1), _rand_bf16(N, K, scale=0.5, seed=2), _rand_bf16(N, seed=3)
+    a, b, bias = rand_bf16(M, K, seed=1), rand_bf16(N, K, scale=0.5, seed=2), rand_bf16(N, seed=3)
     res = torch.randn(M, N, device=DEV, generator=torch.Generator(device=DEV).manual_seed(4))
     outs = []
     for ctas in (0, 5, 1):
@@ -60,7 +56,7 @@ def test_result_independent_of_cta_count(epilogue):
 def test_edges_and_cross_epilogue_consistency(M, N, K):
     """M / N edges (N not a multiple of 8 included); h of the GELU epilogue == the bias epilogue; the residual epilogue ==
     aux + float(bias epilogue), in place or not; dGELU == dGELU(h) applied to the plain GEMM, all bit for bit."""
-    a, b, bias = _rand_bf16(M, K, seed=11), _rand_bf16(N, K, scale=0.5, seed=12), _rand_bf16(N, seed=13)
+    a, b, bias = rand_bf16(M, K, seed=11), rand_bf16(N, K, scale=0.5, seed=12), rand_bf16(N, seed=13)
     t = ops.gemm(a, b, bias=bias)
     torch.cuda.synchronize()
     ref = (a.float() @ b.float().t() + bias.float()).to(torch.bfloat16)
@@ -85,9 +81,9 @@ def test_edges_and_cross_epilogue_consistency(M, N, K):
 
     # dGELU: dG[M, N] = dY[M, K] . W[K, N] (MN-major B) times gelu'(h); the plain GEMM of the same operands gives bf16(acc)
     w = _padded(K, N, torch.bfloat16)  # TMA needs 16-byte row strides
-    w.copy_(_rand_bf16(K, N, scale=0.05, seed=15))
+    w.copy_(rand_bf16(K, N, scale=0.05, seed=15))
     hh = _padded(M, N, torch.bfloat16)
-    hh.copy_(_rand_bf16(M, N, seed=16))
+    hh.copy_(rand_bf16(M, N, seed=16))
     dacc = ops.gemm(a, w, b_mn_major=True)
     dg = ops.gemm(a, w, b_mn_major=True, epilogue=ops.EPI_DGELU_BF16, aux=hh)
     torch.cuda.synchronize()
@@ -100,9 +96,9 @@ def test_edges_and_cross_epilogue_consistency(M, N, K):
 
 def test_conv3x3_through_epilogue_warps():
     B, H, W, Cin, Cout = 2, 16, 16, 64, 200
-    x = _rand_bf16(B, H, W, Cin, seed=21)
-    w = _rand_bf16(Cout, Cin, 3, 3, scale=0.05, seed=22)
-    bias = _rand_bf16(Cout, seed=23)
+    x = rand_bf16(B, H, W, Cin, seed=21)
+    w = rand_bf16(Cout, Cin, 3, 3, scale=0.05, seed=22)
+    bias = rand_bf16(Cout, seed=23)
     wp = ops.pack_conv3x3_weight(w)
     y = ops.conv3x3(x, wp, bias)
     res = torch.randn(B, H, W, Cout, device=DEV, generator=torch.Generator(device=DEV).manual_seed(24))

@@ -351,6 +351,31 @@ def test_persistent_cta_bound_is_a_plain_host_setting():
         lib.b200_set_persistent_ctas(first, 0)
 
 
+# (argument, value stored) for each kernel-variant switch
+SWITCHES = {
+    "b200_set_attention_fwd_version": [(1, 1), (2, 2), (0, 0), (3, 0), (-1, 0)],
+    "b200_set_attention_bwd_version": [(1, 1), (2, 2), (3, 3), (0, 0), (4, 0), (-2, 0)],
+    "b200_set_attention_prefetch": [(1, 1), (0, 0), (5, 1), (-1, 1)],
+    "b200_set_gemm_multicast": [(1, 1), (2, 2), (0, 0), (3, 2), (-4, 0)],
+}
+
+
+@pytest.mark.parametrize("name", sorted(SWITCHES))
+def test_kernel_variant_switches_return_the_previous_value_and_clamp(name):
+    """The variant switches the C-ABI keeps for compatibility (the sm_90a build has one kernel per op, so they change no result)
+    are plain host settings: each returns the previous value and stores its argument clamped to the range it accepts."""
+    setter = getattr(_cabi.lib(), name)
+    first = setter(0)
+    try:
+        prev = 0
+        for arg, stored in SWITCHES[name]:
+            assert setter(arg) == prev, (name, arg)
+            prev = stored
+        assert setter(0) == prev, name
+    finally:
+        setter(first)
+
+
 def test_bench_dp_mode_auto_resolves_by_world_size(monkeypatch):
     """``bench.py --dp-mode auto``: the in-graph bucketed exchange up to 2 GPUs, one all-reduce behind the graph from 3 GPUs up
     (DESIGN.md section 4)."""

@@ -8,8 +8,8 @@ max shows: groups and rows whose mean is hundreds of standard deviations, consta
 Each comparison is against the "eager floor": the error, against the same float64 reference, of the PyTorch op that eager bf16
 autocast runs on the same inputs.  The per-element check counts elements more than one bf16 ulp from bf16(float64 reference) and
 allows no more of them than eager has; the relative L2 error must stay within 1.5x eager's + 1e-6.  Statistics (mean, rstd) must
-be within 4x eager's relative error or 1e-5.  The CPU cases check the float64 references against torch's own ops and the input
-generators against the conditioning they claim; the others need an H100 (pytest -m gpu)."""
+be within 4x eager's relative error or 1e-5.  The references are in _refs.py.  The CPU cases check the input generators against
+the conditioning they claim; the others need an H100 (pytest -m gpu)."""
 import math
 import os
 import sys
@@ -24,68 +24,17 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 
 import cflearn_b200  # noqa: F401,E402
 from cflearn_b200 import _cabi, ops  # noqa: E402
+from _refs import (F64, GROUPS, attention, bf16_ulps_off, groupnorm, layernorm, relerr, softmax_xent,  # noqa: E402
+                   symmetric_xent, with_grads)
 
 DEV = "cuda"
-GROUPS = 32
-F64 = torch.float64
-
-
-# ---- float64 references ------------------------------------------------------------------------------------------------------------
-def gn_ref64(x, gamma, beta, eps, silu):
-    """GroupNorm(32) (+SiLU) of channels-last x [B, HW, C] in float64: (y, mean [B, 32], rstd [B, 32], var [B, 32])."""
-    B, HW, C = x.shape
-    xg = x.to(F64).view(B, HW, GROUPS, C // GROUPS)
-    mean = xg.mean(dim=(1, 3))
-    var = ((xg - mean[:, None, :, None]) ** 2).mean(dim=(1, 3))  # two-pass
-    rstd = (var + eps).rsqrt()
-    z = ((xg - mean[:, None, :, None]) * rstd[:, None, :, None]).reshape(B, HW, C) * gamma.to(F64) + beta.to(F64)
-    return (F.silu(z) if silu else z), mean, rstd, var
-
-
-def ln_ref64(x, gamma, beta, eps):
-    """LayerNorm over the last dim in float64: (y, mean, rstd, var)."""
-    xd = x.to(F64)
-    mean = xd.mean(-1)
-    var = ((xd - mean[:, None]) ** 2).mean(-1)
-    rstd = (var + eps).rsqrt()
-    return (xd - mean[:, None]) * rstd[:, None] * gamma.to(F64) + beta.to(F64), mean, rstd, var
-
-
-def log_softmax_ref64(x):
-    xd = x.to(F64)
-    m = xd.max(-1, keepdim=True).values
-    return xd - m - (xd - m).exp().sum(-1, keepdim=True).log()
-
-
-def attn_ref64(q, k, v, scale, causal):
-    """[B, H, T, D] float64 attention: (out, lse [B, H, Tq])."""
-    s = (q.to(F64) @ k.to(F64).transpose(-1, -2)) * scale
-    if causal:
-        s = s.masked_fill(torch.ones(s.shape[-2], s.shape[-1], dtype=torch.bool, device=s.device).triu(1), float("-inf"))
-    lse = torch.logsumexp(s, -1)
-    return (s - lse[..., None]).exp() @ v.to(F64), lse
 
 
 # ---- checks ------------------------------------------------------------------------------------------------------------------------
-def _relerr(a, ref):
-    ref = ref.to(F64)
-    return ((a.to(F64) - ref).norm() / ref.norm().clamp_min(1e-300)).item()
-
-
-def _ulp_bad(got, ref):
-    """Elements of `got` more than one bf16 ulp from bf16(ref) (NaN counts).  Near zero the ulp is floored at 2^-16 of the largest
-    |ref|: there both eager's and the kernel's fp32 arithmetic leave absolute errors that mean nothing at the tensor's scale."""
-    r = ref.to(torch.bfloat16).to(F64)
-    a = r.abs()
-    ulp = torch.exp2(torch.floor(torch.log2(a.clamp_min(1e-300))) - 7)
-    tol = ulp.clamp_min(2.0 ** -16 * ref.to(F64).abs().max().item())
-    return int((~((got.to(F64) - r).abs() <= tol)).sum().item())
-
-
 def _assert_like_eager(what, got, eager, ref, per_element=True, l2_factor=1.5):
     """``per_element=False`` keeps only the L2 bound (and still counts NaN / inf as failures)."""
-    ours_bad, eager_bad = _ulp_bad(got, ref), _ulp_bad(eager, ref)
-    e_ours, e_eager = _relerr(got, ref), _relerr(eager, ref)
+    ours_bad, eager_bad = bf16_ulps_off(got, ref), bf16_ulps_off(eager, ref)
+    e_ours, e_eager = relerr(got, ref), relerr(eager, ref)
     msg = (f"{what}: {ours_bad} elements more than 1 bf16 ulp from float64 (eager: {eager_bad}), relative L2 {e_ours:.3e} "
            f"(eager: {e_eager:.3e}) of {got.numel()} elements")
     assert bool(torch.isfinite(got).all()) and e_ours <= l2_factor * e_eager + 1e-6, msg
@@ -140,29 +89,6 @@ def gn_slabs(B, HW):
 
 
 # ---- CPU: the references and the generators ----------------------------------------------------------------------------------------
-def test_float64_references_match_torch():
-    g = torch.Generator().manual_seed(0)
-    x = gn_input(2, 49, 64, "mixed", seed=1)
-    gamma, beta = torch.randn(64, generator=g, dtype=F64), torch.randn(64, generator=g, dtype=F64)
-    for silu in (False, True):
-        y, mean, rstd, _ = gn_ref64(x, gamma, beta, 1e-5, silu)
-        want = F.group_norm(x.to(F64).permute(0, 2, 1), GROUPS, gamma, beta, 1e-5).permute(0, 2, 1)
-        assert torch.allclose(y, F.silu(want) if silu else want, rtol=1e-12, atol=1e-12)
-        _, m2, r2 = torch.native_group_norm(x.to(F64).permute(0, 2, 1).contiguous(), gamma, beta, 2, 64, 49, GROUPS, 1e-5)
-        assert torch.allclose(mean, m2, rtol=1e-12, atol=1e-12) and torch.allclose(rstd, r2, rtol=1e-9)
-    xl = torch.randn(37, 40, generator=g, dtype=F64) * 3 + 1e3
-    y, mean, rstd, _ = ln_ref64(xl, gamma[:40], beta[:40], 1e-6)
-    assert torch.allclose(y, F.layer_norm(xl, (40,), gamma[:40], beta[:40], 1e-6), rtol=1e-10, atol=1e-10)
-    logits = torch.randn(9, 31, generator=g, dtype=F64) * 300
-    logits[0, 3] = float("-inf")
-    assert torch.equal(torch.isinf(log_softmax_ref64(logits)), torch.isinf(logits))
-    assert torch.allclose(log_softmax_ref64(logits)[torch.isfinite(logits)], F.log_softmax(logits, -1)[torch.isfinite(logits)], rtol=1e-12)
-    q, k, v = (torch.randn(2, 3, 50, 40, generator=g, dtype=F64) for _ in range(3))
-    for causal in (False, True):
-        o, lse = attn_ref64(q * 10, k, v, 40 ** -0.5, causal)
-        assert torch.allclose(o, F.scaled_dot_product_attention(q * 10, k, v, is_causal=causal), rtol=1e-10, atol=1e-10)
-
-
 @pytest.mark.parametrize("cond", GN_CONDS)
 def test_groupnorm_inputs_have_the_conditioning_they_claim(cond):
     B, HW, C = 3, 256, 320
@@ -209,9 +135,7 @@ def _groupnorm_case(B, H, W, C, cond, silu, seed):
     dy = torch.randn(B, HW, C, generator=g).to(torch.bfloat16).to(DEV)
 
     # float64 reference, forward and backward
-    xd, gd, bd = (t.to(F64).requires_grad_(True) for t in (x, gamma, beta))
-    y64, mean64, rstd64, var64 = gn_ref64(xd, gd, bd, eps, silu)
-    y64.backward(dy.to(F64))
+    (y64, mean64, rstd64, var64), (dx64, dg64, db64) = with_grads(groupnorm, (x, gamma, beta), dy, eps, silu)
     # eager under bf16 autocast: GroupNorm in fp32 on the upcast input (ATen's kernel, which returns its mean / rstd), SiLU in fp32,
     # one bf16 rounding; the input gradient reaches the bf16 input as bf16
     xe = x.float().permute(0, 2, 1).contiguous().requires_grad_(True)
@@ -237,9 +161,9 @@ def _groupnorm_case(B, H, W, C, cond, silu, seed):
     # mean / std ~ 1e3 that moves outputs near zero by more than their own bf16 ulp (the floor eps * mean / std both share).  The
     # SiLU derivative's fast exp2 / reciprocal leave dgamma / dbeta up to ~2x eager's (small) error.
     _assert_like_eager(f"{tag}: y", y, ye, y64, per_element=False)
-    _assert_like_eager(f"{tag}: dx", dx, dx_e, xd.grad, per_element=False)
-    _assert_like_eager(f"{tag}: dgamma", dgamma, ge.grad, gd.grad, per_element=False, l2_factor=4.0)
-    _assert_like_eager(f"{tag}: dbeta", dbeta, be.grad, bd.grad, per_element=False, l2_factor=4.0)
+    _assert_like_eager(f"{tag}: dx", dx, dx_e, dx64, per_element=False)
+    _assert_like_eager(f"{tag}: dgamma", dgamma, ge.grad, dg64, per_element=False, l2_factor=4.0)
+    _assert_like_eager(f"{tag}: dbeta", dbeta, be.grad, db64, per_element=False, l2_factor=4.0)
     # deterministic: a second run is bit-identical
     y2, m2, r2 = ops.groupnorm_silu_fwd(x, gamma, beta, eps, silu=silu)
     dx2, dg2, db2 = ops.groupnorm_silu_bwd(x, dy, gamma, beta, m2, r2, silu=silu)
@@ -283,13 +207,6 @@ def _ln_eager(x32, gamma, beta, eps, dy, out_dtype):
     return ye, mean_e.flatten(), rstd_e.flatten(), xe.grad, ge.grad, be.grad
 
 
-def _ln_ref(x, gamma, beta, eps, dy):
-    xd, gd, bd = (t.to(F64).requires_grad_(True) for t in (x, gamma, beta))
-    y64, mean64, rstd64, var64 = ln_ref64(xd, gd, bd, eps)
-    y64.backward(dy.to(F64))
-    return y64, mean64, rstd64, var64, xd.grad, gd.grad, bd.grad
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("dim", [8, 40, 768, 1024])
 def test_layernorm_fp32(dim):
@@ -303,7 +220,7 @@ def test_layernorm_fp32(dim):
     gamma, beta = torch.randn(dim, generator=g).to(DEV), torch.randn(dim, generator=g).to(DEV)
     dy = torch.randn(rows, dim, generator=g).to(torch.bfloat16).to(DEV)
     dres = torch.randn(rows, dim, generator=g).to(DEV)
-    y64, mean64, rstd64, var64, dx64, dg64, db64 = _ln_ref(x, gamma, beta, eps, dy)
+    (y64, mean64, rstd64, var64), (dx64, dg64, db64) = with_grads(layernorm, (x, gamma, beta), dy, eps)
     ye, mean_e, rstd_e, dx_e, dg_e, db_e = _ln_eager(x.contiguous(), gamma, beta, eps, dy, torch.bfloat16)
 
     y, mean, rstd = ops.layernorm_fwd(xbuf, gamma, beta, eps, rows=rows, dim=dim, ld_x=ld)
@@ -337,7 +254,7 @@ def test_layernorm_bf16(dim):
     gamma, beta = torch.randn(dim, generator=g).to(DEV), torch.randn(dim, generator=g).to(DEV)
     dy = torch.randn(rows, dim, generator=g).to(torch.bfloat16).to(DEV)
     dres = torch.randn(rows, dim, generator=g).to(torch.bfloat16).to(DEV)
-    y64, mean64, rstd64, var64, dx64, dg64, db64 = _ln_ref(x, gamma, beta, eps, dy)
+    (y64, mean64, rstd64, var64), (dx64, dg64, db64) = with_grads(layernorm, (x, gamma, beta), dy, eps)
     ye, mean_e, rstd_e, dx_e, dg_e, db_e = _ln_eager(x.float(), gamma, beta, eps, dy, torch.bfloat16)
     dx_e = dres + dx_e.to(torch.bfloat16)  # eager: the cast back to the bf16 input, then the bf16 residual add
 
@@ -396,10 +313,8 @@ def test_softmax_xent(case):
     loss_mean, loss_rows, dl, bad = ops.softmax_xent(logits, labels, grad_scale=gs, grad_scale_dev=gsd)
     torch.cuda.synchronize()
     sc = gs * (gsd.item() if gsd is not None else 1.0)
-    lsm = log_softmax_ref64(logits)
-    ref_rows = -lsm.gather(1, labels[:, None])[:, 0]
-    onehot = F.one_hot(labels, C).to(F64)
-    dl64 = (lsm.exp() - onehot) * sc / B
+    ref_rows, dl64 = softmax_xent(logits, labels)
+    dl64 = dl64 * sc
     lf = logits.float().requires_grad_(True)
     rows_e = F.cross_entropy(lf, labels, reduction="none")
     rows_e.mean().backward()
@@ -435,17 +350,15 @@ def test_symmetric_xent(case):
     loss = ops.symmetric_xent(logits, dlogits=dl, grad_scale=gs, grad_scale_dev=gsd)
     torch.cuda.synchronize()
     sc = gs * (gsd.item() if gsd is not None else 1.0)
-    ld64 = logits.to(F64).requires_grad_(True)
+    ref, dl64 = symmetric_xent(logits)
     idx = torch.arange(B, device=DEV)
-    ref = -0.5 * (log_softmax_ref64(ld64)[idx, idx].mean() + log_softmax_ref64(ld64.t())[idx, idx].mean())
-    ref.backward()
     lf = logits.float().requires_grad_(True)
     loss_e = 0.5 * (F.cross_entropy(lf, idx) + F.cross_entropy(lf.t(), idx))
     loss_e.backward()
     mag = max(1.0, logits.float()[torch.isfinite(logits.float())].abs().max().item())
     e_ours, e_eager = abs(loss.item() - ref.item()), abs(loss_e.item() - ref.item())
     assert e_ours <= 4 * e_eager + 2.0 ** -23 * mag + 1e-6 * abs(ref.item()), f"{case}: loss error {e_ours:.3e} (eager {e_eager:.3e})"
-    _assert_like_eager(f"symmetric_xent {case}: dlogits", dl, (lf.grad * sc).to(torch.bfloat16), ld64.grad * sc)
+    _assert_like_eager(f"symmetric_xent {case}: dlogits", dl, (lf.grad * sc).to(torch.bfloat16), dl64 * sc)
 
 
 # ---- attention with peaked scores --------------------------------------------------------------------------------------------------
@@ -488,13 +401,10 @@ def _row_errors(x, ref):
 
 def _check_attention(tag, q, k, v, dout, scale, causal, out, lse, dq, dk, dv):
     """q, k, v, dout: bf16 [B, H, T, D] on the device; the kernel's results in the same layout (lse [B, H, Tq])."""
-    qd, kd, vd = (t.to(F64).requires_grad_(True) for t in (q, k, v))
-    o64, lse64 = attn_ref64(qd, kd, vd, scale, causal)
-    o64.backward(dout.to(F64))
+    (o64, lse64), (dq64, dk64, dv64) = with_grads(attention, (q, k, v), dout, scale, causal)
     qe, ke, ve = (t.clone().requires_grad_(True) for t in (q, k, v))
     oe = F.scaled_dot_product_attention(qe, ke, ve, is_causal=causal, scale=scale)
     oe.backward(dout)
-    o64 = o64.detach()
     # out: every row against float64, no further than 2x eager's row error + one bf16 ulp
     ro, re = _row_errors(out, o64), _row_errors(oe, o64)
     bad = ro > 2 * re + 2.0 ** -7
@@ -503,11 +413,11 @@ def _check_attention(tag, q, k, v, dout, scale, causal, out, lse, dq, dk, dv):
                            f"{re.flatten()[w]:.3e})")
     le = (lse.to(F64) - lse64).abs() / lse64.abs().clamp_min(1.0)
     assert le.max().item() <= 1e-3, f"{tag}: lse error {le.max().item():.3e} at flat index {le.argmax().item()}"
-    for name, ours, eager, ref in (("dq", dq, qe.grad, qd.grad), ("dk", dk, ke.grad, kd.grad), ("dv", dv, ve.grad, vd.grad)):
+    for name, ours, eager, ref in (("dq", dq, qe.grad, dq64), ("dk", dk, ke.grad, dk64), ("dv", dv, ve.grad, dv64)):
         if ref.norm().item() == 0.0:  # one key: P = 1 and dS = 0 exactly, so dq / dk are 0 and only rounding noise may remain
-            assert ours.to(F64).norm().item() <= 1e-3 * vd.grad.norm().item(), (tag, name, ours.float().norm().item())
+            assert ours.to(F64).norm().item() <= 1e-3 * dv64.norm().item(), (tag, name, ours.float().norm().item())
             continue
-        e_ours, e_eager = _relerr(ours, ref), _relerr(eager, ref)
+        e_ours, e_eager = relerr(ours, ref), relerr(eager, ref)
         assert e_ours <= 2 * e_eager + 1e-3, f"{tag}: {name} relative L2 {e_ours:.3e} (eager {e_eager:.3e})"
         rms = ref.norm(dim=-1).pow(2).mean().sqrt().item()  # a wrong row stands out against the typical row norm
         r_ours = ((ours.to(F64) - ref).norm(dim=-1) / rms).max().item()
@@ -571,8 +481,8 @@ def test_cross_attention_peaked_causal(Dh):
 # ---- modules on inputs whose channel groups share an offset -------------------------------------------------------------------------
 def _check_modules(ours, eager, fp32):
     for k in ours:
-        floor = _relerr(eager[k], fp32[k].to(F64))
-        e_f, e_e = _relerr(ours[k], fp32[k]), _relerr(ours[k], eager[k])
+        floor = relerr(eager[k], fp32[k].to(F64))
+        e_f, e_e = relerr(ours[k], fp32[k]), relerr(ours[k], eager[k])
         assert e_f <= 1.5 * floor + 1e-6, f"{k}: vs fp32 {e_f:.3e}, eager vs fp32 {floor:.3e}"
         assert e_e <= 2.0 * floor + 1e-6, f"{k}: vs eager {e_e:.3e}, eager vs fp32 {floor:.3e}"
 

@@ -1,5 +1,5 @@
-"""Streamed attention for sequences longer than 256 tokens (b200_attention_long_*): kernel parity against fp32 references and
-torch SDPA, determinism, the T dispatch in ops, and end-to-end training at ViT 384 px / a 300-token text tower.  The CPU case
+"""Streamed attention for sequences longer than 256 tokens (b200_attention_long_*): kernel parity against float64 references
+and torch SDPA, determinism, the T dispatch in ops, and end-to-end training at ViT 384 px / a 300-token text tower.  The CPU case
 checks the geometry limits (the entry points' argument checks are in test_attention_contract.py); the others need an H100
 (pytest -m gpu)."""
 import os
@@ -15,30 +15,12 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 
 import cflearn_b200  # noqa: F401,E402
 from cflearn_b200 import _cabi, ops, registry, vit  # noqa: E402
+from _refs import packed_attention, rand_bf16, relerr, with_grads  # noqa: E402
 
 DEV = "cuda"
 LENGTHS = [257, 300, 384, 577, 1025, 2048, 4096]
 # (B, H) per length: more CTAs than two per SM at every length up to 1025, a small B * H at 2048 / 4096
 SHAPES = {257: (8, 12), 300: (5, 12), 384: (3, 8), 577: (4, 12), 1025: (2, 12), 2048: (1, 8), 4096: (1, 2)}
-
-
-def _rand_bf16(*shape, seed=0):
-    g = torch.Generator(device="cpu").manual_seed(seed)
-    return torch.randn(*shape, generator=g).to(torch.bfloat16).to(DEV)
-
-
-def _relerr(a, b):
-    a, b = a.float(), b.float()
-    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
-
-
-def _attn_ref(qkv, B, T, H, causal):
-    q, k, v = qkv.view(B, T, 3, H, 64).permute(2, 0, 3, 1, 4).float()  # [B, H, T, 64]
-    s = (q @ k.transpose(-1, -2)) * 0.125
-    if causal:
-        s = s.masked_fill(torch.ones(T, T, device=s.device, dtype=torch.bool).triu(1), float("-inf"))
-    o = torch.softmax(s, -1) @ v
-    return o.permute(0, 2, 1, 3).reshape(B * T, H * 64), torch.logsumexp(s, -1)
 
 
 def _long_fwd(qkv, B, T, H, causal):
@@ -62,22 +44,20 @@ def _long_bwd(qkv, out, dout, lse, B, T, H, causal):
 
 def _check_fwd(out, lse, qkv, B, T, H, causal):
     torch.cuda.synchronize()
-    ref_o, ref_lse = _attn_ref(qkv, B, T, H, causal)
-    assert _relerr(out, ref_o) < 5e-3, _relerr(out, ref_o)
-    assert torch.allclose(lse, ref_lse, rtol=1e-4, atol=1e-4), (lse - ref_lse).abs().max().item()
+    ref_o, ref_lse = packed_attention(qkv, B, T, H, causal=causal)
+    assert relerr(out, ref_o) < 5e-3, relerr(out, ref_o)
+    assert torch.allclose(lse.double(), ref_lse, rtol=1e-4, atol=1e-4), (lse.double() - ref_lse).abs().max().item()
     q, k, v = qkv.view(B, T, 3, H, 64).permute(2, 0, 3, 1, 4)
     sdpa = F.scaled_dot_product_attention(q, k, v, is_causal=causal).permute(0, 2, 1, 3).reshape(B * T, H * 64)
-    assert _relerr(out, sdpa) < 5e-3, _relerr(out, sdpa)
+    assert relerr(out, sdpa) < 5e-3, relerr(out, sdpa)
 
 
 def _check_bwd(dqkv, part, qkv, dout, B, T, H, causal):
     torch.cuda.synchronize()
     D = H * 64
-    qf = qkv.float().requires_grad_(True)
-    ref_o, _ = _attn_ref(qf, B, T, H, causal)
-    ref_o.backward(dout.float())
+    _, (ref,) = with_grads(packed_attention, (qkv,), dout, B, T, H, 0.125, causal)
     for name, sl in (("dq", slice(0, D)), ("dk", slice(D, 2 * D)), ("dv", slice(2 * D, 3 * D))):
-        e = _relerr(dqkv[:, sl], qf.grad[:, sl])
+        e = relerr(dqkv[:, sl], ref[:, sl])
         assert e < 1e-2, f"{name}: {e}"
     ref_b = dqkv.float().view(B, T, 3 * D).sum(1)  # fp32 column sums of the bf16 rows returned, per image
     assert (part - ref_b).abs().max().item() <= 1e-5 * ref_b.abs().max().item(), (part - ref_b).abs().max().item()
@@ -89,7 +69,7 @@ def _check_bwd(dqkv, part, qkv, dout, B, T, H, causal):
 @pytest.mark.parametrize("T", LENGTHS)
 def test_long_attention_fwd(T, causal):
     B, H = SHAPES[T]
-    qkv = _rand_bf16(B * T, 3 * H * 64, seed=T)
+    qkv = rand_bf16(B * T, 3 * H * 64, seed=T)
     out, lse = ops.attention_fwd(qkv, B, T, H, causal=causal)
     _check_fwd(out, lse, qkv, B, T, H, causal)
 
@@ -103,8 +83,8 @@ def test_long_attention_bwd(T, causal):
     if T == 4096:
         B, H = 1, 1
     D = H * 64
-    qkv = _rand_bf16(B * T, 3 * D, seed=T + 1)
-    dout = _rand_bf16(B * T, D, seed=T + 2)
+    qkv = rand_bf16(B * T, 3 * D, seed=T + 1)
+    dout = rand_bf16(B * T, D, seed=T + 2)
     out, lse = ops.attention_fwd(qkv, B, T, H, causal=causal)
     dqkv, part = _long_bwd(qkv, out, dout, lse, B, T, H, causal)
     _check_bwd(dqkv, part, qkv, dout, B, T, H, causal)
@@ -124,8 +104,8 @@ def test_long_attention_bwd(T, causal):
 @pytest.mark.parametrize("B,T,H,causal", [(3, 16, 2, False), (5, 77, 8, True), (4, 197, 12, False), (2, 256, 4, False), (2, 256, 3, True)])
 def test_long_entry_points_at_short_T(B, T, H, causal):
     D = H * 64
-    qkv = _rand_bf16(B * T, 3 * D, seed=T + 5)
-    dout = _rand_bf16(B * T, D, seed=T + 6)
+    qkv = rand_bf16(B * T, 3 * D, seed=T + 5)
+    dout = rand_bf16(B * T, D, seed=T + 6)
     out, lse = _long_fwd(qkv, B, T, H, causal)
     _check_fwd(out, lse, qkv, B, T, H, causal)
     dqkv, part = _long_bwd(qkv, out, dout, lse, B, T, H, causal)
@@ -139,7 +119,7 @@ def test_dispatch_boundary():
     # T = 256: the resident kernels, byte-for-byte
     B, T, H = 3, 256, 4
     D = H * 64
-    qkv, dout = _rand_bf16(B * T, 3 * D, seed=11), _rand_bf16(B * T, D, seed=12)
+    qkv, dout = rand_bf16(B * T, 3 * D, seed=11), rand_bf16(B * T, D, seed=12)
     out, lse = ops.attention_fwd(qkv, B, T, H)
     out_r = torch.empty_like(out)
     lse_r = torch.empty_like(lse)
@@ -152,7 +132,7 @@ def test_dispatch_boundary():
     assert torch.equal(dqkv, dqkv_r)
     # T = 257: the streamed kernels
     T = 257
-    qkv, dout = _rand_bf16(B * T, 3 * D, seed=13), _rand_bf16(B * T, D, seed=14)
+    qkv, dout = rand_bf16(B * T, 3 * D, seed=13), rand_bf16(B * T, D, seed=14)
     out, lse = ops.attention_fwd(qkv, B, T, H, causal=True)
     out_l, lse_l = _long_fwd(qkv, B, T, H, True)
     assert torch.equal(out, out_l) and torch.equal(lse, lse_l)
@@ -205,13 +185,13 @@ def test_train_step_parity_384px(name, batch):
     sdg = {k: v.to(DEV) for k, v in sd.items()}
     e_loss, e_grads, e_taps = vo.train_step(sdg, x, y, cfg, autocast_bf16=True, want_taps=True)
     f_loss, f_grads, f_taps = vo.train_step(sdg, x, y, cfg, autocast_bf16=False, want_taps=True)
-    floor = _relerr(e_taps["logits"], f_taps["logits"])
-    assert _relerr(logits, e_taps["logits"]) < VS_EAGER_FACTOR * floor + SLACK
-    assert _relerr(logits, f_taps["logits"]) < VS_FP32_FACTOR * floor + SLACK
+    floor = relerr(e_taps["logits"], f_taps["logits"])
+    assert relerr(logits, e_taps["logits"]) < VS_EAGER_FACTOR * floor + SLACK
+    assert relerr(logits, f_taps["logits"]) < VS_FP32_FACTOR * floor + SLACK
     assert abs(loss.item() - f_loss.item()) < 1.5 * abs(e_loss.item() - f_loss.item()) + 2e-3 * max(1.0, abs(f_loss.item()))
     assert set(grads) == set(e_grads)
     for k in sorted(grads):
-        ours_vs_eager, ours_vs_fp32, eager_vs_fp32 = _relerr(grads[k], e_grads[k]), _relerr(grads[k], f_grads[k]), _relerr(e_grads[k], f_grads[k])
+        ours_vs_eager, ours_vs_fp32, eager_vs_fp32 = relerr(grads[k], e_grads[k]), relerr(grads[k], f_grads[k]), relerr(e_grads[k], f_grads[k])
         assert ours_vs_eager < VS_EAGER_FACTOR * eager_vs_fp32 + SLACK, f"{k}: ours vs eager {ours_vs_eager}, floor {eager_vs_fp32}"
         assert ours_vs_fp32 < VS_FP32_FACTOR * eager_vs_fp32 + SLACK, (k, ours_vs_fp32, eager_vs_fp32)
 
@@ -240,13 +220,13 @@ def test_text_stack_parity_context_300():
     sdg = {k: v.to(DEV) for k, v in sd.items()}
     e_out, e_dx, e_grads = vo.tet_train_step(sdg, x, up, cfg, autocast_bf16=True)
     f_out, f_dx, f_grads = vo.tet_train_step(sdg, x, up, cfg, autocast_bf16=False)
-    floor = _relerr(e_out, f_out)
-    assert _relerr(out, e_out) < VS_EAGER_FACTOR * floor + SLACK and _relerr(out, f_out) < VS_FP32_FACTOR * floor + SLACK
-    dfloor = _relerr(e_dx, f_dx)
-    assert _relerr(xin.grad, e_dx) < VS_EAGER_FACTOR * dfloor + SLACK and _relerr(xin.grad, f_dx) < VS_FP32_FACTOR * dfloor + SLACK
+    floor = relerr(e_out, f_out)
+    assert relerr(out, e_out) < VS_EAGER_FACTOR * floor + SLACK and relerr(out, f_out) < VS_FP32_FACTOR * floor + SLACK
+    dfloor = relerr(e_dx, f_dx)
+    assert relerr(xin.grad, e_dx) < VS_EAGER_FACTOR * dfloor + SLACK and relerr(xin.grad, f_dx) < VS_FP32_FACTOR * dfloor + SLACK
     assert set(grads) == set(e_grads)
     for k in sorted(grads):
-        ours_vs_eager, ours_vs_fp32, eager_vs_fp32 = _relerr(grads[k], e_grads[k]), _relerr(grads[k], f_grads[k]), _relerr(e_grads[k], f_grads[k])
+        ours_vs_eager, ours_vs_fp32, eager_vs_fp32 = relerr(grads[k], e_grads[k]), relerr(grads[k], f_grads[k]), relerr(e_grads[k], f_grads[k])
         assert ours_vs_eager < VS_EAGER_FACTOR * eager_vs_fp32 + SLACK, f"{k}: ours vs eager {ours_vs_eager}, floor {eager_vs_fp32}"
         assert ours_vs_fp32 < VS_FP32_FACTOR * eager_vs_fp32 + SLACK, (k, ours_vs_fp32, eager_vs_fp32)
 

@@ -1,0 +1,109 @@
+"""CPU: every float64 reference in _refs.py against torch's own op on small inputs."""
+import torch
+import torch.nn.functional as F
+
+import _refs as refs
+from test_ill_conditioned_gpu import gn_input
+
+F64 = torch.float64
+
+
+def test_float64_references_match_torch():
+    g = torch.Generator().manual_seed(0)
+    g2 = torch.Generator().manual_seed(1)  # the draws the backward checks add
+    # GroupNorm(32) (+ SiLU) on channels-last rows with every kind of ill-conditioned group, its statistics and its backward
+    x = gn_input(2, 49, 64, "mixed", seed=1)
+    gamma, beta = torch.randn(64, generator=g, dtype=F64), torch.randn(64, generator=g, dtype=F64)
+    dy = torch.randn(2, 49, 64, generator=g2, dtype=F64)
+    for silu in (False, True):
+        (y, mean, rstd, _), grads = refs.with_grads(refs.groupnorm, (x, gamma, beta), dy, 1e-5, silu)
+        xt = x.to(F64).permute(0, 2, 1).requires_grad_(True)
+        gt, bt = gamma.clone().requires_grad_(True), beta.clone().requires_grad_(True)
+        want = F.group_norm(xt, refs.GROUPS, gt, bt, 1e-5)
+        want = (F.silu(want) if silu else want).permute(0, 2, 1)
+        want.backward(dy)
+        assert torch.allclose(y, want.detach(), rtol=1e-12, atol=1e-12)
+        for ours, theirs in zip(grads, (xt.grad.permute(0, 2, 1), gt.grad, bt.grad)):
+            assert torch.allclose(ours, theirs, rtol=1e-9, atol=1e-9)
+        _, m2, r2 = torch.native_group_norm(x.to(F64).permute(0, 2, 1).contiguous(), gamma, beta, 2, 64, 49, refs.GROUPS, 1e-5)
+        assert torch.allclose(mean, m2, rtol=1e-12, atol=1e-12) and torch.allclose(rstd, r2, rtol=1e-9)
+    # LayerNorm on float64, fp32 and bf16 rows, its statistics and its backward
+    xl = torch.randn(37, 40, generator=g, dtype=F64) * 3 + 1e3
+    dyl = torch.randn(37, 40, generator=g2, dtype=F64)
+    for dtype in (F64, torch.float32, torch.bfloat16):
+        xs = xl.to(dtype)
+        (y, mean, rstd, var), grads = refs.with_grads(refs.layernorm, (xs, gamma[:40], beta[:40]), dyl, 1e-6)
+        xt, gt, bt = (t.to(F64).clone().requires_grad_(True) for t in (xs, gamma[:40], beta[:40]))
+        want = F.layer_norm(xt, (40,), gt, bt, 1e-6)
+        want.backward(dyl)
+        assert torch.allclose(y, want.detach(), rtol=1e-10, atol=1e-10)
+        for ours, theirs in zip(grads, (xt.grad, gt.grad, bt.grad)):
+            assert torch.allclose(ours, theirs, rtol=1e-9, atol=1e-9)
+        _, m2, r2 = torch.native_layer_norm(xs.to(F64), (40,), None, None, 1e-6)
+        assert torch.allclose(mean, m2.flatten(), rtol=1e-12) and torch.allclose(rstd, r2.flatten(), rtol=1e-9)
+        assert torch.allclose(var, xs.to(F64).var(-1, unbiased=False), rtol=1e-9)
+    # log-softmax with a -inf logit, softmax cross-entropy and the symmetric cross-entropy
+    logits = torch.randn(9, 31, generator=g, dtype=F64) * 300
+    logits[0, 3] = float("-inf")
+    lsm = refs.log_softmax(logits)
+    assert torch.equal(torch.isinf(lsm), torch.isinf(logits))
+    assert torch.allclose(lsm[torch.isfinite(logits)], F.log_softmax(logits, -1)[torch.isfinite(logits)], rtol=1e-12)
+    labels = torch.randint(0, 31, (9,), generator=g2)
+    labels[0] = 2
+    rows, dl = refs.softmax_xent(logits, labels)
+    lt = logits.clone().requires_grad_(True)
+    want = F.cross_entropy(lt, labels, reduction="none")
+    want.mean().backward()
+    assert torch.allclose(rows, want.detach(), rtol=1e-12) and torch.allclose(dl, lt.grad, rtol=1e-10, atol=1e-14)
+    sq = torch.randn(7, 7, generator=g2, dtype=F64) * 4
+    sq[2, 5] = float("-inf")
+    loss, dsq = refs.symmetric_xent(sq)
+    st = sq.clone().requires_grad_(True)
+    want = 0.5 * (F.cross_entropy(st, torch.arange(7)) + F.cross_entropy(st.t(), torch.arange(7)))
+    want.backward()
+    assert torch.allclose(loss, want.detach(), rtol=1e-12) and torch.allclose(dsq, st.grad, rtol=1e-10, atol=1e-14)
+    # attention on [B, H, T, D] with scale and causal; on rows with Tq != Tk, backward included; on packed qkv rows
+    q, k, v = (torch.randn(2, 3, 50, 40, generator=g, dtype=F64) for _ in range(3))
+    for causal in (False, True):
+        o, lse = refs.attention(q * 10, k, v, 40 ** -0.5, causal)
+        assert torch.allclose(o, F.scaled_dot_product_attention(q * 10, k, v, is_causal=causal), rtol=1e-10, atol=1e-10)
+        s = (q * 10) @ k.transpose(-1, -2) * 40 ** -0.5
+        if causal:
+            s = s.masked_fill(torch.ones(50, 50, dtype=torch.bool).triu(1), float("-inf"))
+        assert torch.allclose(lse, torch.logsumexp(s, -1), rtol=1e-12)
+    B, Tq, Tk, H, Dh = 2, 5, 9, 3, 8
+    qr, kr, vr = (torch.randn(B * T, H * Dh, generator=g2, dtype=F64) for T in (Tq, Tk, Tk))
+    dout = torch.randn(B * Tq, H * Dh, generator=g2, dtype=F64)
+    (o, lse), grads = refs.with_grads(refs.attention_rows, (qr, kr, vr), dout, B, H, 0.3, False)
+    heads = lambda t: t.view(B, -1, H, Dh).permute(0, 2, 1, 3)  # noqa: E731
+    qt, kt, vt = (t.clone().requires_grad_(True) for t in (qr, kr, vr))
+    want = F.scaled_dot_product_attention(heads(qt), heads(kt), heads(vt), scale=0.3).permute(0, 2, 1, 3).reshape(B * Tq, H * Dh)
+    want.backward(dout)
+    assert torch.allclose(o, want.detach(), rtol=1e-10, atol=1e-10) and lse.shape == (B, H, Tq)
+    for ours, theirs in zip(grads, (qt.grad, kt.grad, vt.grad)):
+        assert torch.allclose(ours, theirs, rtol=1e-9, atol=1e-10)
+    qkv = torch.randn(2 * 20, 3 * 2 * 64, generator=g2, dtype=F64)
+    o, lse = refs.packed_attention(qkv, 2, 20, 2, causal=True)
+    pq, pk, pv = qkv.view(2, 20, 3, 2, 64).permute(2, 0, 3, 1, 4)
+    want = F.scaled_dot_product_attention(pq, pk, pv, is_causal=True, scale=0.125).permute(0, 2, 1, 3).reshape(40, 128)
+    assert torch.allclose(o, want, rtol=1e-10, atol=1e-10) and lse.shape == (2, 2, 20)
+    # the 3x3 convolution and its weight gradient (packed order: tap, then channel)
+    xc = torch.randn(2, 5, 6, 8, generator=g2, dtype=F64)
+    w = torch.randn(4, 8, 3, 3, generator=g2, dtype=F64, requires_grad=True)
+    y = F.conv2d(xc.permute(0, 3, 1, 2), w, padding=1)
+    dyc = torch.randn(y.shape, generator=g2, dtype=F64)
+    y.backward(dyc)
+    assert torch.allclose(refs.conv3x3(xc, w.detach()), y.detach().permute(0, 2, 3, 1).reshape(60, 4), rtol=1e-12, atol=1e-12)
+    dw = refs.conv3x3_wgrad(dyc.permute(0, 2, 3, 1).reshape(60, 4), xc)
+    assert torch.allclose(dw, w.grad.permute(0, 2, 3, 1).reshape(4, 72), rtol=1e-10, atol=1e-12)
+    # Adam with L2 weight decay against torch.optim.Adam
+    p0, grad = torch.randn(50, generator=g2, dtype=F64), torch.randn(50, generator=g2, dtype=F64)
+    pt = p0.clone().requires_grad_(True)
+    opt = torch.optim.Adam([pt], lr=1e-2, betas=(0.8, 0.99), eps=1e-6, weight_decay=0.05)
+    for _ in range(4):
+        pt.grad = grad.clone()
+        opt.step()
+    zeros = torch.zeros(50, dtype=F64)
+    p, m, v = refs.adam(p0, grad, zeros, zeros, [1, 2, 3, 4], 1e-2, 0.8, 0.99, 1e-6, 0.05)
+    assert torch.allclose(p, pt.detach(), rtol=1e-12, atol=1e-14)
+    assert torch.allclose(m, opt.state[pt]["exp_avg"], rtol=1e-12) and torch.allclose(v, opt.state[pt]["exp_avg_sq"], rtol=1e-12)

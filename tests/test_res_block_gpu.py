@@ -15,25 +15,16 @@ import cflearn_b200  # noqa: F401,E402
 from cflearn_b200 import ops  # noqa: E402
 from cflearn_b200._cabi import B200Error  # noqa: E402
 from cflearn_b200.unet_blocks import ResidualBlockWithTimeEmbeddingB200 as ResBlock, res_block_forward  # noqa: E402
+from _refs import rand_bf16, relerr  # noqa: E402
 
 DEV = "cuda"
 BF16_MAX = torch.finfo(torch.bfloat16).max
 
 
-def _rand_bf16(*shape, scale=1.0, seed=0):
-    g = torch.Generator(device="cpu").manual_seed(seed)
-    return (torch.randn(*shape, generator=g) * scale).to(torch.bfloat16).to(DEV)
-
-
-def _relerr(a, b):
-    a, b = a.float(), b.float()
-    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
-
-
 def _conv_case(B, side, Cin, Cout, seed):
-    x = _rand_bf16(B, side, side, Cin, seed=seed)
-    w = _rand_bf16(Cout, Cin, 3, 3, scale=(9 * Cin) ** -0.5, seed=seed + 1)
-    bias = _rand_bf16(Cout, scale=0.1, seed=seed + 2)
+    x = rand_bf16(B, side, side, Cin, seed=seed)
+    w = rand_bf16(Cout, Cin, 3, 3, scale=(9 * Cin) ** -0.5, seed=seed + 1)
+    bias = rand_bf16(Cout, scale=0.1, seed=seed + 2)
     return x, ops.pack_conv3x3_weight(w), bias
 
 
@@ -43,7 +34,7 @@ def _conv_case(B, side, Cin, Cout, seed):
 def test_per_image_epilogue(side):
     B, Cin, Cout = 3, 128, 320  # at 8x8 a 128-pixel tile holds two images, and B = 3 leaves the last tile half full
     x, wp, bias = _conv_case(B, side, Cin, Cout, seed=side)
-    t = _rand_bf16(B, Cout, seed=side + 3)
+    t = rand_bf16(B, Cout, seed=side + 3)
     out = ops.conv3x3(x, wp, bias, epilogue=ops.EPI_BIAS_ADD_PER_IMAGE_BF16, aux=t)
     expect = ops.conv3x3(x, wp, bias) + t[:, None, None, :]  # eager's bf16 add of the broadcast table
     assert torch.equal(out, expect)
@@ -54,8 +45,8 @@ def test_clamp_epilogue():
     B, side, Cin, Cout = 2, 16, 64, 256
     x, wp, _ = _conv_case(B, side, Cin, Cout, seed=20)
     # finite sums: the bf16 residual add, bit for bit
-    aux = _rand_bf16(B, side, side, Cout, seed=21)
-    bias = _rand_bf16(Cout, scale=0.1, seed=22)
+    aux = rand_bf16(B, side, side, Cout, seed=21)
+    bias = rand_bf16(Cout, scale=0.1, seed=22)
     out = ops.conv3x3(x, wp, bias, epilogue=ops.EPI_BIAS_RESID_CLAMP_BF16, aux=aux)
     assert torch.equal(out, ops.conv3x3(x, wp, bias) + aux)
     # overflowing sums: +-inf becomes +-bf16 max, as torch.clamp to the finite range does; NaN stays NaN
@@ -78,7 +69,7 @@ def test_clamp_epilogue():
 @pytest.mark.gpu
 @pytest.mark.parametrize("B,HW,C", [(2, 4096, 320), (8, 1024, 640), (3, 64, 2560), (5, 72, 8)])
 def test_colsum_per_image(B, HW, C):
-    x = _rand_bf16(B, HW, C, seed=B + C)
+    x = rand_bf16(B, HW, C, seed=B + C)
     dt, db = ops.colsum_per_image(x)
     dt2, db2 = ops.colsum_per_image(x)
     torch.cuda.synchronize()
@@ -111,9 +102,9 @@ def _inputs(B, Cin, Cout, side, tdim, seed):
 
 def _check(ours, eager, fp32):
     for k in ours:
-        floor = _relerr(eager[k], fp32[k])
-        assert _relerr(ours[k], fp32[k]) <= 1.5 * floor + 1e-6, (k, _relerr(ours[k], fp32[k]), floor)
-        assert _relerr(ours[k], eager[k]) <= 2.0 * floor + 1e-6, (k, _relerr(ours[k], eager[k]), floor)
+        floor = relerr(eager[k], fp32[k])
+        assert relerr(ours[k], fp32[k]) <= 1.5 * floor + 1e-6, (k, relerr(ours[k], fp32[k]), floor)
+        assert relerr(ours[k], eager[k]) <= 2.0 * floor + 1e-6, (k, relerr(ours[k], eager[k]), floor)
 
 
 def _oracle_run(sd, net, tn, up):
@@ -172,7 +163,7 @@ def test_without_time_embedding():
     zero = _run_module(m, net, torch.zeros_like(tn), up)
     for k in none:  # conv1's bias gradient is summed in another order (per image first) when a time embedding is present
         if k == "conv1.bias":
-            assert _relerr(none[k], zero[k]) < 1e-2
+            assert relerr(none[k], zero[k]) < 1e-2
         else:
             assert torch.equal(none[k], zero[k]), k
     sd0 = dict(sd, **{"time_embedding.weight": torch.zeros_like(sd["time_embedding.weight"]),
@@ -190,8 +181,8 @@ def test_res_block_forward_is_the_previous_composition(B, side, Cin, Cout):
     tdim = 1280
     m = ResBlock(Cin, Cout, time_embedding_channels=tdim)
     sd = {"b." + k: v.to(DEV) for k, v in uo.synthetic_state_dict([(k, tuple(v.shape)) for k, v in m.state_dict().items()], seed=3).items()}
-    x = _rand_bf16(B, side, side, Cin, seed=4)
-    tn = _rand_bf16(B, tdim, seed=5)
+    x = rand_bf16(B, side, side, Cin, seed=4)
+    tn = rand_bf16(B, tdim, seed=5)
     ours = res_block_forward(sd, "b.", x, tn)
 
     bf = lambda t: t.to(torch.bfloat16).contiguous()  # noqa: E731
