@@ -19,6 +19,38 @@ def rand_bf16(*shape, scale=1.0, seed=0):
     return (torch.randn(*shape, generator=g) * scale).to(torch.bfloat16).to("cuda")
 
 
+def peaked_qkv(B, H, Tq, Tk, D, scale, causal, seed):
+    """float64 [B, H, T, D] q, k, v whose scaled scores peak at 100..200 for one key per query row.  The dominant key sits in the
+    first key block (row % 3 == 0), at the last key (row % 3 == 1: the last block, a partial tile when Tk % 64 != 0; on causal rows
+    the diagonal, the row's last visible key) or at a random key of the last block (causal: any visible key).  Every other row has a
+    runner-up key within 3 of the peak, so that its gradients are not all rounding noise."""
+    g = torch.Generator().manual_seed(seed)
+    k = torch.randn(B, H, Tk, D, generator=g, dtype=F64)
+    v = torch.randn(B, H, Tk, D, generator=g, dtype=F64)
+    i = torch.arange(Tq).expand(B, H, Tq)
+    r1 = torch.randint(0, 1 << 30, (B, H, Tq), generator=g)
+    r2 = torch.randint(0, 1 << 30, (B, H, Tq), generator=g)
+    blk = min(Tk, 64)
+    if causal:
+        j1 = torch.where(i % 3 == 0, torch.zeros_like(i), torch.where(i % 3 == 1, i, r1 % (i + 1)))
+        j2 = r2 % (i + 1)
+    else:
+        j1 = torch.where(i % 3 == 0, r1 % blk, torch.where(i % 3 == 1, torch.full_like(i, Tk - 1), Tk - 1 - r1 % blk))
+        j2 = r2 % Tk
+    two = (i % 2 == 0) & (j2 != j1)
+    peak = 100 + 100 * torch.rand(B, H, Tq, generator=g, dtype=F64)
+    t1 = peak / scale
+    t2 = (peak - 3 * torch.rand(B, H, Tq, generator=g, dtype=F64)) / scale
+    k1 = k.gather(2, j1[..., None].expand(B, H, Tq, D))
+    k2 = k.gather(2, j2[..., None].expand(B, H, Tq, D))
+    g11, g12, g22 = (k1 * k1).sum(-1), (k1 * k2).sum(-1), (k2 * k2).sum(-1)
+    det = torch.where(two, g11 * g22 - g12 * g12, torch.ones_like(g11))
+    a = torch.where(two, (t1 * g22 - t2 * g12) / det, t1 / g11)  # q = a k1 + c k2: q.k1 = t1 (and q.k2 = t2)
+    c = torch.where(two, (t2 * g11 - t1 * g12) / det, torch.zeros_like(g11))
+    q = a[..., None] * k1 + c[..., None] * k2 + 0.05 * torch.randn(B, H, Tq, D, generator=g, dtype=F64)
+    return q, k, v
+
+
 # ---- error measures ----------------------------------------------------------------------------------------------------------------
 def relerr(a, ref):
     """Relative L2 error of ``a`` against ``ref``, in float64."""
@@ -96,6 +128,80 @@ def packed_attention(qkv, B, T, H, scale=0.125, causal=False):
     """``attention`` of packed rows qkv [B T, 3 H 64] (q | k | v): (out [B T, H 64], lse [B, H, T])."""
     D = H * 64
     return attention_rows(qkv[:, :D], qkv[:, D:2 * D], qkv[:, 2 * D:], B, H, scale, causal)
+
+
+BF16_U = 2.0 ** -8   # unit roundoff of bf16 (8 significant bits): |bf16(x) - x| <= 2^-8 |x|
+FP32_U = 2.0 ** -24  # unit roundoff of fp32: a sum of n exact products is off by at most n 2^-24 times the sum of their magnitudes
+FP32_TINY = 2.0 ** -126  # smallest normal fp32 (and bf16): flush-to-zero arithmetic rounds anything smaller to 0
+ATTN_C = 2.0         # attention_bounds: tolerance = ATTN_C x the first-order error bound
+
+
+def attention_bounds(q, k, v, dout, scale, causal, out):
+    """Per-element error bounds for the attention kernels, on ``attention``'s layout: q / out / dout [B, H, Tq, D], k / v
+    [B, H, Tk, D], ``out`` the kernel's own bf16 output, which its backward reads.  Returns ((o, lse, dq, dk, dv), (tol_o, tol_dq,
+    tol_dk, tol_dv)): the float64 forward and gradients of ``attention`` at these inputs, and for each of o, dq, dk, dv a tensor
+    of its shape that |kernel - float64| must not exceed at any element.
+
+    The tolerances follow the kernels' rounding points (attention_sm90.cu): fp32 scores and softmax, P rounded to bf16 as the
+    A operand of P V and P^T dO, delta = rowsum(dO o out) from the bf16 ``out``, dS = P o (dP - delta) rounded to bf16 as an
+    operand, fp32 accumulation everywhere, dQ / dK scaled in fp32 at the end, every output rounded to bf16 once.  With
+    u = 2^-8 (bf16), g_n = n 2^-24 (an fp32 sum of n exact bf16 x bf16 products), t = 2^-126, |X| elementwise, P the float64
+    softmax and M the 0 / 1 matrix of visible keys:
+
+    scores   S = scale Q K^T over D products, then the fp32 multiply by scale log2(e): each is off by E_ij = g_{D+2} scale (|Q||K|^T)_ij.
+             Softmax moves by at most its exponent's change:  |dP_ij| <= P_ij (E_ij + Ebar_i),  Ebar_i = sum_j P_ij E_ij + 2^-24 (1 +
+             |lse_i|)  (the second term: the stored fp32 lse that the backward recomputes P from).
+    underflow  exp2 runs as ex2.approx.ftz: a probability below t (a score 87 or more under its row's maximum) becomes 0, as does
+             any fp32 value below t, so every P_ij and dS_ij of a visible key and every stored output is also off by up to t.
+    out      o = bf16(sum_j bf16(p_ij) v_j / l_i), p_ij = exp(S_ij - max_j S_ij) and l_i >= 1:
+             tol_o = C [(u + 2 g_Tk) P|V| + (P o (E + Ebar)) |V| + t M|V| + u |o| + t]   (P V and l each over Tk terms).
+    delta    from the kernel's out:  |d delta_i| <= sum_d |dO_id| |out_id - o_id| + g_D sum_d |dO_id| |out_id|.
+    dP       = dO V^T in fp32:  |d dP_ij| <= g_D (|dO||V|^T)_ij.
+    dS       = bf16(P o (dP - delta)):
+             |d dS| <= u |dS| + P o (g_D |dO||V|^T + d delta) + (E + Ebar) o |dS| + t M o (|dP - delta| + 1).
+    dV       = bf16(sum_i bf16(P_ij) dO_i):  tol_dv = C [(u + g_Tq) P^T|dO| + (P o (E + Ebar))^T |dO| + t M^T|dO| + u |dv| + t].
+    dQ       = bf16(scale sum_j bf16(dS_ij) K_j):  tol_dq = C [scale (|d dS| |K| + g_Tk |dS||K|) + u |dq| + t];
+    dK       likewise over the queries:  tol_dk = C [scale (|d dS|^T |Q| + g_Tq |dS|^T|Q|) + u |dk| + t].
+
+    C = ATTN_C = 2 covers what the first-order bound drops: products of two error terms and the few-ulp fp32 error of the
+    exp2 / log / reciprocal approximations.  Where a quantity is exact in both -- o with V = 0, every gradient with dO = 0 -- the
+    tolerance falls to the underflow floor, a few t.  Masked (causal) keys have P = 0 and add nothing."""
+    qd, kd, vd, dod, od = (t.to(F64) for t in (q, k, v, dout, out))
+    Tq, Tk, D = qd.shape[-2], kd.shape[-2], qd.shape[-1]
+    s = (qd @ kd.transpose(-1, -2)) * scale
+    seen = torch.ones(Tq, Tk, dtype=F64, device=s.device)
+    if causal:
+        seen = seen.tril()
+        s = s.masked_fill(seen == 0, float("-inf"))
+    lse = torch.logsumexp(s, -1)
+    p = (s - lse[..., None]).exp()
+    o = p @ vd
+    dp_delta = dod @ vd.transpose(-1, -2) - (dod * o).sum(-1)[..., None]
+    ds = p * dp_delta
+    dq, dk, dv = scale * (ds @ kd), scale * (ds.transpose(-1, -2) @ qd), p.transpose(-1, -2) @ dod
+
+    gD, u, t = (D + 2) * FP32_U, BF16_U, FP32_TINY
+    aq, ak, av, ado = qd.abs(), kd.abs(), vd.abs(), dod.abs()
+    e = gD * scale * (aq @ ak.transpose(-1, -2))
+    e = e + (p * e).sum(-1, keepdim=True) + FP32_U * (1 + lse.abs())[..., None]  # E + Ebar
+    pe = p * e
+    ddelta = (ado * (od - o).abs()).sum(-1) + gD * (ado * od.abs()).sum(-1)
+    dds = u * ds.abs() + p * (gD * (ado @ av.transpose(-1, -2)) + ddelta[..., None]) + e * ds.abs() + t * seen * (dp_delta.abs() + 1)
+    tol_o = ATTN_C * ((u + 2 * Tk * FP32_U) * (p @ av) + pe @ av + t * (seen @ av) + u * o.abs() + t)
+    tol_dv = ATTN_C * ((u + Tq * FP32_U) * (p.transpose(-1, -2) @ ado) + pe.transpose(-1, -2) @ ado + t * (seen.transpose(-1, -2) @ ado) +
+                       u * dv.abs() + t)
+    tol_dq = ATTN_C * (scale * ((dds + Tk * FP32_U * ds.abs()) @ ak) + u * dq.abs() + t)
+    tol_dk = ATTN_C * (scale * ((dds + Tq * FP32_U * ds.abs()).transpose(-1, -2) @ aq) + u * dk.abs() + t)
+    return (o, lse, dq, dk, dv), (tol_o, tol_dq, tol_dk, tol_dv)
+
+
+def attention_bounds_rows(q, k, v, dout, B, H, scale, causal, out):
+    """``attention_bounds`` on the kernels' row layout (as ``attention_rows``): q / out / dout [B Tq, H Dh], k / v [B Tk, H Dh].
+    Everything comes back in that layout (lse [B, H, Tq])."""
+    heads = lambda t: t.reshape(B, -1, H, t.shape[1] // H).permute(0, 2, 1, 3)  # noqa: E731
+    rows = lambda t: t.permute(0, 2, 1, 3).reshape(-1, t.shape[1] * t.shape[3])  # noqa: E731
+    (o, lse, dq, dk, dv), tols = attention_bounds(heads(q), heads(k), heads(v), heads(dout), scale, causal, heads(out))
+    return (rows(o), lse, rows(dq), rows(dk), rows(dv)), tuple(rows(t) for t in tols)
 
 
 def layernorm(x, gamma, beta, eps):

@@ -24,7 +24,7 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 
 import cflearn_b200  # noqa: F401,E402
 from cflearn_b200 import _cabi, ops  # noqa: E402
-from _refs import (F64, GROUPS, attention, bf16_ulps_off, groupnorm, layernorm, relerr, softmax_xent,  # noqa: E402
+from _refs import (F64, GROUPS, attention, bf16_ulps_off, groupnorm, layernorm, peaked_qkv, relerr, softmax_xent,  # noqa: E402
                    symmetric_xent, with_grads)
 
 DEV = "cuda"
@@ -362,38 +362,6 @@ def test_symmetric_xent(case):
 
 
 # ---- attention with peaked scores --------------------------------------------------------------------------------------------------
-def peaked_qkv(B, H, Tq, Tk, D, scale, causal, seed):
-    """float64 [B, H, T, D] q, k, v whose scaled scores peak at 100..200 for one key per query row.  The dominant key sits in the
-    first key block (row % 3 == 0), at the last key (row % 3 == 1: the last block, a partial tile when Tk % 64 != 0; on causal rows
-    the diagonal, the row's last visible key) or at a random key of the last block (causal: any visible key).  Every other row has a
-    runner-up key within 3 of the peak, so that its gradients are not all rounding noise."""
-    g = torch.Generator().manual_seed(seed)
-    k = torch.randn(B, H, Tk, D, generator=g, dtype=F64)
-    v = torch.randn(B, H, Tk, D, generator=g, dtype=F64)
-    i = torch.arange(Tq).expand(B, H, Tq)
-    r1 = torch.randint(0, 1 << 30, (B, H, Tq), generator=g)
-    r2 = torch.randint(0, 1 << 30, (B, H, Tq), generator=g)
-    blk = min(Tk, 64)
-    if causal:
-        j1 = torch.where(i % 3 == 0, torch.zeros_like(i), torch.where(i % 3 == 1, i, r1 % (i + 1)))
-        j2 = r2 % (i + 1)
-    else:
-        j1 = torch.where(i % 3 == 0, r1 % blk, torch.where(i % 3 == 1, torch.full_like(i, Tk - 1), Tk - 1 - r1 % blk))
-        j2 = r2 % Tk
-    two = (i % 2 == 0) & (j2 != j1)
-    peak = 100 + 100 * torch.rand(B, H, Tq, generator=g, dtype=F64)
-    t1 = peak / scale
-    t2 = (peak - 3 * torch.rand(B, H, Tq, generator=g, dtype=F64)) / scale
-    k1 = k.gather(2, j1[..., None].expand(B, H, Tq, D))
-    k2 = k.gather(2, j2[..., None].expand(B, H, Tq, D))
-    g11, g12, g22 = (k1 * k1).sum(-1), (k1 * k2).sum(-1), (k2 * k2).sum(-1)
-    det = torch.where(two, g11 * g22 - g12 * g12, torch.ones_like(g11))
-    a = torch.where(two, (t1 * g22 - t2 * g12) / det, t1 / g11)  # q = a k1 + c k2: q.k1 = t1 (and q.k2 = t2)
-    c = torch.where(two, (t2 * g11 - t1 * g12) / det, torch.zeros_like(g11))
-    q = a[..., None] * k1 + c[..., None] * k2 + 0.05 * torch.randn(B, H, Tq, D, generator=g, dtype=F64)
-    return q, k, v
-
-
 def _row_errors(x, ref):
     """Per-row L2 error of [..., T, D] tensors, relative to the row's own norm."""
     return (x.to(F64) - ref).norm(dim=-1) / ref.norm(dim=-1).clamp_min(1e-300)

@@ -107,3 +107,48 @@ def test_float64_references_match_torch():
     p, m, v = refs.adam(p0, grad, zeros, zeros, [1, 2, 3, 4], 1e-2, 0.8, 0.99, 1e-6, 0.05)
     assert torch.allclose(p, pt.detach(), rtol=1e-12, atol=1e-14)
     assert torch.allclose(m, opt.state[pt]["exp_avg"], rtol=1e-12) and torch.allclose(v, opt.state[pt]["exp_avg_sq"], rtol=1e-12)
+
+
+def test_attention_bounds():
+    g = torch.Generator().manual_seed(2)
+    bf = lambda *s: torch.randn(*s, generator=g).to(torch.bfloat16)  # noqa: E731
+    B, H, Tq, Tk, D, scale = 2, 3, 7, 9, 16, 0.3
+    q, dout, k, v = bf(B, H, Tq, D), bf(B, H, Tq, D), bf(B, H, Tk, D), bf(B, H, Tk, D)
+    for causal, kk, vv in ((False, k, v), (True, k[:, :, :Tq], v[:, :, :Tq])):
+        # the float64 values it returns are attention's forward and autograd gradients
+        (o, lse, dq, dk, dv), tols = refs.attention_bounds(q, kk, vv, dout, scale, causal, q)
+        (o2, lse2), grads = refs.with_grads(refs.attention, (q, kk, vv), dout, scale, causal)
+        assert torch.allclose(o, o2, rtol=1e-12, atol=1e-14) and torch.allclose(lse, lse2, rtol=1e-12)
+        for ours, theirs in zip((dq, dk, dv), grads):
+            assert torch.allclose(ours, theirs, rtol=1e-10, atol=1e-12)
+        assert [t.shape for t in tols] == [o.shape, dq.shape, dk.shape, dv.shape] and all((t > 0).all() for t in tols)
+        # the row-layout wrapper is the same computation on [B T, H D] rows
+        rows = lambda t: t.permute(0, 2, 1, 3).reshape(-1, H * D)  # noqa: E731
+        r_vals, r_tols = refs.attention_bounds_rows(rows(q), rows(kk), rows(vv), rows(dout), B, H, scale, causal, rows(q))
+        assert torch.allclose(r_vals[1], lse, rtol=1e-14)
+        for a, b in zip((r_vals[0],) + r_vals[2:] + r_tols, (o, dq, dk, dv) + tols):
+            assert torch.allclose(a, rows(b), rtol=1e-12, atol=1e-15)
+
+    # nothing above the underflow floor (2^-126 flushes) where the quantity is exact: o with V = 0, every gradient with dO = 0
+    (o, *_), (tol_o, *_) = refs.attention_bounds(q, k, torch.zeros_like(v), dout, scale, False, torch.zeros_like(q))
+    assert torch.equal(o, torch.zeros_like(o, dtype=F64)) and (tol_o <= 2.0 ** -100).all()
+    _, (_, *tol_grads) = refs.attention_bounds(q, k, v, torch.zeros_like(dout), scale, False, q)
+    assert all((t <= 2.0 ** -100).all() for t in tol_grads)
+    # one key: P = 1, out = v exactly, dS = 0, so dq = dk = 0 and their tolerance is only the fp32 rounding of dP and delta
+    k1, v1 = k[:, :, :1], v[:, :, :1]
+    (o, _, dq, dk, dv), (tol_o, tol_dq, tol_dk, tol_dv) = refs.attention_bounds(q, k1, v1, dout, scale, False, v1.expand(-1, -1, Tq, -1))
+    assert torch.equal(o, v1.to(F64).expand_as(o)) and dq.abs().max() < 1e-12 and dk.abs().max() < 1e-12
+    w = dout.to(F64).abs() @ v1.to(F64).abs().transpose(-1, -2)  # sum_d |dO_id| |v_d|: the magnitude of dP and delta
+    assert (tol_dq <= 2.0 ** -14 * scale * (w @ k1.to(F64).abs())).all()
+    assert (tol_dk <= 2.0 ** -14 * scale * (w.transpose(-1, -2) @ q.to(F64).abs())).all()
+    assert (tol_dv >= 2.0 ** -8 * dv.abs()).all() and (tol_o >= 2.0 ** -8 * o.abs()).all()
+
+    # monotone: a larger |V| never shrinks tol_o, a larger |dO| never shrinks tol_dv (and doubling either doubles them)
+    grow = lambda t: (t.float() * (1 + torch.rand(t.shape, generator=g))).to(torch.bfloat16)  # noqa: E731
+    for causal, kk, vv in ((False, k, v), (True, k[:, :, :Tq], v[:, :, :Tq])):
+        base = refs.attention_bounds(q, kk, vv, dout, scale, causal, q)[1]
+        bigger_v = refs.attention_bounds(q, kk, grow(vv), dout, scale, causal, q)[1]
+        bigger_do = refs.attention_bounds(q, kk, vv, grow(dout), scale, causal, q)[1]
+        assert (bigger_v[0] >= base[0]).all() and (bigger_do[3] >= base[3]).all()
+        assert torch.allclose(refs.attention_bounds(q, kk, 2 * vv, dout, scale, causal, q)[1][0], 2 * base[0], rtol=1e-12)
+        assert torch.allclose(refs.attention_bounds(q, kk, vv, 2 * dout, scale, causal, q)[1][3], 2 * base[3], rtol=1e-12)
