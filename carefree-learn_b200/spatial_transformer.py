@@ -17,18 +17,21 @@ LayerNorm gradient is rounded to bf16 before the bf16 add of the residual branch
 Activations live channels-last: a ``torch.channels_last`` input is used with no copy (a contiguous NCHW one costs one permute),
 and the output is [B, C, H, W] with channels-last strides.  Each block is one ``autograd.Function`` (and the whole transformer
 one more) that keeps the activations it needs through ``save_for_backward`` (so ``retain_graph``, saved-tensor hooks and
-autograd's in-place checks apply as for any other op); ``use_checkpoint=True`` is accepted but nothing is recomputed -- it changes
-memory, not results.  Dropout > 0, hooks (ToMe / style reference, inference features), ``use_linear=True`` and activations
+autograd's in-place checks apply as for any other op).  With ``use_checkpoint=True`` a block keeps only its inputs and reruns
+its forward in backward (``checkpoint.py``): the same results bit for bit, one block's activations held instead of every
+block's.  In ``SpatialTransformerB200`` the outer GroupNorm and 1x1 convolutions keep their tensors either way, as the
+reference checkpoints the blocks alone.  Dropout > 0, hooks (ToMe / style reference, inference features), ``use_linear=True`` and activations
 other than GEGLU are refused.
 """
 from __future__ import annotations
 
+from functools import partial
 from typing import Any, Dict, List, Optional, Sequence, Tuple
 
 import torch
 from torch import Tensor, nn
 
-from . import ops
+from . import checkpoint, ops
 from ._cabi import B200Error
 from .attention import CrossAttentionB200, _bf, _Linear, attention_backward, attention_forward
 
@@ -104,30 +107,45 @@ def _context_grad(dcs: List[Optional[Tensor]], meta) -> Optional[Tensor]:
     return total.view(meta[1])
 
 
+def _block_build(heads: int, net: Tensor, context: Optional[Tensor], *params: Tensor) -> Tuple[Tensor, tuple]:
+    """_BlockFn's forward on its inputs: (the block's output [B, T, C], what ``_block_backward`` reads)."""
+    B, T, C = net.shape
+    x3, saved = _block_forward(net.reshape(B * T, C).contiguous(), _context_rows(context), params, B, heads)
+    return x3.view(B, T, C), saved
+
+
+def _rows_build(B: int, heads: int, x0: Tensor, c: Optional[Tensor], *params: Tensor) -> Tuple[Tensor, tuple]:
+    """One block of _SpatialTransformerFn on its inputs: token rows x0 [M, C] and context rows c."""
+    return _block_forward(x0, c, params, B, heads)
+
+
 class _BlockFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, net: Tensor, context: Optional[Tensor], heads: int, *params: Tensor):  # type: ignore[override]
-        B, T, C = net.shape
-        x3, saved = _block_forward(net.reshape(B * T, C).contiguous(), _context_rows(context), params, B, heads)
-        ctx.save_for_backward(*saved)
-        ctx.meta = (B, heads, net.shape, _context_meta(context))
-        return x3.view(B, T, C)
+    def forward(ctx, net: Tensor, context: Optional[Tensor], heads: int, use_checkpoint: bool, *params: Tensor):  # type: ignore[override]
+        out, kept = checkpoint.run(partial(_block_build, heads), (net, context, *params), use_checkpoint)
+        ctx.save_for_backward(*kept)
+        ctx.meta = (net.shape[0], heads, net.shape, _context_meta(context), use_checkpoint)
+        return out
 
     @staticmethod
     def backward(ctx, dout: Tensor):  # type: ignore[override]
-        B, heads, shape, context = ctx.meta
-        dx, dc, grads = _block_backward(ctx.saved_tensors, _bf(dout.reshape(-1, shape[-1])), B, heads)
-        return (dx.view(shape), _context_grad([dc], context), None, *grads)
+        B, heads, shape, context, use_checkpoint = ctx.meta
+        saved = checkpoint.rebuild(partial(_block_build, heads), ctx.saved_tensors, use_checkpoint)
+        dx, dc, grads = _block_backward(saved, _bf(dout.reshape(-1, shape[-1])), B, heads)
+        return (dx.view(shape), _context_grad([dc], context), None, None, *grads)
 
 
 class _SpatialTransformerFn(torch.autograd.Function):
+    """``use_checkpoint``: one flag per block, as each of the reference's blocks checkpoints itself.  The outer GroupNorm and
+    1x1 convolutions always keep their tensors; a checkpointed block keeps only its inputs, and backward rebuilds it just
+    before its own backward, so at most one block's rebuilt activations are alive at a time."""
+
     @staticmethod
-    def forward(ctx, net: Tensor, context: Optional[Tensor], heads: int, *params: Tensor):  # type: ignore[override]
+    def forward(ctx, net: Tensor, context: Optional[Tensor], heads: int, use_checkpoint: Tuple[bool, ...], *params: Tensor):  # type: ignore[override]
         B, C, H, W = net.shape
         M = B * H * W
         gn_w, gn_b, w_in, b_in = params[:4]
         w_out, b_out = params[-2:]
-        nblocks = (len(params) - 6) // BLOCK_PARAMS
         L = w_in.shape[0]
         xt = net.permute(0, 2, 3, 1).contiguous().view(B, H * W, C)  # a view when net is channels-last
         gn_w32, gn_b32 = gn_w.float().contiguous(), gn_b.float().contiguous()
@@ -135,31 +153,39 @@ class _SpatialTransformerFn(torch.autograd.Function):
         w_in_b = _bf(w_in.reshape(L, C))
         t = ops.gemm(yn.view(M, C), w_in_b, bias=_bf(b_in))
         c = _context_rows(context)
-        saved_blocks: List = []
-        for i in range(nblocks):
-            t, s = _block_forward(t, c, params[4 + BLOCK_PARAMS * i: 4 + BLOCK_PARAMS * (i + 1)], B, heads)
-            saved_blocks += s
+        build = partial(_rows_build, B, heads)
+        kept_blocks: List = []
+        for i, ckpt in enumerate(use_checkpoint):
+            t, kept = checkpoint.run(build, (t, c, *params[4 + BLOCK_PARAMS * i: 4 + BLOCK_PARAMS * (i + 1)]), ckpt)
+            kept_blocks.append(kept)
         w_out_b = _bf(w_out.reshape(C, L))
         out = ops.gemm(t, w_out_b, bias=_bf(b_out), epilogue=ops.EPI_BIAS_RESID_BF16, aux=xt.view(M, C))
-        ctx.save_for_backward(xt, yn, gm, gr, gn_w32, gn_b32, w_in_b, t, w_out_b, *saved_blocks)
-        ctx.meta = (B, C, H, W, L, heads, _context_meta(context), w_in.shape, w_out.shape)
+        ctx.save_for_backward(xt, yn, gm, gr, gn_w32, gn_b32, w_in_b, t, w_out_b, *(s for kept in kept_blocks for s in kept))
+        ctx.meta = (B, C, H, W, L, heads, _context_meta(context), w_in.shape, w_out.shape, use_checkpoint,
+                    [len(kept) for kept in kept_blocks])
         return out.view(B, H, W, C).permute(0, 3, 1, 2)
 
     @staticmethod
     def backward(ctx, dout: Tensor):  # type: ignore[override]
         saved = ctx.saved_tensors
         xt, yn, gm, gr, gn_w32, gn_b32, w_in_b, t, w_out_b = saved[:9]
-        saved_blocks = [saved[9 + BLOCK_SAVED * i: 9 + BLOCK_SAVED * (i + 1)] for i in range((len(saved) - 9) // BLOCK_SAVED)]
-        B, C, H, W, L, heads, context, w_in_shape, w_out_shape = ctx.meta
+        B, C, H, W, L, heads, context, w_in_shape, w_out_shape, use_checkpoint, sizes = ctx.meta
+        kept_blocks, start = [], 9
+        for n in sizes:
+            kept_blocks.append(saved[start:start + n])
+            start += n
         M, dev = B * H * W, dout.device
         dt = dout.permute(0, 2, 3, 1).to(torch.bfloat16).contiguous().view(M, C)
         dw_out = ops.wgrad(dt, t, torch.empty((C, L), dtype=torch.float32, device=dev))
         db_out = ops.colsum(dt, torch.empty(C, dtype=torch.float32, device=dev))
         dtl = ops.gemm(dt, w_out_b, b_mn_major=True)
+        build = partial(_rows_build, B, heads)
         block_grads: List[List[Tensor]] = []
         dcs: List[Optional[Tensor]] = []
-        for s in reversed(saved_blocks):
+        for kept, ckpt in zip(reversed(kept_blocks), reversed(use_checkpoint)):
+            s = checkpoint.rebuild(build, kept, ckpt)
             dtl, dc, g = _block_backward(s, dtl, B, heads)
+            del s  # a rebuilt block's activations are released before the block below it is rebuilt
             block_grads.insert(0, g)
             dcs.append(dc)
         dw_in = ops.wgrad(dtl, yn.view(M, C), torch.empty((L, C), dtype=torch.float32, device=dev))
@@ -168,7 +194,7 @@ class _SpatialTransformerFn(torch.autograd.Function):
         dxg, dgn_w, dgn_b = ops.groupnorm_silu_bwd(xt, dyn.view(B, H * W, C), gn_w32, gn_b32, gm, gr, silu=False)
         dx = (dxg.view(M, C) + dt).view(B, H, W, C).permute(0, 3, 1, 2)  # GroupNorm path + the final residual, a bf16 add
         flat = [g for gs in block_grads for g in gs]
-        return (dx, _context_grad(dcs, context), None, dgn_w, dgn_b, dw_in.view(w_in_shape), db_in, *flat,
+        return (dx, _context_grad(dcs, context), None, None, dgn_w, dgn_b, dw_in.view(w_in_shape), db_in, *flat,
                 dw_out.view(w_out_shape), db_out)
 
 
@@ -231,7 +257,7 @@ class SpatialTransformerBlockB200(nn.Module):
         if latent_dim % 8 != 0:
             raise NotImplementedError("SpatialTransformerBlockB200: the feed-forward width must be a multiple of 8")
         self.num_heads = num_heads
-        self.use_checkpoint = use_checkpoint  # accepted: activations are saved, not recomputed (same results, more memory)
+        self.use_checkpoint = use_checkpoint  # keep only the inputs and recompute the activations in backward
         # registration order of the reference: attn1, ff, attn2, norm1..3 (state_dict order)
         self.attn1 = CrossAttentionB200(query_dim=query_dim, num_heads=num_heads, head_dim=head_dim)
         self.ff = _FeedForwardParams(query_dim, latent_dim)
@@ -253,7 +279,7 @@ class SpatialTransformerBlockB200(nn.Module):
 
     def forward(self, net: Tensor, context: Optional[Tensor] = None) -> Tensor:
         _check_input(net, "SpatialTransformerBlockB200")
-        return _BlockFn.apply(net, context, self.num_heads, *self._block_params())
+        return _BlockFn.apply(net, context, self.num_heads, self.use_checkpoint, *self._block_params())
 
 
 class SpatialTransformerB200(nn.Module):
@@ -285,4 +311,5 @@ class SpatialTransformerB200(nn.Module):
         for b in self.blocks:
             params += b._block_params()
         params += [self.from_latent.weight, self.from_latent.bias]
-        return _SpatialTransformerFn.apply(net, context, self.num_heads, *params)
+        use_checkpoint = tuple(bool(b.use_checkpoint) for b in self.blocks)
+        return _SpatialTransformerFn.apply(net, context, self.num_heads, use_checkpoint, *params)

@@ -21,19 +21,22 @@ embedding's weight / bias gradients from dt and dtime = silu_backward(bf16(dt . 
 intended difference from eager: the backward treats the clamp as the identity, where eager zeroes the gradient of an element
 whose sum overflowed bf16 (a block whose output overflows is already broken; the clamp only keeps the forward finite).
 
-``ResidualBlockWithTimeEmbeddingB200`` is the drop-in module (one ``autograd.Function`` that keeps its activations through
-``save_for_backward``); ``res_block_forward`` runs the same forward on a state dict.  Up / down-sampling, the timestep MLP and
-the assembled UNet with its training step are the open part of row N3.
+``ResidualBlockWithTimeEmbeddingB200`` is the drop-in module: one ``autograd.Function`` that keeps its activations through
+``save_for_backward``, or with ``use_checkpoint=True`` keeps only its inputs and reruns the forward at the start of backward
+(``checkpoint.py``: the same gradients bit for bit, less memory held between forward and backward).  ``res_block_forward``
+runs the same forward on a state dict.  Up / down-sampling, the timestep MLP and the assembled UNet with its training step are
+the open part of row N3.
 """
 from __future__ import annotations
 
+from functools import partial
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 import torch.nn.functional as F
 from torch import Tensor, nn
 
-from . import ops
+from . import checkpoint, ops
 from ._cabi import B200Error
 from .attention import _bf
 
@@ -141,24 +144,33 @@ def res_block_forward(sd: Dict[str, Tensor], prefix: str, net: Tensor, time_net:
 # ------------------------------------------------------------------------------------------------------------------------------
 # module
 # ------------------------------------------------------------------------------------------------------------------------------
+def _build(eps: float, net: Tensor, time_net: Optional[Tensor], *params: Optional[Tensor]) -> Tuple[Tensor, tuple]:
+    """The Function's forward on its inputs: (out [B, Cout, H, W] with channels-last strides, what ``res_block_bwd`` reads)."""
+    xt = net.permute(0, 2, 3, 1).contiguous()  # a view when net is channels-last
+    out, saved = res_block_fwd(xt, time_net, params, eps)
+    return out.permute(0, 3, 1, 2), saved
+
+
 class _ResBlockFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, net: Tensor, time_net: Optional[Tensor], eps: float, *params: Optional[Tensor]):  # type: ignore[override]
-        xt = net.permute(0, 2, 3, 1).contiguous()  # a view when net is channels-last
-        out, saved = res_block_fwd(xt, time_net, params, eps)
-        ctx.save_for_backward(*saved)
-        return out.permute(0, 3, 1, 2)
+    def forward(ctx, net: Tensor, time_net: Optional[Tensor], eps: float, use_checkpoint: bool, *params: Optional[Tensor]):  # type: ignore[override]
+        ctx.eps, ctx.use_checkpoint = eps, use_checkpoint
+        out, kept = checkpoint.run(partial(_build, eps), (net, time_net, *params), use_checkpoint)
+        ctx.save_for_backward(*kept)
+        return out
 
     @staticmethod
     def backward(ctx, dout: Tensor):  # type: ignore[override]
-        dx, dtime, grads = res_block_bwd(ctx.saved_tensors, dout.permute(0, 2, 3, 1).to(torch.bfloat16).contiguous())
-        return (dx.permute(0, 3, 1, 2), dtime, None, *grads)
+        saved = checkpoint.rebuild(partial(_build, ctx.eps), ctx.saved_tensors, ctx.use_checkpoint)
+        dx, dtime, grads = res_block_bwd(saved, dout.permute(0, 2, 3, 1).to(torch.bfloat16).contiguous())
+        return (dx.permute(0, 3, 1, 2), dtime, None, None, *grads)
 
 
 class ResidualBlockWithTimeEmbeddingB200(nn.Module):
     """Drop-in for cflearn's ``ResidualBlockWithTimeEmbedding`` on the native kernels (bf16 activations, fp32 parameters; CUDA
     only).  ``forward(net, time_net=None)`` takes bf16 [B, Cin, H, W] (channels-last preferred: used without a copy) and a bf16
-    [B, time_embedding_channels] time embedding, and returns bf16 [B, Cout, H, W] with channels-last strides."""
+    [B, time_embedding_channels] time embedding, and returns bf16 [B, Cout, H, W] with channels-last strides.
+    ``use_checkpoint=True`` keeps only the inputs for backward and recomputes the activations there (the same gradients)."""
 
     def __init__(self, in_channels: int, out_channels: Optional[int] = None, *, signal_dim: int = 2, dropout: float = 0.0,
                  norm_eps: float = 1.0e-6, use_conv_shortcut: bool = False, integrate_upsample: bool = False,
@@ -182,7 +194,7 @@ class ResidualBlockWithTimeEmbeddingB200(nn.Module):
         self.in_channels = in_channels
         self.out_channels = out_channels
         self.norm_eps = norm_eps
-        self.use_checkpoint = use_checkpoint  # accepted: activations are saved, not recomputed (same results, more memory)
+        self.use_checkpoint = use_checkpoint  # keep only the inputs and recompute the activations in backward
         # registration order of the reference (state_dict order): norm1, conv1, time_embedding, norm2, conv2, shortcut
         self.norm1 = nn.GroupNorm(32, in_channels, eps=norm_eps)
         self.conv1 = nn.Conv2d(in_channels, out_channels, 3, 1, 1)
@@ -215,4 +227,4 @@ class ResidualBlockWithTimeEmbeddingB200(nn.Module):
                 raise B200Error(f"{what} needs CUDA tensors (there is no CPU fallback)")
             if t is not None and t.dtype != torch.bfloat16:
                 raise B200Error(f"{what}: net and time_net must be bf16 (the UNet's activations under bf16 autocast)")
-        return _ResBlockFn.apply(net, time_net, self.norm_eps, *self._params())
+        return _ResBlockFn.apply(net, time_net, self.norm_eps, self.use_checkpoint, *self._params())
