@@ -188,7 +188,8 @@ class CLIPB200(nn.Module):
         return [self.vit.arena, self.text_transformer.arena, self.glue]
 
     def _collect_glue_grads(self) -> None:
-        """autograd hands the loose parameters' gradients over as separate tensors: move them into the glue arena."""
+        """autograd hands the loose parameters' gradients over as separate tensors: move them into the glue arena.  Once they
+        are its views, autograd accumulates the next backward's gradients into them in place."""
         with torch.no_grad():
             for k in self._glue_keys:
                 p = self.glue.params[k]
@@ -201,7 +202,9 @@ class CLIPB200(nn.Module):
 
     def train_step(self, image: Tensor, text: Tensor) -> Tensor:
         """forward + symmetric cross-entropy + backward (+ data parallel: the towers' bucket reducers run inside their
-        backward, the loose parameters are all-reduced here); returns the loss (fp32 scalar on the device)."""
+        backward, the loose parameters are all-reduced here); returns the loss (fp32 scalar on the device).  Under
+        gradient accumulation the trainer runs every micro-batch but a window's last in ``dp.no_sync``, so both exchanges
+        happen once per window, on the accumulated gradients."""
         loss = symmetric_cross_entropy(self.forward(image, text))
         loss.backward()
         self._collect_glue_grads()

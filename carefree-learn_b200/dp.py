@@ -13,6 +13,7 @@ finding 3: the reference defines multi-GPU parity only mathematically).
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes
 import os
 from typing import Any, Dict, List, Optional, Tuple, Union
@@ -224,6 +225,26 @@ def attach_native_reducers(module, comm: NativeComm) -> List[NativeBucketReducer
 def detach_reducers(module) -> None:
     for t in _towers(module):
         t.engine.reducer = None
+
+
+@contextlib.contextmanager
+def no_sync(module):
+    """Backward without the gradient exchange, like DDP's ``no_sync``: inside, the towers' bucket reducers and a module's
+    all-reduce of its loose parameters (``module.comm``) are switched off.  Gradient accumulation runs every micro-batch
+    of a window but the last inside it, so the window's sum is exchanged once, by its last backward."""
+    towers = _towers(module)
+    reducers = [t.engine.reducer for t in towers]
+    comm = getattr(module, "comm", None)
+    try:
+        detach_reducers(module)
+        if hasattr(module, "towers"):
+            module.comm = None
+        yield
+    finally:
+        for t, red in zip(towers, reducers):
+            t.engine.reducer = red
+        if hasattr(module, "towers"):
+            module.comm = comm
 
 
 def attach_reducer(module, process_group=None) -> GradBucketReducer:

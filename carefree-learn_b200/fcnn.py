@@ -114,5 +114,5 @@ class FCNNB200(nn.Module):
         the gradient arena, overwritten every call) and returns (loss, predictions)."""
         self.arena.ensure()  # may re-create the gradient arena
         pred, loss = self._launch(x, y=y, grads=self.arena.grad, loss_weights=loss_weights)
-        self.arena.publish_grads(self.arena.grad, list(self.arena.params))
+        self.arena.publish_grads(list(self.arena.params))
         return loss, pred

@@ -373,9 +373,10 @@ def attention_fwd(qkv: Tensor, B: int, T: int, H: int, *, scale: Optional[float]
 
 
 def attention_bwd(qkv: Tensor, out: Tensor, dout: Tensor, lse: Tensor, B: int, T: int, H: int, *, scale: Optional[float] = None, causal: bool = False, dqkv: Optional[Tensor] = None,
-                  dbias: Optional[Tensor] = None) -> Tensor:
+                  dbias: Optional[Tensor] = None, accumulate: bool = False) -> Tensor:
     """dqkv (bf16 [B*T, 3*H*64]).  ``dbias`` (fp32 [3*H*64]): also receives the bf16-rounded column sums of dqkv -- the
-    gradient of the packed qkv bias -- accumulated inside the kernel (no separate pass over dqkv)."""
+    gradient of the packed qkv bias -- accumulated inside the kernel (no separate pass over dqkv); ``accumulate``: added to
+    ``dbias`` instead of overwriting it."""
     what, D = "attention_bwd", H * 64
     _check(what, "qkv", qkv, _BF16, rows=B * T, width=3 * D)
     _check(what, "out", out, _BF16, rows=B * T, width=D)
@@ -395,7 +396,7 @@ def attention_bwd(qkv: Tensor, out: Tensor, dout: Tensor, lse: Tensor, B: int, T
         call("b200_attention_long_bwd", qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr(), dqkv.data_ptr(), B, T, H, 64, sc,
              int(causal), _ptr(part), ws.data_ptr(), _stream())
     if dbias is not None:
-        _colsum_finish(part, 3 * D, B, 0, 3 * D, dbias, round_bf16=True)
+        _colsum_finish(part, 3 * D, B, 0, 3 * D, dbias, round_bf16=True, accumulate=accumulate)
     return dqkv
 
 

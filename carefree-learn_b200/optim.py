@@ -11,10 +11,13 @@ live on the device, so the update can be replayed from a CUDA graph while a sche
 Adam`` (IDLModel.train, cflearn/schema.py:1174-1294, minus its per-step host work) into ONE CUDA graph.  With more
 than one rank the all-reduces are nodes of the same graph: each transformer block's bucket is reduced on a forked
 communication stream through the library's own NCCL communicator (``dp.NativeComm``) while the backward of the
-earlier blocks is still running.
+earlier blocks is still running.  With gradient accumulation over K micro-batches it captures two graphs in one memory
+pool: a micro-step (forward, loss, backward adding to the gradient arenas) and the window's closing step (the same, then
+the exchange, clipping and Adam).
 """
 from __future__ import annotations
 
+import contextlib
 from typing import Any, Dict, List, Optional
 
 import torch
@@ -215,16 +218,26 @@ class GraphedTrainStep:
     Data parallel (``comm``: a ``dp.NativeComm``): the graph also holds the gradient exchange -- the model's bucket
     reducers launch ``ncclAllReduce`` per transformer block on a forked stream as soon as that block's gradients are
     complete -- and the Adam update behind the join.  ``inputs``: the static input tensors (default: an image batch
-    [batch, C, S, S] fp32 and int64 labels [batch, 1] for the classifier)."""
+    [batch, C, S, S] fp32 and int64 labels [batch, 1] for the classifier).
+
+    ``grad_accumulate=K``: one optimizer update per K calls of ``step`` (the reference's ``TrainerConfig.grad_accumulate``).
+    Every call runs forward, loss and a backward that adds to the gradient arenas, which are zeroed (one ``fill`` launch per
+    arena) before a window's first call; the K-th call also exchanges the summed gradients, clips them and steps Adam.
+    ``updated`` says whether the last call did.  K = 1 is the single graph described above."""
 
     def __init__(self, model: Any, optimizer: ArenaAdam, batch: int, warmup: int = 2, comm: Any = None, flat: bool = False,
-                 inputs: Optional[List[Tensor]] = None):
+                 inputs: Optional[List[Tensor]] = None, grad_accumulate: int = 1):
+        if grad_accumulate < 1:
+            raise ValueError(f"grad_accumulate must be >= 1, got {grad_accumulate}")
         if not optimizer.capturable:
             raise ValueError("GraphedTrainStep needs ArenaAdam(capturable=True)")
         from . import _cabi, dp
 
         self.world = 1 if comm is None else comm.world
         self.comm = comm
+        self.accumulate = int(grad_accumulate)
+        self.micro = 0  # calls of the current window so far
+        self.updated = False
         # flat=True (A/B switch): the graph stops after backward; ONE all-reduce per gradient arena and Adam are
         # enqueued behind every replay -- the un-overlapped schedule
         self.flat = bool(flat) and self.world > 1
@@ -247,6 +260,9 @@ class GraphedTrainStep:
         self.x, self.labels = inputs[0], inputs[-1]
         self.loss = torch.zeros((), dtype=torch.float32, device=dev)
         self.bad_label = torch.zeros(1, dtype=torch.int32, device=dev)
+        if self.accumulate > 1:  # every backward from here on adds to the arenas, the captured ones included
+            for a in arenas:
+                a.publish_grads(list(a.params))
         # warm up on a side stream (allocator pools, workspaces, lazy function attributes, NCCL connections), then
         # capture.  Warm-up steps run real Adam updates on an all-zero batch, so everything they touch is put back.
         state = optimizer.state_tensors()
@@ -255,16 +271,28 @@ class GraphedTrainStep:
         s.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(s):
             for _ in range(warmup):
+                if self.accumulate > 1:
+                    self._eager(update=False)
                 self._eager()
         torch.cuda.current_stream().wait_stream(s)
         torch.cuda.synchronize()
+        # one pool for both graphs: they never run at the same time, so the micro-step's activations reuse the closing step's
+        pool = torch.cuda.graph_pool_handle()
+        self.micro_graph: Optional[torch.cuda.CUDAGraph] = None
+        self.launches_per_micro_replay: Optional[int] = None
+        if self.accumulate > 1:
+            self.micro_graph = torch.cuda.CUDAGraph()
+            n0 = _cabi.launch_count()
+            with torch.cuda.graph(self.micro_graph, pool=pool, capture_error_mode="thread_local"):
+                self._eager(update=False)
+            self.launches_per_micro_replay = _cabi.launch_count() - n0
         self.graph = torch.cuda.CUDAGraph()
         n0 = _cabi.launch_count()
         # thread_local: only THIS thread is held to the capture rules -- a torch.distributed watchdog thread polling its own
         # events (the process group that bootstrapped the communicator) must not invalidate the capture
-        with torch.cuda.graph(self.graph, capture_error_mode="thread_local"):
+        with torch.cuda.graph(self.graph, pool=pool, capture_error_mode="thread_local"):
             self._eager()
-        self.launches_per_replay = _cabi.launch_count() - n0  # b200 kernels inside one replay of the graph
+        self.launches_per_replay = _cabi.launch_count() - n0  # b200 kernels inside one replay of the (closing) graph
         with torch.no_grad():
             for dst, src in zip(state, snap):
                 dst.copy_(src)
@@ -272,13 +300,18 @@ class GraphedTrainStep:
             optimizer.step_count = int(optimizer.step_dev.item())
         torch.cuda.synchronize()
 
-    def _eager(self) -> None:
-        self.optimizer.zero_grad()
-        loss = self.model.train_step(*self.inputs)  # DP: the reducers all-reduce bucket by bucket inside backward
+    def _eager(self, update: bool = True) -> None:
+        """One step; ``update=False``: a micro-step of a window, which only adds its gradients to the arenas."""
+        from . import dp
+
+        if self.accumulate == 1:
+            self.optimizer.zero_grad()
+        with contextlib.nullcontext() if update else dp.no_sync(self.model):
+            loss = self.model.train_step(*self.inputs)  # DP: the reducers all-reduce bucket by bucket inside backward
         hook = getattr(self.model, "clip_norm_hook", None)
-        if hook is not None and not self.flat:
+        if update and hook is not None and not self.flat:
             hook()  # device-side clip coefficient (trainer.B200TrainStep): captured with the step
-        if not self.flat:
+        if update and not self.flat:
             self.optimizer.step()
         self.loss.copy_(loss)
         flag = getattr(self.model, "last_bad_flag", None)
@@ -289,6 +322,14 @@ class GraphedTrainStep:
         self.optimizer.sync_hyper()  # lr schedule: 24 bytes host->device when (and only when) a value changed
         for dst, src in zip(self.inputs, inputs):
             dst.copy_(src.reshape(dst.shape), non_blocking=True)
+        if self.accumulate > 1 and self.micro == 0:
+            for a in self.optimizer.arenas():
+                ops.fill_f32(a.grad, 0.0)
+        self.micro = (self.micro + 1) % self.accumulate
+        self.updated = self.micro == 0
+        if not self.updated:
+            self.micro_graph.replay()
+            return self.loss
         self.graph.replay()
         if self.flat:
             for a in self.optimizer.arenas():
@@ -307,6 +348,9 @@ class GraphedTrainStep:
             torch.cuda.synchronize()
             self.graph.reset()
             self.graph = None
+            if self.micro_graph is not None:
+                self.micro_graph.reset()
+                self.micro_graph = None
 
     def check_labels(self) -> None:
         """Synchronises and raises ``ValueError`` if the last replay saw a label outside [0, num_classes)."""

@@ -14,24 +14,38 @@ gradient clipping, the fused multi-arena Adam, and any ``torch.optim.lr_schedule
 ``WarmupScheduler`` (cflearn/schedulers.py:126-171; pipeline/blocks/basic.py:334-352) -- driving the learning rate through
 ``optimizer.param_groups``.  With ``graph=True`` everything up to and including Adam is ONE CUDA graph; the scheduler's new
 learning rate reaches the captured kernels through 24 bytes of device memory, never by re-capturing.
+
+``grad_accumulate=K`` follows the reference's ``TrainerConfig.grad_accumulate`` (schema.py:1276-1290, 1888): backward runs
+on every micro-batch and the update (clip, optimizer, scheduler) only on every K-th call, counting from the first; the
+loss is not divided by K, so the update sees the sum of the K micro-batch gradients.  The gradients add up in place in
+the arenas.  With a communicator they are exchanged once per window, by its last backward: that gives avg_r(sum_k g)
+where DDP without ``no_sync`` gives sum_k avg_r(g) -- equal but for the order of the fp32 additions, and K - 1 fewer
+exchanges per window.
 """
 from __future__ import annotations
 
+import contextlib
 from typing import Any, List, Optional
 
 import torch
 from torch import Tensor
 
+from . import dp
 from .optim import ArenaAdam, GraphedTrainStep
 
 
 class B200TrainStep:
     def __init__(self, model: Any, optimizer: ArenaAdam, *, scheduler: Any = None, clip_norm: float = 0.0, comm: Any = None,
-                 graph: bool = False, batch: Optional[int] = None, static_inputs: Optional[List[Tensor]] = None, flat: bool = False):
+                 graph: bool = False, batch: Optional[int] = None, static_inputs: Optional[List[Tensor]] = None, flat: bool = False,
+                 grad_accumulate: int = 1):
+        if grad_accumulate < 1:
+            raise ValueError(f"grad_accumulate must be >= 1, got {grad_accumulate}")
         self.model, self.optimizer, self.scheduler = model, optimizer, scheduler
         self.clip_norm = float(clip_norm)
         self.comm = comm
+        self.accumulate = int(grad_accumulate)
         self.steps = 0
+        self.updated = False  # whether the last ``step`` ran the optimizer
         self._graph: Optional[GraphedTrainStep] = None
         if self.clip_norm > 0.0 and not optimizer.capturable:
             raise ValueError("clip_norm > 0 needs ArenaAdam(capturable=True)")
@@ -42,10 +56,9 @@ class B200TrainStep:
             if batch is None and static_inputs is None:
                 raise ValueError("graph=True needs the batch size (or the static input tensors)")
             self._graph = GraphedTrainStep(model, optimizer, batch or static_inputs[0].shape[0], comm=comm, inputs=static_inputs,
-                                           flat=flat)  # flat: ONE all-reduce behind the graph instead of in-graph buckets
+                                           flat=flat,  # flat: ONE all-reduce behind the graph instead of in-graph buckets
+                                           grad_accumulate=self.accumulate)
         elif comm is not None and comm.world > 1:
-            from . import dp
-
             dp.attach_native_reducers(model, comm)
 
     def close(self) -> None:
@@ -55,16 +68,22 @@ class B200TrainStep:
             self._graph = None
 
     def step(self, *batch: Tensor) -> Tensor:
-        """One optimisation step on ``batch`` (device tensors or pinned host tensors); returns the loss (device scalar)."""
+        """One micro-batch on ``batch`` (device tensors or pinned host tensors); returns its loss (device scalar).  Every
+        ``grad_accumulate``-th call also updates the parameters; ``updated`` says whether this one did."""
         if self._graph is not None:
             loss = self._graph.step(*batch)
+            self.updated = self._graph.updated
         else:
-            self.optimizer.zero_grad()                      # schema.py:984 (moved to the front: backward overwrites the arena)
-            loss = self.model.train_step(*batch)            # autocast forward + loss + accelerator.backward   schema.py:1266-1276,980
-            if self.clip_norm > 0.0:
-                self.optimizer.clip_grad_norm_(self.clip_norm)  # trainer.clip_norm_step()                     schema.py:982
-            self.optimizer.step()                           # schema.py:983
-        if self.scheduler is not None:
+            first, self.updated = self.steps % self.accumulate == 0, (self.steps + 1) % self.accumulate == 0
+            if first:
+                self.optimizer.zero_grad()                  # schema.py:984 (moved to the front: the window's first backward overwrites the arena)
+            with contextlib.nullcontext() if self.updated else dp.no_sync(self.model):
+                loss = self.model.train_step(*batch)        # autocast forward + loss + accelerator.backward   schema.py:1266-1276,980
+            if self.updated:
+                if self.clip_norm > 0.0:
+                    self.optimizer.clip_grad_norm_(self.clip_norm)  # trainer.clip_norm_step()                 schema.py:982
+                self.optimizer.step()                       # schema.py:983
+        if self.updated and self.scheduler is not None:
             self.scheduler.step()                           # writes optimizer.param_groups[0]["lr"]; reaches the device on the next step
         self.steps += 1
         return loss

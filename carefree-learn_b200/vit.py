@@ -54,7 +54,6 @@ class ParamArena:
         self.flat: Optional[Tensor] = None
         self.flat_bf16: Optional[Tensor] = None
         self.grad: Optional[Tensor] = None
-        self.grad_scratch: Optional[Tensor] = None
         self.params: Dict[str, nn.Parameter] = {}
         self._bf16_version = -1
 
@@ -80,7 +79,6 @@ class ParamArena:
         self.flat = flat
         self.flat_bf16 = torch.zeros(self.total, dtype=torch.bfloat16, device=dev) if dev.type == "cuda" else None
         self.grad = torch.zeros(self.total, dtype=torch.float32, device=dev)
-        self.grad_scratch = None
         self._bf16_version = -1
 
     def ensure(self) -> None:
@@ -113,30 +111,30 @@ class ParamArena:
         """[lo, hi) of the arena holding ``keys``, which are consecutive in the layout (one all-reduce bucket)."""
         return self.offsets[keys[0]], self.offsets[keys[-1]] + _padded(self.shapes[keys[-1]])
 
-    def grad_arena(self, keys: List[str]) -> Tensor:
-        """Where a backward writes: the main gradient arena (overwrite), unless some parameter already holds a gradient
-        (gradient accumulation): then the scratch arena, added on by ``publish_grads``."""
-        if not any(self.params[k].grad is not None for k in keys):
-            return self.grad
-        if self.grad_scratch is None:
-            self.grad_scratch = torch.zeros_like(self.grad)
-        return self.grad_scratch
-
-    def publish_grads(self, G: Tensor, keys: List[str]) -> None:
-        """Make ``p.grad`` views of the gradient arena (no copies), after a backward wrote ``G`` (see ``grad_arena``)."""
+    def claim_grads(self, keys: List[str]) -> bool:
+        """Before a backward over ``keys``: whether it adds to the gradient arena in place (``True``: eager's ``p.grad += g``)
+        or overwrites it.  It overwrites while no parameter holds a gradient.  Once one does (gradient accumulation), every
+        ``p.grad`` that is not yet its arena view is folded in first -- a missing one as zeros, any other tensor copied -- so
+        that the arena holds every gradient the backward adds to.  After ``publish_grads`` the gradients are live (each
+        ``p.grad`` its arena view) and the next backward accumulates with no extra pass."""
+        if all(self.params[k].grad is None for k in keys):
+            return False
         with torch.no_grad():
             for key in keys:
-                p = self.params[key]
-                v = self.view(self.grad, key)
-                if G is self.grad:
-                    if p.grad is None or p.grad.data_ptr() != v.data_ptr():
-                        p.grad = v
-                else:  # accumulation step: G is the scratch arena
-                    if p.grad is None:
-                        v.copy_(self.view(G, key))
-                        p.grad = v
-                    else:
-                        p.grad.add_(self.view(G, key))
+                p, v = self.params[key], self.view(self.grad, key)
+                if p.grad is None:
+                    ops.fill_f32(v, 0.0)
+                elif p.grad.data_ptr() != v.data_ptr():
+                    v.copy_(p.grad)
+        return True
+
+    def publish_grads(self, keys: List[str]) -> None:
+        """Make each ``p.grad`` of ``keys`` its view of the gradient arena (no copies)."""
+        for key in keys:
+            p = self.params[key]
+            v = self.view(self.grad, key)
+            if p.grad is None or p.grad.data_ptr() != v.data_ptr():
+                p.grad = v
 
 
 def _register_dotted(root: nn.Module, key: str, param: nn.Parameter) -> None:
@@ -311,52 +309,56 @@ class ViTEngine:
         return out, (net, mean1, rstd1, ln1, qkv, attn, lse, mid, mean2, rstd2, ln2, h, act)
 
     def block_backward(self, i: int, saved: Tuple[Tensor, ...], dnet: Tensor, dnet_bf: Tensor, G: Tensor, B: int,
-                       *, ff2_bias_done: bool = True, next_ff2_bias: bool = True) -> None:
+                       *, ff2_bias_done: bool = True, next_ff2_bias: bool = True, accumulate: bool = False) -> None:
         """Backward of block ``i``.  ``dnet`` (fp32) / ``dnet_bf`` (its bf16 rounding) hold the gradient of the block's
         output and are OVERWRITTEN with the gradient of its input.  ``ff2_bias_done``: this block's FF2 bias gradient was
         already emitted by the producer of ``dnet_bf``; ``next_ff2_bias``: emit block ``i-1``'s from the last LayerNorm
-        backward here (both fusions remove a pass over the [M, D] gradient)."""
+        backward here (both fusions remove a pass over the [M, D] gradient).  ``accumulate``: the parameter gradients are
+        added to ``G`` instead of overwriting it."""
         g, A = self.geo, self.arena
         T, D, M = g.T, g.D, B * g.T
         dev = dnet.device
         b = f"encoder.mixing_blocks.{i}."
         net, mean1, rstd1, ln1, qkv, attn, lse, mid, mean2, rstd2, ln2, h, act = saved
         if not ff2_bias_done:
-            ops.colsum(dnet_bf, A.g(b + "channel_mixing.net.3.linear.bias", G))
+            ops.colsum(dnet_bf, A.g(b + "channel_mixing.net.3.linear.bias", G), accumulate=accumulate)
         # FeedForward: net_out = mid + W2 gelu(W1 ln2 + b1) + b2
         ff1_bias = A.g(b + "channel_mixing.net.0.linear.bias", G)
         shrink, self.shrink_next = self.shrink_next, 0  # the previous block's bucket is being all-reduced right now
         dh = ops.gemm(dnet_bf, A.w(b + "channel_mixing.net.3.linear.weight"), b_mn_major=True,
                       epilogue=ops.EPI_DQGELU_BF16 if g.quick_gelu else ops.EPI_DGELU_BF16, aux=h,
                       max_ctas=(ops.num_sms() - shrink) if shrink else 0)
-        ops.wgrad(dnet_bf, act, A.g(b + "channel_mixing.net.3.linear.weight", G))
+        ops.wgrad(dnet_bf, act, A.g(b + "channel_mixing.net.3.linear.weight", G), accumulate=accumulate)
         dln2 = ops.gemm(dh, A.w(b + "channel_mixing.net.0.linear.weight"), b_mn_major=True)
-        ops.wgrad(dh, ln2, A.g(b + "channel_mixing.net.0.linear.weight", G))
-        ops.colsum(dh, ff1_bias)
+        ops.wgrad(dh, ln2, A.g(b + "channel_mixing.net.0.linear.weight", G), accumulate=accumulate)
+        ops.colsum(dh, ff1_bias, accumulate=accumulate)
         dmid = torch.empty((M, D), dtype=torch.float32, device=dev)
         dmid_bf = torch.empty((M, D), dtype=torch.bfloat16, device=dev)
         ops.layernorm_bwd(dln2, mid, A.p(b + "channel_norm.weight"), mean2, rstd2, rows=M, dim=D, ld_x=D, dres=dnet,
                           dx_out=dmid, ld_dx=D, dx_bf16=dmid_bf,
                           dgamma=A.g(b + "channel_norm.weight", G), dbeta=A.g(b + "channel_norm.bias", G),
-                          dx_colsum=A.g(b + "token_mixing.net.out_linear.linear.bias", G))
+                          dx_colsum=A.g(b + "token_mixing.net.out_linear.linear.bias", G), accumulate=accumulate)
         # attention: mid = net + Wo attn + bo
         dattn = ops.gemm(dmid_bf, A.w(b + "token_mixing.net.out_linear.linear.weight"), b_mn_major=True)
-        ops.wgrad(dmid_bf, attn, A.g(b + "token_mixing.net.out_linear.linear.weight", G))
-        dqkv = ops.attention_bwd(qkv, attn, dattn, lse, B, T, g.H, causal=g.causal, dbias=A.g(b + "token_mixing.net.qkv_bias", G))
+        ops.wgrad(dmid_bf, attn, A.g(b + "token_mixing.net.out_linear.linear.weight", G), accumulate=accumulate)
+        dqkv = ops.attention_bwd(qkv, attn, dattn, lse, B, T, g.H, causal=g.causal, dbias=A.g(b + "token_mixing.net.qkv_bias", G),
+                                 accumulate=accumulate)
         dln1 = ops.gemm(dqkv, A.w(b + "token_mixing.net.in_w"), b_mn_major=True)
-        ops.wgrad(dqkv, ln1, A.g(b + "token_mixing.net.in_w", G))
+        ops.wgrad(dqkv, ln1, A.g(b + "token_mixing.net.in_w", G), accumulate=accumulate)
         ops.layernorm_bwd(dln1, net, A.p(b + "token_norm.weight"), mean1, rstd1, rows=M, dim=D, ld_x=D, dres=dmid,
                           dx_out=dnet, ld_dx=D, dx_bf16=dnet_bf,
                           dgamma=A.g(b + "token_norm.weight", G), dbeta=A.g(b + "token_norm.bias", G),
-                          dx_colsum=A.g(f"encoder.mixing_blocks.{i - 1}.channel_mixing.net.3.linear.bias", G) if (i > 0 and next_ff2_bias) else None)
+                          dx_colsum=A.g(f"encoder.mixing_blocks.{i - 1}.channel_mixing.net.3.linear.bias", G) if (i > 0 and next_ff2_bias) else None,
+                          accumulate=accumulate)
 
-    def stem_backward(self, sv: "_Saved", dnet: Tensor, G: Tensor) -> None:
+    def stem_backward(self, sv: "_Saved", dnet: Tensor, G: Tensor, *, accumulate: bool = False) -> None:
         """tokens = cat(cls, patches) + pos ; patches = conv(x): pos / cls / conv weight (+ bias) gradients."""
         g, A = self.geo, self.arena
-        dpatch = ops.assemble_tokens_bwd(dnet, A.g("encoder.pos_encoding.pos_encoding", G), A.g("encoder.head_token", G), sv.B, g.np, g.D)
-        ops.wgrad(dpatch, sv.cols, A.g("to_patches.projection.weight", G).view(g.D, -1))
+        dpatch = ops.assemble_tokens_bwd(dnet, A.g("encoder.pos_encoding.pos_encoding", G), A.g("encoder.head_token", G), sv.B, g.np, g.D,
+                                         accumulate=accumulate)
+        ops.wgrad(dpatch, sv.cols, A.g("to_patches.projection.weight", G).view(g.D, -1), accumulate=accumulate)
         if g.conv_bias:
-            ops.colsum(dpatch, A.g("to_patches.projection.bias", G))
+            ops.colsum(dpatch, A.g("to_patches.projection.bias", G), accumulate=accumulate)
 
     # ---- forward ------------------------------------------------------------------------------------------
     def encoder_forward(self, x: Tensor, want_f32: bool) -> Tuple[Tensor, Optional[Tensor], _Saved]:
@@ -405,22 +407,23 @@ class ViTEngine:
     def projection_forward(self, enc_bf16: Tensor) -> Tensor:
         return ops.gemm(enc_bf16, self.arena.w("output_projection"), b_mn_major=True)  # [B, D] . [D, out] -> bf16 [B, out]
 
-    def projection_backward(self, sv: _Saved, d_out: Tensor, G: Tensor) -> Tensor:
+    def projection_backward(self, sv: _Saved, d_out: Tensor, G: Tensor, *, accumulate: bool = False) -> Tensor:
         A = self.arena
         d_enc = ops.gemm(d_out, A.w("output_projection"))                      # [B, out] . [D, out]^T -> bf16 [B, D]
-        ops.wgrad(sv.enc_bf16, d_out, A.g("output_projection", G))             # enc^T . d_out -> [D, out]
+        ops.wgrad(sv.enc_bf16, d_out, A.g("output_projection", G), accumulate=accumulate)  # enc^T . d_out -> [D, out]
         return d_enc
 
     # ---- backward -----------------------------------------------------------------------------------------
-    def head_backward(self, sv: _Saved, dlogits: Tensor, G: Tensor) -> Tensor:
+    def head_backward(self, sv: _Saved, dlogits: Tensor, G: Tensor, *, accumulate: bool = False) -> Tensor:
         A = self.arena
         d_enc = ops.gemm(dlogits, A.w("head.linear.weight"), b_mn_major=True)  # [B, D] bf16
-        ops.wgrad(dlogits, sv.enc_bf16, A.g("head.linear.weight", G))
-        ops.colsum(dlogits, A.g("head.linear.bias", G))
+        ops.wgrad(dlogits, sv.enc_bf16, A.g("head.linear.weight", G), accumulate=accumulate)
+        ops.colsum(dlogits, A.g("head.linear.bias", G), accumulate=accumulate)
         return d_enc
 
-    def encoder_backward(self, sv: _Saved, d_enc_bf16: Tensor, G: Tensor) -> Optional[Tensor]:
-        """Writes every encoder parameter gradient into the flat arena ``G`` (overwrite semantics).  ``d_enc_bf16``: the
+    def encoder_backward(self, sv: _Saved, d_enc_bf16: Tensor, G: Tensor, *, accumulate: bool = False) -> Optional[Tensor]:
+        """Writes every encoder parameter gradient into the flat arena ``G`` (overwriting it, or adding to it with
+        ``accumulate``; activation gradients are never accumulated).  ``d_enc_bf16``: the
         gradient of the head LayerNorm's output -- bf16 [B, D] (vision: it feeds a bf16 matmul) or, in token mode,
         fp32 [B*T, D] (the LayerNorm output itself is what the module returns).  Token mode returns the gradient of the
         embedded input [B, T, D]."""
@@ -433,20 +436,20 @@ class ViTEngine:
             dnet_bf = torch.empty((M, D), dtype=torch.bfloat16, device=dev)
             ops.layernorm_bwd(d_enc_bf16, sv.net_last, A.p(g.head_norm_key + "weight"), sv.head_mean, sv.head_rstd,
                               rows=M, dim=D, ld_x=D, dres=None, dx_out=dnet, ld_dx=D, dx_bf16=dnet_bf,
-                              dgamma=A.g(g.head_norm_key + "weight", G), dbeta=A.g(g.head_norm_key + "bias", G))
+                              dgamma=A.g(g.head_norm_key + "weight", G), dbeta=A.g(g.head_norm_key + "bias", G), accumulate=accumulate)
         else:
             ops.fill_f32(dnet, 0.0)
             ops.layernorm_bwd(d_enc_bf16, sv.net_last, A.p(g.head_norm_key + "weight"), sv.head_mean, sv.head_rstd,
                               rows=B, dim=D, ld_x=T * D, dres=None, dx_out=dnet, ld_dx=T * D, dx_bf16=None,
-                              dgamma=A.g(g.head_norm_key + "weight", G), dbeta=A.g(g.head_norm_key + "bias", G))
+                              dgamma=A.g(g.head_norm_key + "weight", G), dbeta=A.g(g.head_norm_key + "bias", G), accumulate=accumulate)
             dnet_bf = ops.cast_bf16(dnet)
         # bias gradient of the last block's FF2 (dY = dnet_bf); every other Linear whose dY comes out of a LayerNorm
         # backward gets its bias gradient from that kernel (dx_colsum)
-        ops.colsum(dnet_bf, A.g(f"encoder.mixing_blocks.{g.L - 1}.channel_mixing.net.3.linear.bias", G))
+        ops.colsum(dnet_bf, A.g(f"encoder.mixing_blocks.{g.L - 1}.channel_mixing.net.3.linear.bias", G), accumulate=accumulate)
         if red is not None:
             red.ready("tail", G)
         for i in reversed(range(g.L)):
-            self.block_backward(i, sv.blocks[i], dnet, dnet_bf, G, B)
+            self.block_backward(i, sv.blocks[i], dnet, dnet_bf, G, B, accumulate=accumulate)
             sv.blocks[i] = None  # release this block's activations
             if red is not None:
                 red.ready(i, G)
@@ -454,12 +457,13 @@ class ViTEngine:
             dpre = torch.empty_like(dnet)
             ops.layernorm_bwd(dnet, sv.emb_in, A.p("encoder.embedding_norm.weight"), sv.emb_mean, sv.emb_rstd, rows=M, dim=D, ld_x=D,
                               dres=None, dx_out=dpre, ld_dx=D, dx_bf16=None,
-                              dgamma=A.g("encoder.embedding_norm.weight", G), dbeta=A.g("encoder.embedding_norm.bias", G))
+                              dgamma=A.g("encoder.embedding_norm.weight", G), dbeta=A.g("encoder.embedding_norm.bias", G),
+                              accumulate=accumulate)
             dnet = dpre
         if g.tokens:  # net = x + pos: the input gradient is dnet itself
-            ops.add_pos_bwd(dnet, A.g("encoder.pos_encoding.pos_encoding", G), B, T, D)
+            ops.add_pos_bwd(dnet, A.g("encoder.pos_encoding.pos_encoding", G), B, T, D, accumulate=accumulate)
         else:
-            self.stem_backward(sv, dnet, G)
+            self.stem_backward(sv, dnet, G, accumulate=accumulate)
         if red is not None:
             red.ready("stem", G)
         return dnet.view(B, T, D) if g.tokens else None
@@ -477,20 +481,21 @@ class ViTEngine:
             return self.projection_forward(enc_bf16), sv
         return (enc_f32.view(sv.B, g.T, g.D) if g.tokens else enc_f32), sv
 
-    def stack_backward(self, sv: _Saved, d_out: Tensor, G: Tensor, head: bool) -> Optional[Tensor]:
-        """Backward of ``stack_forward`` from the gradient of its output; returns the input gradient in token mode."""
+    def stack_backward(self, sv: _Saved, d_out: Tensor, G: Tensor, head: bool, *, accumulate: bool = False) -> Optional[Tensor]:
+        """Backward of ``stack_forward`` from the gradient of its output (``accumulate``: added to ``G``); returns the input
+        gradient in token mode."""
         g = self.geo
         if head:
             if d_out.dtype != torch.bfloat16:
                 raise B200Error("classifier backward expects a bf16 gradient for the bf16 logits")
-            d_enc = self.head_backward(sv, ops.tma_aligned(d_out), G)
+            d_enc = self.head_backward(sv, ops.tma_aligned(d_out), G, accumulate=accumulate)
         elif g.tokens:  # fp32: the LayerNorm output is the module output
             d_enc = d_out.contiguous().float().view(-1, g.D)
         else:  # under autocast the encoder output feeds a bf16 matmul, so its gradient is bf16-representable
             d_enc = d_out.contiguous() if d_out.dtype == torch.bfloat16 else ops.cast_bf16(d_out.contiguous().float())
             if g.out_dim is not None:
-                d_enc = self.projection_backward(sv, d_enc, G)
-        return self.encoder_backward(sv, d_enc, G)
+                d_enc = self.projection_backward(sv, d_enc, G, accumulate=accumulate)
+        return self.encoder_backward(sv, d_enc, G, accumulate=accumulate)
 
 
 # -----------------------------------------------------------------------------------------------------------------
@@ -498,8 +503,9 @@ class ViTEngine:
 # -----------------------------------------------------------------------------------------------------------------
 class _StackFn(torch.autograd.Function):
     """The whole native stack of one module as ONE autograd node (``ViTEngine.stack_forward``).  Its backward writes every
-    parameter gradient into the gradient arena and publishes them as ``p.grad`` views, so autograd receives ``None`` for
-    the parameters; only token mode returns an input gradient."""
+    parameter gradient into the gradient arena -- overwriting it, or adding to it in place while the parameters hold
+    gradients (``ParamArena.claim_grads``) -- and publishes them as ``p.grad`` views, so autograd receives ``None`` for the
+    parameters; only token mode returns an input gradient."""
 
     @staticmethod
     def forward(ctx: Any, engine: ViTEngine, keys: List[str], head: bool, x: Tensor, *params: Tensor) -> Tensor:
@@ -510,11 +516,11 @@ class _StackFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx: Any, d_out: Tensor) -> Tuple[Any, ...]:
         eng, keys = ctx.engine, ctx.keys
-        G = eng.arena.grad_arena(keys)
-        d_in = eng.stack_backward(ctx.sv, d_out, G, ctx.head)
+        accumulate = eng.arena.claim_grads(keys)
+        d_in = eng.stack_backward(ctx.sv, d_out, eng.arena.grad, ctx.head, accumulate=accumulate)
         if eng.reducer is not None:
             eng.reducer.finish()
-        eng.arena.publish_grads(G, keys)
+        eng.arena.publish_grads(keys)
         ctx.sv = None
         return (None, None, None, d_in) + (None,) * len(keys)
 
