@@ -2,7 +2,7 @@
 
 ``CrossAttentionB200`` is a drop-in for the reference module: same constructor keywords, the same fp32 parameters under the
 same ``state_dict`` keys (``to_q.weight``, ``to_k.weight``, ``to_v.weight``, ``out_linear.0.weight``, ``out_linear.0.bias``).
-Its forward and backward are one ``autograd.Function`` over ``attention_forward`` / ``attention_backward``, which the
+Its forward and backward are one ``checkpoint.OpFn`` node over ``attention_forward`` / ``attention_backward``, which the
 SpatialTransformerBlock (``spatial_transformer.py``) calls as well; every product is the wgmma GEMM (``ops.gemm`` / ``ops.wgrad``) or the
 streamed attention (``ops.cross_attention_fwd/_bwd``), which reads q / k / v as column slices of the projection outputs:
 
@@ -18,17 +18,29 @@ likewise the k and v contributions to the context gradient.  Dropout > 0 and att
 """
 from __future__ import annotations
 
+from dataclasses import dataclass
 from typing import Optional, Tuple
 
 import torch
 from torch import Tensor, nn
 
-from . import ops
+from . import checkpoint, ops
 from ._cabi import B200Error
 
 
 def _bf(t: Tensor) -> Tensor:
     return t.to(torch.bfloat16).contiguous()
+
+
+def _rows(t: Optional[Tensor]) -> Optional[Tensor]:
+    """[..., D] -> contiguous bf16 [rows, D] (a view of a contiguous bf16 tensor); None stays None."""
+    return None if t is None else _bf(t.reshape(-1, t.shape[-1]))
+
+
+def _check_cuda(what: str, *tensors: Optional[Tensor]) -> None:
+    """Refuses CPU tensors before any launch: the native modules have no CPU fallback."""
+    if any(t is not None and not t.is_cuda for t in tensors):
+        raise B200Error(f"{what} needs CUDA tensors (there is no CPU fallback)")
 
 
 def attention_forward(x: Tensor, c: Optional[Tensor], wq: Tensor, wk: Tensor, wv: Tensor, wo: Tensor, bo: Tensor, B: int, heads: int,
@@ -91,25 +103,18 @@ def attention_backward(saved: tuple, dy: Tensor, B: int, heads: int):
     return dx, dc, dwq, dwk, dwv, dwo, dbo
 
 
-class _CrossAttentionFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, net: Tensor, context: Optional[Tensor], wq: Tensor, wk: Tensor, wv: Tensor, wo: Tensor, bo: Tensor, heads: int):  # type: ignore[override]
-        B, Tq, Dq = net.shape
-        x = _bf(net.reshape(B * Tq, Dq))
-        c = None if context is None else _bf(context.reshape(-1, context.shape[-1]))
-        y, saved = attention_forward(x, c, wq, wk, wv, wo, bo, B, heads)
-        ctx.save_for_backward(*saved)
-        ctx.meta = (B, heads, net.dtype, net.shape, None if context is None else (context.dtype, context.shape))
-        return y.view(B, Tq, Dq)
+@dataclass(frozen=True)
+class _AttentionOp:
+    """CrossAttentionB200 as a ``checkpoint.OpFn`` op on (net [B, Tq, Dq], context [B, Tk, Dc] or None, wq, wk, wv, wo, bo)."""
+    B: int
+    heads: int
 
-    @staticmethod
-    def backward(ctx, dy: Tensor):  # type: ignore[override]
-        B, heads, net_dtype, net_shape, ctx_meta = ctx.meta
-        saved = ctx.saved_tensors
-        M, Dq = saved[0].shape
-        dx, dc, dwq, dwk, dwv, dwo, dbo = attention_backward(saved, _bf(dy.reshape(M, Dq)), B, heads)
-        dctx = None if dc is None else dc.to(ctx_meta[0]).view(ctx_meta[1])
-        return dx.to(net_dtype).view(net_shape), dctx, dwq, dwk, dwv, dwo, dbo, None
+    def forward(self, net: Tensor, context: Optional[Tensor], *params: Tensor) -> Tuple[Tensor, tuple]:
+        y, saved = attention_forward(_rows(net), _rows(context), *params, self.B, self.heads)
+        return y.view(net.shape), saved
+
+    def backward(self, saved: tuple, dy: Tensor) -> tuple:
+        return attention_backward(saved, _rows(dy), self.B, self.heads)
 
 
 class _Linear(nn.Module):
@@ -146,7 +151,8 @@ class CrossAttentionB200(nn.Module):
     def forward(self, net: Tensor, *, context: Optional[Tensor] = None, mask: Optional[Tensor] = None) -> Tensor:
         if mask is not None:
             raise NotImplementedError("CrossAttentionB200: attention masks are not supported")
-        if not net.is_cuda:
-            raise B200Error("CrossAttentionB200 needs CUDA tensors (there is no CPU fallback)")
+        _check_cuda("CrossAttentionB200", net, context)
+        B, _, _ = net.shape  # tokens [B, Tq, query_dim]
         lin = self.out_linear[0]
-        return _CrossAttentionFn.apply(net, context, self.to_q.weight, self.to_k.weight, self.to_v.weight, lin.weight, lin.bias, self.num_heads)
+        return checkpoint.OpFn.apply(_AttentionOp(B, self.num_heads), False, net, context, self.to_q.weight, self.to_k.weight,
+                                     self.to_v.weight, lin.weight, lin.bias)

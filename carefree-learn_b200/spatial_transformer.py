@@ -15,17 +15,16 @@ three elementwise gradients are eager's roundings (dh = bf16(da g), dg = bf16(da
 LayerNorm gradient is rounded to bf16 before the bf16 add of the residual branch's gradient, as eager does.
 
 Activations live channels-last: a ``torch.channels_last`` input is used with no copy (a contiguous NCHW one costs one permute),
-and the output is [B, C, H, W] with channels-last strides.  Each block is one ``autograd.Function`` (and the whole transformer
-one more) that keeps the activations it needs through ``save_for_backward`` (so ``retain_graph``, saved-tensor hooks and
-autograd's in-place checks apply as for any other op).  With ``use_checkpoint=True`` a block keeps only its inputs and reruns
-its forward in backward (``checkpoint.py``): the same results bit for bit, one block's activations held instead of every
-block's.  In ``SpatialTransformerB200`` the outer GroupNorm and 1x1 convolutions keep their tensors either way, as the
-reference checkpoints the blocks alone.  Dropout > 0, hooks (ToMe / style reference, inference features), ``use_linear=True`` and activations
-other than GEGLU are refused.
+and the output is [B, C, H, W] with channels-last strides.  A block is one ``checkpoint.OpFn`` node that keeps the activations
+its backward reads, or with ``use_checkpoint=True`` only its inputs, rerunning its forward in backward: the same results bit for
+bit, one block's activations held instead of every block's.  ``SpatialTransformerB200`` is a chain of such nodes: GroupNorm and
+to_latent, each block as it runs standalone (with its own ``use_checkpoint``), then from_latent with the residual.  The outer
+two keep their tensors either way, as the reference checkpoints the blocks alone.  Dropout > 0, hooks (ToMe / style
+reference, inference features), ``use_linear=True`` and activations other than GEGLU are refused.
 """
 from __future__ import annotations
 
-from functools import partial
+from dataclasses import dataclass
 from typing import Any, Dict, List, Optional, Sequence, Tuple
 
 import torch
@@ -33,22 +32,21 @@ from torch import Tensor, nn
 
 from . import checkpoint, ops
 from ._cabi import B200Error
-from .attention import CrossAttentionB200, _bf, _Linear, attention_backward, attention_forward
+from .attention import CrossAttentionB200, _bf, _check_cuda, _Linear, _rows, attention_backward, attention_forward
 
 LN_EPS = 1e-5  # nn.LayerNorm's default (api.py:792-794)
 GN_EPS = 1e-6  # SpatialTransformer.norm (api.py:838)
-BLOCK_PARAMS = 20  # tensors per block handed to the autograd Functions, in _block_params order
-BLOCK_SAVED = 37   # tensors (or Nones) per block kept for backward: 17 of its own + 10 per attention
+BLOCK_PARAMS = 20  # tensors per block handed to _block_forward, in _block_params order
 
 
 # ------------------------------------------------------------------------------------------------------------------------------
 # one block: functional forward / backward on [M, C] bf16 token rows
 # ------------------------------------------------------------------------------------------------------------------------------
 def _block_forward(x0: Tensor, c: Optional[Tensor], P: Sequence[Tensor], B: int, heads: int) -> Tuple[Tensor, tuple]:
-    """Returns (x3 bf16 [M, C], a flat tuple of BLOCK_SAVED tensors / Nones for save_for_backward)."""
+    """Returns (x3 bf16 [M, C], a flat tuple of 37 tensors / Nones for save_for_backward: 17 of its own + 10 per attention)."""
     a1, a2 = P[0:5], P[5:10]
     w1, b1, w2, b2 = P[10:14]
-    g1, be1, g2, be2, g3, be3 = (t.float().contiguous() for t in P[14:20])  # the kernels read fp32 [C]
+    g1, be1, g2, be2, g3, be3 = (t.float().contiguous() for t in P[14:BLOCK_PARAMS])  # the kernels read fp32 [C]
     y1, m1, r1 = ops.layernorm_bf16_fwd(x0, g1, be1, LN_EPS)
     x1, s1 = attention_forward(y1, None, *a1, B, heads, resid=x0)
     y2, m2, r2 = ops.layernorm_bf16_fwd(x1, g2, be2, LN_EPS)
@@ -61,8 +59,8 @@ def _block_forward(x0: Tensor, c: Optional[Tensor], P: Sequence[Tensor], B: int,
 
 
 def _block_backward(saved: tuple, dx3: Tensor, B: int, heads: int) -> Tuple[Tensor, Optional[Tensor], List[Tensor]]:
-    """dx3: bf16 [M, C], the gradient of the block's output.  Returns (dx0 bf16, dcontext bf16 or None, the 20 parameter
-    gradients in _block_params order)."""
+    """dx3: bf16 [M, C], the gradient of the block's output.  Returns (dx0 bf16, dcontext bf16 or None, the BLOCK_PARAMS
+    parameter gradients in _block_params order)."""
     x0, x1, x2, m1, r1, m2, r2, m3, r3, y3, hg, act, w1b, w2b, g1, g2, g3 = saved[:17]
     s1, s2 = saved[17:27], saved[27:37]
     dev = dx3.device
@@ -81,121 +79,65 @@ def _block_backward(saved: tuple, dx3: Tensor, B: int, heads: int) -> Tuple[Tens
     return dx0, dc, [*ga1, *ga2, dw1, db1, dw2, db2, dg1, dbe1, dg2, dbe2, dg3, dbe3]
 
 
-def _check_input(net: Tensor, what: str) -> None:
-    if not net.is_cuda:
-        raise B200Error(f"{what} needs CUDA tensors (there is no CPU fallback)")
-    if net.dtype != torch.bfloat16:
-        raise B200Error(f"{what}: the input must be bf16 (the residual stream of the UNet under bf16 autocast)")
+@dataclass(frozen=True)
+class _BlockOp:
+    """SpatialTransformerBlockB200 as a ``checkpoint.OpFn`` op on (net [B, T, C], context [B, Tk, Dc] or None, the
+    BLOCK_PARAMS parameters in _block_params order)."""
+    B: int
+    heads: int
+
+    def forward(self, net: Tensor, context: Optional[Tensor], *params: Tensor) -> Tuple[Tensor, tuple]:
+        x3, saved = _block_forward(_rows(net), _rows(context), params, self.B, self.heads)
+        return x3.view(net.shape), saved
+
+    def backward(self, saved: tuple, dout: Tensor) -> tuple:
+        dx, dc, grads = _block_backward(saved, _rows(dout), self.B, self.heads)
+        return (dx, dc, *grads)
 
 
-def _context_rows(context: Optional[Tensor]) -> Optional[Tensor]:
-    return None if context is None else _bf(context.reshape(-1, context.shape[-1]))
+class _LatentIn:
+    """SpatialTransformerB200's GroupNorm and to_latent as an op on (xt [B, H, W, C] channels-last, norm w / b, to_latent
+    w / b): the tokens [B, H*W, L]."""
 
-
-def _context_meta(context: Optional[Tensor]):
-    return None if context is None else (context.dtype, context.shape)
-
-
-def _context_grad(dcs: List[Optional[Tensor]], meta) -> Optional[Tensor]:
-    """The context's gradient: each block's bf16 contribution in the context's dtype, summed in that dtype (autograd's sum)."""
-    if meta is None:
-        return None
-    total = None
-    for dc in dcs:
-        g = dc.to(meta[0])
-        total = g if total is None else total + g
-    return total.view(meta[1])
-
-
-def _block_build(heads: int, net: Tensor, context: Optional[Tensor], *params: Tensor) -> Tuple[Tensor, tuple]:
-    """_BlockFn's forward on its inputs: (the block's output [B, T, C], what ``_block_backward`` reads)."""
-    B, T, C = net.shape
-    x3, saved = _block_forward(net.reshape(B * T, C).contiguous(), _context_rows(context), params, B, heads)
-    return x3.view(B, T, C), saved
-
-
-def _rows_build(B: int, heads: int, x0: Tensor, c: Optional[Tensor], *params: Tensor) -> Tuple[Tensor, tuple]:
-    """One block of _SpatialTransformerFn on its inputs: token rows x0 [M, C] and context rows c."""
-    return _block_forward(x0, c, params, B, heads)
-
-
-class _BlockFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, net: Tensor, context: Optional[Tensor], heads: int, use_checkpoint: bool, *params: Tensor):  # type: ignore[override]
-        out, kept = checkpoint.run(partial(_block_build, heads), (net, context, *params), use_checkpoint)
-        ctx.save_for_backward(*kept)
-        ctx.meta = (net.shape[0], heads, net.shape, _context_meta(context), use_checkpoint)
-        return out
-
-    @staticmethod
-    def backward(ctx, dout: Tensor):  # type: ignore[override]
-        B, heads, shape, context, use_checkpoint = ctx.meta
-        saved = checkpoint.rebuild(partial(_block_build, heads), ctx.saved_tensors, use_checkpoint)
-        dx, dc, grads = _block_backward(saved, _bf(dout.reshape(-1, shape[-1])), B, heads)
-        return (dx.view(shape), _context_grad([dc], context), None, None, *grads)
-
-
-class _SpatialTransformerFn(torch.autograd.Function):
-    """``use_checkpoint``: one flag per block, as each of the reference's blocks checkpoints itself.  The outer GroupNorm and
-    1x1 convolutions always keep their tensors; a checkpointed block keeps only its inputs, and backward rebuilds it just
-    before its own backward, so at most one block's rebuilt activations are alive at a time."""
-
-    @staticmethod
-    def forward(ctx, net: Tensor, context: Optional[Tensor], heads: int, use_checkpoint: Tuple[bool, ...], *params: Tensor):  # type: ignore[override]
-        B, C, H, W = net.shape
-        M = B * H * W
-        gn_w, gn_b, w_in, b_in = params[:4]
-        w_out, b_out = params[-2:]
+    def forward(self, xt: Tensor, gn_w: Tensor, gn_b: Tensor, w_in: Tensor, b_in: Tensor) -> Tuple[Tensor, tuple]:
+        B, H, W, C = xt.shape
         L = w_in.shape[0]
-        xt = net.permute(0, 2, 3, 1).contiguous().view(B, H * W, C)  # a view when net is channels-last
         gn_w32, gn_b32 = gn_w.float().contiguous(), gn_b.float().contiguous()
-        yn, gm, gr = ops.groupnorm_silu_fwd(xt, gn_w32, gn_b32, GN_EPS, silu=False)
+        yn, gm, gr = ops.groupnorm_silu_fwd(xt.view(B, H * W, C), gn_w32, gn_b32, GN_EPS, silu=False)
         w_in_b = _bf(w_in.reshape(L, C))
-        t = ops.gemm(yn.view(M, C), w_in_b, bias=_bf(b_in))
-        c = _context_rows(context)
-        build = partial(_rows_build, B, heads)
-        kept_blocks: List = []
-        for i, ckpt in enumerate(use_checkpoint):
-            t, kept = checkpoint.run(build, (t, c, *params[4 + BLOCK_PARAMS * i: 4 + BLOCK_PARAMS * (i + 1)]), ckpt)
-            kept_blocks.append(kept)
-        w_out_b = _bf(w_out.reshape(C, L))
-        out = ops.gemm(t, w_out_b, bias=_bf(b_out), epilogue=ops.EPI_BIAS_RESID_BF16, aux=xt.view(M, C))
-        ctx.save_for_backward(xt, yn, gm, gr, gn_w32, gn_b32, w_in_b, t, w_out_b, *(s for kept in kept_blocks for s in kept))
-        ctx.meta = (B, C, H, W, L, heads, _context_meta(context), w_in.shape, w_out.shape, use_checkpoint,
-                    [len(kept) for kept in kept_blocks])
-        return out.view(B, H, W, C).permute(0, 3, 1, 2)
+        t = ops.gemm(yn.view(B * H * W, C), w_in_b, bias=_bf(b_in))
+        return t.view(B, H * W, L), (xt, yn, gm, gr, gn_w32, gn_b32, w_in_b)
 
-    @staticmethod
-    def backward(ctx, dout: Tensor):  # type: ignore[override]
-        saved = ctx.saved_tensors
-        xt, yn, gm, gr, gn_w32, gn_b32, w_in_b, t, w_out_b = saved[:9]
-        B, C, H, W, L, heads, context, w_in_shape, w_out_shape, use_checkpoint, sizes = ctx.meta
-        kept_blocks, start = [], 9
-        for n in sizes:
-            kept_blocks.append(saved[start:start + n])
-            start += n
-        M, dev = B * H * W, dout.device
-        dt = dout.permute(0, 2, 3, 1).to(torch.bfloat16).contiguous().view(M, C)
-        dw_out = ops.wgrad(dt, t, torch.empty((C, L), dtype=torch.float32, device=dev))
-        db_out = ops.colsum(dt, torch.empty(C, dtype=torch.float32, device=dev))
-        dtl = ops.gemm(dt, w_out_b, b_mn_major=True)
-        build = partial(_rows_build, B, heads)
-        block_grads: List[List[Tensor]] = []
-        dcs: List[Optional[Tensor]] = []
-        for kept, ckpt in zip(reversed(kept_blocks), reversed(use_checkpoint)):
-            s = checkpoint.rebuild(build, kept, ckpt)
-            dtl, dc, g = _block_backward(s, dtl, B, heads)
-            del s  # a rebuilt block's activations are released before the block below it is rebuilt
-            block_grads.insert(0, g)
-            dcs.append(dc)
+    def backward(self, saved: tuple, dout: Tensor) -> tuple:
+        xt, yn, gm, gr, gn_w32, gn_b32, w_in_b = saved
+        B, H, W, C = xt.shape
+        L, M, dev = w_in_b.shape[0], B * H * W, dout.device
+        dtl = _rows(dout)
         dw_in = ops.wgrad(dtl, yn.view(M, C), torch.empty((L, C), dtype=torch.float32, device=dev))
         db_in = ops.colsum(dtl, torch.empty(L, dtype=torch.float32, device=dev))
         dyn = ops.gemm(dtl, w_in_b, b_mn_major=True)
-        dxg, dgn_w, dgn_b = ops.groupnorm_silu_bwd(xt, dyn.view(B, H * W, C), gn_w32, gn_b32, gm, gr, silu=False)
-        dx = (dxg.view(M, C) + dt).view(B, H, W, C).permute(0, 3, 1, 2)  # GroupNorm path + the final residual, a bf16 add
-        flat = [g for gs in block_grads for g in gs]
-        return (dx, _context_grad(dcs, context), None, None, dgn_w, dgn_b, dw_in.view(w_in_shape), db_in, *flat,
-                dw_out.view(w_out_shape), db_out)
+        dxg, dgn_w, dgn_b = ops.groupnorm_silu_bwd(xt.view(B, H * W, C), dyn.view(B, H * W, C), gn_w32, gn_b32, gm, gr, silu=False)
+        return dxg, dgn_w, dgn_b, dw_in, db_in
+
+
+class _LatentOut:
+    """SpatialTransformerB200's from_latent and the residual as an op on (t [B, H*W, L], xt [B, H, W, C], from_latent w / b):
+    bf16(bf16(from_latent(t)) + xt) in the GEMM's epilogue, [B, C, H, W] with channels-last strides."""
+
+    def forward(self, t: Tensor, xt: Tensor, w_out: Tensor, b_out: Tensor) -> Tuple[Tensor, tuple]:
+        B, H, W, C = xt.shape
+        w_out_b = _bf(w_out.reshape(C, t.shape[-1]))
+        out = ops.gemm(_rows(t), w_out_b, bias=_bf(b_out), epilogue=ops.EPI_BIAS_RESID_BF16, aux=_rows(xt))
+        return out.view(B, H, W, C).permute(0, 3, 1, 2), (t, w_out_b)
+
+    def backward(self, saved: tuple, dout: Tensor) -> tuple:
+        t, w_out_b = saved
+        C, L = w_out_b.shape
+        dev = dout.device
+        dt = dout.permute(0, 2, 3, 1).to(torch.bfloat16).contiguous().view(-1, C)
+        dw_out = ops.wgrad(dt, _rows(t), torch.empty((C, L), dtype=torch.float32, device=dev))
+        db_out = ops.colsum(dt, torch.empty(C, dtype=torch.float32, device=dev))
+        return ops.gemm(dt, w_out_b, b_mn_major=True), dt, dw_out, db_out  # the residual's gradient is dt itself
 
 
 # ------------------------------------------------------------------------------------------------------------------------------
@@ -278,8 +220,10 @@ class SpatialTransformerBlockB200(nn.Module):
         return out
 
     def forward(self, net: Tensor, context: Optional[Tensor] = None) -> Tensor:
-        _check_input(net, "SpatialTransformerBlockB200")
-        return _BlockFn.apply(net, context, self.num_heads, self.use_checkpoint, *self._block_params())
+        _check_cuda("SpatialTransformerBlockB200", net, context)
+        if net.dtype != torch.bfloat16:
+            raise B200Error("SpatialTransformerBlockB200: the input must be bf16 (the residual stream of the UNet under bf16 autocast)")
+        return checkpoint.OpFn.apply(_BlockOp(net.shape[0], self.num_heads), self.use_checkpoint, net, context, *self._block_params())
 
 
 class SpatialTransformerB200(nn.Module):
@@ -306,10 +250,12 @@ class SpatialTransformerB200(nn.Module):
         self.from_latent = _Conv1x1Params(latent, in_channels, zero=True)
 
     def forward(self, net: Tensor, context: Optional[Tensor] = None) -> Tensor:
-        _check_input(net, "SpatialTransformerB200")
-        params = [self.norm.weight, self.norm.bias, self.to_latent.weight, self.to_latent.bias]
-        for b in self.blocks:
-            params += b._block_params()
-        params += [self.from_latent.weight, self.from_latent.bias]
-        use_checkpoint = tuple(bool(b.use_checkpoint) for b in self.blocks)
-        return _SpatialTransformerFn.apply(net, context, self.num_heads, use_checkpoint, *params)
+        _check_cuda("SpatialTransformerB200", net, context)
+        if net.dtype != torch.bfloat16:
+            raise B200Error("SpatialTransformerB200: the input must be bf16 (the residual stream of the UNet under bf16 autocast)")
+        # a view when net is channels-last; autograd adds xt's two gradients (GroupNorm path, residual) and the blocks' context ones
+        xt = net.permute(0, 2, 3, 1).contiguous()
+        t = checkpoint.OpFn.apply(_LatentIn(), False, xt, self.norm.weight, self.norm.bias, self.to_latent.weight, self.to_latent.bias)
+        for block in self.blocks:
+            t = block(t, context)
+        return checkpoint.OpFn.apply(_LatentOut(), False, t, xt, self.from_latent.weight, self.from_latent.bias)

@@ -21,15 +21,15 @@ embedding's weight / bias gradients from dt and dtime = silu_backward(bf16(dt . 
 intended difference from eager: the backward treats the clamp as the identity, where eager zeroes the gradient of an element
 whose sum overflowed bf16 (a block whose output overflows is already broken; the clamp only keeps the forward finite).
 
-``ResidualBlockWithTimeEmbeddingB200`` is the drop-in module: one ``autograd.Function`` that keeps its activations through
-``save_for_backward``, or with ``use_checkpoint=True`` keeps only its inputs and reruns the forward at the start of backward
-(``checkpoint.py``: the same gradients bit for bit, less memory held between forward and backward).  ``res_block_forward``
+``ResidualBlockWithTimeEmbeddingB200`` is the drop-in module: one ``checkpoint.OpFn`` node over ``res_block_fwd`` /
+``res_block_bwd`` that keeps their saved tensors, or with ``use_checkpoint=True`` keeps only its inputs and reruns the forward
+at the start of backward (the same gradients bit for bit, less memory held between forward and backward).  ``res_block_forward``
 runs the same forward on a state dict.  Up / down-sampling, the timestep MLP and the assembled UNet with its training step are
 the open part of row N3.
 """
 from __future__ import annotations
 
-from functools import partial
+from dataclasses import dataclass
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
@@ -38,7 +38,7 @@ from torch import Tensor, nn
 
 from . import checkpoint, ops
 from ._cabi import B200Error
-from .attention import _bf
+from .attention import _bf, _check_cuda
 
 MAX_CHANNELS = 2560  # GroupNorm kernels
 
@@ -144,26 +144,20 @@ def res_block_forward(sd: Dict[str, Tensor], prefix: str, net: Tensor, time_net:
 # ------------------------------------------------------------------------------------------------------------------------------
 # module
 # ------------------------------------------------------------------------------------------------------------------------------
-def _build(eps: float, net: Tensor, time_net: Optional[Tensor], *params: Optional[Tensor]) -> Tuple[Tensor, tuple]:
-    """The Function's forward on its inputs: (out [B, Cout, H, W] with channels-last strides, what ``res_block_bwd`` reads)."""
-    xt = net.permute(0, 2, 3, 1).contiguous()  # a view when net is channels-last
-    out, saved = res_block_fwd(xt, time_net, params, eps)
-    return out.permute(0, 3, 1, 2), saved
+@dataclass(frozen=True)
+class _ResBlockOp:
+    """ResidualBlockWithTimeEmbeddingB200 as a ``checkpoint.OpFn`` op on (net [B, Cin, H, W], time_net or None, *_params()):
+    the NHWC kernels on net's channels-last view, the output [B, Cout, H, W] and dx with channels-last strides."""
+    eps: float
 
+    def forward(self, net: Tensor, time_net: Optional[Tensor], *params: Optional[Tensor]) -> Tuple[Tensor, tuple]:
+        xt = net.permute(0, 2, 3, 1).contiguous()  # a view when net is channels-last
+        out, saved = res_block_fwd(xt, time_net, params, self.eps)
+        return out.permute(0, 3, 1, 2), saved
 
-class _ResBlockFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, net: Tensor, time_net: Optional[Tensor], eps: float, use_checkpoint: bool, *params: Optional[Tensor]):  # type: ignore[override]
-        ctx.eps, ctx.use_checkpoint = eps, use_checkpoint
-        out, kept = checkpoint.run(partial(_build, eps), (net, time_net, *params), use_checkpoint)
-        ctx.save_for_backward(*kept)
-        return out
-
-    @staticmethod
-    def backward(ctx, dout: Tensor):  # type: ignore[override]
-        saved = checkpoint.rebuild(partial(_build, ctx.eps), ctx.saved_tensors, ctx.use_checkpoint)
+    def backward(self, saved: tuple, dout: Tensor) -> tuple:
         dx, dtime, grads = res_block_bwd(saved, dout.permute(0, 2, 3, 1).to(torch.bfloat16).contiguous())
-        return (dx.permute(0, 3, 1, 2), dtime, None, None, *grads)
+        return (dx.permute(0, 3, 1, 2), dtime, *grads)
 
 
 class ResidualBlockWithTimeEmbeddingB200(nn.Module):
@@ -222,9 +216,7 @@ class ResidualBlockWithTimeEmbeddingB200(nn.Module):
             tdim = self.time_embedding.in_features
             if tuple(time_net.shape) != (B, tdim) or tdim % 8 != 0:
                 raise B200Error(f"{what}: time_net must be [B, {tdim}] with a width that is a multiple of 8")
-        for t in (net, time_net):
-            if t is not None and not t.is_cuda:
-                raise B200Error(f"{what} needs CUDA tensors (there is no CPU fallback)")
-            if t is not None and t.dtype != torch.bfloat16:
-                raise B200Error(f"{what}: net and time_net must be bf16 (the UNet's activations under bf16 autocast)")
-        return _ResBlockFn.apply(net, time_net, self.norm_eps, self.use_checkpoint, *self._params())
+        _check_cuda(what, net, time_net)
+        if any(t is not None and t.dtype != torch.bfloat16 for t in (net, time_net)):
+            raise B200Error(f"{what}: net and time_net must be bf16 (the UNet's activations under bf16 autocast)")
+        return checkpoint.OpFn.apply(_ResBlockOp(self.norm_eps), self.use_checkpoint, net, time_net, *self._params())

@@ -260,8 +260,8 @@ def test_checkpointed_block_holds_its_inputs_alone(which):
 
 @pytest.mark.gpu
 def test_checkpointed_transformer_holds_block_inputs_alone():
-    """The outer GroupNorm and 1x1 convolutions keep their 9 tensors; each checkpointed block keeps its token rows, the context
-    rows and its 20 parameters, nothing it computes."""
+    """The outer GroupNorm and 1x1 convolutions keep their 9 tensors; each checkpointed block keeps its tokens, the context and
+    its 20 parameters, nothing it computes."""
     layers = 2
     m, inputs, up = _transformer(320, 16, layers)
     _run(m, inputs, [up], True)
