@@ -261,6 +261,175 @@ def conv3x3_wgrad(dy, x):
     return dy.to(F64).t() @ cols
 
 
+def conv3x3_dgrad(dy, w):
+    """Input gradient of ``conv3x3`` for dy [B, H, W, Cout] and w [Cout, Cin, 3, 3]: [B H W, Cin]."""
+    B, H, W, _ = dy.shape
+    dx = F.conv_transpose2d(dy.to(F64).permute(0, 3, 1, 2), w.to(F64), padding=1)
+    return dx.permute(0, 2, 3, 1).reshape(B * H * W, -1)
+
+
+# ---- exact operands for the GEMM and the 3x3 convolution ---------------------------------------------------------------------------
+# bf16 operands that are small integers times a power of two per row of A and per column of B (per image and per output channel
+# for the convolution): every product of one output shares the unit 2^(row exponent + column exponent).  With sum_k |a_k b_k|
+# below EXACT_BUDGET units, every product and every partial sum -- in any order, in any adder of at least 23 bits that aligns or
+# truncates -- is an exact multiple of that unit, so the fp32 accumulator holds the float64 value exactly and the kernels' bf16
+# results are fixed to the bit.  The exponents stay inside fp32's normal range: no expected value depends on flush-to-zero.
+EXACT_BUDGET = 2 ** 22
+INT_BUDGET = 2 ** 20  # the random integers' share; a cancelling pair (products +-2^20) takes at most the other 2^21
+CANCEL = 2 ** 10      # operand magnitude of a cancelling pair
+
+
+def bf16(x):
+    """bf16 of x, rounded once to fp32 first: what a kernel's fp32 value becomes when it stores bf16."""
+    return x.to(torch.float32).to(torch.bfloat16)
+
+
+def exact_ints(shape, K, seed):
+    """Integers uniform in [-q, q], q in {1, 3, 7, 15} the largest with K q^2 <= INT_BUDGET (float64, CPU)."""
+    q = max(q for q in (1, 3, 7, 15) if K * q * q <= INT_BUDGET)
+    g = torch.Generator().manual_seed(seed)
+    return torch.randint(-q, q + 1, tuple(shape), generator=g).to(F64)
+
+
+def exact_scaled(ints, exp):
+    """bf16 ints * 2^exp (``exp`` broadcast to ``ints``), checked to be exact."""
+    v = ints * torch.exp2(torch.as_tensor(exp, dtype=F64))
+    out = v.to(torch.bfloat16)
+    assert torch.equal(out.to(F64), v), "operand not exact in bf16"
+    return out
+
+
+def exponents(n, lo, hi, seed):
+    """n exponents uniform in [lo, hi] (float64, CPU)."""
+    return torch.randint(lo, hi + 1, (n,), generator=torch.Generator().manual_seed(seed)).to(F64)
+
+
+def cancel_pairs(K, kind):
+    """k positions (+, -) of the cancelling pair: inside one k16 step, across the first two 64-deep k-blocks, or at the two ends of
+    the reduction (a split apart whenever there are two splits); None without cancellation."""
+    if kind is None:
+        return None
+    k = {"k16": (K - 16, K - 13) if K >= 16 else None, "kblock": (63, 64) if K > 64 else None, "split": (0, K - 1) if K > 1 else None}[kind]
+    assert k is not None, f"no {kind} cancellation at K = {K}"
+    return k
+
+
+def exact_operands(M, N, K, a_exp, b_exp, cancel=None, seed=0):
+    """A [M, K] and B [N, K] (bf16, CPU): integers times 2^a_exp[m] per row of A and 2^b_exp[n] per row of B.  ``cancel`` = (k+, k-,
+    ...): both columns of a pair in A hold 2^10, B holds +2^10 at k+ and -2^10 at k-, so every output gets products +2^20 and -2^20
+    units that cancel next to the small terms.  Asserts the exactness budget (one pair fits in it)."""
+    ia, ib = exact_ints((M, K), K, seed), exact_ints((N, K), K, seed + 1)
+    for kp, kn in zip(cancel[::2], cancel[1::2]) if cancel is not None else ():
+        ia[:, kp] = ia[:, kn] = CANCEL
+        ib[:, kp], ib[:, kn] = CANCEL, -CANCEL
+    worst = (ia.abs() @ ib.abs().t()).max().item()
+    assert worst < EXACT_BUDGET, f"sum |a b| = {worst} units, over the 2^22 budget"
+    return exact_scaled(ia, a_exp[:, None]), exact_scaled(ib, b_exp[:, None])
+
+
+def exact_conv_operands(B, H, W, Cin, Cout, x_exp, w_exp, seed=0):
+    """x [B, H, W, Cin] and w [Cout, Cin, 3, 3] (bf16, CPU) for ``conv3x3``: integers times 2^x_exp[b] per image and 2^w_exp[co] per
+    output channel.  Asserts the exactness budget over the 9 Cin products of every output."""
+    ix, iw = exact_ints((B, H, W, Cin), 9 * Cin, seed), exact_ints((Cout, Cin, 3, 3), 9 * Cin, seed + 1)
+    worst = conv3x3(ix.abs(), iw.abs()).max().item()
+    assert worst < EXACT_BUDGET, f"sum |x w| = {worst} units, over the 2^22 budget"
+    return exact_scaled(ix, x_exp[:, None, None, None]), exact_scaled(iw, w_exp[:, None, None, None])
+
+
+def exact_wgrad_operands(B, H, W, Cin, Cout, x_exp, dy_exp, seed=0):
+    """x [B, H, W, Cin] and dy [B H W, Cout] (bf16, CPU) for ``conv3x3_wgrad``: integers times 2^x_exp[ci] per input channel and
+    2^dy_exp[co] per output channel.  Asserts the exactness budget over the B H W products of every weight."""
+    ix, idy = exact_ints((B, H, W, Cin), B * H * W, seed), exact_ints((B * H * W, Cout), B * H * W, seed + 1)
+    worst = conv3x3_wgrad(idy.abs(), ix.abs()).max().item()
+    assert worst < EXACT_BUDGET, f"sum |dy x| = {worst} units, over the 2^22 budget"
+    return exact_scaled(ix, x_exp), exact_scaled(idy, dy_exp)
+
+
+# ---- the GEMM epilogues at their rounding points ------------------------------------------------------------------------------------
+GELU_ATOL = 2e-6  # the GEMM's fast erf is accurate to ~1e-7 absolute where GELU is nearly zero, per unit of the factor scaling it
+
+
+def gelu(x):
+    return 0.5 * x * (1.0 + torch.erf(x / math.sqrt(2.0)))
+
+
+def gelu_grad(x):
+    return 0.5 * (1.0 + torch.erf(x / math.sqrt(2.0))) + x * torch.exp(-0.5 * x * x) / math.sqrt(2.0 * math.pi)
+
+
+def splitk_ranges(K, splits):
+    """[k0, k1) of each split-K plane: the 64-deep k-blocks divided as evenly as the GEMM divides them, at most one split each."""
+    nkb = (K + 63) // 64
+    s = min(splits, nkb)
+    return [(nkb * sp // s * 64, min(K, nkb * (sp + 1) // s * 64)) for sp in range(s)]
+
+
+def gemm_t(acc, bias=None):
+    """t = bf16(acc + bias) as the GEMM rounds it: the fp32 sum of the fp32 accumulator and the bf16 bias, then bf16.  ``acc`` is the
+    exact float64 product (which the fp32 accumulator holds exactly on exact operands)."""
+    s = acc.to(F64) if bias is None else acc.to(F64) + bias.to(F64)
+    return bf16(s)
+
+
+def add_bf16(t, aux, clamp=False):
+    """bf16(float(t) + float(aux)) in fp32 (epilogues 9, 10, 11); ``clamp`` (11): +-inf become +-bf16 max, NaN stays."""
+    s = (t.float() + aux.float()).to(torch.bfloat16)
+    if clamp:
+        big = torch.finfo(torch.bfloat16).max
+        s = torch.where(torch.isinf(s), torch.where(s > 0, big, -big).to(torch.bfloat16), s)
+    return s
+
+
+def gemm_epilogue(epi, t, aux=None):
+    """The outputs of GEMM epilogue ``epi`` given t: bf16(acc + bias), or bf16(acc) for the backward epilogues 3, 6 and 8 (for 7, t is
+    hg [M, 2F]; for 8, da [M, F]).  ``aux``: the epilogue's aux rows (10: already one row per pixel).  Returns {name: (expected, tol)}:
+    tol None means bit for bit (bf16 or fp32 values); otherwise |got - expected| <= tol elementwise, float64, for the outputs that are
+    transcendental functions of t.  Their ulp counts are the ones the footprint and exhaustive GELU tests allow."""
+    td = t.to(F64)
+    u = 2.0 ** -7
+
+    def tol(ulps, ref, factor=1.0, mag=None):
+        return ulps * u * (ref.abs() if mag is None else mag) + GELU_ATOL * (factor.abs() if torch.is_tensor(factor) else factor)
+
+    if epi in (0, 1, 5, 7):
+        out = {"out0": (t, None)}
+        if epi == 1:
+            ref = gelu(td)
+            out["out1"] = (ref, tol(1, ref))
+        elif epi == 5:  # eager's three bf16 roundings: 1.702 h, sigmoid, the product
+            ref = td * bf16(torch.sigmoid(bf16(1.702 * td).to(F64))).to(F64)
+            out["out1"] = (ref, tol(2, ref))
+        elif epi == 7:
+            Fd = t.shape[1] // 2
+            h, gate = td[:, :Fd], td[:, Fd:]
+            ref = h * bf16(gelu(gate)).to(F64)
+            out["out1"] = (ref, tol(1, ref, h))
+        return out
+    if epi == 2:
+        return {"out0": (aux.float() + t.float(), None)}
+    if epi in (9, 10, 11):
+        return {"out0": (add_bf16(t, aux, clamp=epi == 11), None)}
+    h = aux.to(F64)
+    if epi == 3:
+        ref = td * gelu_grad(h)
+        return {"out0": (ref, tol(2, ref, td))}
+    if epi == 6:  # autograd of h * sigmoid(1.702 h) on bf16 tensors, one rounding per kernel; the two paths into h may cancel
+        s = bf16(torch.sigmoid(bf16(1.702 * h).to(F64))).to(F64)
+        gh1 = bf16(td * s).to(F64)
+        gt = bf16(bf16(bf16(td * h).to(F64) * bf16(1 - s).to(F64)).to(F64) * s).to(F64)
+        gh2 = bf16(1.702 * gt).to(F64)
+        ref = gh1 + gh2
+        return {"out0": (ref, tol(3, ref, td, gh1.abs() + gh2.abs()))}
+    if epi == 8:  # dh = bf16(da g), dgate = bf16(gelu'(gate) bf16(da h)), g = bf16(gelu(gate))
+        Fd = t.shape[1]
+        hh, gate = h[:, :Fd], h[:, Fd:]
+        dh = td * bf16(gelu(gate)).to(F64)
+        dgate = gelu_grad(gate) * bf16(td * hh).to(F64)
+        ref = torch.cat([dh, dgate], 1)
+        return {"out0": (ref, tol(2, ref, torch.cat([td, td * hh], 1)))}
+    raise ValueError(f"no reference for epilogue {epi}")
+
+
 def adam(p, g, m, v, steps, lr, b1, b2, eps, wd, grad_scale=1.0):
     """Adam with L2 weight decay (torch.optim.Adam's update) over the step numbers ``steps``: (params, exp_avg, exp_avg_sq)."""
     p, m, v = p.to(F64).clone(), m.to(F64).clone(), v.to(F64).clone()

@@ -21,8 +21,8 @@ import torch.nn.functional as F
 
 import cflearn_b200  # noqa: F401  (registers the package)
 from cflearn_b200 import _cabi
-from _refs import (adam, assert_ulp, attention_rows, conv3x3, conv3x3_wgrad, first_bad, groupnorm, layernorm, packed_attention, relerr,
-                   with_grads)
+from _refs import (adam, assert_ulp, attention_rows, bf16, conv3x3, conv3x3_wgrad, first_bad, gelu, gelu_grad, groupnorm, layernorm,
+                   packed_attention, relerr, with_grads)
 
 DEV = "cuda"
 GUARD_BYTES = 65536
@@ -192,10 +192,6 @@ def call(name, *args):
 # ------------------------------------------------------------------------------------------------------------------------
 # value checks (the float64 references of _refs.py, on the CPU)
 # ------------------------------------------------------------------------------------------------------------------------
-def bf16(x):
-    return x.to(torch.float32).to(torch.bfloat16)
-
-
 def assert_close(got, ref, what, rtol, atol_rel=0.0):
     g, r = got.double(), ref.double()
     tol = rtol * r.abs() + atol_rel * r.abs().max().clamp_min(1e-30) + 1e-30
@@ -219,14 +215,6 @@ def assert_equal(got, ref, what):
 def rand(shape, seed, scale=1.0, dtype=torch.bfloat16):
     g = torch.Generator().manual_seed(seed)
     return (torch.randn(*shape, generator=g, dtype=torch.float64) * scale).to(dtype)
-
-
-def gelu(x):
-    return 0.5 * x * (1.0 + torch.erf(x / math.sqrt(2.0)))
-
-
-def gelu_grad(x):
-    return 0.5 * (1.0 + torch.erf(x / math.sqrt(2.0))) + x * torch.exp(-0.5 * x * x) / math.sqrt(2.0 * math.pi)
 
 
 # ------------------------------------------------------------------------------------------------------------------------

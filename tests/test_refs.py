@@ -152,3 +152,58 @@ def test_attention_bounds():
         assert (bigger_v[0] >= base[0]).all() and (bigger_do[3] >= base[3]).all()
         assert torch.allclose(refs.attention_bounds(q, kk, 2 * vv, dout, scale, causal, q)[1][0], 2 * base[0], rtol=1e-12)
         assert torch.allclose(refs.attention_bounds(q, kk, vv, 2 * dout, scale, causal, q)[1][3], 2 * base[3], rtol=1e-12)
+
+
+def test_gemm_and_conv_references():
+    g = torch.Generator().manual_seed(3)
+    # the input gradient of the 3x3 convolution against autograd of F.conv2d
+    xc = torch.randn(2, 5, 6, 8, generator=g, dtype=F64, requires_grad=True)
+    w = torch.randn(4, 8, 3, 3, generator=g, dtype=F64)
+    y = F.conv2d(xc.permute(0, 3, 1, 2), w, padding=1)
+    dyc = torch.randn(y.shape, generator=g, dtype=F64)
+    y.backward(dyc)
+    assert torch.allclose(refs.conv3x3_dgrad(dyc.permute(0, 2, 3, 1), w), xc.grad.reshape(60, 8), rtol=1e-12, atol=1e-12)
+    # exact operands: bf16 ints times 2^exp per row, the cancelling pair in place, the budget enforced
+    ea, eb = refs.exponents(5, -20, 20, 1), refs.exponents(3, -20, 20, 2)
+    A, B = refs.exact_operands(5, 3, 100, ea, eb, cancel=refs.cancel_pairs(100, "kblock"))
+    assert (A[:, 63].double() == 2.0 ** (10 + ea)).all() and (B[:, 64].double() == -(2.0 ** (10 + eb))).all()
+    units = (A.double() * torch.exp2(-ea)[:, None]).abs() @ (B.double() * torch.exp2(-eb)[:, None]).abs().t()
+    assert units.max() < refs.EXACT_BUDGET and torch.equal(units, units.round())
+    x, wc = refs.exact_conv_operands(2, 4, 4, 64, 8, refs.exponents(2, -3, 3, 3), refs.exponents(8, -3, 3, 4))
+    assert x.dtype == wc.dtype == torch.bfloat16 and x.shape == (2, 4, 4, 64) and wc.shape == (8, 64, 3, 3)
+    xw, dyw = refs.exact_wgrad_operands(1, 8, 8, 64, 8, refs.exponents(64, -3, 3, 5), refs.exponents(8, -3, 3, 6)[None, :])
+    assert xw.shape == (1, 8, 8, 64) and dyw.shape == (64, 8)
+    assert refs.splitk_ranges(200, 5) == [(0, 64), (64, 128), (128, 192), (192, 200)]
+    # t = bf16(fp32(acc + bias)): ties go to even (257 -> 256, 259 -> 260); the fp32 rounding comes first (2^24 + 1 + 2^-30)
+    acc = torch.tensor([[257.0, 259.0, 2.0 ** 24 + 1]], dtype=F64)
+    t = refs.gemm_t(acc, torch.tensor([0.0, 0.0, 2.0 ** -30], dtype=torch.bfloat16))
+    assert t.float().tolist() == [[256.0, 260.0, 2.0 ** 24]]
+    # the bf16 adds and the clamp of epilogue 11
+    big = torch.finfo(torch.bfloat16).max
+    s = refs.add_bf16(torch.tensor([big, -big, 1.0, float("nan")]).to(torch.bfloat16), torch.tensor([big, -big, 2.0 ** -8, 0.0]).to(torch.bfloat16), clamp=True)
+    assert s[:3].float().tolist() == [big, -big, 1.0] and torch.isnan(s[3])
+    # the epilogues of functions of t against torch: GELU, dGELU, QuickGELU (eager's roundings on bf16 tensors), GEGLU and dGEGLU
+    tb = (torch.randn(6, 16, generator=g) * 2).to(torch.bfloat16)
+    hb = (torch.randn(6, 16, generator=g) * 2).to(torch.bfloat16)
+    out = refs.gemm_epilogue(1, tb)
+    assert torch.equal(out["out0"][0], tb) and out["out0"][1] is None
+    assert torch.allclose(out["out1"][0], F.gelu(tb.double()), rtol=1e-12, atol=1e-15)
+    hd = hb.double().requires_grad_(True)
+    F.gelu(hd).backward(tb.double())
+    assert torch.allclose(refs.gemm_epilogue(3, tb, hb)["out0"][0], hd.grad, rtol=1e-12, atol=1e-15)
+    eager = tb * torch.sigmoid(tb * 1.702)  # bf16 CPU tensors: one rounding per op
+    assert torch.equal(refs.bf16(refs.gemm_epilogue(5, tb)["out1"][0]), eager)
+    hq = hb.clone().requires_grad_(True)
+    (hq * torch.sigmoid(hq * 1.702)).backward(tb)
+    ref6, tol6 = refs.gemm_epilogue(6, tb, hb)["out0"]
+    assert ((hq.grad.double() - ref6).abs() <= tol6).all()
+    hg = torch.cat([tb, hb], 1)
+    ref7, _ = refs.gemm_epilogue(7, hg)["out1"]
+    assert torch.allclose(ref7, tb.double() * F.gelu(hb.double()).to(torch.bfloat16).double(), rtol=1e-12, atol=1e-15)
+    hgd = hg.double().requires_grad_(True)
+    (hgd[:, :16] * F.gelu(hgd[:, 16:])).backward(tb.double())
+    ref8, tol8 = refs.gemm_epilogue(8, tb, hg)["out0"]
+    assert ((ref8 - hgd.grad).abs() <= tol8).all()
+    aux = torch.randn(6, 16, generator=g)
+    assert torch.equal(refs.gemm_epilogue(2, tb, aux)["out0"][0], aux + tb.float())
+    assert torch.equal(refs.gemm_epilogue(9, tb, hb)["out0"][0], (tb.float() + hb.float()).to(torch.bfloat16))
