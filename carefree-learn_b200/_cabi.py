@@ -1,4 +1,4 @@
-"""ctypes binding of ``libb200_cflearn.so`` (the C-ABI declared in ``include/b200_cflearn.h``).
+"""ctypes binding of ``libb200_cflearn.so`` (the C-ABI declared in ``include/b200_cflearn.h`` and ``include/b200_cflearn_ext.h``).
 
 The library is the product: there is no CPU or PyTorch fallback.  Importing this module never raises (so the
 CPU test-suite can inspect the symbol table), but every compute entry point raises ``B200Error`` loudly when the
@@ -95,6 +95,16 @@ SIGNATURES: Dict[str, Any] = {
     "b200_comm_nccl_version": (c_int, []),
 }
 
+# The entry points declared in include/b200_cflearn_ext.h (after version 4 of the main header), exported by the same library.
+EXT_SIGNATURES: Dict[str, Any] = {
+    "b200_conv3x3_s2_nhwc_bf16": (c_int, [_P, _P, _P, _P, _P, _LL, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
+    "b200_conv3x3_s2_dgrad_nhwc_bf16": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
+    "b200_conv3x3_s2_wgrad_nhwc_bf16": (c_int, [_P, _LL, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
+    "b200_conv3x3_up2_nhwc_bf16": (c_int, [_P, _P, _P, _P, _P, _LL, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
+    "b200_upsample_nearest2x_bf16": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
+    "b200_sum2x2_bf16": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
+}
+
 _lib: Optional[ctypes.CDLL] = None
 _load_error: Optional[str] = None
 
@@ -111,7 +121,7 @@ def _load() -> None:
         return
     try:
         lib = ctypes.CDLL(LIB_PATH)
-        for name, (res, args) in SIGNATURES.items():
+        for name, (res, args) in {**SIGNATURES, **EXT_SIGNATURES}.items():
             fn = getattr(lib, name)
             fn.restype = res
             fn.argtypes = args
@@ -147,6 +157,10 @@ def lib() -> ctypes.CDLL:
 
 def exported_symbols() -> List[str]:
     return [name for name in SIGNATURES if hasattr(lib(), name)]
+
+
+def exported_ext_symbols() -> List[str]:
+    return [name for name in EXT_SIGNATURES if hasattr(lib(), name)]
 
 
 def last_error() -> str:

@@ -51,6 +51,6 @@ int configure_smem(Kernel kernel, int smem, bool (&configured)[64]) {
 }
 
 int make_tmap(CUtensorMap* out, const void* base, int elem_bytes, int rank, const uint64_t* dims,
-              const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes);
+              const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes, const uint32_t* elem_strides = nullptr);
 
 }  // namespace b200

@@ -40,6 +40,7 @@
 #include <utility>
 
 #include "b200_internal.h"
+#include "../../include/b200_cflearn_ext.h"
 #include "ptx.cuh"
 
 namespace b200 {
@@ -121,9 +122,62 @@ struct GemmParams {
     // an M tile is 128 consecutive pixels (whole image rows), k-block kb = (tap, 64-channel block), and the A tile of a tap is
     // the SAME box shifted by (kx - 1, ky - 1) -- TMA zero-fills what falls outside the image: the padding costs nothing
     int conv, conv_h, conv_w, conv_cin;
+    // The tap-to-box mapping and the output addressing of the convolution, by kind (CONV_*).  Its GEMM rows are one grid, or four
+    // parity classes of [B, conv_h, conv_w] pixels, class c at rows [c class_stride, c class_stride + class_rows) (class_stride:
+    // class_rows rounded up to whole tiles).  k-block (tap j, 64 channels) of class c loads the activation box at (x, y conv_ys)
+    // shifted by conv_tap(); a parity class writes grid pixel (b, m, n) of class c = (py, px) to output pixel (b, 2m + py, 2n + px)
+    // of a 2 conv_h x 2 conv_w image.  (Three ints: a larger parameter block costs the plain GEMMs' staging loop its unrolling.)
+    int conv_kind, class_rows, class_stride;
 };
 
+// CONV_S1 / CONV_S2: the nine taps of a 3x3 / padding 1 convolution at stride 1 / 2 (the activation map is then 2 conv_h x
+// 2 conv_w with element strides 2); CONV_UP2: the nearest-2x upsampling convolution, four classes of nine taps;
+// CONV_S2_DGRAD: the stride-2 input gradient, four classes of 1, 2, 2, 4 taps.
+enum : int { CONV_S1 = 1, CONV_S2 = 2, CONV_UP2 = 3, CONV_S2_DGRAD = 4 };
+
+__host__ __device__ __forceinline__ int conv_classes(int kind) { return kind >= CONV_UP2 ? 4 : 1; }
+__host__ __device__ __forceinline__ int conv_ys(int kind) { return kind == CONV_S2 ? 2 : 1; }
+// taps of class c, and the taps of the classes before it (the class's first B column in taps)
+__host__ __device__ __forceinline__ int conv_class_taps(int kind, int c) {
+    return kind == CONV_S2_DGRAD ? ((c >> 1) + 1) * ((c & 1) + 1) : 9;
+}
+__host__ __device__ __forceinline__ int conv_class_tap0(int kind, int c) { return kind == CONV_S2_DGRAD ? 2 * c - (c > 0) : 0; }
+
+// box offset (dx, dy) of tap j of class c
+__device__ __forceinline__ void conv_tap(int kind, int c, int j, int& dx, int& dy) {
+    const int py = c >> 1, px = c & 1;
+    if (kind == CONV_UP2) {  // upsampled row 2m + py + ky - 1 is x row m + floor((py + ky - 1) / 2); columns alike
+        dy = (py + j / 3 + 1) / 2 - 1;
+        dx = (px + j % 3 + 1) / 2 - 1;
+    } else if (kind == CONV_S2_DGRAD) {
+        // dx row 2m + py takes ky = 1 from dy row m (py = 0), or ky = 0 from row m + 1 and ky = 2 from row m (py = 1); columns
+        // alike.  Taps in row-major (ky, kx) order.
+        const int nx = px + 1, jy = j / nx, jx = j - jy * nx;
+        dy = py && jy == 0 ? 1 : 0;
+        dx = px && jx == 0 ? 1 : 0;
+    } else {
+        dy = j / 3 - 1;
+        dx = j % 3 - 1;
+    }
+}
+
+// Output row of GEMM row `row`: itself, or its pixel of the 2x-sized image under a parity-class scatter.
+__device__ __forceinline__ long long conv_out_row(const GemmParams& p, int row) {
+    if (conv_classes(p.conv_kind) == 1) return row;
+    const int c = row / p.class_stride, q = row - c * p.class_stride;
+    const int n = q % p.conv_w, t = q / p.conv_w, m = t % p.conv_h, b = t / p.conv_h;
+    return (static_cast<long long>(b) * 2 * p.conv_h + 2 * m + (c >> 1)) * (2 * p.conv_w) + 2 * n + (c & 1);
+}
+
+// Rows of m tile m_t the epilogue writes (a parity class ends inside its last tile).
+__device__ __forceinline__ int tile_rows(const GemmParams& p, int m_t) {
+    const int m0 = m_t * BM;
+    if (conv_classes(p.conv_kind) == 1) return min(BM, p.M - m0);
+    return min(BM, p.class_rows - (m0 - (m0 / p.class_stride) * p.class_stride));
+}
+
 // Work unit u -> (m tile, n tile, split, k-block range).  Consecutive units share the m tile (A stays in L2).
+template <bool CONV>
 __device__ __forceinline__ void decode_unit(const GemmParams& p, int u, int& m_t, int& n_t, int& sp, int& kb0, int& kb1) {
     n_t = u % p.num_n_tiles;
     int r = u / p.num_n_tiles;
@@ -131,6 +185,9 @@ __device__ __forceinline__ void decode_unit(const GemmParams& p, int u, int& m_t
     m_t = r / p.splits;
     kb0 = static_cast<int>((static_cast<long long>(p.num_kb) * sp) / p.splits);
     kb1 = static_cast<int>((static_cast<long long>(p.num_kb) * (sp + 1)) / p.splits);
+    if constexpr (CONV) {
+        if (conv_classes(p.conv_kind) > 1) kb1 = conv_class_taps(p.conv_kind, (m_t * BM) / p.class_stride) * (p.conv_cin / BK);  // (one split)
+    }
 }
 
 // one k-block (BK = 64 = four k16 steps) of this warpgroup's 64 x 256 accumulator; scale_d = 0 on a unit's first k-block
@@ -160,9 +217,9 @@ __device__ __forceinline__ void store_partial_pair(const GemmParams& p, int sp, 
 // n_ok: how many of the 8 columns are inside N (8 on every interior chunk).  Element for element the same arithmetic as
 // the per-pair epilogue it replaces, so results are bit-identical.  h8 (dGELU / dQuickGELU only): the chunk's h when n_ok == 8,
 // loaded by the caller rows ahead (see the epilogue loop).
-template <int EPI, bool QUICK>
+template <int EPI, bool QUICK, bool CONV>
 __device__ __forceinline__ void epi_chunk(const GemmParams& p, int row, int col, const uint32_t (&t)[4], int n_ok, const uint4& h8) {
-    const long long off = static_cast<long long>(row) * p.ldo + col;
+    const long long off = (CONV ? conv_out_row(p, row) : row) * p.ldo + col;
     uint32_t o[4];  // the bf16 output (out0) of the bf16 variants
     if constexpr (EPI == EPI_BIAS_BF16) {
 #pragma unroll
@@ -209,7 +266,8 @@ __device__ __forceinline__ void epi_chunk(const GemmParams& p, int row, int col,
     } else if constexpr (EPI == EPI_BIAS_RESID_BF16 || EPI == EPI_BIAS_ADD_PER_IMAGE_BF16 || EPI == EPI_BIAS_RESID_CLAMP_BF16) {
         // out0(bf16) = bf16(float(bf16(acc + bias)) + float(aux(bf16)))     (aux may alias out0)
         // per image: aux is a [B, ldo] table, one row per image of the convolution (a 128-row tile may hold two images)
-        const long long aux_off = EPI == EPI_BIAS_ADD_PER_IMAGE_BF16 ? static_cast<long long>(row / (p.conv_h * p.conv_w)) * p.ldo + col : off;
+        const int grid_row = CONV && conv_classes(p.conv_kind) > 1 ? row % p.class_stride : row;
+        const long long aux_off = EPI == EPI_BIAS_ADD_PER_IMAGE_BF16 ? static_cast<long long>(grid_row / (p.conv_h * p.conv_w)) * p.ldo + col : off;
         const __nv_bfloat16* src = reinterpret_cast<const __nv_bfloat16*>(p.aux) + aux_off;
         uint32_t rw[4] = {0u, 0u, 0u, 0u};
         if (n_ok == 8) {
@@ -313,7 +371,9 @@ __device__ __forceinline__ uint32_t staging_offset(int r, int chunk) {
 // QUICK (GELU / dGELU variants only): QuickGELU instead of the exact erf GELU.  A template parameter, not a runtime flag,
 // so the other variants carry none of its registers.
 // TA / TB: 1 = that operand is MN-major.
-template <int EPI, bool QUICK, int TA, int TB>
+// CONV: the forward / input-gradient convolution entries (A behind the 4-D tap map, parity classes, scattered output rows); a
+// separate instantiation, so the plain GEMMs carry none of its addressing.
+template <int EPI, bool QUICK, int TA, int TB, bool CONV>
 __global__ void __launch_bounds__(GemmCfg<EPI>::THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
     using Cfg = GemmCfg<EPI>;
@@ -352,10 +412,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             uint32_t sphase = 0;
             for (int u = blockIdx.x; u < total_units; u += gridDim.x) {
                 int m_t, n_t, sp, kb0, kb1;
-                decode_unit(p, u, m_t, n_t, sp, kb0, kb1);
+                decode_unit<CONV>(p, u, m_t, n_t, sp, kb0, kb1);
                 const int col = n_t * BN + lane * 8;
                 const int n_ok = min(8, max(0, (kEpi[EPI].cols == COLS_F ? p.N >> 1 : p.N) - col));
-                const int rows = min(BM, p.M - m_t * BM);
+                const int rows = CONV ? tile_rows(p, m_t) : min(BM, p.M - m_t * BM);
                 if constexpr (kEpi[EPI].aux == AUX_ROWS_BF16 || kEpi[EPI].aux == AUX_ROWS_F32) {
                     // pull the tile's aux rows into L2 while its MMAs still run: three warps cannot hide HBM latency alone.
                     // Rows are 16-byte aligned and padded to ldo >= the 16-byte-rounded width, so no byte past a row is named.
@@ -364,11 +424,11 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                     const uint32_t bytes = static_cast<uint32_t>((min(BN, p.N - n0) * eb + 15) & ~15);
                     const uint8_t* aux = reinterpret_cast<const uint8_t*>(p.aux);
                     for (int r = threadIdx.x - 9 * 32; r < rows; r += 32 * Cfg::EPI_WARPS)
-                        bulk_prefetch_l2(aux + (static_cast<long long>(m_t * BM + r) * p.ldo + n0) * eb, bytes);
+                        bulk_prefetch_l2(aux + ((CONV ? conv_out_row(p, m_t * BM + r) : m_t * BM + r) * p.ldo + n0) * eb, bytes);
                 }
                 if constexpr (kEpi[EPI].aux == AUX_IMAGE_BF16) {  // the table has one row per image: prefetch the tile's images
-                    const int hw = p.conv_h * p.conv_w, n0 = n_t * BN;
-                    const int img0 = (m_t * BM) / hw, img1 = (m_t * BM + rows - 1) / hw;
+                    const int hw = p.conv_h * p.conv_w, n0 = n_t * BN, q0 = CONV ? (m_t * BM) % p.class_stride : m_t * BM;
+                    const int img0 = q0 / hw, img1 = (q0 + rows - 1) / hw;
                     const uint32_t bytes = static_cast<uint32_t>((min(BN, p.N - n0) * 2 + 15) & ~15);
                     const uint8_t* aux = reinterpret_cast<const uint8_t*>(p.aux);
                     for (int b = img0 + threadIdx.x - 9 * 32; b <= img1; b += 32 * Cfg::EPI_WARPS)
@@ -420,7 +480,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                                 if (n_ok == 8 && rn < rows) hq[i] = *reinterpret_cast<const uint4*>(hrows + static_cast<long long>(rn) * p.ldo);
                                 const uint4 v = *reinterpret_cast<const uint4*>(staging + staging_offset(r, lane));
                                 const uint32_t t[4] = {v.x, v.y, v.z, v.w};
-                                if (n_ok > 0) epi_chunk<EPI, QUICK>(p, m_t * BM + r, col, t, n_ok, h8);
+                                if (n_ok > 0) epi_chunk<EPI, QUICK, CONV>(p, m_t * BM + r, col, t, n_ok, h8);
                             }
                         }
                     }
@@ -430,7 +490,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                     for (int r = warp - 9; r < rows; r += Cfg::EPI_WARPS) {
                         const uint4 v = *reinterpret_cast<const uint4*>(staging + staging_offset(r, lane));
                         const uint32_t t[4] = {v.x, v.y, v.z, v.w};
-                        if (n_ok > 0) epi_chunk<EPI, QUICK>(p, m_t * BM + r, col, t, n_ok, make_uint4(0u, 0u, 0u, 0u));
+                        if (n_ok > 0) epi_chunk<EPI, QUICK, CONV>(p, m_t * BM + r, col, t, n_ok, make_uint4(0u, 0u, 0u, 0u));
                     }
                 }
                 mbar_arrive(staging_empty);
@@ -449,20 +509,22 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             uint32_t phase = 0;
             for (int u = blockIdx.x; u < total_units; u += gridDim.x) {
                 int m_t, n_t, sp, kb0, kb1;
-                decode_unit(p, u, m_t, n_t, sp, kb0, kb1);
+                decode_unit<CONV>(p, u, m_t, n_t, sp, kb0, kb1);
                 const int m0 = m_t * BM, n0 = n_t * BN;
                 for (int kb = kb0; kb < kb1; ++kb) {
                     mbar_wait(&empty_bar[stage], phase ^ 1u);
                     uint8_t* a_dst = sA + stage * A_STAGE_BYTES;
                     uint8_t* b_dst = sB + stage * B_STAGE_BYTES;
                     mbar_expect_tx(&full_bar[stage], A_STAGE_BYTES + B_STAGE_BYTES);
-                    if (p.conv == 1) {
+                    const int cls = CONV ? m0 / p.class_stride : 0;
+                    if constexpr (CONV) {
                         const int cpb = p.conv_cin / BK;
                         const int tap = kb / cpb, c0 = (kb - tap * cpb) * BK;
-                        const int ky = tap / 3, kx = tap - ky * 3;
-                        const int hw = p.conv_h * p.conv_w;
-                        const int bimg = m0 / hw, y0 = (m0 - bimg * hw) / p.conv_w;
-                        tma_load_4d(a_dst, &tmA, &full_bar[stage], c0, kx - 1, y0 + ky - 1, bimg);
+                        const int hw = p.conv_h * p.conv_w, q0 = m0 - cls * p.class_stride;
+                        const int bimg = q0 / hw, y0 = (q0 - bimg * hw) / p.conv_w;
+                        int dx, dy;
+                        conv_tap(p.conv_kind, cls, tap, dx, dy);
+                        tma_load_4d(a_dst, &tmA, &full_bar[stage], c0, dx, y0 * conv_ys(p.conv_kind) + dy, bimg);
                     } else if constexpr (!TA) {
                         tma_load_2d(a_dst, &tmA, &full_bar[stage], kb * BK, m0);
                     } else {
@@ -481,14 +543,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                             const int tap = n / p.conv_cin, c0 = n - tap * p.conv_cin;
                             const int ky = tap / 3, kx = tap - ky * 3;
                             // (boxes past N = 9 Cin: tap >= 9 lands outside the image -> zero fill, bytes still credited)
-                            tma_load_4d(b_dst + i * MN_BOX_BYTES, &tmB, &full_bar[stage], c0, kx - 1, tap < 9 ? y0 + ky - 1 : -65536, bimg);
+                            tma_load_4d(b_dst + i * MN_BOX_BYTES, &tmB, &full_bar[stage], c0, kx - 1, tap < 9 ? y0 * conv_ys(p.conv_kind) + ky - 1 : -65536, bimg);
                         }
                     } else if constexpr (kEpi[EPI].cols == COLS_F_PAIRED) {
                         // W1 behind a 3-D map {K, F, 2}: one box = 128 h rows then the matching 128 gate rows (rows past F
                         // zero-filled), so the B tile holds [h | gate] of the same 128 columns
                         tma_load_3d(b_dst, &tmB, &full_bar[stage], kb * BK, n_t * (BN / 2), 0);
                     } else if constexpr (!TB) {
-                        tma_load_2d(b_dst, &tmB, &full_bar[stage], kb * BK, n0);
+                        tma_load_2d(b_dst, &tmB, &full_bar[stage], ((CONV ? conv_class_tap0(p.conv_kind, cls) * (p.conv_cin / BK) : 0) + kb) * BK, n0);
                     } else {
 #pragma unroll
                         for (int i = 0; i < BN / 64; ++i)
@@ -511,7 +573,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     uint32_t phase = 0, sphase = 0;
     for (int u = blockIdx.x; u < total_units; u += gridDim.x) {
         int m_t, n_t, sp, kb0, kb1;
-        decode_unit(p, u, m_t, n_t, sp, kb0, kb1);
+        decode_unit<CONV>(p, u, m_t, n_t, sp, kb0, kb1);
         float acc[128];
         int prev = -1;
         for (int kb = kb0; kb < kb1; ++kb) {
@@ -626,7 +688,7 @@ static int ensure_current_context() {
 
 // rank-2/3 tiled map; dims/box innermost first; strides in BYTES for dims 1.. (rank-1 entries)
 int make_tmap(CUtensorMap* out, const void* base, int elem_bytes, int rank, const uint64_t* dims,
-              const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes) {
+              const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes, const uint32_t* elem_strides) {
     PFN_encodeTiled fn = get_encode_fn();
     if (!fn) return set_error(B200_ERR_DRIVER, "cuTensorMapEncodeTiled entry point unavailable");
     CUtensorMapDataType dt = elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
@@ -641,7 +703,7 @@ int make_tmap(CUtensorMap* out, const void* base, int elem_bytes, int rank, cons
     for (int i = 0; i < rank; ++i) {
         gdim[i] = dims[i];
         bx[i] = box[i];
-        es[i] = 1;
+        es[i] = elem_strides != nullptr ? elem_strides[i] : 1;
     }
     for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_bytes[i];
     if (!aligned(16, {base})) return set_error(B200_ERR_ALIGN, "tensor base not 16 B aligned");
@@ -701,12 +763,12 @@ extern "C" int b200_set_persistent_ctas(int n, int launches) {
 // only recorded and returned.
 static int g_gemm_multicast = 0;
 
-template <int EPI, bool QUICK, int TA, int TB>
+template <int EPI, bool QUICK, int TA, int TB, bool CONV = false>
 static int launch_gemm_impl(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int grid, cudaStream_t stream) {
     using Cfg = GemmCfg<EPI>;
     static bool configured[64] = {};
-    if (const int rc = configure_smem(gemm_bf16_kernel<EPI, QUICK, TA, TB>, Cfg::SMEM_BYTES, configured)) return rc;
-    gemm_bf16_kernel<EPI, QUICK, TA, TB><<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
+    if (const int rc = configure_smem(gemm_bf16_kernel<EPI, QUICK, TA, TB, CONV>, Cfg::SMEM_BYTES, configured)) return rc;
+    gemm_bf16_kernel<EPI, QUICK, TA, TB, CONV><<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(B200_ERR_LAUNCH, cudaGetErrorString(e));
     count_launch(1);
@@ -729,6 +791,20 @@ constexpr std::array<std::array<GemmLauncher, 4>, sizeof...(P)> launcher_table(s
 
 // indexed by (public epilogue, 2 TA + TB)
 static constexpr auto kLaunch = launcher_table(std::make_integer_sequence<int, kNumEpi>{});
+
+// the convolution-forward instance of public epilogue P (operands (0, 0)), or nullptr where the convolutions do not offer it
+template <int P>
+constexpr GemmLauncher conv_launcher() {
+    if constexpr ((kEpi[P].entries & ENTRY_CONV3X3) != 0) return &launch_gemm_impl<kEpi[P].kernel, kEpi[P].quick, 0, 0, true>;
+    else return nullptr;
+}
+
+template <int... P>
+constexpr std::array<GemmLauncher, sizeof...(P)> conv_launcher_table(std::integer_sequence<int, P...>) {
+    return {{conv_launcher<P>()...}};
+}
+
+static constexpr auto kLaunchConv = conv_launcher_table(std::make_integer_sequence<int, kNumEpi>{});
 
 }  // namespace b200
 
@@ -761,7 +837,9 @@ extern "C" int b200_gemm_pick_splits(int M, int N, int K) {
     return best;
 }
 
-struct ConvGeom { int B, H, W, Cin, mode; };  // mode 1: forward / input gradient (A behind the 4-D map); 2: weight gradient (B)
+// mode 1: forward / input gradient (A behind the 4-D map); 2: weight gradient (B).  B, H, W: the grid of the GEMM rows (mode 1) or
+// of the reduction's pixels (mode 2); kind: CONV_* (the activation is 2H x 2W for CONV_S2).
+struct ConvGeom { int B, H, W, Cin, mode, kind; };
 
 // Every argument check of the GEMM entries, before any tensor map is encoded: a call is refused the same way with or without
 // a device.  conv_fwd: the call comes from b200_conv3x3_nhwc_bf16.
@@ -813,11 +891,13 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
             // channels-last activation [B, H, W, Cin]: dims {Cin, W, H, B}; box = 64 channels x 128 consecutive pixels
             const int hb = cg->H < BM / cg->W ? cg->H : BM / cg->W;      // image rows per tile
             const int nb = BM / (cg->W * hb);                             // images per tile (> 1 only when H * W < 128)
-            uint64_t d4[4] = {static_cast<uint64_t>(cg->Cin), static_cast<uint64_t>(cg->W), static_cast<uint64_t>(cg->H), static_cast<uint64_t>(cg->B)};
-            uint64_t s4[3] = {static_cast<uint64_t>(cg->Cin) * 2, static_cast<uint64_t>(cg->W) * cg->Cin * 2,
-                              static_cast<uint64_t>(cg->H) * cg->W * cg->Cin * 2};
-            uint32_t b4[4] = {BK, static_cast<uint32_t>(cg->W), static_cast<uint32_t>(hb), static_cast<uint32_t>(nb)};
-            if ((rc = make_tmap(&tmA, A, 2, 4, d4, s4, b4, 128)) != 0) return rc;
+            const uint32_t st = conv_ys(cg->kind);
+            const uint64_t sw = st * static_cast<uint64_t>(cg->W), sh = st * static_cast<uint64_t>(cg->H);
+            uint64_t d4[4] = {static_cast<uint64_t>(cg->Cin), sw, sh, static_cast<uint64_t>(cg->B)};
+            uint64_t s4[3] = {static_cast<uint64_t>(cg->Cin) * 2, sw * cg->Cin * 2, sh * sw * cg->Cin * 2};
+            uint32_t b4[4] = {BK, static_cast<uint32_t>(sw), st * hb, static_cast<uint32_t>(nb)};
+            const uint32_t es[4] = {1, st, st, 1};
+            if ((rc = make_tmap(&tmA, A, 2, 4, d4, s4, b4, 128, es)) != 0) return rc;
         } else {
         if (!a_mn) { d[0] = K; d[1] = M; bx[0] = BK; bx[1] = BM; }
         else       { d[0] = M; d[1] = K; bx[0] = 64; bx[1] = BK; }
@@ -827,11 +907,13 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
         if (cg != nullptr && cg->mode == 2) {
             // weight gradient: the activation as the MN-major B operand, box = 64 channels x 64 consecutive pixels (one k-block)
             const int hb = BK / cg->W;
-            uint64_t d4[4] = {static_cast<uint64_t>(cg->Cin), static_cast<uint64_t>(cg->W), static_cast<uint64_t>(cg->H), static_cast<uint64_t>(cg->B)};
-            uint64_t s4[3] = {static_cast<uint64_t>(cg->Cin) * 2, static_cast<uint64_t>(cg->W) * cg->Cin * 2,
-                              static_cast<uint64_t>(cg->H) * cg->W * cg->Cin * 2};
-            uint32_t b4[4] = {64, static_cast<uint32_t>(cg->W), static_cast<uint32_t>(hb), 1};
-            if ((rc = make_tmap(&tmB, B, 2, 4, d4, s4, b4, 128)) != 0) return rc;
+            const uint32_t st = conv_ys(cg->kind);
+            const uint64_t sw = st * static_cast<uint64_t>(cg->W), sh = st * static_cast<uint64_t>(cg->H);
+            uint64_t d4[4] = {static_cast<uint64_t>(cg->Cin), sw, sh, static_cast<uint64_t>(cg->B)};
+            uint64_t s4[3] = {static_cast<uint64_t>(cg->Cin) * 2, sw * cg->Cin * 2, sh * sw * cg->Cin * 2};
+            uint32_t b4[4] = {64, static_cast<uint32_t>(sw), st * hb, 1};
+            const uint32_t es[4] = {1, st, st, 1};
+            if ((rc = make_tmap(&tmB, B, 2, 4, d4, s4, b4, 128, es)) != 0) return rc;
         } else if (e.cols == COLS_F_PAIRED) {
             // W1 [2F, ldb] as {K, F, 2}: one box is 128 rows of the h half and the same 128 rows of the gate half
             const uint64_t F = static_cast<uint64_t>(n_cols);
@@ -846,13 +928,20 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
         if ((rc = make_tmap(&tmB, B, 2, 2, d, s, bx, 128)) != 0) return rc;
         }
     }
-    GemmParams p;
+    GemmParams p{};
     p.conv = cg != nullptr ? cg->mode : 0;
     p.conv_h = cg != nullptr ? cg->H : 0;
     p.conv_w = cg != nullptr ? cg->W : 0;
     p.conv_cin = cg != nullptr ? cg->Cin : 0;
     p.M = M; p.N = N; p.K = K;
     p.num_m_tiles = (M + BM - 1) / BM;
+    p.conv_kind = cg != nullptr ? cg->kind : 0;
+    p.class_rows = M;
+    p.class_stride = p.num_m_tiles * BM;
+    if (cg != nullptr && conv_classes(cg->kind) > 1) {  // M = 4 class_stride
+        p.class_rows = cg->B * cg->H * cg->W;
+        p.class_stride = M / 4;
+    }
     const int tile_n = e.cols == COLS_F_PAIRED ? BN / 2 : BN;
     p.num_n_tiles = (n_cols + tile_n - 1) / tile_n;
     p.splits = splits;
@@ -866,6 +955,7 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
     int grid = persistent_ctas();
     if (max_ctas > 0 && max_ctas < grid) grid = max_ctas;
     if (units < grid) grid = static_cast<int>(units);
+    if (cg != nullptr && cg->mode == 1) return kLaunchConv[epilogue](tmA, tmB, p, grid, stream);  // (admitted by check_gemm_args)
     return kLaunch[epilogue][2 * a_mn + b_mn](tmA, tmB, p, grid, stream);
 }
 
@@ -891,7 +981,7 @@ extern "C" int b200_conv3x3_nhwc_bf16(const void* x, const void* w_packed, const
     if (W > BM || BM % W != 0) return refuse(B200_ERR_ARG, "conv3x3", "the image width must divide 128");
     const int hb = H < BM / W ? H : BM / W;
     if (H % hb != 0 || BM % (W * hb) != 0) return refuse(B200_ERR_ARG, "conv3x3", "H must be a multiple of 128 / W (or H * W must divide 128)");
-    ConvGeom cg{B, H, W, Cin, 1};
+    const ConvGeom cg{B, H, W, Cin, 1, CONV_S1};
     const long long M = static_cast<long long>(B) * H * W;
     if (M > 0x7fffffffll) return refuse(B200_ERR_ARG, "conv3x3", "too many pixels");
     return gemm_dispatch(x, Cin, 0, w_packed, 9ll * Cin, 0, static_cast<int>(M), Cout, 9 * Cin, epilogue, bias, out0, nullptr, aux, ldo, 1, 0,
@@ -911,7 +1001,66 @@ extern "C" int b200_conv3x3_wgrad_nhwc_bf16(const void* dy, long long ld_dy, con
     if ((static_cast<long long>(H) * W) % BK != 0) return refuse(B200_ERR_ARG, "conv3x3 wgrad", "H * W must be a multiple of 64");
     const long long K = static_cast<long long>(B) * H * W;
     if (K > 0x7fffffffll) return refuse(B200_ERR_ARG, "conv3x3 wgrad", "too many pixels");
-    ConvGeom cg{B, H, W, Cin, 2};
+    const ConvGeom cg{B, H, W, Cin, 2, CONV_S1};
     return gemm_dispatch(dy, ld_dy, 1, x, Cin, 1, Cout, 9 * Cin, static_cast<int>(K), EPI_PARTIAL_F32, nullptr, partials, nullptr, nullptr,
                          9ll * Cin, splits, 0, stream, &cg);
+}
+
+// ------------------------------------------------------------------------------------------------
+// resampling convolutions (include/b200_cflearn_ext.h): the same main loop with other tap tables and output addressing
+// ------------------------------------------------------------------------------------------------
+// The size checks every resampling entry shares.  (H, W) is the lower-resolution side; (h, w) the grid the GEMM tiles;
+// red / outc: the reduction's and the output's channels.
+static int check_resample(const char* entry, int B, int H, int W, int red, int outc, bool even, int h, int w) {
+    if (B <= 0 || H <= 0 || W <= 0 || red <= 0 || outc <= 0) return refuse(B200_ERR_ARG, entry, "non-positive size");
+    if (even && (H % 2 != 0 || W % 2 != 0)) return refuse(B200_ERR_ARG, entry, "H and W must be even");
+    if (red % BK != 0) return refuse(B200_ERR_ARG, entry, "the reduction's channel count must be a multiple of 64");
+    if (outc % 8 != 0) return refuse(B200_ERR_ARG, entry, "the output's channel count must be a multiple of 8");
+    if (w > BM || BM % w != 0) return refuse(B200_ERR_ARG, entry, "the grid width must divide 128");
+    const int hb = h < BM / w ? h : BM / w;
+    if (h % hb != 0 || BM % (w * hb) != 0) return refuse(B200_ERR_ARG, entry, "the grid height must be a multiple of 128 / width (or height * width must divide 128)");
+    if (4ll * B * (2 * H) * (2 * W) > 0x7fffffffll) return refuse(B200_ERR_ARG, entry, "too many pixels");
+    return 0;
+}
+
+// four parity classes of a [B, h, w] grid, each padded to whole tiles: the GEMM's M
+static int class_m(const ConvGeom& g) {
+    const long long rows = static_cast<long long>(g.B) * g.H * g.W;
+    return static_cast<int>(4 * ((rows + BM - 1) / BM) * BM);
+}
+
+extern "C" int b200_conv3x3_s2_nhwc_bf16(const void* x, const void* w_packed, const void* bias, void* out0, const void* aux, long long ldo,
+                                         int B, int H, int W, int Cin, int Cout, int epilogue, cudaStream_t stream) {
+    if (const int rc = check_resample("conv3x3_s2", B, H, W, Cin, Cout, true, H / 2, W / 2)) return rc;
+    const ConvGeom cg{B, H / 2, W / 2, Cin, 1, CONV_S2};
+    return gemm_dispatch(x, Cin, 0, w_packed, 9ll * Cin, 0, B * (H / 2) * (W / 2), Cout, 9 * Cin, epilogue, bias, out0, nullptr, aux, ldo,
+                         1, 0, stream, &cg);
+}
+
+extern "C" int b200_conv3x3_s2_dgrad_nhwc_bf16(const void* dy, const void* w_dgrad, void* dx, int B, int H, int W, int Cin, int Cout,
+                                               cudaStream_t stream) {
+    if (const int rc = check_resample("conv3x3_s2 dgrad", B, H, W, Cout, Cin, true, H / 2, W / 2)) return rc;
+    const ConvGeom cg{B, H / 2, W / 2, Cout, 1, CONV_S2_DGRAD};
+    return gemm_dispatch(dy, Cout, 0, w_dgrad, 9ll * Cout, 0, class_m(cg), Cin, 9 * Cout, EPI_BIAS_BF16, nullptr, dx, nullptr, nullptr, Cin,
+                         1, 0, stream, &cg);
+}
+
+extern "C" int b200_conv3x3_s2_wgrad_nhwc_bf16(const void* dy, long long ld_dy, const void* x, void* partials, int B, int H, int W, int Cin,
+                                               int Cout, int splits, cudaStream_t stream) {
+    const char* what = "conv3x3_s2 wgrad";
+    if (const int rc = check_resample(what, B, H, W, Cin, Cout, true, H / 2, W / 2)) return rc;
+    const int h = H / 2, w = W / 2;
+    if (w > BK || BK % w != 0) return refuse(B200_ERR_ARG, what, "the grid width must divide 64");
+    if ((h * w) % BK != 0) return refuse(B200_ERR_ARG, what, "the grid's height * width must be a multiple of 64");
+    const ConvGeom cg{B, h, w, Cin, 2, CONV_S2};
+    return gemm_dispatch(dy, ld_dy, 1, x, Cin, 1, Cout, 9 * Cin, B * h * w, EPI_PARTIAL_F32, nullptr, partials, nullptr, nullptr, 9ll * Cin,
+                         splits, 0, stream, &cg);
+}
+
+extern "C" int b200_conv3x3_up2_nhwc_bf16(const void* x, const void* w_packed, const void* bias, void* out0, const void* aux, long long ldo,
+                                          int B, int H, int W, int Cin, int Cout, int epilogue, cudaStream_t stream) {
+    if (const int rc = check_resample("conv3x3_up2", B, H, W, Cin, Cout, false, H, W)) return rc;
+    const ConvGeom cg{B, H, W, Cin, 1, CONV_UP2};
+    return gemm_dispatch(x, Cin, 0, w_packed, 9ll * Cin, 0, class_m(cg), Cout, 9 * Cin, epilogue, bias, out0, nullptr, aux, ldo, 1, 0,
+                         stream, &cg);
 }

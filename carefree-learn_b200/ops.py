@@ -762,3 +762,104 @@ def conv3x3(x: Tensor, w_packed: Tensor, bias: Optional[Tensor] = None, *, epilo
     out = torch.empty((B, H, W, Cout), dtype=dtype, device=x.device)
     call("b200_conv3x3_nhwc_bf16", x.data_ptr(), w_packed.data_ptr(), _ptr(bias), out.data_ptr(), _ptr(aux), Cout, B, H, W, Cin, Cout, epilogue, _stream())
     return out
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# resampling convolutions of the SD-v1.5 UNet (include/b200_cflearn_ext.h)
+# ----------------------------------------------------------------------------------------------------------------
+def _conv_resample(entry: str, what: str, x: Tensor, w_packed: Tensor, bias: Optional[Tensor], epilogue: int, aux: Optional[Tensor],
+                   Ho: int, Wo: int) -> Tensor:
+    B, H, W, Cin = x.shape
+    _check(what, "w_packed", w_packed, _BF16, (None, 9 * Cin))
+    Cout = w_packed.shape[0]
+    _check(what, "bias", bias, None, contiguous=False, optional=True)
+    dtype, aux_kind, _ = EPILOGUES.get(epilogue, (_BF16, None, None))  # the C side refuses the others
+    if aux_kind:
+        _check(what, "aux", aux, dtype, rows=B if aux_kind == "image" else B * Ho * Wo, width=Cout)
+    else:
+        _check(what, "aux", aux, None, contiguous=False, optional=True)
+    out = torch.empty((B, Ho, Wo, Cout), dtype=dtype, device=x.device)
+    call(entry, x.data_ptr(), w_packed.data_ptr(), _ptr(bias), out.data_ptr(), _ptr(aux), Cout, B, H, W, Cin, Cout, epilogue, _stream())
+    return out
+
+
+def conv3x3_s2(x: Tensor, w_packed: Tensor, bias: Optional[Tensor] = None, *, epilogue: int = EPI_BIAS_BF16,
+               aux: Optional[Tensor] = None) -> Tensor:
+    """3x3 convolution with stride 2 and zero padding 1: x bf16 [B, H, W, Cin] channels-last, w_packed bf16 [Cout, 9 * Cin] ->
+    [B, H/2, W/2, Cout].  ``epilogue`` / ``aux`` as ``conv3x3`` (aux rows: the output's pixels)."""
+    _check("conv3x3_s2", "x", x, _BF16, (None, None, None, None))
+    return _conv_resample("b200_conv3x3_s2_nhwc_bf16", "conv3x3_s2", x, w_packed, bias, epilogue, aux, x.shape[1] // 2, x.shape[2] // 2)
+
+
+def conv3x3_up2(x: Tensor, w_packed: Tensor, bias: Optional[Tensor] = None, *, epilogue: int = EPI_BIAS_BF16,
+                aux: Optional[Tensor] = None) -> Tensor:
+    """Nearest 2x upsampling then a 3x3 / padding 1 convolution, in one implicit GEMM that never writes the upsampled image:
+    x bf16 [B, H, W, Cin] channels-last, w_packed bf16 [Cout, 9 * Cin] -> [B, 2H, 2W, Cout].  ``epilogue`` / ``aux`` as
+    ``conv3x3`` (aux rows: the output's pixels)."""
+    _check("conv3x3_up2", "x", x, _BF16, (None, None, None, None))
+    return _conv_resample("b200_conv3x3_up2_nhwc_bf16", "conv3x3_up2", x, w_packed, bias, epilogue, aux, 2 * x.shape[1], 2 * x.shape[2])
+
+
+# taps (ky, kx) of the input-gradient parity classes (py, px) of the stride-2 convolution, in b200_conv3x3_s2_dgrad_nhwc_bf16's order
+_S2_DGRAD_TAPS = [(ky, kx) for py in (0, 1) for px in (0, 1) for ky in ((1,) if py == 0 else (0, 2)) for kx in ((1,) if px == 0 else (0, 2))]
+
+
+def pack_conv3x3_weight_s2_dgrad(w: Tensor) -> Tensor:
+    """[Cout, Cin, 3, 3] -> bf16 [Cin, 9 * Cout]: the weights of ``conv3x3_s2_dgrad``, class by class and tap by tap."""
+    if tuple(w.shape[2:]) != (3, 3):
+        raise B200Error("pack_conv3x3_weight_s2_dgrad: 3x3 kernels only")
+    return torch.cat([w[:, :, ky, kx].t() for ky, kx in _S2_DGRAD_TAPS], dim=1).to(torch.bfloat16).contiguous()
+
+
+def conv3x3_s2_dgrad(dy: Tensor, w_dgrad: Tensor) -> Tensor:
+    """Input gradient of ``conv3x3_s2``: dy bf16 [B, H/2, W/2, Cout], w_dgrad = ``pack_conv3x3_weight_s2_dgrad(w)`` -> bf16
+    [B, H, W, Cin]."""
+    what = "conv3x3_s2_dgrad"
+    _check(what, "dy", dy, _BF16, (None, None, None, None))
+    B, h, w, Cout = dy.shape
+    _check(what, "w_dgrad", w_dgrad, _BF16, (None, 9 * Cout))
+    Cin = w_dgrad.shape[0]
+    dx = torch.empty((B, 2 * h, 2 * w, Cin), dtype=torch.bfloat16, device=dy.device)
+    call("b200_conv3x3_s2_dgrad_nhwc_bf16", dy.data_ptr(), w_dgrad.data_ptr(), dx.data_ptr(), B, 2 * h, 2 * w, Cin, Cout, _stream())
+    return dx
+
+
+def conv3x3_s2_wgrad(dy: Tensor, x: Tensor, out: Optional[Tensor] = None, *, round_bf16: bool = True, accumulate: bool = False) -> Tensor:
+    """Weight gradient of ``conv3x3_s2``: dy bf16 [B, H/2, W/2, Cout], x bf16 [B, H, W, Cin] -> fp32 [Cout, 9 * Cin], packed as
+    ``conv3x3_wgrad``'s."""
+    what = "conv3x3_s2_wgrad"
+    _check(what, "x", x, _BF16, (None, None, None, None))
+    B, H, W, Cin = x.shape
+    _check(what, "dy", dy, _BF16, (B, H // 2, W // 2, None))
+    Cout = dy.shape[3]
+    if out is None:
+        out = torch.empty((Cout, 9 * Cin), dtype=torch.float32, device=x.device)
+        accumulate = False
+    _check(what, "out", out, _F32, (Cout, 9 * Cin))
+    n = Cout * 9 * Cin
+    splits = pick_splits(Cout, 9 * Cin, B * (H // 2) * (W // 2))
+    part = WORKSPACE.get(x.device, splits * n, "splitk")[: splits * n]
+    call("b200_conv3x3_s2_wgrad_nhwc_bf16", dy.data_ptr(), Cout, x.data_ptr(), part.data_ptr(), B, H, W, Cin, Cout, splits, _stream())
+    call("b200_splitk_reduce", part.data_ptr(), splits, n, out.data_ptr(), int(round_bf16), int(accumulate), _stream())
+    return out
+
+
+def upsample_nearest2x(x: Tensor) -> Tensor:
+    """Nearest 2x upsampling of bf16 [B, H, W, C] (channels-last): [B, 2H, 2W, C], an exact copy."""
+    _check("upsample_nearest2x", "x", x, _BF16, (None, None, None, None))
+    B, H, W, C = x.shape
+    out = torch.empty((B, 2 * H, 2 * W, C), dtype=torch.bfloat16, device=x.device)
+    call("b200_upsample_nearest2x_bf16", x.data_ptr(), out.data_ptr(), B, H, W, C, _stream())
+    return out
+
+
+def sum2x2(x: Tensor) -> Tensor:
+    """The backward of ``upsample_nearest2x``: bf16 [B, 2H, 2W, C] -> bf16 [B, H, W, C], each 2x2 block summed in fp32 and
+    rounded once."""
+    _check("sum2x2", "x", x, _BF16, (None, None, None, None))
+    B, H2, W2, C = x.shape
+    if H2 % 2 or W2 % 2:
+        raise B200Error(f"sum2x2: x must have even height and width, got {list(x.shape)}")
+    out = torch.empty((B, H2 // 2, W2 // 2, C), dtype=torch.bfloat16, device=x.device)
+    call("b200_sum2x2_bf16", x.data_ptr(), out.data_ptr(), B, H2 // 2, W2 // 2, C, _stream())
+    return out

@@ -220,3 +220,137 @@ class ResidualBlockWithTimeEmbeddingB200(nn.Module):
         if any(t is not None and t.dtype != torch.bfloat16 for t in (net, time_net)):
             raise B200Error(f"{what}: net and time_net must be bf16 (the UNet's activations under bf16 autocast)")
         return checkpoint.OpFn.apply(_ResBlockOp(self.norm_eps), self.use_checkpoint, net, time_net, *self._params())
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# resampling: ResDownsample / ResUpsample with use_conv (cflearn/modules/core/convs/residual.py:86-151)
+# ------------------------------------------------------------------------------------------------------------------------------
+def _tiles(what: str, h: int, w: int, wgrad: bool) -> None:
+    """The tile rules of the implicit-GEMM convolutions on an h x w grid (``wgrad``: also those of the weight gradient)."""
+    if w > 128 or 128 % w != 0 or h % min(h, 128 // w) != 0:
+        raise B200Error(f"{what}: a {h} x {w} grid is not tiled by 128-pixel tiles of whole rows (the width must divide 128, the "
+                        "height be a multiple of 128 / width)")
+    if wgrad and (w > 64 or 64 % w != 0 or (h * w) % 64 != 0):
+        raise B200Error(f"{what}: the weight gradient's {h} x {w} grid needs a width that divides 64 and h * w a multiple of 64")
+
+
+def check_resample_geometry(what: str, up: bool, H: int, W: int, Cin: int, Cout: int) -> None:
+    """Raise ``B200Error`` (with the reason) for shapes the resampling kernels do not take; H x W is the input's size."""
+    for name, c in (("Cin", Cin), ("Cout", Cout)):
+        if c <= 0 or c % 64 != 0:
+            raise B200Error(f"{what}: {name} = {c} must be a positive multiple of 64 (the convolutions reduce over 64-channel blocks)")
+    if up:  # fused forward on the H x W grid; backward: stride-1 input and weight gradients at 2H x 2W
+        _tiles(what, H, W, False)
+        _tiles(what, 2 * H, 2 * W, True)
+    else:
+        if H % 2 or W % 2:
+            raise B200Error(f"{what}: H = {H} and W = {W} must be even")
+        _tiles(what, H // 2, W // 2, True)
+
+
+def _bias_rows(bias: Tensor, B: int) -> Tensor:
+    """The bias as a per-image table [B, Cout] for the per-image epilogue with no bias of its own: bf16(bf16(conv) + bias), the
+    two roundings of eager's biased convolution on CUDA (DESIGN.md section 2)."""
+    return _bf(bias).expand(B, -1).contiguous()
+
+
+def _nhwc(t: Tensor) -> Tensor:
+    return t.permute(0, 2, 3, 1).to(torch.bfloat16).contiguous()  # a view when t is channels-last bf16
+
+
+@dataclass(frozen=True)
+class _DownsampleOp:
+    """ResDownsampleB200 as a ``checkpoint.OpFn`` op on (net [B, Cin, H, W], weight, bias); keeps only its input (and the
+    parameters) for backward."""
+
+    def forward(self, net: Tensor, weight: Tensor, bias: Tensor) -> Tuple[Tensor, tuple]:
+        out = ops.conv3x3_s2(_nhwc(net), ops.pack_conv3x3_weight(weight), epilogue=ops.EPI_BIAS_ADD_PER_IMAGE_BF16,
+                             aux=_bias_rows(bias, net.shape[0]))
+        return out.permute(0, 3, 1, 2), (net, weight)
+
+    def backward(self, saved: tuple, dout: Tensor) -> tuple:
+        net, weight = saved
+        Cout, Cin = weight.shape[:2]
+        d = _nhwc(dout)
+        dw = ops.unpack_conv3x3_weight(ops.conv3x3_s2_wgrad(d, _nhwc(net)), Cin)
+        db = ops.colsum(d.view(-1, Cout), torch.empty(Cout, dtype=torch.float32, device=d.device))
+        dx = ops.conv3x3_s2_dgrad(d, ops.pack_conv3x3_weight_s2_dgrad(weight))
+        return dx.permute(0, 3, 1, 2), dw, db
+
+
+@dataclass(frozen=True)
+class _UpsampleOp:
+    """ResUpsampleB200 as a ``checkpoint.OpFn`` op on (net [B, Cin, H, W], weight, bias); keeps only its low-resolution input (and
+    the parameters) for backward.  Backward holds two transient 2H x 2W tensors: the upsampled input for the weight gradient and
+    the input gradient before its 2x2 sum."""
+
+    def forward(self, net: Tensor, weight: Tensor, bias: Tensor) -> Tuple[Tensor, tuple]:
+        out = ops.conv3x3_up2(_nhwc(net), ops.pack_conv3x3_weight(weight), epilogue=ops.EPI_BIAS_ADD_PER_IMAGE_BF16,
+                              aux=_bias_rows(bias, net.shape[0]))
+        return out.permute(0, 3, 1, 2), (net, weight)
+
+    def backward(self, saved: tuple, dout: Tensor) -> tuple:
+        net, weight = saved
+        Cout, Cin = weight.shape[:2]
+        d = _nhwc(dout)
+        dw = ops.unpack_conv3x3_weight(ops.conv3x3_wgrad(d, ops.upsample_nearest2x(_nhwc(net))), Cin)
+        db = ops.colsum(d.view(-1, Cout), torch.empty(Cout, dtype=torch.float32, device=d.device))
+        dx = ops.sum2x2(ops.conv3x3(d, ops.pack_conv3x3_weight_dgrad(weight)))
+        return dx.permute(0, 3, 1, 2), dw, db
+
+
+def _resample_options(what: str, use_conv: bool, signal_dim: int, padding: int) -> None:
+    if not use_conv:
+        raise NotImplementedError(f"{what}: use_conv=False (average pooling / a bare interpolation) is not supported")
+    if signal_dim != 2:
+        raise NotImplementedError(f"{what}: signal_dim={signal_dim} is not supported (2-D signals only)")
+    if padding != 1:
+        raise NotImplementedError(f"{what}: padding={padding} is not supported (padding=1 only)")
+
+
+class _Resample(nn.Module):
+    """The forward of both resampling modules: bf16 [B, Cin, H, W] (either memory format; CUDA only) -> bf16 [B, Cout, H', W']
+    with channels-last strides, through one ``checkpoint.OpFn`` node."""
+
+    UP = False
+
+    def _run(self, conv: nn.Conv2d, net: Tensor) -> Tensor:
+        what = type(self).__name__
+        if net.dim() != 4 or net.shape[1] != conv.in_channels:
+            raise B200Error(f"{what}: net must be [B, {conv.in_channels}, H, W]")
+        check_resample_geometry(what, self.UP, net.shape[2], net.shape[3], conv.in_channels, conv.out_channels)
+        _check_cuda(what, net)
+        if net.dtype != torch.bfloat16:
+            raise B200Error(f"{what}: net must be bf16 (the UNet's activations under bf16 autocast)")
+        op = _UpsampleOp() if self.UP else _DownsampleOp()
+        return checkpoint.OpFn.apply(op, False, net, conv.weight, conv.bias)
+
+
+class ResDownsampleB200(_Resample):
+    """Drop-in for cflearn's ``ResDownsample`` with ``use_conv=True`` on the native kernels: a 3x3 convolution with stride 2 and
+    padding 1 (``net`` is a Conv2d, as in the reference's state dict)."""
+
+    def __init__(self, in_channels: int, use_conv: bool, *, signal_dim: int = 2, out_channels: Optional[int] = None,
+                 padding: int = 1) -> None:
+        super().__init__()
+        _resample_options("ResDownsampleB200", use_conv, signal_dim, padding)
+        self.net = nn.Conv2d(in_channels, out_channels or in_channels, 3, stride=2, padding=padding)
+
+    def forward(self, net: Tensor) -> Tensor:
+        return self._run(self.net, net)
+
+
+class ResUpsampleB200(_Resample):
+    """Drop-in for cflearn's ``ResUpsample`` with ``use_conv=True`` on the native kernels: nearest 2x upsampling and a 3x3 /
+    padding 1 convolution (``conv``), fused so that the upsampled image is never written in the forward."""
+
+    UP = True
+
+    def __init__(self, in_channels: int, use_conv: bool, *, signal_dim: int = 2, out_channels: Optional[int] = None,
+                 padding: int = 1) -> None:
+        super().__init__()
+        _resample_options("ResUpsampleB200", use_conv, signal_dim, padding)
+        self.conv = nn.Conv2d(in_channels, out_channels or in_channels, 3, padding=padding)
+
+    def forward(self, net: Tensor) -> Tensor:
+        return self._run(self.conv, net)
