@@ -109,6 +109,112 @@ def spatial_transformer(sd: StateDict, p: str, net: Tensor, context: Optional[Te
     return inp + F.conv2d(net, sd[p + "from_latent.weight"], sd[p + "from_latent.bias"])
 
 
+# ------------------------------------------------------------------------------------------------------------------------------
+# the same computations with every op boundary returned, for the per-op teacher-forced tests (tests/test_unet_ops_gpu.py).
+# ``out`` of each is bit-identical to the function above it (tests/test_oracle.py).  Where one tensor feeds two paths (x into
+# GroupNorm and the shortcut, a context into several blocks), each path reads its own ``view_as`` of it, so that one backward
+# yields each path's gradient apart (the views change no value and no op).  Every non-leaf entry can ``retain_grad()``.
+# ------------------------------------------------------------------------------------------------------------------------------
+def res_block_ops(sd: StateDict, p: str, net: Tensor, time_net: Tensor) -> Dict[str, Tensor]:
+    """``res_block``'s op boundaries: x, x_gn / x_sc (the GroupNorm and shortcut paths' views of x), gn1, silu1, conv1 (with its
+    bias), time_silu, t, h (conv1 + t), gn2, silu2, conv2, shortcut (1x1 conv, when the width changes), sum (pre-clamp), out."""
+    o: Dict[str, Tensor] = {"x": net, "x_gn": net.view_as(net), "x_sc": net.view_as(net)}
+    o["gn1"] = _gn(sd, p + "norm1.", o["x_gn"], 1e-5)
+    o["silu1"] = F.silu(o["gn1"])
+    o["conv1"] = F.conv2d(o["silu1"], sd[p + "conv1.weight"], sd[p + "conv1.bias"], padding=1)
+    inp = o["x_sc"]
+    if p + "shortcut.weight" in sd:
+        inp = o["shortcut"] = F.conv2d(o["x_sc"], sd[p + "shortcut.weight"], sd[p + "shortcut.bias"])
+    o["time_silu"] = F.silu(time_net)
+    o["t"] = F.linear(o["time_silu"], sd[p + "time_embedding.weight"], sd[p + "time_embedding.bias"])
+    o["h"] = o["conv1"] + o["t"][..., None, None]
+    o["gn2"] = _gn(sd, p + "norm2.", o["h"], 1e-5)
+    o["silu2"] = F.silu(o["gn2"])
+    o["conv2"] = F.conv2d(o["silu2"], sd[p + "conv2.weight"], sd[p + "conv2.bias"], padding=1)
+    o["sum"] = inp + o["conv2"]
+    fi = torch.finfo(o["sum"].dtype)
+    o["out"] = o["sum"].clamp(fi.min, fi.max)
+    return o
+
+
+def cross_attention_ops(sd: StateDict, p: str, net: Tensor, context: Optional[Tensor], heads: int) -> Dict[str, Tensor]:
+    """``cross_attention``'s op boundaries: x, q, k, v (the projections, [B, T, L]), attn (the attention output with the heads
+    unfolded, [B, Tq, L]) and out (out_linear)."""
+    b, tq, dq = net.shape
+    ctx = net if context is None else context
+    o: Dict[str, Tensor] = {"x": net}
+    o["q"] = F.linear(net, sd[p + "to_q.weight"])
+    o["k"] = F.linear(ctx, sd[p + "to_k.weight"])
+    o["v"] = F.linear(ctx, sd[p + "to_v.weight"])
+
+    def fold(z: Tensor) -> Tensor:
+        bb, t, d = z.shape
+        return z.view(bb, t, heads, d // heads).permute(0, 2, 1, 3).reshape(bb * heads, t, d // heads)
+
+    out = F.scaled_dot_product_attention(fold(o["q"]).contiguous(), fold(o["k"]).contiguous(), fold(o["v"]).contiguous(), None, 0.0)
+    o["attn"] = out.reshape(b, heads, tq, dq // heads).permute(0, 2, 1, 3).contiguous().view(b, tq, dq)
+    o["out"] = F.linear(o["attn"], sd[p + "out_linear.0.weight"], sd[p + "out_linear.0.bias"])
+    return o
+
+
+def transformer_block_ops(sd: StateDict, p: str, net: Tensor, context: Optional[Tensor], heads: int) -> Dict[str, Tensor]:
+    """``transformer_block``'s op boundaries: x, ln1, attn1.* (``cross_attention_ops`` of the self-attention), x1 (its residual
+    sum), ln2, attn2.*, x2, ln3, hg (the GEGLU projection), h / gate (its halves), gelu, prod (h * gelu), ff2, out."""
+    d = net.shape[-1]
+    ln = lambda i, z: F.layer_norm(z, (d,), sd[p + f"norm{i}.weight"], sd[p + f"norm{i}.bias"], 1e-5)  # noqa: E731
+    o: Dict[str, Tensor] = {"x": net}
+    o["ln1"] = ln(1, net)
+    o.update({"attn1." + k: v for k, v in cross_attention_ops(sd, p + "attn1.", o["ln1"], None, heads).items() if k != "x"})
+    o["x1"] = o["attn1.out"] + net
+    o["ln2"] = ln(2, o["x1"])
+    o.update({"attn2." + k: v for k, v in cross_attention_ops(sd, p + "attn2.", o["ln2"], context, heads).items() if k != "x"})
+    o["x2"] = o["attn2.out"] + o["x1"]
+    o["ln3"] = ln(3, o["x2"])
+    o["hg"] = F.linear(o["ln3"], sd[p + "ff.net.0.net.weight"], sd[p + "ff.net.0.net.bias"])
+    o["h"], o["gate"] = o["hg"].chunk(2, dim=-1)
+    o["gelu"] = F.gelu(o["gate"])
+    o["prod"] = o["h"] * o["gelu"]
+    o["ff2"] = F.linear(o["prod"], sd[p + "ff.net.2.linear.weight"], sd[p + "ff.net.2.linear.bias"])
+    o["out"] = o["ff2"] + o["x2"]
+    return o
+
+
+def spatial_transformer_ops(sd: StateDict, p: str, net: Tensor, context: Optional[Tensor], heads: int) -> Dict[str, Tensor]:
+    """``spatial_transformer``'s op boundaries: x, x_gn / x_res (the GroupNorm and residual paths' views of x), gn, latent_in (to_latent),
+    tokens ([B, HW, C]), blocks.{i}.* (``transformer_block_ops``, with blocks.{i}.context the block's view of the context), latent
+    ([B, C, H, W]), latent_out (from_latent) and out."""
+    b, c, h, w = net.shape
+    o: Dict[str, Tensor] = {"x": net, "x_gn": net.view_as(net), "x_res": net.view_as(net)}
+    o["gn"] = _gn(sd, p + "norm.", o["x_gn"], 1e-6)
+    o["latent_in"] = F.conv2d(o["gn"], sd[p + "to_latent.weight"], sd[p + "to_latent.bias"])
+    t = o["tokens"] = o["latent_in"].permute(0, 2, 3, 1).reshape(b, h * w, c)
+    i = 0
+    while p + f"blocks.{i}.norm1.weight" in sd:
+        q = f"blocks.{i}."
+        ctx = None if context is None else context.view_as(context)
+        if ctx is not None:
+            o[q + "context"] = ctx
+        o.update({q + k: v for k, v in transformer_block_ops(sd, p + q, t, ctx, heads).items() if k != "x"})
+        t = o[q + "out"]
+        i += 1
+    o["latent"] = t.permute(0, 2, 1).contiguous().view(b, c, h, w)
+    o["latent_out"] = F.conv2d(o["latent"], sd[p + "from_latent.weight"], sd[p + "from_latent.bias"])
+    o["out"] = o["x_res"] + o["latent_out"]
+    return o
+
+
+def resample_ops(sd: StateDict, p: str, net: Tensor) -> Dict[str, Tensor]:
+    """The op boundaries of the resampling child at ``p`` as ``_sequential`` runs it: ResDownsample (``net.weight``: x, out) or
+    ResUpsample (``conv.weight``: x, up = the nearest 2x copy, out)."""
+    o: Dict[str, Tensor] = {"x": net}
+    if p + "net.weight" in sd:
+        o["out"] = F.conv2d(net, sd[p + "net.weight"], sd[p + "net.bias"], stride=2, padding=1)
+    else:
+        o["up"] = F.interpolate(net, scale_factor=2, mode="nearest")
+        o["out"] = F.conv2d(o["up"], sd[p + "conv.weight"], sd[p + "conv.bias"], padding=1)
+    return o
+
+
 def _sequential(sd: StateDict, p: str, net: Tensor, time_net: Tensor, context: Optional[Tensor], heads: int) -> Tensor:
     """TimestepAttnSequential.forward (unet.py:31-45): children dispatched by type; here by the parameter names they own."""
     j = 0

@@ -268,6 +268,42 @@ def conv3x3_dgrad(dy, w):
     return dx.permute(0, 2, 3, 1).reshape(B * H * W, -1)
 
 
+def _nchw(t):
+    return t.to(F64).permute(0, 3, 1, 2)
+
+
+def _nhwc(t):
+    return t.permute(0, 2, 3, 1)
+
+
+def conv3x3_s2(x, w):
+    """3x3 / stride 2 / zero padding 1 convolution of channels-last x [B, H, W, Cin] with w [Cout, Cin, 3, 3]: [B, H/2, W/2, Cout]."""
+    return _nhwc(F.conv2d(_nchw(x), w.to(F64), stride=2, padding=1))
+
+
+def conv3x3_up2(x, w):
+    """Nearest 2x upsampling of channels-last x [B, H, W, Cin], then ``conv3x3`` with w: [B, 2H, 2W, Cout]."""
+    return _nhwc(F.conv2d(F.interpolate(_nchw(x), scale_factor=2, mode="nearest"), w.to(F64), padding=1))
+
+
+def conv3x3_s2_dgrad(dy, w, H, W):
+    """Input gradient of ``conv3x3_s2`` for dy [B, H/2, W/2, Cout] and w [Cout, Cin, 3, 3]: [B, H, W, Cin]."""
+    B, Cin = dy.shape[0], w.shape[1]
+    return _nhwc(torch.nn.grad.conv2d_input((B, Cin, H, W), w.to(F64), _nchw(dy), stride=2, padding=1))
+
+
+def conv3x3_s2_wgrad(dy, x):
+    """Weight gradient of ``conv3x3_s2`` for dy [B, H/2, W/2, Cout]: [Cout, 9 Cin] in the kernels' packed order (tap, then channel)."""
+    w_shape = (dy.shape[3], x.shape[3], 3, 3)
+    return torch.nn.grad.conv2d_weight(_nchw(x), w_shape, _nchw(dy), stride=2, padding=1).permute(0, 2, 3, 1).reshape(w_shape[0], -1)
+
+
+def colsum_per_image(x):
+    """Column sums of x [B, ..., C] per image and over all rows: (per_image [B, C], total [C])."""
+    xd = x.to(F64).reshape(x.shape[0], -1, x.shape[-1])
+    return xd.sum(1), xd.sum((0, 1))
+
+
 # ---- exact operands for the GEMM and the 3x3 convolution ---------------------------------------------------------------------------
 # bf16 operands that are small integers times a power of two per row of A and per column of B (per image and per output channel
 # for the convolution): every product of one output shares the unit 2^(row exponent + column exponent).  With sum_k |a_k b_k|

@@ -342,3 +342,45 @@ def test_mixing_block_ops_is_the_same_computation_as_mixing_block():
             a = vo.mixing_block(sd, 1, x, cfg["latent_dim"] // 64, 1e-6)
             b = vo.mixing_block_ops(sd, 1, x, cfg["latent_dim"] // 64, 1e-6)["out"]
         assert torch.equal(a, b)
+
+
+
+def test_unet_block_ops_are_the_same_computations_as_the_blocks():
+    """oracle/unet_oracle.py's *_ops (op boundaries exposed for tests/test_unet_ops_gpu.py) == the block functions, bit for bit, in
+    fp32 and under bf16 autocast: every ResBlock, SpatialTransformer (and its SpatialTransformerBlock and two CrossAttentions),
+    ResDownsample and ResUpsample of the tiny UNet, each on an input of its own width."""
+    import unet_oracle as uo
+
+    with _pin("unet_tiny") as (fx, _):
+        shapes = [(k, tuple(v)) for k, v in fx["shapes"]]
+    cfg = uo.unet_config(fx["config_name"])
+    sd = uo.synthetic_state_dict(shapes, seed=3)
+    heads = cfg["num_heads"]
+    g = torch.Generator().manual_seed(4)
+    time_net = torch.randn(2, sd["time_embedding.2.weight"].shape[0], generator=g)
+    context = torch.randn(2, 5, cfg["context_dim"], generator=g)
+    children = {k[: -len(s)]: s for k in sd for s in ("norm1.weight", "to_latent.weight", "net.weight", "conv.weight") if k.endswith(s)}
+    # not the transformer blocks' own norm1 / GEGLU ``net.weight``
+    children = {q: s for q, s in children.items() if ".blocks." not in q}
+    seen = set()
+    for autocast in (False, True):
+        with torch.autocast("cpu", dtype=torch.bfloat16, enabled=autocast):
+            for q, kind in sorted(children.items()):
+                w = sd[q + kind]
+                x = torch.randn(2, w.shape[0] if w.dim() == 1 else w.shape[1], 8, 8, generator=g)  # the child's input width
+                seen.add(kind)
+                if kind == "norm1.weight":
+                    assert torch.equal(uo.res_block_ops(sd, q, x, time_net)["out"], uo.res_block(sd, q, x, time_net)), q
+                elif kind == "to_latent.weight":
+                    assert torch.equal(uo.spatial_transformer_ops(sd, q, x, context, heads)["out"],
+                                       uo.spatial_transformer(sd, q, x, context, heads)), q
+                    tok, b = torch.randn(2, 64, x.shape[1], generator=g), q + "blocks.0."
+                    assert torch.equal(uo.transformer_block_ops(sd, b, tok, context, heads)["out"],
+                                       uo.transformer_block(sd, b, tok, context, heads)), b
+                    for a, ctx in (("attn1.", None), ("attn2.", context)):
+                        assert torch.equal(uo.cross_attention_ops(sd, b + a, tok, ctx, heads)["out"],
+                                           uo.cross_attention(sd, b + a, tok, ctx, heads)), b + a
+                else:  # _sequential runs the child alone when it is child 0 of a prefix of its own
+                    one = {"r.0." + k[len(q):]: v for k, v in sd.items() if k.startswith(q)}
+                    assert torch.equal(uo.resample_ops(sd, q, x)["out"], uo._sequential(one, "r.", x, time_net, None, heads)), q
+    assert seen == {"norm1.weight", "to_latent.weight", "net.weight", "conv.weight"}

@@ -207,3 +207,24 @@ def test_gemm_and_conv_references():
     aux = torch.randn(6, 16, generator=g)
     assert torch.equal(refs.gemm_epilogue(2, tb, aux)["out0"][0], aux + tb.float())
     assert torch.equal(refs.gemm_epilogue(9, tb, hb)["out0"][0], (tb.float() + hb.float()).to(torch.bfloat16))
+
+
+def test_resample_and_per_image_references():
+    """The stride-2 / nearest-2x convolution references and their gradients against torch's autograd of the same fp32 ops, and the
+    per-image column sums against a loop over images."""
+    g = torch.Generator().manual_seed(7)
+    x = torch.randn(2, 8, 6, 5, generator=g)  # channels-last [B, H, W, Cin]
+    w = torch.randn(4, 5, 3, 3, generator=g)
+    xf, wf = x.permute(0, 3, 1, 2).clone().requires_grad_(True), w.clone().requires_grad_(True)
+    y = F.conv2d(xf, wf, stride=2, padding=1)
+    dy = torch.randn(y.shape, generator=g)
+    y.backward(dy)
+    dy_nhwc = dy.permute(0, 2, 3, 1)
+    assert torch.allclose(refs.conv3x3_s2(x, w).float(), y.detach().permute(0, 2, 3, 1), atol=1e-5)
+    assert torch.allclose(refs.conv3x3_s2_dgrad(dy_nhwc, w, 8, 6).float(), xf.grad.permute(0, 2, 3, 1), atol=1e-5)
+    assert torch.allclose(refs.conv3x3_s2_wgrad(dy_nhwc, x).float(), wf.grad.permute(0, 2, 3, 1).reshape(4, -1), atol=1e-4)
+    up = F.conv2d(F.interpolate(x.permute(0, 3, 1, 2), scale_factor=2, mode="nearest"), w, padding=1)
+    assert torch.allclose(refs.conv3x3_up2(x, w).float(), up.permute(0, 2, 3, 1), atol=1e-5)
+    per, tot = refs.colsum_per_image(x)
+    assert torch.allclose(per.float(), torch.stack([x[b].reshape(-1, 5).sum(0) for b in range(2)]), atol=1e-5)
+    assert torch.allclose(tot.float(), x.reshape(-1, 5).sum(0), atol=1e-5)

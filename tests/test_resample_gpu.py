@@ -20,21 +20,13 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 import cflearn_b200  # noqa: F401,E402
 from cflearn_b200 import ops  # noqa: E402
 from cflearn_b200.unet_blocks import ResDownsampleB200, ResUpsampleB200, ResidualBlockWithTimeEmbeddingB200  # noqa: E402
-from _refs import bf16, exact_ints, exact_scaled, exponents, first_bad, relerr  # noqa: E402
+from _refs import (bf16, conv3x3_s2, conv3x3_s2_dgrad, conv3x3_s2_wgrad, conv3x3_up2, exact_ints, exact_scaled, exponents,  # noqa: E402
+                   first_bad, relerr)
 from test_kernel_footprint_gpu import Case, S, assert_equal, call, rand  # noqa: E402
 
 DEV = "cuda"
 F64 = torch.float64
 CL = torch.channels_last
-grad_input, grad_weight = torch.nn.grad.conv2d_input, torch.nn.grad.conv2d_weight
-
-
-def nchw(t):
-    return t.to(F64).permute(0, 3, 1, 2)
-
-
-def nhwc(t):
-    return t.permute(0, 2, 3, 1)
 
 
 def packed(w):
@@ -43,22 +35,7 @@ def packed(w):
 
 
 # float64 references on channels-last tensors (CPU)
-def ref_down(x, w):
-    return nhwc(F.conv2d(nchw(x), w.to(F64), stride=2, padding=1))
-
-
-def ref_up(x, w):
-    return nhwc(F.conv2d(F.interpolate(nchw(x), scale_factor=2, mode="nearest"), w.to(F64), padding=1))
-
-
-def ref_down_dgrad(dy, w, H, W):
-    B, Cin = dy.shape[0], w.shape[1]
-    return nhwc(grad_input((B, Cin, H, W), w.to(F64), nchw(dy), stride=2, padding=1))
-
-
-def ref_down_wgrad(dy, x):
-    w_shape = (dy.shape[3], x.shape[3], 3, 3)
-    return packed(grad_weight(nchw(x), w_shape, nchw(dy), stride=2, padding=1))
+ref_down, ref_up, ref_down_dgrad, ref_down_wgrad = conv3x3_s2, conv3x3_up2, conv3x3_s2_dgrad, conv3x3_s2_wgrad
 
 
 def sum2x2_ref(x):
