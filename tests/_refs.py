@@ -475,3 +475,263 @@ def adam(p, g, m, v, steps, lr, b1, b2, eps, wd, grad_scale=1.0):
         v = b2 * v + (1 - b2) * gg * gg
         p = p - lr / (1 - b1 ** t) * m / (v.sqrt() / math.sqrt(1 - b2 ** t) + eps)
     return p, m, v
+
+
+# ---- the fused FCNN step ----------------------------------------------------------------------------------------------------------------
+# b200_fcnn_step (csrc/mlp.cu) runs Linear -> ReLU -> ... -> Linear in fp32, one thread per sample, every sum an FFMA chain in a fixed
+# order: the forward z = fma(W_jk, a_k, ...) from z = b_j (or +0) over k; the output gradient of the multi_task[mae, mse] loss
+# (w_mae sign(d) + 2 w_mse d) * inv with d = pred - y and inv = fp32(1 / (M nout)), or a given dpred; per 128-row block, each weight
+# gradient fma(d_j[r], a_k[r], ...) over the block's 128 rows (rows past M carry d = 0), each bias gradient the plain sum of those d_j,
+# the loss sum_j (w_mae |d| + w_mse d^2) summed over the block then times inv; each input gradient fma(d_j, W_jk, ...) over j, kept
+# where the stored activation is > 0; finally b200_colsum_finish adds the block partials.
+FCNN_BUDGET = 2 ** 24  # an fp32 sum of multiples of q whose magnitudes add up to less than 2^24 q is exact in any order
+FCNN_C = 2.0           # fcnn_bounds: tolerance = FCNN_C x the first-order error bound
+
+
+def fcnn_layers(params, dims, woff, boff):
+    """[(W_l [dims[l+1], dims[l]], b_l [dims[l+1]] or None)] of the arena ``params`` (float64 views)."""
+    p = params.to(F64)
+    return [(p[woff[l]:woff[l] + dims[l] * dims[l + 1]].view(dims[l + 1], dims[l]),
+             p[boff[l]:boff[l] + dims[l + 1]] if boff[l] >= 0 else None) for l in range(len(dims) - 1)]
+
+
+def fcnn_forward(x, layers):
+    """(pre-activations z_l, activations a_l) of the network: a_0 = x, a_{l+1} = relu(z_{l+1}) except the output a_L = z_L."""
+    acts, pre = [x.to(F64)], []
+    for l, (W, b) in enumerate(layers):
+        z = acts[-1] @ W.t() + (0.0 if b is None else b) + 0.0
+        pre.append(z)
+        acts.append(torch.relu(z) if l + 1 < len(layers) else z)
+    return pre, acts
+
+
+def fcnn_step(x, params, dims, woff, boff, y=None, dpred=None, w_mae=1.0, w_mse=1.0):
+    """The fused FCNN step in float64: (pred [M, nout], loss (0-dim; None with dpred), gradient arena [P]).  With ``y`` the loss is
+    w_mae mean|pred - y| + w_mse mean (pred - y)^2, the mean over all M nout elements; otherwise ``dpred`` is d(pred).  torch's rules:
+    the L1 gradient is sign(d), 0 at d = 0; the ReLU gradient is 0 where the activation is 0 (threshold_backward), the boundary z = 0
+    included.  The arena's gaps get gradient 0.  An exact zero comes out as +0, as in the kernel, whose sums start from +0.
+
+    The kernel's one rounding that no choice of operands removes is its fp32 inv = 1 / (M nout): it is exact only when M nout is a power
+    of two, so only then can the kernel's loss and gradients of the fused loss equal these bit for bit."""
+    layers = fcnn_layers(params, dims, woff, boff)
+    _, acts = fcnn_forward(x, layers)
+    pred = acts[-1]
+    loss = None
+    if y is not None:
+        d = pred - y.to(F64)
+        n = d.numel()
+        loss = (w_mae * d.abs() + w_mse * d * d).sum() / n
+        g = (w_mae * torch.sign(d) + 2 * w_mse * d) / n + 0.0
+    else:
+        g = dpred.to(F64)
+    grads = torch.zeros(params.numel(), dtype=F64, device=pred.device)
+    for l in reversed(range(len(layers))):
+        W, b = layers[l]
+        grads[woff[l]:woff[l] + W.numel()] = (g.t() @ acts[l]).reshape(-1) + 0.0
+        if b is not None:
+            grads[boff[l]:boff[l] + b.numel()] = g.sum(0) + 0.0
+        if l > 0:
+            g = torch.where(acts[l] > 0, g @ W, torch.zeros_like(acts[l])) + 0.0
+    return pred, loss, grads
+
+
+def fcnn_bounds(x, params, dims, woff, boff, y=None, dpred=None, w_mae=1.0, w_mse=1.0):
+    """(pred, loss, grads) of ``fcnn_step`` and, for each, a tolerance of its shape that |kernel - float64| must not exceed anywhere.
+
+    First-order propagation of the kernel's fp32 roundings, with u = 2^-24, g_n = n u for a fixed-order sum of n terms (an FFMA chain
+    rounds once per term), |X| elementwise and B = ceil(blocks / 8) + 8 the adds of b200_colsum_finish:
+    forward   dz_{l+1} = g_{in} (|b| + |a_l| |W|^T) + da_l |W|^T;  da_{l+1} = dz_{l+1} (ReLU does not expand an error); tol_pred = C dz_L.
+    residual  dd = dz_L + u |d|.
+    dpred     dg = 0.  Fused loss: dg = [2 w_mse dd + 4 u (w_mae + 2 w_mse |d|)] / n (the product 2 w_mse d, the add, the product with
+              inv and inv's own rounding), plus 2 w_mae / n where |d| <= dd: there sign(d) may flip.
+    loss      tol = C [sum (w_mae + 2 w_mse |d|) dd + (3 u + g_{nout + 9 + B}) sum (w_mae |d| + w_mse d^2)] / n: each term's two products
+              and add, then the thread's sum over nout, the 32-lane tree (5), the four warps (2), the product with inv and its error (2).
+    weights   tol = C [g_{128 + B} |D|^T |a_l| + dD^T |a_l| + |D|^T da_l], D the layer's output gradient; biases C [g_{128 + B} sum |D| +
+              sum dD].
+    inputs    t = D W: dt = g_out |D| |W| + dD |W|; kept where a_l > 0, and where |z_l| <= dz_l the kernel may mask otherwise: there
+              the error may be |t| + dt.
+    C = FCNN_C = 2 covers the products of two error terms the first order drops."""
+    u, C = FP32_U, FCNN_C
+    layers = fcnn_layers(params, dims, woff, boff)
+    pre, acts = fcnn_forward(x, layers)
+    pred = acts[-1]
+    M, nout = pred.shape
+    blocks = -(-M // 128)
+    B = -(-blocks // 8) + 8
+    da, dzs = torch.zeros_like(acts[0]), []
+    for l, (W, b) in enumerate(layers):
+        mag = acts[l].abs() @ W.abs().t() + (0.0 if b is None else b.abs())
+        da = dims[l] * u * mag + da @ W.abs().t()
+        dzs.append(da)
+    loss = tol_loss = None
+    if y is not None:
+        d = pred - y.to(F64)
+        n = d.numel()
+        dd = da + u * d.abs()
+        terms = w_mae * d.abs() + w_mse * d * d
+        loss = terms.sum() / n
+        tol_loss = C * (((w_mae + 2 * w_mse * d.abs()) * dd).sum() + (3 * u + (nout + 9 + B) * u) * terms.sum()) / n
+        g = (w_mae * torch.sign(d) + 2 * w_mse * d) / n + 0.0
+        dg = (2 * w_mse * dd + 4 * u * (w_mae + 2 * w_mse * d.abs())) / n + (2 * w_mae / n) * (d.abs() <= dd)
+    else:
+        g = dpred.to(F64)
+        dg = torch.zeros_like(g)
+    grads = torch.zeros(params.numel(), dtype=F64, device=pred.device)
+    tol = torch.zeros_like(grads)
+    dacts = [torch.zeros_like(acts[0])] + dzs  # the error of each activation
+    for l in reversed(range(len(layers))):
+        W, b = layers[l]
+        a, ag = acts[l], acts[l].abs()
+        grads[woff[l]:woff[l] + W.numel()] = (g.t() @ a).reshape(-1) + 0.0
+        tol[woff[l]:woff[l] + W.numel()] = C * ((128 + B) * u * (g.abs().t() @ ag) + dg.t() @ ag + g.abs().t() @ dacts[l]).reshape(-1)
+        if b is not None:
+            grads[boff[l]:boff[l] + b.numel()] = g.sum(0) + 0.0
+            tol[boff[l]:boff[l] + b.numel()] = C * ((128 + B) * u * g.abs().sum(0) + dg.sum(0))
+        if l > 0:
+            t = g @ W
+            dt = dims[l + 1] * u * (g.abs() @ W.abs()) + dg @ W.abs()
+            live, unsure = a > 0, pre[l - 1].abs() <= dacts[l]
+            g = torch.where(live, t, torch.zeros_like(t)) + 0.0
+            dg = torch.where(live, dt, torch.zeros_like(dt)) + torch.where(unsure, t.abs() + dt, torch.zeros_like(dt))
+    return (pred, loss, grads), (C * dzs[-1], tol_loss, tol)
+
+
+def _quantum(v):
+    """The largest power of two that divides the dyadic float v (> 0)."""
+    q = 2.0 ** math.floor(math.log2(abs(v)))
+    while v / q != round(v / q):
+        q /= 2
+    return q
+
+
+FCNN_FANS = (64.0, 16.0, 8.0, 4.0, 2.0, 1.0)  # exact_fcnn_operands tries the densest weights first
+
+
+def exact_fcnn_operands(dims, M, bias, seed, *, y=False, w_mae=1.0, w_mse=1.0, fan=None, gaps=True, arena_len=None, layout=None):
+    """fp32 operands of the fused FCNN step on which every product and partial sum of the kernel is exact, so that its pred, loss
+    and gradients equal ``fcnn_step``'s bit for bit.  ``bias``: one bool per layer.  Returns a dict: x [M, dims[0]], y or dpred
+    [M, nout], params (the arena, NaN in every gap), woff, boff, and the planted zeros: relu_zeros [(layer, row, unit)] whose ReLU
+    input is exactly 0, residual_zeros [(row, unit)] where pred - y is exactly 0.
+
+    Values are small integers times a power of two: x in [-3, 3] 2^ex; W_l in {-1, 0, 1} (one nonzero in 16 is +-3; hidden layers
+    three quarters positive, or all where a unit has one input, so that units stay alive) times 2^e_l, each weight nonzero with probability fan / min(in, out), so that
+    activation l is a multiple of q_l = 2^(ex + e_0 + ... + e_{l-1}); b_l in [-2, 4] q_{l+1} (the output layer's in [-4, 4]); dpred
+    in [-3, 3] 2^ed; y = pred + {-2, -1, 1, 2} q_L.  Exponents differ per layer, so a value taken from the wrong layer is off by a power
+    of two.  Planted zeros: in hidden layers with a bias, the bias of every unit j = 1 mod 3 is minus its pre-activation on one row
+    (a ReLU input of exactly 0); in hidden layers without one, one unit's weights are all 0; residuals 2, 7, 12, ... (row-major) are
+    exactly 0.
+
+    Asserts that every intermediate stays under FCNN_BUDGET units of its quantum, measured on the network run on absolute values:
+    forward sums, y and the residuals, the loss terms summed over all rows, the output gradient, every weight and bias gradient
+    summed over all M rows (which bounds each 128-row block and the sum of the blocks), and every input gradient.  Without ``fan``
+    the densest of FCNN_FANS that keeps the budget is taken.  ``y=True`` (the fused loss) needs M nout a power of two: the kernel's
+    fp32 1 / (M nout) is exact only then.  ``layout`` = (woff, boff, P) places the tensors as given; otherwise they go in a shuffled
+    order with gaps of 0..5 floats (``gaps``), the arena padded to ``arena_len``."""
+    if fan is None:
+        for f in FCNN_FANS[:-1]:
+            try:
+                return exact_fcnn_operands(dims, M, bias, seed, y=y, w_mae=w_mae, w_mse=w_mse, fan=f, gaps=gaps, arena_len=arena_len,
+                                           layout=layout)
+            except AssertionError as err:
+                if "budget" not in str(err):
+                    raise
+        fan = FCNN_FANS[-1]
+    L, nout = len(dims) - 1, dims[-1]
+    n = M * nout
+    assert not y or n & (n - 1) == 0, f"the fused loss is exact only for M nout a power of two, not {n}"
+    g = torch.Generator().manual_seed(seed)
+    ri = lambda lo, hi, shape=(): torch.randint(lo, hi + 1, shape, generator=g).to(F64)  # noqa: E731
+    ex, ed = int(ri(-3, 3)), int(ri(-3, 3))
+    cum = [ex]  # log2 of each activation's quantum: steps of -2..2, kept within [-4, 4]
+    for _ in range(L):
+        cum.append(min(4, max(-4, cum[-1] + int(ri(-2, 2)))))
+    es = [c1 - c0 for c0, c1 in zip(cum, cum[1:])]
+    qs = [2.0 ** c for c in cum]
+    x = ri(-3, 3, (M, dims[0])) * qs[0]
+    Ws, bs, relu_zeros, a = [], [], [], x
+    for l in range(L):
+        n_in, n_out, hidden = dims[l], dims[l + 1], l + 1 < L
+        u = lambda: torch.rand(n_out, n_in, generator=g, dtype=F64)  # noqa: E731
+        sign = torch.where(u() < (0.5 if not hidden else 0.25 if n_in > 1 else 0.0), -1.0, 1.0)
+        mag = torch.where(u() < 1 / 16, 3.0, 1.0)
+        wi = torch.where(u() < fan / min(n_in, n_out), sign * mag, 0.0).to(F64)
+        if hidden and not bias[l] and n_out > 1:
+            j = int(ri(0, n_out - 1))
+            wi[j] = 0.0
+            relu_zeros += [(l, r, j) for r in range(M)]
+        W = wi * 2.0 ** es[l]
+        z = a @ W.t() + 0.0
+        b = None
+        if bias[l]:
+            b = ri(-2 if hidden else -4, 4, (n_out,)) * qs[l + 1]
+            if hidden:
+                for j in range(1, n_out, 3):
+                    r = int(ri(0, M - 1))
+                    b[j] = -z[r, j] + 0.0
+                    relu_zeros.append((l, r, j))
+            z = z + b + 0.0
+        Ws.append(W)
+        bs.append(b)
+        a = torch.relu(z) if hidden else z
+    pred, residual_zeros = a, []
+    if y:
+        di = ri(1, 2, (M, nout)) * torch.where(torch.rand(M, nout, generator=g) < 0.5, -1.0, 1.0).to(F64)
+        di.view(-1)[2::5] = 0.0
+        residual_zeros = [divmod(i, nout) for i in range(2, n, 5)]
+        target = pred + di * qs[L] + 0.0
+    else:
+        target = ri(-3, 3, (M, nout)) * 2.0 ** ed
+
+    def check(units, what):
+        worst = units.max().item()
+        assert worst < FCNN_BUDGET, f"{what}: {worst:.0f} units, over the 2^24 budget"
+
+    A = [x.abs()]
+    for l in range(L):
+        A.append(A[l] @ Ws[l].abs().t() + (0.0 if bs[l] is None else bs[l].abs()))
+        check(A[l + 1] / qs[l + 1], f"layer {l} forward sum")
+    if y:
+        d = pred - target
+        check(target.abs() / qs[L], "y")
+        check(d.abs() / qs[L], "residual")
+        qt = min([_quantum(w) * q for w, q in ((w_mae, qs[L]), (w_mse, qs[L] ** 2)) if w != 0] or [1.0])
+        check((w_mae * d.abs() + w_mse * d * d).sum() / qt, "loss sum")
+        D = ((w_mae * torch.sign(d) + 2 * w_mse * d) / n).abs()
+        G = min([_quantum(w) * q for w, q in ((w_mae, 1.0), (w_mse, 2 * qs[L])) if w != 0] or [1.0]) / n
+    else:
+        D, G = target.abs(), 2.0 ** ed
+    check(D / G, "output gradient")
+    for l in reversed(range(L)):
+        check((D.t() @ A[l]) / (G * qs[l]), f"layer {l} weight gradient")
+        check(D.sum(0) / G, f"layer {l} bias gradient")
+        if l > 0:
+            D, G = D @ Ws[l].abs(), G * 2.0 ** es[l]
+            check(D / G, f"layer {l} input gradient")
+    assert min(qs + [G]) >= 2.0 ** -100, "a quantum near fp32's subnormal range"
+
+    names = [("w", l) for l in range(L)] + [("b", l) for l in range(L) if bias[l]]
+    if layout is not None:
+        woff, boff, P = list(layout[0]), list(layout[1]), layout[2]
+    else:
+        if gaps:
+            names = [names[i] for i in torch.randperm(len(names), generator=g).tolist()]
+        woff, boff, cur = [0] * L, [-1] * L, 0
+        for kind, l in names:
+            cur += int(ri(0, 5)) if gaps else 0
+            (woff if kind == "w" else boff)[l] = cur
+            cur += dims[l] * dims[l + 1] if kind == "w" else dims[l + 1]
+        P = cur + (int(ri(1, 3)) if gaps else 0)
+        if arena_len is not None:
+            assert arena_len >= P, f"the network needs {P} floats, more than arena_len {arena_len}"
+            P = arena_len
+    params = torch.full((P,), float("nan"), dtype=F64)
+    for l in range(L):
+        params[woff[l]:woff[l] + Ws[l].numel()] = Ws[l].reshape(-1)
+        if bs[l] is not None:
+            params[boff[l]:boff[l] + dims[l + 1]] = bs[l]
+    out = dict(x=x.float(), params=params.float(), woff=woff, boff=boff, relu_zeros=relu_zeros, residual_zeros=residual_zeros)
+    out["y" if y else "dpred"] = target.float()
+    for name in ("x", "params", "y" if y else "dpred"):
+        v, t = out[name].double(), {"x": x, "params": params}.get(name, target)
+        assert torch.equal(v[~t.isnan()], t[~t.isnan()]), f"{name} not exact in fp32"
+    return out

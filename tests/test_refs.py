@@ -228,3 +228,63 @@ def test_resample_and_per_image_references():
     per, tot = refs.colsum_per_image(x)
     assert torch.allclose(per.float(), torch.stack([x[b].reshape(-1, 5).sum(0) for b in range(2)]), atol=1e-5)
     assert torch.allclose(tot.float(), x.reshape(-1, 5).sum(0), atol=1e-5)
+
+
+def test_fcnn_reference():
+    """fcnn_step against torch's autograd of the same float64 network (Linear, ReLU, l1_loss, mse_loss) on an arena with gaps and a
+    layer without bias, with ReLU inputs and residuals planted at exactly 0; fcnn_bounds returns the same values."""
+    g = torch.Generator().manual_seed(8)
+    dims, woff, boff, P = [5, 7, 6, 3], [50, 0, 100], [90, -1, 120], 126
+    halves = lambda *shape: torch.randint(-6, 7, shape, generator=g).to(F64) / 2  # noqa: E731  (sums exact: the zeros below are 0)
+    params = torch.full((P,), float("nan"), dtype=F64)
+    x = halves(9, 5)
+    for l in range(3):
+        params[woff[l]:woff[l] + dims[l] * dims[l + 1]] = halves(dims[l] * dims[l + 1])
+        if boff[l] >= 0:
+            params[boff[l]:boff[l] + dims[l + 1]] = halves(dims[l + 1])
+    # pre-activation of unit 2, row 4 exactly 0 (the bias cancels it)
+    W0 = params[woff[0]:woff[0] + 35].view(7, 5)
+    params[boff[0] + 2] = -(x[4] @ W0[2])
+    y, dpred = halves(9, 3) + 0.25, halves(9, 3)
+    keys = [(woff[l], dims[l] * dims[l + 1]) for l in range(3)] + [(boff[l], dims[l + 1]) for l in range(3) if boff[l] >= 0]
+
+    def autograd(target, w, use_dpred):
+        leaves = [params[o:o + n].clone().requires_grad_(True) for o, n in keys]
+        W = [leaves[l].view(dims[l + 1], dims[l]) for l in range(3)]
+        b = {0: leaves[3], 2: leaves[4]}
+        a = x
+        for l in range(3):
+            a = F.linear(a, W[l], b.get(l))
+            if l < 2:
+                a = torch.relu(a)
+        pred = a
+        if use_dpred:
+            pred.backward(target)
+            loss = None
+        else:
+            loss = w[0] * F.l1_loss(pred, target) + w[1] * F.mse_loss(pred, target)
+            loss.backward()
+        grads = torch.zeros(P, dtype=F64)
+        for (o, n), t in zip(keys, leaves):
+            grads[o:o + n] = t.grad
+        return pred.detach(), loss, grads
+
+    _, acts = refs.fcnn_forward(x, refs.fcnn_layers(params, dims, woff, boff))
+    y_zero = y.clone()
+    y_zero[1, 2] = acts[-1][1, 2]  # residual exactly 0: sign(0) = 0
+    assert acts[1][4, 2] == 0
+    for kw, w in ((dict(y=y_zero), (0.5, 2.0)), (dict(y=y), (1.0, 0.0)), (dict(dpred=dpred), (1.0, 1.0))):
+        pred, loss, grads = refs.fcnn_step(x, params, dims, woff, boff, w_mae=w[0], w_mse=w[1], **kw)
+        want_pred, want_loss, want_grads = autograd(kw.get("y", kw.get("dpred")), w, "dpred" in kw)
+        assert torch.allclose(pred, want_pred, rtol=1e-12, atol=1e-12)
+        assert (loss is None) == (want_loss is None) and (loss is None or torch.allclose(loss, want_loss, rtol=1e-12))
+        bad = ~torch.isclose(grads, want_grads, rtol=1e-10, atol=1e-12)
+        assert not bad.any(), (kw.keys(), torch.nonzero(bad).flatten().tolist(), grads[bad], want_grads[bad])
+        gaps = torch.ones(P, dtype=torch.bool)
+        for o, n in keys:
+            gaps[o:o + n] = False
+        assert (grads[gaps] == 0).all() and not torch.signbit(grads).logical_and(grads == 0).any()
+        (p2, l2, g2), (tp, tl, tg) = refs.fcnn_bounds(x, params, dims, woff, boff, w_mae=w[0], w_mse=w[1], **kw)
+        assert torch.equal(p2, pred) and torch.equal(g2, grads) and (l2 is None or torch.equal(l2, loss))
+        assert tp.shape == pred.shape and tg.shape == grads.shape and (tp > 0).all() and (tg[~gaps] >= 0).all()
+        assert (tl is None) == (loss is None) and (tl is None or tl > 0)
