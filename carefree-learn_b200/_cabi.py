@@ -103,6 +103,8 @@ EXT_SIGNATURES: Dict[str, Any] = {
     "b200_conv3x3_up2_nhwc_bf16": (c_int, [_P, _P, _P, _P, _P, _LL, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     "b200_upsample_nearest2x_bf16": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
     "b200_sum2x2_bf16": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
+    "b200_pad_channels_bf16": (c_int, [_P, c_int, c_int, _P, c_int, c_int, c_int, c_int, c_int, _P]),
+    "b200_noise_prediction_loss_bf16": (c_int, [_P, _P, c_int, _P, _P, _P, c_int, _LL, _P]),
 }
 
 _lib: Optional[ctypes.CDLL] = None

@@ -863,3 +863,48 @@ def sum2x2(x: Tensor) -> Tensor:
     out = torch.empty((B, H2 // 2, W2 // 2, C), dtype=torch.bfloat16, device=x.device)
     call("b200_sum2x2_bf16", x.data_ptr(), out.data_ptr(), B, H2 // 2, W2 // 2, C, _stream())
     return out
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# the two ends of the SD-v1.5 UNet's training step (include/b200_cflearn_ext.h)
+# ----------------------------------------------------------------------------------------------------------------
+def _layout(what: str, name: str, t: Tensor, dtypes: Tuple[torch.dtype, ...]) -> bool:
+    """True for a dense channels-last [B, C, H, W] CUDA tensor, False for a contiguous NCHW one; anything else is refused."""
+    ok = t is not None and t.is_cuda and t.dtype in dtypes and t.dim() == 4
+    cl = ok and t.is_contiguous(memory_format=torch.channels_last)
+    if not ok or not (cl or t.is_contiguous()):
+        got = "None" if t is None else f"{t.dtype} {list(t.shape)} with strides {list(t.stride())} on {t.device}"
+        raise B200Error(f"{what}: {name} must be a CUDA {' or '.join(str(d) for d in dtypes)} tensor [B, C, H, W], contiguous NCHW or "
+                        f"channels-last (got {got})")
+    return cl and not t.is_contiguous()
+
+
+def pad_channels(x: Tensor, cp: int) -> Tensor:
+    """x fp32 or bf16 [B, C, H, W] (contiguous NCHW or channels-last) -> bf16 [B, H, W, cp] with channels >= C zero: the
+    round-to-nearest-even cast autocast applies, then zero padding to a width the convolutions take."""
+    cl = _layout("pad_channels", "x", x, (_F32, _BF16))
+    B, C, H, W = x.shape
+    out = torch.empty((B, H, W, cp), dtype=torch.bfloat16, device=x.device)
+    call("b200_pad_channels_bf16", x.data_ptr(), int(x.dtype == _F32), int(cl), out.data_ptr(), B, C, H, W, cp, _stream())
+    return out
+
+
+def noise_prediction_loss(pred: Tensor, noise: Tensor, *, grad_out: Optional[Tensor] = None) -> Tensor:
+    """The DDPM noise-prediction loss mean_b(mean_chw((pred - noise)^2)) of pred bf16 [B, C, H, W] and noise (fp32 or bf16, the
+    same shape and memory format; contiguous NCHW or channels-last).  Without ``grad_out``: the fp32 loss [1].  With it (fp32
+    [1] on the device, the loss's upstream gradient): d loss / d pred, bf16 in pred's layout."""
+    what = "noise_prediction_loss"
+    cl = _layout(what, "pred", pred, (_BF16,))
+    if _layout(what, "noise", noise, (_F32, _BF16)) != cl or noise.shape != pred.shape:
+        raise B200Error(f"{what}: noise must have pred's shape {list(pred.shape)} and memory format")
+    _check(what, "grad_out", grad_out, _F32, (1,), optional=True)
+    B = pred.shape[0]
+    N = pred.numel() // max(B, 1)
+    loss = dpred = None
+    if grad_out is None:
+        loss = torch.empty(1, dtype=torch.float32, device=pred.device)
+    else:
+        dpred = torch.empty_like(pred)
+    call("b200_noise_prediction_loss_bf16", pred.data_ptr(), noise.data_ptr(), int(noise.dtype == _F32), _ptr(loss), _ptr(dpred),
+         _ptr(grad_out), B, N, _stream())
+    return loss if grad_out is None else dpred

@@ -64,6 +64,29 @@ int b200_upsample_nearest2x_bf16(const void* x, void* out, int B, int H, int W, 
  * out [B, H, W, C] (dense) from x [B, 2H, 2W, C] (dense); C % 8 == 0. */
 int b200_sum2x2_bf16(const void* x, void* out, int B, int H, int W, int C, cudaStream_t stream);
 
+/* ---------------------------------------------------------------------------------------------------------
+ * The two ends of the SD-v1.5 UNet's training step (cflearn/modules/multimodal/diffusion/unet.py:215-275 and
+ * cflearn/models/cv/diffusion.py:44-94).
+ * --------------------------------------------------------------------------------------------------------- */
+
+/* Channel padding: out [B, H, W, Cp] bf16 (dense, channels-last) from x [B, C, H, W], channels >= C set to +0.  x is fp32
+ * (x_f32 = 1, rounded to nearest even) or bf16 (copied bit for bit), dense NCHW (x_channels_last = 0) or dense channels-last
+ * (1).  0 < C <= Cp, Cp % 8 == 0, H * W < 2^31, B * H * W * Cp <= 2^38.  The 4-channel stem and head run on the 64-channel
+ * convolutions through it. */
+int b200_pad_channels_bf16(const void* x, int x_f32, int x_channels_last, void* out, int B, int C, int H, int W, int Cp,
+                           cudaStream_t stream);
+
+/* The DDPM noise-prediction loss at DDPMStep's defaults (l2, eps parameterization, l_simple_weight 1, log_var 0, no ELBO
+ * term): mean over b of (mean over the N = C H W elements of image b of (pred - noise)^2).  pred: bf16, noise: fp32
+ * (noise_f32 = 1) or bf16, both [B, N] rows (the images of NCHW and of channels-last tensors alike), in the same layout.  Give
+ * exactly one of
+ *   loss (fp32 [1]): the loss, in a fixed order (one CTA: per-image partials, then their mean), bit-identical run to run;
+ *   dpred (bf16 [B, N], pred's layout) with grad_out (fp32 [1] on the device, the loss's upstream gradient): the gradient with
+ *   eager's fp32 operations, bf16(fl(2 fl(pred - noise)) fl(fl(grad_out fl(1/B)) fl(1/N))).
+ * B * N <= 2^38.  Each call is one launch. */
+int b200_noise_prediction_loss_bf16(const void* pred, const void* noise, int noise_f32, float* loss, void* dpred,
+                                    const float* grad_out, int B, long long N, cudaStream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
