@@ -69,35 +69,42 @@ def attention_forward(x: Tensor, c: Optional[Tensor], wq: Tensor, wk: Tensor, wv
     return y, (x, c, q, k, v, o, lse, w_in, w_kv, w_o)
 
 
-def attention_backward(saved: tuple, dy: Tensor, B: int, heads: int):
+def attention_backward(saved: tuple, dy: Tensor, B: int, heads: int, pg: Optional[checkpoint.ParamGrads] = None):
     """Backward of ``attention_forward`` for dy bf16 [B*Tq, Dq] (the gradient of y; with ``resid`` the residual's own
     gradient is dy as well, which the caller adds).  Returns (dx bf16, dc bf16 or None, dwq, dwk, dwv, dwo, dbo), the weight
-    and bias gradients fp32 and rounded to bf16 like eager's."""
+    and bias gradients fp32 and rounded to bf16 like eager's.  ``pg``: where they go, numbered wq, wk, wv, wo, bo from 0
+    (default: fresh tensors)."""
     x, c, q, k, v, o, lse, w_in, w_kv, w_o = saved
     M, Dq = x.shape
     L = q.shape[1]
-    dwo = torch.empty(w_o.shape, dtype=torch.float32, device=dy.device)
-    dbo = torch.empty(Dq, dtype=torch.float32, device=dy.device)
-    ops.wgrad(dy, o, dwo)
-    ops.colsum(dy, dbo)
+    dev = dy.device
+    pg = pg or checkpoint.NO_GRADS
+    dwo = pg.out(3, tuple(w_o.shape), dev)
+    dbo = pg.out(4, (Dq,), dev)
+    ops.wgrad(dy, o, dwo, **pg.mode)
+    ops.colsum(dy, dbo, **pg.mode)
     do = ops.gemm(dy, w_o, b_mn_major=True)
     if c is None:
-        dqkv = torch.empty((M, 3 * L), dtype=torch.bfloat16, device=dy.device)
+        dqkv = torch.empty((M, 3 * L), dtype=torch.bfloat16, device=dev)
         ops.cross_attention_bwd(q, k, v, o, do, lse, B, heads, dq=dqkv[:, :L], dk=dqkv[:, L:2 * L], dv=dqkv[:, 2 * L:])
-        dw = torch.empty((3 * L, Dq), dtype=torch.float32, device=dy.device)
-        ops.wgrad(dqkv, x, dw)
+        dw, direct = pg.span((0, 1, 2), (3 * L, Dq), dev)  # the arena views of [Wq; Wk; Wv] when they are adjacent
+        ops.wgrad(dqkv, x, dw, **(pg.mode if direct else {}))
         dwq, dwk, dwv = dw[:L], dw[L:2 * L], dw[2 * L:]
+        if not direct:
+            dwq, dwk, dwv = pg.put(0, dwq), pg.put(1, dwk), pg.put(2, dwv)
         dx = ops.gemm(dqkv, w_in, b_mn_major=True)
         dc = None
     else:
-        dq = torch.empty((M, L), dtype=torch.bfloat16, device=dy.device)
-        dkv = torch.empty((c.shape[0], 2 * L), dtype=torch.bfloat16, device=dy.device)
+        dq = torch.empty((M, L), dtype=torch.bfloat16, device=dev)
+        dkv = torch.empty((c.shape[0], 2 * L), dtype=torch.bfloat16, device=dev)
         ops.cross_attention_bwd(q, k, v, o, do, lse, B, heads, dq=dq, dk=dkv[:, :L], dv=dkv[:, L:])
-        dwq = torch.empty((L, Dq), dtype=torch.float32, device=dy.device)
-        dwkv = torch.empty((2 * L, c.shape[1]), dtype=torch.float32, device=dy.device)
-        ops.wgrad(dq, x, dwq)
-        ops.wgrad(dkv, c, dwkv)
+        dwq = pg.out(0, (L, Dq), dev)
+        dwkv, direct = pg.span((1, 2), (2 * L, c.shape[1]), dev)
+        ops.wgrad(dq, x, dwq, **pg.mode)
+        ops.wgrad(dkv, c, dwkv, **(pg.mode if direct else {}))
         dwk, dwv = dwkv[:L], dwkv[L:]
+        if not direct:
+            dwk, dwv = pg.put(1, dwk), pg.put(2, dwv)
         dx = ops.gemm(dq, w_in, b_mn_major=True)
         dc = ops.gemm(dkv, w_kv, b_mn_major=True)
     return dx, dc, dwq, dwk, dwv, dwo, dbo
@@ -113,8 +120,9 @@ class _AttentionOp:
         y, saved = attention_forward(_rows(net), _rows(context), *params, self.B, self.heads)
         return y.view(net.shape), saved
 
-    def backward(self, saved: tuple, dy: Tensor) -> tuple:
-        return attention_backward(saved, _rows(dy), self.B, self.heads)
+    def backward(self, saved: tuple, dy: Tensor, pg: Optional[checkpoint.ParamGrads] = None) -> tuple:
+        pg = pg or checkpoint.NO_GRADS
+        return attention_backward(saved, _rows(dy), self.B, self.heads, pg.sub(2))
 
 
 class _Linear(nn.Module):

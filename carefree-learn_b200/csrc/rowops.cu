@@ -13,6 +13,7 @@
 
 #include "b200_internal.h"
 #include "ptx.cuh"
+#include "../../include/b200_cflearn_ext.h"
 
 namespace b200 {
 
@@ -898,7 +899,9 @@ __global__ void fill_f32_kernel(float* __restrict__ dst, float v, long long n) {
     else for (long long k = i; k < n; ++k) dst[k] = v;
 }
 
-// Adam over the flat parameter arena (torch.optim.Adam semantics, no amsgrad; L2 weight decay added to the grad)
+// Adam over the flat parameter arena (torch.optim.Adam semantics, no amsgrad; L2 weight decay added to the grad).
+// kDecoupled: AdamW (torch.optim.AdamW's order): p <- p (1 - lr wd) first, then the Adam update with no L2 term.
+template <bool kDecoupled>
 __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
                             float* __restrict__ v, long long n4, float lr, float b1, float b2, float eps, float wd,
                             float bc1, float bc2_sqrt, const int* __restrict__ step_dev) {
@@ -914,8 +917,10 @@ __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, 
     float4 mm = reinterpret_cast<float4*>(m)[i];
     float4 vv = reinterpret_cast<float4*>(v)[i];
     const float step = lr / bc1;
+    const float keep = 1.0f - lr * wd;
     auto upd = [&](float& pw, float gw, float& mw, float& vw) {
-        gw += wd * pw;
+        if (kDecoupled) pw *= keep;
+        else gw += wd * pw;
         mw += (gw - mw) * (1.0f - b1);
         vw = vw * b2 + (1.0f - b2) * gw * gw;
         const float denom = sqrtf(vw) / bc2_sqrt + eps;
@@ -935,7 +940,8 @@ __global__ void increment_kernel(int* counter) { counter[0] += 1; }
 // Same update with EVERY hyper-parameter read from device memory (hyper = {lr, beta1, beta2, eps, weight_decay, grad_scale}):
 // a captured CUDA graph then follows a learning-rate schedule (the reference's default scheduler is "warmup",
 // cflearn/pipeline/blocks/basic.py:334-352) by rewriting 24 bytes between replays.  grad_scale multiplies the gradient
-// first (1 / world_size after a SUM all-reduce, or a clip coefficient, cflearn/schema.py:981-982).
+// first (1 / world_size after a SUM all-reduce, or a clip coefficient, cflearn/schema.py:981-982).  kDecoupled as adam_kernel.
+template <bool kDecoupled>
 __global__ void adam_dev_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
                                 float* __restrict__ v, long long n4, const float* __restrict__ hyper,
                                 const int* __restrict__ step_dev) {
@@ -950,8 +956,14 @@ __global__ void adam_dev_kernel(float* __restrict__ p, const float* __restrict__
     float4 mm = reinterpret_cast<float4*>(m)[i];
     float4 vv = reinterpret_cast<float4*>(v)[i];
     const float step = lr / bc1;
+    const float keep = 1.0f - lr * wd;
     auto upd = [&](float& pw, float gw, float& mw, float& vw) {
-        gw = gw * gs + wd * pw;
+        if (kDecoupled) {
+            pw *= keep;
+            gw *= gs;
+        } else {
+            gw = gw * gs + wd * pw;
+        }
         mw += (gw - mw) * (1.0f - b1);
         vw = vw * b2 + (1.0f - b2) * gw * gw;
         const float denom = sqrtf(vw) / bc2_sqrt + eps;
@@ -1354,10 +1366,9 @@ extern "C" int b200_cast_f32_to_bf16(const float* src, void* dst_bf16, long long
     cast_f32_bf16_kernel<<<static_cast<unsigned>((thr + 255) / 256), 256, 0, stream>>>(src, reinterpret_cast<__nv_bfloat16*>(dst_bf16), n);
     return check_launch("cast_f32_bf16");
 }
-extern "C" int b200_adam_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n,
-                              float lr, float beta1, float beta2, float eps, float weight_decay, int step,
-                              int* step_dev, cudaStream_t stream) {
-    const char* E = "adam_step";
+template <bool kDecoupled>
+static int adam_step_host(const char* E, float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n, float lr,
+                          float beta1, float beta2, float eps, float weight_decay, int step, int* step_dev, cudaStream_t stream) {
     if (n <= 0 || n % 4 != 0) return refuse(B200_ERR_ARG, E, "n must be a positive multiple of 4");
     if (step_dev == nullptr && step < 1) return refuse(B200_ERR_ARG, E, "step >= 1 (or pass step_dev)");
     if (!params || !grads || !exp_avg || !exp_avg_sq) return refuse(B200_ERR_ARG, E, "null pointer");
@@ -1372,13 +1383,14 @@ extern "C" int b200_adam_step(float* params, const float* grads, float* exp_avg,
     const float bc1 = 1.0f - powf(beta1, t);
     const float bc2_sqrt = sqrtf(1.0f - powf(beta2, t));
     const long long n4 = n / 4;
-    adam_kernel<<<static_cast<unsigned>((n4 + 255) / 256), 256, 0, stream>>>(params, grads, exp_avg, exp_avg_sq, n4, lr, beta1,
-                                                                          beta2, eps, weight_decay, bc1, bc2_sqrt, step_dev);
-    return check_launch("adam_step");
+    adam_kernel<kDecoupled><<<static_cast<unsigned>((n4 + 255) / 256), 256, 0, stream>>>(params, grads, exp_avg, exp_avg_sq, n4, lr,
+                                                                                      beta1, beta2, eps, weight_decay, bc1, bc2_sqrt,
+                                                                                      step_dev);
+    return check_launch(E);
 }
-extern "C" int b200_adam_step_dev(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n,
-                                  const float* hyper_dev, int* step_dev, int increment, cudaStream_t stream) {
-    const char* E = "adam_step_dev";
+template <bool kDecoupled>
+static int adam_step_dev_host(const char* E, float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n,
+                              const float* hyper_dev, int* step_dev, int increment, cudaStream_t stream) {
     if (n <= 0 || n % 4 != 0) return refuse(B200_ERR_ARG, E, "n must be a positive multiple of 4");
     if (!params || !grads || !exp_avg || !exp_avg_sq || !hyper_dev || !step_dev) return refuse(B200_ERR_ARG, E, "null pointer");
     if (!aligned(16, {params, grads, exp_avg, exp_avg_sq})) return refuse(B200_ERR_ALIGN, E, "arenas not 16-byte aligned");
@@ -1389,8 +1401,29 @@ extern "C" int b200_adam_step_dev(float* params, const float* grads, float* exp_
         if (rc) return rc;
     }
     const long long n4 = n / 4;
-    adam_dev_kernel<<<static_cast<unsigned>((n4 + 255) / 256), 256, 0, stream>>>(params, grads, exp_avg, exp_avg_sq, n4, hyper_dev, step_dev);
-    return check_launch("adam_step_dev");
+    adam_dev_kernel<kDecoupled><<<static_cast<unsigned>((n4 + 255) / 256), 256, 0, stream>>>(params, grads, exp_avg, exp_avg_sq, n4,
+                                                                                          hyper_dev, step_dev);
+    return check_launch(E);
+}
+extern "C" int b200_adam_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n,
+                              float lr, float beta1, float beta2, float eps, float weight_decay, int step,
+                              int* step_dev, cudaStream_t stream) {
+    return adam_step_host<false>("adam_step", params, grads, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps, weight_decay, step,
+                                 step_dev, stream);
+}
+extern "C" int b200_adam_step_dev(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n,
+                                  const float* hyper_dev, int* step_dev, int increment, cudaStream_t stream) {
+    return adam_step_dev_host<false>("adam_step_dev", params, grads, exp_avg, exp_avg_sq, n, hyper_dev, step_dev, increment, stream);
+}
+extern "C" int b200_adamw_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n,
+                               float lr, float beta1, float beta2, float eps, float weight_decay, int step,
+                               int* step_dev, cudaStream_t stream) {
+    return adam_step_host<true>("adamw_step", params, grads, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps, weight_decay, step,
+                                step_dev, stream);
+}
+extern "C" int b200_adamw_step_dev(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n,
+                                   const float* hyper_dev, int* step_dev, int increment, cudaStream_t stream) {
+    return adam_step_dev_host<true>("adamw_step_dev", params, grads, exp_avg, exp_avg_sq, n, hyper_dev, step_dev, increment, stream);
 }
 extern "C" int b200_fill_f32(float* dst, float value, long long n, cudaStream_t stream) {
     const char* E = "fill";

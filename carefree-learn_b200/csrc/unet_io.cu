@@ -1,5 +1,6 @@
 // The two ends of the SD-v1.5 UNet's training step (include/b200_cflearn_ext.h): the channel padding that lets the 4-channel
-// stem and head run on the 64-channel implicit-GEMM convolutions, and the DDPM noise-prediction loss with its gradient.
+// stem and head run on the 64-channel implicit-GEMM convolutions (plain, or fused with the DDPM noising of the latent), and the
+// DDPM noise-prediction loss with its gradient.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -16,8 +17,15 @@ namespace b200 {
 __device__ __forceinline__ uint16_t to_bf16_bits(float v) { return __bfloat16_as_ushort(__float2bfloat16_rn(v)); }
 __device__ __forceinline__ uint16_t to_bf16_bits(uint16_t v) { return v; }
 
-template <typename T, bool kChannelsLast>
-__global__ void pad_channels_kernel(const T* __restrict__ x, uint4* __restrict__ out, long long groups, int C, int HW, int Cp8) {
+// The element reads are a Source's: src(i, b) returns the bf16 bits of element i (of image b) of the real channels.
+template <typename T>
+struct CastSource {
+    const T* x;
+    __device__ __forceinline__ uint16_t operator()(long long i, long long) const { return to_bf16_bits(x[i]); }
+};
+
+template <bool kChannelsLast, typename Source>
+__global__ void pad_channels_kernel(Source src, uint4* __restrict__ out, long long groups, int C, int HW, int Cp8) {
     const long long g = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (g >= groups) return;
     const int c0 = static_cast<int>(g % Cp8) * 8;
@@ -29,11 +37,40 @@ __global__ void pad_channels_kernel(const T* __restrict__ x, uint4* __restrict__
     for (int k = 0; k < 4; ++k) {
         uint32_t lo = 0, hi = 0;
         const int c = c0 + 2 * k;
-        if (c < C) lo = to_bf16_bits(kChannelsLast ? x[pix * C + c] : x[(b * C + c) * HW + p]);
-        if (c + 1 < C) hi = to_bf16_bits(kChannelsLast ? x[pix * C + c + 1] : x[(b * C + c + 1) * HW + p]);
+        if (c < C) lo = src(kChannelsLast ? pix * C + c : (b * C + c) * HW + p, b);
+        if (c + 1 < C) hi = src(kChannelsLast ? pix * C + c + 1 : (b * C + c + 1) * HW + p, b);
         w[k] = lo | (hi << 16);
     }
     out[g] = make_uint4(w[0], w[1], w[2], w[3]);
+}
+
+// ---- DDPM noising ----------------------------------------------------------------------------------------------------------------
+// bf16(fl(fl(a[t_b] x0) + fl(s[t_b] noise))): q_sample's `w_net * net + w_noise * noise` in fp32 with no contraction, then autocast's
+// cast at the stem.  A timestep outside [0, T) reads no table entry: it sets *bad and the image's elements become NaN.
+struct QSampleSource {
+    const float* x0;
+    const float* noise;
+    const long long* t;
+    const float* a;
+    const float* s;
+    long long T;
+    int* bad;
+    __device__ __forceinline__ uint16_t operator()(long long i, long long b) const {
+        const long long tb = t[b];
+        if (tb < 0 || tb >= T) {
+            atomicExch(bad, 1);
+            return 0x7fc0u;  // bf16 NaN
+        }
+        return to_bf16_bits(__fadd_rn(__fmul_rn(a[tb], x0[i]), __fmul_rn(s[tb], noise[i])));
+    }
+};
+
+template <typename Source>
+static void launch_pad(Source src, bool channels_last, uint4* out, int B, int C, int H, int W, int Cp, cudaStream_t stream) {
+    const long long groups = static_cast<long long>(B) * H * W * (Cp / 8);
+    const unsigned grid = static_cast<unsigned>((groups + 255) / 256);
+    if (channels_last) pad_channels_kernel<true><<<grid, 256, 0, stream>>>(src, out, groups, C, H * W, Cp / 8);
+    else pad_channels_kernel<false><<<grid, 256, 0, stream>>>(src, out, groups, C, H * W, Cp / 8);
 }
 
 // ---- the noise-prediction loss ---------------------------------------------------------------------------------------------------
@@ -103,14 +140,9 @@ extern "C" int b200_pad_channels_bf16(const void* x, int x_f32, int x_channels_l
     if (x == nullptr || out == nullptr) return refuse(B200_ERR_ARG, E, "null pointer");
     if (!aligned(x_f32 ? 4 : 2, {x})) return refuse(B200_ERR_ALIGN, E, "x not aligned to its element size");
     if (!aligned(16, {out})) return refuse(B200_ERR_ALIGN, E, "out not 16-byte aligned");
-    const long long groups = static_cast<long long>(B) * H * W * (Cp / 8);
-    const unsigned grid = static_cast<unsigned>((groups + 255) / 256);
     uint4* o = reinterpret_cast<uint4*>(out);
-    const int HW = H * W;
-    if (x_f32 && x_channels_last) pad_channels_kernel<float, true><<<grid, 256, 0, stream>>>(static_cast<const float*>(x), o, groups, C, HW, Cp / 8);
-    else if (x_f32) pad_channels_kernel<float, false><<<grid, 256, 0, stream>>>(static_cast<const float*>(x), o, groups, C, HW, Cp / 8);
-    else if (x_channels_last) pad_channels_kernel<uint16_t, true><<<grid, 256, 0, stream>>>(static_cast<const uint16_t*>(x), o, groups, C, HW, Cp / 8);
-    else pad_channels_kernel<uint16_t, false><<<grid, 256, 0, stream>>>(static_cast<const uint16_t*>(x), o, groups, C, HW, Cp / 8);
+    if (x_f32) launch_pad(CastSource<float>{static_cast<const float*>(x)}, x_channels_last != 0, o, B, C, H, W, Cp, stream);
+    else launch_pad(CastSource<uint16_t>{static_cast<const uint16_t*>(x)}, x_channels_last != 0, o, B, C, H, W, Cp, stream);
     return check_launch("pad_channels");
 }
 
@@ -140,4 +172,25 @@ extern "C" int b200_noise_prediction_loss_bf16(const void* pred, const void* noi
     if (noise_f32) noise_loss_grad_kernel<<<grid, 256, 0, stream>>>(p, nf, total, inv_b, inv_n, grad_out, d);
     else noise_loss_grad_kernel<<<grid, 256, 0, stream>>>(p, nb, total, inv_b, inv_n, grad_out, d);
     return check_launch("noise_prediction_loss_grad");
+}
+
+extern "C" int b200_q_sample_pad_bf16(const float* x0, const float* noise, int channels_last, const long long* timesteps,
+                                      const float* sqrt_alphas_cumprod, const float* sqrt_one_minus_alphas_cumprod, long long T,
+                                      int* bad_flag, void* out, int B, int C, int H, int W, int Cp, cudaStream_t stream) {
+    const char* E = "q_sample_pad";
+    if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || Cp <= 0 || T <= 0) return refuse(B200_ERR_ARG, E, "non-positive size");
+    if (Cp % 8 != 0) return refuse(B200_ERR_ARG, E, "Cp must be a multiple of 8");
+    if (C > Cp) return refuse(B200_ERR_ARG, E, "C must be at most Cp");
+    if (channels_last != 0 && channels_last != 1) return refuse(B200_ERR_ARG, E, "flags must be 0 or 1");
+    if (static_cast<long long>(H) * W > 0x7fffffffll) return refuse(B200_ERR_ARG, E, "H * W must be at most 2^31 - 1");
+    if (static_cast<long long>(B) * H * W > kMaxElements / Cp) return refuse(B200_ERR_ARG, E, "too many elements");
+    if (x0 == nullptr || noise == nullptr || timesteps == nullptr || sqrt_alphas_cumprod == nullptr ||
+        sqrt_one_minus_alphas_cumprod == nullptr || bad_flag == nullptr || out == nullptr)
+        return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(4, {x0, noise, sqrt_alphas_cumprod, sqrt_one_minus_alphas_cumprod, bad_flag}) || !aligned(8, {timesteps}))
+        return refuse(B200_ERR_ALIGN, E, "pointers not aligned to their element size");
+    if (!aligned(16, {out})) return refuse(B200_ERR_ALIGN, E, "out not 16-byte aligned");
+    launch_pad(QSampleSource{x0, noise, timesteps, sqrt_alphas_cumprod, sqrt_one_minus_alphas_cumprod, T, bad_flag}, channels_last != 0,
+               reinterpret_cast<uint4*>(out), B, C, H, W, Cp, stream);
+    return check_launch("q_sample_pad");
 }

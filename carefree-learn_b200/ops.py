@@ -616,23 +616,25 @@ def scatter_rows(dout: Tensor, pos: Tensor, T: int) -> Tensor:
 # optimizer, fused FCNN
 # ----------------------------------------------------------------------------------------------------------------
 def adam_step(params: Tensor, grads: Tensor, exp_avg: Tensor, exp_avg_sq: Tensor, *, hyper: Sequence[float] = (), step: int = 0,
-              hyper_dev: Optional[Tensor] = None, step_dev: Optional[Tensor] = None, increment: bool = True) -> None:
+              hyper_dev: Optional[Tensor] = None, step_dev: Optional[Tensor] = None, increment: bool = True,
+              decoupled: bool = False) -> None:
     """One Adam update (torch.optim.Adam without amsgrad) of contiguous fp32 tensors of equal numel, in place.  Either with host
     ``hyper`` = (lr, beta1, beta2, eps, weight_decay) at step count ``step`` >= 1, or with every hyper-parameter on the device:
     ``hyper_dev`` fp32 [6] = (lr, beta1, beta2, eps, weight_decay, grad_scale) and the step counter ``step_dev`` int32 [1],
-    incremented first when ``increment`` (so the update can be replayed from a CUDA graph)."""
-    what = "adam_step"
+    incremented first when ``increment`` (so the update can be replayed from a CUDA graph).  ``decoupled``: AdamW
+    (torch.optim.AdamW's order, p (1 - lr weight_decay) first, then the update with no L2 term)."""
+    what = "adamw_step" if decoupled else "adam_step"
     _check(what, "params", params, _F32)
     n = params.numel()
     for name, t in (("grads", grads), ("exp_avg", exp_avg), ("exp_avg_sq", exp_avg_sq)):
         _check(what, name, t, _F32, numel=n)
     if hyper_dev is None:
-        call("b200_adam_step", params.data_ptr(), grads.data_ptr(), exp_avg.data_ptr(), exp_avg_sq.data_ptr(), n, *hyper, step, None,
-             _stream())
+        call("b200_adamw_step" if decoupled else "b200_adam_step", params.data_ptr(), grads.data_ptr(), exp_avg.data_ptr(),
+             exp_avg_sq.data_ptr(), n, *hyper, step, None, _stream())
         return
     _check(what, "hyper_dev", hyper_dev, _F32, (6,))
     _check(what, "step_dev", step_dev, torch.int32, (1,))
-    call("b200_adam_step_dev", params.data_ptr(), grads.data_ptr(), exp_avg.data_ptr(), exp_avg_sq.data_ptr(), n, hyper_dev.data_ptr(),
+    call("b200_adamw_step_dev" if decoupled else "b200_adam_step_dev", params.data_ptr(), grads.data_ptr(), exp_avg.data_ptr(), exp_avg_sq.data_ptr(), n, hyper_dev.data_ptr(),
          step_dev.data_ptr(), int(increment), _stream())
 
 
@@ -737,10 +739,15 @@ def conv3x3_wgrad(dy: Tensor, x: Tensor, out: Optional[Tensor] = None, *, round_
     return out
 
 
+def conv3x3_weight_view(w_packed: Tensor, cin: int) -> Tensor:
+    """[Cout, 9 * Cin] (tap-major) -> a [Cout, Cin, 3, 3] view of it in the reference's Conv2d.weight index order."""
+    co = w_packed.shape[0]
+    return w_packed.view(co, 3, 3, cin).permute(0, 3, 1, 2)
+
+
 def unpack_conv3x3_weight(w_packed: Tensor, cin: int) -> Tensor:
     """[Cout, 9 * Cin] (tap-major) -> [Cout, Cin, 3, 3], the reference's Conv2d.weight layout."""
-    co = w_packed.shape[0]
-    return w_packed.view(co, 3, 3, cin).permute(0, 3, 1, 2).contiguous()
+    return conv3x3_weight_view(w_packed, cin).contiguous()
 
 
 def conv3x3(x: Tensor, w_packed: Tensor, bias: Optional[Tensor] = None, *, epilogue: int = EPI_BIAS_BF16, aux: Optional[Tensor] = None) -> Tensor:
@@ -887,6 +894,27 @@ def pad_channels(x: Tensor, cp: int) -> Tensor:
     out = torch.empty((B, H, W, cp), dtype=torch.bfloat16, device=x.device)
     call("b200_pad_channels_bf16", x.data_ptr(), int(x.dtype == _F32), int(cl), out.data_ptr(), B, C, H, W, cp, _stream())
     return out
+
+
+def q_sample_pad(x0: Tensor, noise: Tensor, timesteps: Tensor, sqrt_alphas_cumprod: Tensor, sqrt_one_minus_alphas_cumprod: Tensor,
+                 cp: int) -> Tuple[Tensor, Tensor]:
+    """DDPM noising into the stem's input: x0 and noise fp32 [B, C, H, W] (both contiguous NCHW or both channels-last),
+    timesteps int64 [B], the two fp32 [T] tables -> (bf16 [B, H, W, cp] = bf16(a[t] x0 + s[t] noise) in fp32 with no contraction,
+    channels >= C zero; int32 [1] flag, non-zero if a timestep was outside [0, T), whose image is then NaN)."""
+    what = "q_sample_pad"
+    cl = _layout(what, "x0", x0, (_F32,))
+    if _layout(what, "noise", noise, (_F32,)) != cl or noise.shape != x0.shape:
+        raise B200Error(f"{what}: noise must have x0's shape {list(x0.shape)} and memory format")
+    B, C, H, W = x0.shape
+    _check(what, "timesteps", timesteps, torch.int64, (B,))
+    _check(what, "sqrt_alphas_cumprod", sqrt_alphas_cumprod, _F32, (None,))
+    T = sqrt_alphas_cumprod.shape[0]
+    _check(what, "sqrt_one_minus_alphas_cumprod", sqrt_one_minus_alphas_cumprod, _F32, (T,))
+    out = torch.empty((B, H, W, cp), dtype=torch.bfloat16, device=x0.device)
+    bad = torch.zeros(1, dtype=torch.int32, device=x0.device)
+    call("b200_q_sample_pad_bf16", x0.data_ptr(), noise.data_ptr(), int(cl), timesteps.data_ptr(), sqrt_alphas_cumprod.data_ptr(),
+         sqrt_one_minus_alphas_cumprod.data_ptr(), T, bad.data_ptr(), out.data_ptr(), B, C, H, W, cp, _stream())
+    return out, bad
 
 
 def noise_prediction_loss(pred: Tensor, noise: Tensor, *, grad_out: Optional[Tensor] = None) -> Tensor:

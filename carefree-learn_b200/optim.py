@@ -30,6 +30,8 @@ class ArenaAdam(torch.optim.Optimizer):
     """A real ``torch.optim.Optimizer`` (so ``torch.optim.lr_scheduler`` classes -- and the reference's own ``WarmupScheduler``,
     cflearn/schedulers.py:126-171 -- accept it), with ONE parameter group holding every parameter of the module's arenas."""
 
+    decoupled = False  # weight decay as an L2 term in the gradient (torch.optim.Adam)
+
     def __init__(self, module: Any, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8, weight_decay: float = 0.0,
                  capturable: bool = False):
         self.module = module
@@ -153,9 +155,10 @@ class ArenaAdam(torch.optim.Optimizer):
         for idx, a in enumerate(self.arenas()):
             if self.capturable:
                 ops.adam_step(a.flat, a.grad, self.exp_avgs[idx], self.exp_avg_sqs[idx], hyper_dev=self.hyper_dev, step_dev=self.step_dev,
-                              increment=idx == 0)
+                              increment=idx == 0, decoupled=self.decoupled)
             else:
-                ops.adam_step(a.flat, a.grad, self.exp_avgs[idx], self.exp_avg_sqs[idx], hyper=(lr, b1, b2, eps, wd), step=self.step_count)
+                ops.adam_step(a.flat, a.grad, self.exp_avgs[idx], self.exp_avg_sqs[idx], hyper=(lr, b1, b2, eps, wd), step=self.step_count,
+                              decoupled=self.decoupled)
 
     def zero_grad(self, set_to_none: bool = True) -> None:
         if set_to_none:
@@ -205,6 +208,17 @@ class ArenaAdam(torch.optim.Optimizer):
                 self.step_dev.fill_(self.step_count)
         if self.capturable:
             self.sync_hyper()
+
+
+class ArenaAdamW(ArenaAdam):
+    """``torch.optim.AdamW`` (the zoo's DDPM optimizer ``"adamw"``, cflearn/optimizers.py:31; weight decay 0.01 by default) on
+    the arenas: the same fused kernels with decoupled decay, p <- p (1 - lr weight_decay) before the Adam update."""
+
+    decoupled = True
+
+    def __init__(self, module: Any, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8, weight_decay: float = 1e-2,
+                 capturable: bool = False):
+        super().__init__(module, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, capturable=capturable)
 
 
 class GraphedTrainStep:

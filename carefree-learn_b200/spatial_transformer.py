@@ -58,24 +58,26 @@ def _block_forward(x0: Tensor, c: Optional[Tensor], P: Sequence[Tensor], B: int,
     return x3, (x0, x1, x2, m1, r1, m2, r2, m3, r3, y3, hg, act, w1b, w2b, g1, g2, g3, *s1, *s2)
 
 
-def _block_backward(saved: tuple, dx3: Tensor, B: int, heads: int) -> Tuple[Tensor, Optional[Tensor], List[Tensor]]:
+def _block_backward(saved: tuple, dx3: Tensor, B: int, heads: int, pg: Optional[checkpoint.ParamGrads] = None
+                    ) -> Tuple[Tensor, Optional[Tensor], List[Tensor]]:
     """dx3: bf16 [M, C], the gradient of the block's output.  Returns (dx0 bf16, dcontext bf16 or None, the BLOCK_PARAMS
-    parameter gradients in _block_params order)."""
+    parameter gradients in _block_params order).  ``pg``: where they go, numbered in that order (default: fresh tensors)."""
     x0, x1, x2, m1, r1, m2, r2, m3, r3, y3, hg, act, w1b, w2b, g1, g2, g3 = saved[:17]
     s1, s2 = saved[17:27], saved[27:37]
     dev = dx3.device
+    pg = pg or checkpoint.NO_GRADS
     # feed-forward: FF2's weight / bias gradients, its dgrad through GEGLU's backward (one epilogue), then FF1
-    dw2 = ops.wgrad(dx3, act, torch.empty(w2b.shape, dtype=torch.float32, device=dev))
-    db2 = ops.colsum(dx3, torch.empty(w2b.shape[0], dtype=torch.float32, device=dev))
+    dw2 = ops.wgrad(dx3, act, pg.out(12, tuple(w2b.shape), dev), **pg.mode)
+    db2 = ops.colsum(dx3, pg.out(13, (w2b.shape[0],), dev), **pg.mode)
     dhg = ops.gemm(dx3, w2b, b_mn_major=True, epilogue=ops.EPI_DGEGLU_BF16, aux=hg)
-    dw1 = ops.wgrad(dhg, y3, torch.empty(w1b.shape, dtype=torch.float32, device=dev))
-    db1 = ops.colsum(dhg, torch.empty(w1b.shape[0], dtype=torch.float32, device=dev))
+    dw1 = ops.wgrad(dhg, y3, pg.out(10, tuple(w1b.shape), dev), **pg.mode)
+    db1 = ops.colsum(dhg, pg.out(11, (w1b.shape[0],), dev), **pg.mode)
     dy3 = ops.gemm(dhg, w1b, b_mn_major=True)
-    dx2, dg3, dbe3 = ops.layernorm_bf16_bwd(dy3, x2, g3, m3, r3, dres=dx3)
-    dy2, dc, *ga2 = attention_backward(s2, dx2, B, heads)
-    dx1, dg2, dbe2 = ops.layernorm_bf16_bwd(dy2, x1, g2, m2, r2, dres=dx2)
-    dy1, _, *ga1 = attention_backward(s1, dx1, B, heads)
-    dx0, dg1, dbe1 = ops.layernorm_bf16_bwd(dy1, x0, g1, m1, r1, dres=dx1)
+    dx2, dg3, dbe3 = ops.layernorm_bf16_bwd(dy3, x2, g3, m3, r3, dres=dx3, **pg.norm_kw(18, 19))
+    dy2, dc, *ga2 = attention_backward(s2, dx2, B, heads, pg.sub(5))
+    dx1, dg2, dbe2 = ops.layernorm_bf16_bwd(dy2, x1, g2, m2, r2, dres=dx2, **pg.norm_kw(16, 17))
+    dy1, _, *ga1 = attention_backward(s1, dx1, B, heads, pg)
+    dx0, dg1, dbe1 = ops.layernorm_bf16_bwd(dy1, x0, g1, m1, r1, dres=dx1, **pg.norm_kw(14, 15))
     return dx0, dc, [*ga1, *ga2, dw1, db1, dw2, db2, dg1, dbe1, dg2, dbe2, dg3, dbe3]
 
 
@@ -90,8 +92,9 @@ class _BlockOp:
         x3, saved = _block_forward(_rows(net), _rows(context), params, self.B, self.heads)
         return x3.view(net.shape), saved
 
-    def backward(self, saved: tuple, dout: Tensor) -> tuple:
-        dx, dc, grads = _block_backward(saved, _rows(dout), self.B, self.heads)
+    def backward(self, saved: tuple, dout: Tensor, pg: Optional[checkpoint.ParamGrads] = None) -> tuple:
+        pg = pg or checkpoint.NO_GRADS
+        dx, dc, grads = _block_backward(saved, _rows(dout), self.B, self.heads, pg.sub(2))
         return (dx, dc, *grads)
 
 
@@ -108,15 +111,17 @@ class _LatentIn:
         t = ops.gemm(yn.view(B * H * W, C), w_in_b, bias=_bf(b_in))
         return t.view(B, H * W, L), (xt, yn, gm, gr, gn_w32, gn_b32, w_in_b)
 
-    def backward(self, saved: tuple, dout: Tensor) -> tuple:
+    def backward(self, saved: tuple, dout: Tensor, pg: Optional[checkpoint.ParamGrads] = None) -> tuple:
+        pg = pg or checkpoint.NO_GRADS
         xt, yn, gm, gr, gn_w32, gn_b32, w_in_b = saved
         B, H, W, C = xt.shape
         L, M, dev = w_in_b.shape[0], B * H * W, dout.device
         dtl = _rows(dout)
-        dw_in = ops.wgrad(dtl, yn.view(M, C), torch.empty((L, C), dtype=torch.float32, device=dev))
-        db_in = ops.colsum(dtl, torch.empty(L, dtype=torch.float32, device=dev))
+        dw_in = ops.wgrad(dtl, yn.view(M, C), pg.out(3, (L, C), dev), **pg.mode)
+        db_in = ops.colsum(dtl, pg.out(4, (L,), dev), **pg.mode)
         dyn = ops.gemm(dtl, w_in_b, b_mn_major=True)
-        dxg, dgn_w, dgn_b = ops.groupnorm_silu_bwd(xt.view(B, H * W, C), dyn.view(B, H * W, C), gn_w32, gn_b32, gm, gr, silu=False)
+        dxg, dgn_w, dgn_b = ops.groupnorm_silu_bwd(xt.view(B, H * W, C), dyn.view(B, H * W, C), gn_w32, gn_b32, gm, gr, silu=False,
+                                                   **pg.norm_kw(1, 2))
         return dxg, dgn_w, dgn_b, dw_in, db_in
 
 
@@ -130,13 +135,14 @@ class _LatentOut:
         out = ops.gemm(_rows(t), w_out_b, bias=_bf(b_out), epilogue=ops.EPI_BIAS_RESID_BF16, aux=_rows(xt))
         return out.view(B, H, W, C).permute(0, 3, 1, 2), (t, w_out_b)
 
-    def backward(self, saved: tuple, dout: Tensor) -> tuple:
+    def backward(self, saved: tuple, dout: Tensor, pg: Optional[checkpoint.ParamGrads] = None) -> tuple:
+        pg = pg or checkpoint.NO_GRADS
         t, w_out_b = saved
         C, L = w_out_b.shape
         dev = dout.device
         dt = dout.permute(0, 2, 3, 1).to(torch.bfloat16).contiguous().view(-1, C)
-        dw_out = ops.wgrad(dt, _rows(t), torch.empty((C, L), dtype=torch.float32, device=dev))
-        db_out = ops.colsum(dt, torch.empty(C, dtype=torch.float32, device=dev))
+        dw_out = ops.wgrad(dt, _rows(t), pg.out(2, (C, L), dev), **pg.mode)
+        db_out = ops.colsum(dt, pg.out(3, (C,), dev), **pg.mode)
         return ops.gemm(dt, w_out_b, b_mn_major=True), dt, dw_out, db_out  # the residual's gradient is dt itself
 
 

@@ -61,23 +61,25 @@ class _TimeMLPOp:
         a = F.silu(h).contiguous()  # eager's F.silu on the bf16 tensor (fp32 maths, bf16 result)
         return ops.gemm(a, w2b, bias=_bf(b2)), (e, h, a, w0b, w2b)
 
-    def backward(self, saved: tuple, dt: Tensor) -> tuple:
+    def backward(self, saved: tuple, dt: Tensor, pg: Optional[checkpoint.ParamGrads] = None) -> tuple:
+        pg = pg or checkpoint.NO_GRADS
         e, h, a, w0b, w2b = saved
         dev = dt.device
         dt = dt.to(torch.bfloat16).contiguous()
-        dw2 = ops.wgrad(dt, a, _f32(*w2b.shape, device=dev))
-        db2 = ops.colsum(dt, _f32(w2b.shape[0], device=dev))
+        dw2 = ops.wgrad(dt, a, pg.out(3, tuple(w2b.shape), dev), **pg.mode)
+        db2 = ops.colsum(dt, pg.out(4, (w2b.shape[0],), dev), **pg.mode)
         dh = torch.ops.aten.silu_backward(ops.gemm(dt, w2b, b_mn_major=True), h).contiguous()
-        dw0 = ops.wgrad(dh, e, _f32(*w0b.shape, device=dev))
-        db0 = ops.colsum(dh, _f32(w0b.shape[0], device=dev))
+        dw0 = ops.wgrad(dh, e, pg.out(1, tuple(w0b.shape), dev), **pg.mode)
+        db0 = ops.colsum(dh, pg.out(2, (w0b.shape[0],), dev), **pg.mode)
         return None, dw0, db0, dw2, db2
 
 
-def stem_conv(net: Tensor, weight: Tensor, bias: Tensor) -> Tuple[Tensor, Tensor, Tensor]:
+def stem_conv(net: Tensor, weight: Tensor, bias: Tensor, padded: bool = False) -> Tuple[Tensor, Tensor, Tensor]:
     """Conv2d(C, Cout, 3, padding 1) of net fp32 / bf16 [B, C, H, W] (C <= 64): the input zero-padded to 64 channels (x, bf16
-    [B, H, W, 64]) and the weight to [Cout, 64, 3, 3] (wp).  Returns (out bf16 [B, H, W, Cout] = bf16(bf16(conv) + bias), x, wp)."""
-    C = net.shape[1]
-    x = ops.pad_channels(net, PAD_CHANNELS)
+    [B, H, W, 64]) and the weight to [Cout, 64, 3, 3] (wp).  Returns (out bf16 [B, H, W, Cout] = bf16(bf16(conv) + bias), x, wp).
+    ``padded``: net is already x (``ops.q_sample_pad``'s output)."""
+    C = weight.shape[1]
+    x = net if padded else ops.pad_channels(net, PAD_CHANNELS)
     wp = F.pad(weight, (0, 0, 0, 0, 0, PAD_CHANNELS - C))
     out = ops.conv3x3(x, ops.pack_conv3x3_weight(wp), epilogue=ops.EPI_BIAS_ADD_PER_IMAGE_BF16, aux=_bias_rows(bias, net.shape[0]))
     return out, x, wp
@@ -118,18 +120,20 @@ def head_conv_bwd(dout: Tensor, y: Tensor, wp: Tensor) -> Tuple[Tensor, Tensor, 
 @dataclass(frozen=True)
 class _StemOp:
     """input_blocks.0.0 as an op on (net [B, C, H, W] fp32 / bf16, weight, bias).  ``need_dx``: the latent requires grad (a
-    DDPM's noised latent does not)."""
+    DDPM's noised latent does not).  ``padded``: net is the stem's padded bf16 input [B, H, W, 64] (the DDPM's noised latent)."""
     channels: int
     need_dx: bool
+    padded: bool = False
 
     def forward(self, net: Tensor, weight: Tensor, bias: Tensor) -> Tuple[Tensor, tuple]:
-        out, x, wp = stem_conv(net, weight, bias)
+        out, x, wp = stem_conv(net, weight, bias, self.padded)
         return out.permute(0, 3, 1, 2), (x, wp)
 
-    def backward(self, saved: tuple, dout: Tensor) -> tuple:
+    def backward(self, saved: tuple, dout: Tensor, pg: Optional[checkpoint.ParamGrads] = None) -> tuple:
+        pg = pg or checkpoint.NO_GRADS
         x, wp = saved
         dx, dw, db = stem_conv_bwd(_nhwc(dout), x, wp, self.channels, self.need_dx)
-        return None if dx is None else dx.permute(0, 3, 1, 2), dw, db
+        return None if dx is None else dx.permute(0, 3, 1, 2), pg.put(1, dw), pg.put(2, db)
 
 
 @dataclass(frozen=True)
@@ -146,14 +150,15 @@ class _HeadOp:
         out, wp = head_conv(y.view(B, H, W, C), weight, bias)
         return out.permute(0, 3, 1, 2), (xt, y, m, r, g, b, wp)
 
-    def backward(self, saved: tuple, dout: Tensor) -> tuple:
+    def backward(self, saved: tuple, dout: Tensor, pg: Optional[checkpoint.ParamGrads] = None) -> tuple:
+        pg = pg or checkpoint.NO_GRADS
         xt, y, m, r, g, b, wp = saved
         B, H, W, C = xt.shape
         if not (dout.is_contiguous() or dout.is_contiguous(memory_format=torch.channels_last)):
             dout = dout.contiguous()
         dy, dw, db = head_conv_bwd(dout, y.view(B, H, W, C), wp)
-        dx, dg, dbe = ops.groupnorm_silu_bwd(xt.view(B, H * W, C), dy.view(B, H * W, C), g, b, m, r)
-        return dx.view(B, H, W, C).permute(0, 3, 1, 2), dg, dbe, dw, db
+        dx, dg, dbe = ops.groupnorm_silu_bwd(xt.view(B, H * W, C), dy.view(B, H * W, C), g, b, m, r, **pg.norm_kw(1, 2))
+        return dx.view(B, H, W, C).permute(0, 3, 1, 2), dg, dbe, pg.put(3, dw), pg.put(4, db)
 
 
 def timestep_embedding(timesteps: Tensor, frequency: Tensor) -> Tensor:
@@ -297,6 +302,8 @@ class UNetDiffuserB200(nn.Module):
             head_conv.bias.zero_()
         self.head = nn.Sequential(nn.GroupNorm(32, c), nn.SiLU(), head_conv)
 
+    _grad_arena: Optional["UNetGradArena"] = None  # set by enable_grad_arena
+
     def check_geometry(self, B: int, H: int, W: int) -> None:
         """Raise one ``B200Error`` naming the first level (and the rule) whose H x W grid the blocks cannot tile."""
         for level in range(self.levels):
@@ -345,9 +352,29 @@ class UNetDiffuserB200(nn.Module):
         _check_cuda(what, net, timesteps, context)
         if not (net.is_contiguous() or net.is_contiguous(memory_format=torch.channels_last)):
             net = net.contiguous()
+        return self._body(net, False, timesteps, context)
+
+    def forward_padded(self, x: Tensor, timesteps: Tensor, context: Optional[Tensor] = None) -> Tensor:
+        """``forward`` on the stem's padded input x, bf16 [B, H, W, 64] with channels >= in_channels zero (``ops.q_sample_pad``'s
+        output, which needs no gradient)."""
+        what = "UNetDiffuserB200"
+        if x.dim() != 4 or x.shape[3] != PAD_CHANNELS or x.dtype != torch.bfloat16 or not x.is_contiguous():
+            raise B200Error(f"{what}: the padded input must be contiguous bf16 [B, H, W, {PAD_CHANNELS}]")
+        B, H, W, _ = x.shape
+        if timesteps.shape != (B,):
+            raise B200Error(f"{what}: timesteps must be [B] = [{B}]")
+        if context is not None and (context.dim() != 3 or context.shape[0] != B or context.shape[2] != self.context_dim):
+            raise B200Error(f"{what}: context must be [B, Tk, {self.context_dim}]")
+        self.check_geometry(B, H, W)
+        _check_cuda(what, x, timesteps, context)
+        return self._body(x, True, timesteps, context)
+
+    def _body(self, net: Tensor, padded: bool, timesteps: Tensor, context: Optional[Tensor]) -> Tensor:
+        if self._grad_arena is not None:
+            self._grad_arena.begin()
         time_net = self._time_mlp(timestep_embedding(timesteps, self._frequency))
         ctx = None if context is None else context.to(torch.bfloat16)  # autocast's cast at to_k / to_v, made once
-        h = self._stem(net)
+        h = self._stem(net, padded)
         skips = [h]
         for blocks in self.input_blocks[1:]:
             h = self._run(blocks, h, time_net, ctx)
@@ -361,10 +388,121 @@ class UNetDiffuserB200(nn.Module):
         te = self.time_embedding
         return checkpoint.OpFn.apply(_TimeMLPOp(), False, emb, te[0].weight, te[0].bias, te[2].weight, te[2].bias)
 
-    def _stem(self, net: Tensor) -> Tensor:
+    def _stem(self, net: Tensor, padded: bool = False) -> Tensor:
         stem = self.input_blocks[0][0]
-        return checkpoint.OpFn.apply(_StemOp(self.in_channels, net.requires_grad), False, net, stem.weight, stem.bias)
+        return checkpoint.OpFn.apply(_StemOp(self.in_channels, net.requires_grad, padded), False, net, stem.weight, stem.bias)
 
     def _head(self, net: Tensor) -> Tensor:
         gn, conv = self.head[0], self.head[2]
         return checkpoint.OpFn.apply(_HeadOp(gn.eps), False, net, gn.weight, gn.bias, conv.weight, conv.bias)
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# the flat gradient arena
+# ------------------------------------------------------------------------------------------------------------------------------
+SHRINK_LAUNCHES = 4  # persistent launches (convolutions, GEMMs) that leave the communicator's SMs free after a bucket starts
+
+
+def bucket_plan(unet: UNetDiffuserB200) -> List[Tuple[str, List[str]]]:
+    """The all-reduce buckets in the order backward completes them, each a top-level child: ``head``, the output blocks last
+    first, ``residual``, the input blocks last first, then ``stem``: the stem and the timestep MLP, whose gradient is complete
+    only once every ResBlock has added its share.  Keys are ``unet.named_parameters()`` names, in state_dict order inside a
+    bucket."""
+    names = [n for n, _ in unet.named_parameters()]
+
+    def under(prefix: str) -> List[str]:
+        return [n for n in names if n.startswith(prefix + ".")]
+
+    plan = [("head", under("head"))]
+    plan += [(f"output_blocks.{i}", under(f"output_blocks.{i}")) for i in reversed(range(len(unet.output_blocks)))]
+    plan += [("residual", under("residual"))]
+    plan += [(f"input_blocks.{i}", under(f"input_blocks.{i}")) for i in reversed(range(1, len(unet.input_blocks)))]
+    plan += [("stem", under("input_blocks.0") + under("time_embedding"))]
+    return plan
+
+
+class UNetGradArena:
+    """The UNet's parameters in one ``vit.ParamArena`` laid out by ``bucket_plan``, each parameter carrying a
+    ``checkpoint.GradSlot``: every op's backward writes its parameter gradients straight into their views (overwriting, or adding
+    while the parameters hold gradients, ``ParamArena.claim_grads``), and ``p.grad`` is the view.  When a bucket's last gradient
+    is written it is handed to ``reducer.ready`` (``dp.NativeBucketReducer``), which all-reduces it on a side stream while
+    backward goes on; the persistent kernels launched next then leave the communicator's SMs free (``shrink_next``).
+
+    It offers what ``dp`` reads of a transformer engine (``buckets()``, ``reducer``, ``shrink_next``), so the DDPM module hands
+    it out as both its ``geo`` and its ``engine``.
+
+    The arena is built on the parameters' device by its first ``arena.ensure()`` (the UNet's forward calls ``begin``, which
+    does it, and rebuilds it after ``.to(device)``), so a module constructed on the host holds no second copy there.  Each forward
+    also restarts the buckets' counts: a bucket is complete when each of its trainable parameters' gradients was written once
+    since (``check``)."""
+
+    def __init__(self, unet: UNetDiffuserB200) -> None:
+        from .vit import ParamArena
+
+        params = dict(unet.named_parameters())
+        self.plan = bucket_plan(unet)
+        self.arena = ParamArena([(k, tuple(params[k].shape)) for _, keys in self.plan for k in keys], bf16_shadow=False)
+        self.arena.params = {k: params[k] for _, keys in self.plan for k in keys}  # attached by the first ensure()
+        self.reducer: Any = None
+        self._shrunk = False
+        self._buckets = {name: checkpoint.Bucket(name, len(keys), self._ready) for name, keys in self.plan}
+        for name, keys in self.plan:
+            for k in keys:
+                setattr(params[k], checkpoint.SLOT_ATTR, checkpoint.GradSlot(self.arena, k, self._buckets[name]))
+        self._params = params
+        self._unet = unet
+        unet._grad_arena = self
+
+    def buckets(self) -> Dict[str, List[List[str]]]:
+        return {name: [keys] for name, keys in self.plan}
+
+    def begin(self) -> None:
+        """At the start of a forward: the arena on the parameters' device, and every bucket waiting for the gradients of its
+        trainable parameters (a frozen parameter's op skips its slot)."""
+        self.arena.ensure()
+        for name, keys in self.plan:
+            self._buckets[name].reset(sum(self._params[k].requires_grad for k in keys))
+
+    def check(self) -> None:
+        """Raise ``B200Error`` unless every bucket was completed exactly once since the last forward, i.e. each was handed to the
+        reducer after all of its gradients were written: anything else would skip or truncate a bucket's exchange."""
+        bad = [f"{b.name} ({b.size - b.left} of {b.size} written)" for b in self._buckets.values() if b.left != 0]
+        if bad:
+            raise B200Error("UNetGradArena: gradient buckets not completed exactly once by this backward (one forward, then one "
+                            f"backward per exchange): {', '.join(bad)}")
+
+    def end_backward(self) -> None:
+        """Lift what is left of a lowered persistent grid, so that it cannot reach the next step's launches."""
+        if self._shrunk:
+            from . import _cabi
+            _cabi.lib().b200_set_persistent_ctas(0, 0)
+            self._shrunk = False
+
+    def _ready(self, name: str) -> None:
+        if self.reducer is not None:
+            self.reducer.ready(name)
+
+    @property
+    def shrink_next(self) -> int:
+        return 0
+
+    @shrink_next.setter
+    def shrink_next(self, ctas: int) -> None:
+        if ctas > 0:
+            from . import _cabi
+            _cabi.lib().b200_set_persistent_ctas(ops.num_sms() - ctas, SHRINK_LAUNCHES)
+            self._shrunk = True
+
+    def close(self) -> None:
+        """Take the slots off the parameters: their gradients go back to autograd."""
+        for p in self._params.values():
+            if hasattr(p, checkpoint.SLOT_ATTR):
+                delattr(p, checkpoint.SLOT_ATTR)
+        self._unet._grad_arena = None
+
+
+def enable_grad_arena(unet: UNetDiffuserB200) -> UNetGradArena:
+    """Put the UNet's parameters in a flat arena whose gradient views their ops' backwards write directly (``UNetGradArena``).
+    Keys, shapes and ``state_dict`` order do not change; the arena is built on the parameters' device by the next forward (or
+    ``arena.ensure()``).  ``close()`` on the result turns it off."""
+    return UNetGradArena(unet)

@@ -90,41 +90,49 @@ def res_block_fwd(x: Tensor, time_net: Optional[Tensor], P: Sequence[Optional[Te
     return out, (x, y1, h, y2, m1, r1, m2, r2, time_net, ta, g1f, be1f, g2f, be2f, w1, w2, wtb, wsb)
 
 
-def res_block_bwd(saved: Sequence[Optional[Tensor]], dout: Tensor) -> Tuple[Tensor, Optional[Tensor], List[Optional[Tensor]]]:
+def res_block_bwd(saved: Sequence[Optional[Tensor]], dout: Tensor, pg: Optional[checkpoint.ParamGrads] = None
+                  ) -> Tuple[Tensor, Optional[Tensor], List[Optional[Tensor]]]:
     """dout: contiguous bf16 [B, H, W, Cout].  Returns (dx bf16 [B, H, W, Cin], dtime bf16 [B, tdim] or None, the parameter
-    gradients in ``res_block_fwd``'s P order: time-embedding ones None without a time input, shortcut ones None without one)."""
+    gradients in ``res_block_fwd``'s P order: time-embedding ones None without a time input, shortcut ones None without one).
+    ``pg``: where the parameter gradients go, numbered in P order (default: fresh tensors)."""
     x, y1, h, y2, m1, r1, m2, r2, time_net, ta, g1f, be1f, g2f, be2f, w1, w2, wtb, wsb = saved
     B, H, W, Cin = x.shape
     Cout = w1.shape[0]
     HW, M, dev = H * W, B * H * W, dout.device
+    pg = pg or checkpoint.NO_GRADS
     f32 = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)  # noqa: E731
     d2 = dout.view(M, Cout)
     # conv2: weight, bias (= the shortcut's bias gradient too) and input gradients
-    dw2 = ops.unpack_conv3x3_weight(ops.conv3x3_wgrad(dout, y2.view(B, H, W, Cout)), Cout)
-    db2 = ops.colsum(d2, f32(Cout))
+    dw2 = pg.put(8, ops.conv3x3_weight_view(ops.conv3x3_wgrad(dout, y2.view(B, H, W, Cout)), Cout))
+    shared_bias = wsb is not None and pg.dest(9) is not None  # one column sum feeds two arena views
+    db2 = ops.colsum(d2, f32(Cout)) if shared_bias else ops.colsum(d2, pg.out(9, (Cout,), dev), **pg.mode)
     dy2 = ops.conv3x3(dout, ops.pack_conv3x3_weight_dgrad(w2))
-    dh, dg2, dbe2 = ops.groupnorm_silu_bwd(h.view(B, HW, Cout), dy2.view(B, HW, Cout), g2f, be2f, m2, r2)
+    dh, dg2, dbe2 = ops.groupnorm_silu_bwd(h.view(B, HW, Cout), dy2.view(B, HW, Cout), g2f, be2f, m2, r2, **pg.norm_kw(6, 7))
     # one pass over dh: the time embedding's upstream gradient [B, Cout] and conv1's bias gradient
     if time_net is None:
-        dt, db1 = None, ops.colsum(dh.view(M, Cout), f32(Cout))
+        dt, db1 = None, ops.colsum(dh.view(M, Cout), pg.out(3, (Cout,), dev), **pg.mode)
     else:
         dt, db1 = ops.colsum_per_image(dh)
+        db1 = pg.put(3, db1)
     dhv = dh.view(B, H, W, Cout)
-    dw1 = ops.unpack_conv3x3_weight(ops.conv3x3_wgrad(dhv, y1.view(B, H, W, Cin)), Cin)
+    dw1 = pg.put(2, ops.conv3x3_weight_view(ops.conv3x3_wgrad(dhv, y1.view(B, H, W, Cin)), Cin))
     dy1 = ops.conv3x3(dhv, ops.pack_conv3x3_weight_dgrad(w1))
-    dxg, dg1, dbe1 = ops.groupnorm_silu_bwd(x.view(B, HW, Cin), dy1.view(B, HW, Cin), g1f, be1f, m1, r1)
+    dxg, dg1, dbe1 = ops.groupnorm_silu_bwd(x.view(B, HW, Cin), dy1.view(B, HW, Cin), g1f, be1f, m1, r1, **pg.norm_kw(0, 1))
     # the shortcut path, added to GroupNorm1's gradient in one bf16 add
     dws = dbs = None
     if wsb is None:
         dx = dxg.view(M, Cin) + d2
     else:
-        dws = ops.wgrad(d2, x.view(M, Cin), f32(Cout, Cin)).view(Cout, Cin, 1, 1)
-        dbs = db2.clone()
+        dws = ops.wgrad(d2, x.view(M, Cin), pg.out(10, (Cout, Cin), dev), **pg.mode).view(Cout, Cin, 1, 1)
+        if shared_bias:
+            dbs, db2 = pg.put(11, db2), pg.put(9, db2)
+        else:
+            dbs = pg.put(11, db2.clone())
         dx = dxg.view(M, Cin) + ops.gemm(d2, wsb, b_mn_major=True)
     dtime = dwt = dbt = None
     if time_net is not None:  # [B, tdim] glue, the ops eager runs
-        dwt = ops.wgrad(dt, ta, f32(*wtb.shape))
-        dbt = ops.colsum(dt, f32(Cout))
+        dwt = ops.wgrad(dt, ta, pg.out(4, tuple(wtb.shape), dev), **pg.mode)
+        dbt = ops.colsum(dt, pg.out(5, (Cout,), dev), **pg.mode)
         dtime = torch.ops.aten.silu_backward(ops.gemm(dt, wtb, b_mn_major=True), time_net)
     return dx.view(B, H, W, Cin), dtime, [dg1, dbe1, dw1, db1, dwt, dbt, dg2, dbe2, dw2, db2, dws, dbs]
 
@@ -155,8 +163,9 @@ class _ResBlockOp:
         out, saved = res_block_fwd(xt, time_net, params, self.eps)
         return out.permute(0, 3, 1, 2), saved
 
-    def backward(self, saved: tuple, dout: Tensor) -> tuple:
-        dx, dtime, grads = res_block_bwd(saved, dout.permute(0, 2, 3, 1).to(torch.bfloat16).contiguous())
+    def backward(self, saved: tuple, dout: Tensor, pg: Optional[checkpoint.ParamGrads] = None) -> tuple:
+        pg = pg or checkpoint.NO_GRADS
+        dx, dtime, grads = res_block_bwd(saved, dout.permute(0, 2, 3, 1).to(torch.bfloat16).contiguous(), pg.sub(2))
         return (dx.permute(0, 3, 1, 2), dtime, *grads)
 
 
@@ -268,12 +277,13 @@ class _DownsampleOp:
                              aux=_bias_rows(bias, net.shape[0]))
         return out.permute(0, 3, 1, 2), (net, weight)
 
-    def backward(self, saved: tuple, dout: Tensor) -> tuple:
+    def backward(self, saved: tuple, dout: Tensor, pg: Optional[checkpoint.ParamGrads] = None) -> tuple:
+        pg = pg or checkpoint.NO_GRADS
         net, weight = saved
         Cout, Cin = weight.shape[:2]
         d = _nhwc(dout)
-        dw = ops.unpack_conv3x3_weight(ops.conv3x3_s2_wgrad(d, _nhwc(net)), Cin)
-        db = ops.colsum(d.view(-1, Cout), torch.empty(Cout, dtype=torch.float32, device=d.device))
+        dw = pg.put(1, ops.conv3x3_weight_view(ops.conv3x3_s2_wgrad(d, _nhwc(net)), Cin))
+        db = ops.colsum(d.view(-1, Cout), pg.out(2, (Cout,), d.device), **pg.mode)
         dx = ops.conv3x3_s2_dgrad(d, ops.pack_conv3x3_weight_s2_dgrad(weight))
         return dx.permute(0, 3, 1, 2), dw, db
 
@@ -289,12 +299,13 @@ class _UpsampleOp:
                               aux=_bias_rows(bias, net.shape[0]))
         return out.permute(0, 3, 1, 2), (net, weight)
 
-    def backward(self, saved: tuple, dout: Tensor) -> tuple:
+    def backward(self, saved: tuple, dout: Tensor, pg: Optional[checkpoint.ParamGrads] = None) -> tuple:
+        pg = pg or checkpoint.NO_GRADS
         net, weight = saved
         Cout, Cin = weight.shape[:2]
         d = _nhwc(dout)
-        dw = ops.unpack_conv3x3_weight(ops.conv3x3_wgrad(d, ops.upsample_nearest2x(_nhwc(net))), Cin)
-        db = ops.colsum(d.view(-1, Cout), torch.empty(Cout, dtype=torch.float32, device=d.device))
+        dw = pg.put(1, ops.conv3x3_weight_view(ops.conv3x3_wgrad(d, ops.upsample_nearest2x(_nhwc(net))), Cin))
+        db = ops.colsum(d.view(-1, Cout), pg.out(2, (Cout,), d.device), **pg.mode)
         dx = ops.sum2x2(ops.conv3x3(d, ops.pack_conv3x3_weight_dgrad(weight)))
         return dx.permute(0, 3, 1, 2), dw, db
 

@@ -40,10 +40,12 @@ def _padded(shape: Tuple[int, ...]) -> int:
 # parameter arena
 # -----------------------------------------------------------------------------------------------------------------
 class ParamArena:
-    """Flat fp32 parameters + bf16 shadow + flat fp32 gradients, addressed by reference ``state_dict`` key."""
+    """Flat fp32 parameters + bf16 shadow + flat fp32 gradients, addressed by reference ``state_dict`` key.  ``bf16_shadow=False``:
+    no shadow (a module whose ops cast their own weights)."""
 
-    def __init__(self, spec: List[Tuple[str, Tuple[int, ...]]]):
+    def __init__(self, spec: List[Tuple[str, Tuple[int, ...]]], bf16_shadow: bool = True):
         self.spec = list(spec)
+        self.bf16_shadow = bf16_shadow
         self.offsets: Dict[str, int] = {}
         off = 0
         for key, shape in self.spec:
@@ -77,13 +79,16 @@ class ParamArena:
                 v.copy_(p.data.to(torch.float32))
                 p.data = v
         self.flat = flat
-        self.flat_bf16 = torch.zeros(self.total, dtype=torch.bfloat16, device=dev) if dev.type == "cuda" else None
+        self.flat_bf16 = torch.zeros(self.total, dtype=torch.bfloat16, device=dev) if dev.type == "cuda" and self.bf16_shadow else None
         self.grad = torch.zeros(self.total, dtype=torch.float32, device=dev)
         self._bf16_version = -1
 
     def ensure(self) -> None:
-        """Cheap aliasing check: ``module.to(device)`` / ``load_state_dict(assign=True)`` break the views."""
-        assert self.flat is not None
+        """Cheap aliasing check: ``module.to(device)`` / ``load_state_dict(assign=True)`` break the views.  An arena whose
+        parameters were given but not yet attached (``flat`` None) is built here, on their device."""
+        if self.flat is None:
+            self.rebuild()
+            return
         base = self.flat.data_ptr()
         ok = True
         for key, p in self.params.items():

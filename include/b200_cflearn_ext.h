@@ -87,6 +87,28 @@ int b200_pad_channels_bf16(const void* x, int x_f32, int x_channels_last, void* 
 int b200_noise_prediction_loss_bf16(const void* pred, const void* noise, int noise_f32, float* loss, void* dpred,
                                     const float* grad_out, int B, long long N, cudaStream_t stream);
 
+/* DDPM noising fused into the stem's input (q_sample, cflearn/modules/multimodal/diffusion/samplers/schema.py:94-108, before the
+ * stem's autocast cast): out [B, H, W, Cp] bf16 (dense, channels-last) with, for channel c < C of image b and t = timesteps[b],
+ * bf16(fl(fl(sqrt_alphas_cumprod[t] x0) + fl(sqrt_one_minus_alphas_cumprod[t] noise))) -- two fp32 products and their fp32 sum,
+ * no contraction -- and channels >= C set to +0.  x0, noise: fp32 [B, C, H, W], both dense NCHW (channels_last = 0) or both
+ * dense channels-last (1); timesteps: int64 [B]; the two tables: fp32 [T].  A timestep outside [0, T) reads no table entry: it
+ * sets *bad_flag = 1 (int32, never cleared here) and the image's channels < C are NaN.  0 < C <= Cp, Cp % 8 == 0, H * W < 2^31,
+ * B * H * W * Cp <= 2^38.  One launch, on the pad_channels kernel. */
+int b200_q_sample_pad_bf16(const float* x0, const float* noise, int channels_last, const long long* timesteps,
+                           const float* sqrt_alphas_cumprod, const float* sqrt_one_minus_alphas_cumprod, long long T, int* bad_flag,
+                           void* out, int B, int C, int H, int W, int Cp, cudaStream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------
+ * AdamW on the flat fp32 arenas (torch.optim.AdamW without amsgrad; the zoo's DDPM trains with "adamw",
+ * cflearn/optimizers.py:31): b200_adam_step / b200_adam_step_dev with decoupled weight decay, in torch.optim.AdamW's order:
+ * p <- p (1 - lr weight_decay) first, then the Adam update with no L2 term in the gradient.  Same arguments, rules and device
+ * hyper block {lr, beta1, beta2, eps, weight_decay, grad_scale} (grad_scale multiplies the gradient) as the Adam entries.
+ * --------------------------------------------------------------------------------------------------------- */
+int b200_adamw_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n, float lr, float beta1,
+                    float beta2, float eps, float weight_decay, int step, int* step_dev, cudaStream_t stream);
+int b200_adamw_step_dev(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n, const float* hyper_dev,
+                        int* step_dev, int increment, cudaStream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
