@@ -106,6 +106,8 @@ EXT_SIGNATURES: Dict[str, Any] = {
     "b200_pad_channels_bf16": (c_int, [_P, c_int, c_int, _P, c_int, c_int, c_int, c_int, c_int, _P]),
     "b200_noise_prediction_loss_bf16": (c_int, [_P, _P, c_int, _P, _P, _P, c_int, _LL, _P]),
     "b200_q_sample_pad_bf16": (c_int, [_P, _P, c_int, _P, _P, _P, _LL, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
+    "b200_ddim_step_bf16": (c_int, [_P, _P, c_float, _P, _P, _P, _P, c_int, c_float, _P, c_int, _P, _P, _P, c_int, c_int, c_int, c_int,
+                                    c_int, c_int, _P]),
     "b200_adamw_step": (c_int, [_P, _P, _P, _P, _LL, c_float, c_float, c_float, c_float, c_float, c_int, _P, _P]),
     "b200_adamw_step_dev": (c_int, [_P, _P, _P, _P, _LL, _P, _P, c_int, _P]),
 }

@@ -124,6 +124,88 @@ __global__ void noise_loss_grad_kernel(const __nv_bfloat16* __restrict__ pred, c
     dpred[i] = __float2bfloat16_rn(__fmul_rn(__fmul_rn(2.0f, d), g));
 }
 
+// ---- one DDIM denoising step ---------------------------------------------------------------------------------------------------
+// The reference's DDIMSampler update (samplers/ddim.py:195-239, schema.py:255) with its rounding points: classifier-free guidance
+// as eager's three bf16 tensor ops, then the fp32 update, each operation rounded, in the reference's order.  The per-step scalars
+// come from coef[step] = {s1m, sqrt_a, sqrt_ap, c_dir, sigma} (fp32, computed on the host as the reference computes them).
+constexpr int kDdimCoefs = 5;
+
+__device__ __forceinline__ float bf16_round(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
+
+struct DdimArgs {
+    const __nv_bfloat16* eps;     // [B, H, W, C]
+    const __nv_bfloat16* eps_u;   // [B, H, W, C] or nullptr
+    float scale;
+    int guided;                   // eps_u given and scale != 1
+    float* x;                     // [B, C, H, W]
+    const float* noise;           // [B, C, H, W]
+    const float* coef;            // [S, kDdimCoefs]
+    const long long* ts_table;    // [S]
+    int S;
+    float temperature;
+    const int* step_dev;
+    int* bad;
+    uint4* next_in;               // [copies B, H, W, Cp]
+    long long* next_ts;           // [copies B]
+    int copies, B, C, HW, Cp8;
+    long long groups;             // B HW Cp8
+};
+
+// One thread per 8 channels of one pixel of next_in, as pad_channels_kernel: the threads whose group holds real channels also
+// advance x for those channels.  Reads of the counter and the table are uniform across the grid.
+__global__ void ddim_step_kernel(DdimArgs a) {
+    const long long g = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    const int step = *a.step_dev;
+    const bool ok = step >= 0 && step < a.S;
+    const bool has_next = ok && step + 1 < a.S;
+    if (has_next && g < static_cast<long long>(a.copies) * a.B) a.next_ts[g] = a.ts_table[step + 1];
+    if (g >= a.groups) return;
+    const int c0 = static_cast<int>(g % a.Cp8) * 8;
+    const long long pix = g / a.Cp8;  // b HW + p
+    const long long b = pix / a.HW;
+    const long long p = pix - b * a.HW;
+    if (!ok) {
+        if (g == 0) atomicExch(a.bad, 1);
+        for (int c = c0; c < c0 + 8 && c < a.C; ++c) a.x[(b * a.C + c) * a.HW + p] = __int_as_float(0x7fc00000);
+        return;
+    }
+    float s1m = 0.f, sqrt_a = 1.f, sqrt_ap = 0.f, c_dir = 0.f, sigma = 0.f;
+    if (c0 < a.C) {
+        const float* k = a.coef + static_cast<long long>(step) * kDdimCoefs;
+        s1m = k[0], sqrt_a = k[1], sqrt_ap = k[2], c_dir = k[3], sigma = k[4];
+    }
+    uint32_t w[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        uint32_t half[2] = {0u, 0u};
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int c = c0 + 2 * j + h;
+            if (c >= a.C) continue;
+            float e = __bfloat162float(a.eps[pix * a.C + c]);
+            if (a.guided) {  // eps_uncond + scale * (eps - eps_uncond), three bf16 tensor ops
+                const float u = __bfloat162float(a.eps_u[pix * a.C + c]);
+                const float d = bf16_round(__fsub_rn(e, u));
+                const float m = bf16_round(__fmul_rn(a.scale, d));
+                e = bf16_round(__fadd_rn(u, m));
+            }
+            const long long i = (b * a.C + c) * a.HW + p;
+            const float x0 = __fdiv_rn(__fsub_rn(a.x[i], __fmul_rn(s1m, e)), sqrt_a);
+            const float dir = __fmul_rn(c_dir, e);
+            const float nz = __fmul_rn(__fmul_rn(sigma, a.noise[i]), a.temperature);
+            const float out = __fadd_rn(__fadd_rn(__fmul_rn(sqrt_ap, x0), dir), nz);
+            a.x[i] = out;
+            half[h] = to_bf16_bits(out);
+        }
+        w[j] = half[0] | (half[1] << 16);
+    }
+    if (!has_next) return;
+    const uint4 v = make_uint4(w[0], w[1], w[2], w[3]);
+    for (int k = 0; k < a.copies; ++k) a.next_in[g + k * a.groups] = v;
+}
+
+__global__ void ddim_increment_kernel(int* counter) { counter[0] += 1; }
+
 }  // namespace b200
 
 using namespace b200;
@@ -193,4 +275,41 @@ extern "C" int b200_q_sample_pad_bf16(const float* x0, const float* noise, int c
     launch_pad(QSampleSource{x0, noise, timesteps, sqrt_alphas_cumprod, sqrt_one_minus_alphas_cumprod, T, bad_flag}, channels_last != 0,
                reinterpret_cast<uint4*>(out), B, C, H, W, Cp, stream);
     return check_launch("q_sample_pad");
+}
+
+extern "C" int b200_ddim_step_bf16(const void* eps, const void* eps_uncond, float guidance_scale, float* x, const float* noise,
+                                   const float* coef, const long long* ts_table, int S, float temperature,
+                                   int* step_dev, int increment, int* bad_flag, void* next_in, long long* next_ts, int copies,
+                                   int B, int C, int H, int W, int Cp, cudaStream_t stream) {
+    const char* E = "ddim_step";
+    if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || Cp <= 0 || S <= 0) return refuse(B200_ERR_ARG, E, "non-positive size");
+    if (Cp % 8 != 0) return refuse(B200_ERR_ARG, E, "Cp must be a multiple of 8");
+    if (C > Cp) return refuse(B200_ERR_ARG, E, "C must be at most Cp");
+    if (copies != 1 && copies != 2) return refuse(B200_ERR_ARG, E, "copies must be 1 or 2");
+    if (increment != 0 && increment != 1) return refuse(B200_ERR_ARG, E, "increment must be 0 or 1");
+    if (copies == 2 && eps_uncond == nullptr) return refuse(B200_ERR_ARG, E, "copies = 2 needs eps_uncond");
+    if (static_cast<long long>(H) * W > 0x7fffffffll) return refuse(B200_ERR_ARG, E, "H * W must be at most 2^31 - 1");
+    if (static_cast<long long>(B) * H * W > kMaxElements / (2 * Cp)) return refuse(B200_ERR_ARG, E, "too many elements");
+    if (eps == nullptr || x == nullptr || noise == nullptr || coef == nullptr || ts_table == nullptr || step_dev == nullptr ||
+        bad_flag == nullptr || next_in == nullptr || next_ts == nullptr)
+        return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(2, {eps, eps_uncond}) || !aligned(4, {x, noise, coef, step_dev, bad_flag}) || !aligned(8, {ts_table, next_ts}))
+        return refuse(B200_ERR_ALIGN, E, "pointers not aligned to their element size");
+    if (!aligned(16, {next_in})) return refuse(B200_ERR_ALIGN, E, "next_in not 16-byte aligned");
+    DdimArgs a;
+    a.eps = static_cast<const __nv_bfloat16*>(eps);
+    a.eps_u = static_cast<const __nv_bfloat16*>(eps_uncond);
+    a.scale = guidance_scale;
+    a.guided = eps_uncond != nullptr && guidance_scale != 1.0f;
+    a.x = x, a.noise = noise, a.coef = coef, a.ts_table = ts_table, a.S = S, a.temperature = temperature;
+    a.step_dev = step_dev, a.bad = bad_flag;
+    a.next_in = static_cast<uint4*>(next_in), a.next_ts = next_ts;
+    a.copies = copies, a.B = B, a.C = C, a.HW = H * W, a.Cp8 = Cp / 8;
+    a.groups = static_cast<long long>(B) * H * W * (Cp / 8);
+    const long long threads = a.groups > 2ll * B ? a.groups : 2ll * B;
+    ddim_step_kernel<<<static_cast<unsigned>((threads + 255) / 256), 256, 0, stream>>>(a);
+    int rc = check_launch("ddim_step");
+    if (rc || !increment) return rc;
+    ddim_increment_kernel<<<1, 1, 0, stream>>>(step_dev);  // after the step: the kernel above only reads the counter
+    return check_launch("ddim_step_increment");
 }

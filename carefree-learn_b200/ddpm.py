@@ -13,8 +13,11 @@ completes them, and all-reduced bucket by bucket when a communicator is attached
 what ``optim.ArenaAdam`` / ``ArenaAdamW``, ``trainer.B200TrainStep`` and ``optim.GraphedTrainStep`` drive, so the whole step --
 draws, noising, forward, loss, backward, exchange, clipping and the update -- is one CUDA graph.
 
-Not implemented, and refused by name: other parameterizations than ``eps``, a learned log-variance, EMA and condition models
-(pass the encoded context as ``cond``).  Sampling is not part of this module.
+Sampling is the reference's default, DDIM with classifier-free guidance (``ddim.DDIMSamplerB200``): ``sample`` / ``decode``
+run one CUDA-graph replay per denoising step.
+
+Not implemented, and refused by name: other parameterizations than ``eps``, a learned log-variance, EMA, condition models other
+than "identity" (pass the encoded context as ``cond``) and samplers other than "ddim".
 """
 from __future__ import annotations
 
@@ -25,12 +28,19 @@ import torch
 from torch import Tensor, nn
 
 from . import ops
+from .ddim import DDIMSamplerB200
 from ._cabi import B200Error
 from .unet import PAD_CHANNELS, UNetDiffuserB200, enable_grad_arena, noise_prediction_loss
 
 PREDICTIONS_KEY = "predictions"  # cflearn/constants.py
 NOISE_KEY = "noise"  # DDPM.noise_key (ddpm.py:99)
 TIMESTEPS_KEY = "timesteps"  # DDPM.timesteps_key (ddpm.py:100)
+IDENTITY_CONDITION_MODEL = "identity"  # DDPM.identity_condition_model (ddpm.py:101)
+
+
+def _check_sampler(sampler: str) -> None:
+    if sampler != "ddim":
+        raise NotImplementedError(f"DDPMB200: sampler={sampler!r} is not supported (ddim only)")
 
 
 def make_beta_schedule(schedule: str, timesteps: int, linear_start: float, linear_end: float, cosine_s: float) -> np.ndarray:
@@ -50,15 +60,21 @@ def make_beta_schedule(schedule: str, timesteps: int, linear_start: float, linea
     raise ValueError(f"unrecognized schedule '{schedule}' occurred")
 
 
-def noise_tables(timesteps: int = 1000, given_betas: Optional[np.ndarray] = None, beta_schedule: str = "linear",
-                 linear_start: float = 1.0e-4, linear_end: float = 2.0e-2, cosine_s: float = 8.0e-3) -> Tuple[Tensor, Tensor]:
-    """(sqrt(alphas_cumprod), sqrt(1 - alphas_cumprod)) as fp32 [T]: _register_noise_schedule (ddpm.py:599-629) in float64, then
-    one rounding to fp32."""
+def alphas_cumprod_table(timesteps: int = 1000, given_betas: Optional[np.ndarray] = None, beta_schedule: str = "linear",
+                         linear_start: float = 1.0e-4, linear_end: float = 2.0e-2, cosine_s: float = 8.0e-3) -> np.ndarray:
+    """alphas_cumprod as _register_noise_schedule (ddpm.py:608-616) computes it: float64 [T]."""
     if given_betas is not None:
         betas = np.asarray(given_betas, dtype=np.float64)
     else:
         betas = make_beta_schedule(beta_schedule, timesteps, linear_start, linear_end, cosine_s)
-    alphas_cumprod = np.cumprod(1.0 - betas, axis=0)
+    return np.cumprod(1.0 - betas, axis=0)
+
+
+def noise_tables(timesteps: int = 1000, given_betas: Optional[np.ndarray] = None, beta_schedule: str = "linear",
+                 linear_start: float = 1.0e-4, linear_end: float = 2.0e-2, cosine_s: float = 8.0e-3) -> Tuple[Tensor, Tensor]:
+    """(sqrt(alphas_cumprod), sqrt(1 - alphas_cumprod)) as fp32 [T]: _register_noise_schedule (ddpm.py:599-629) in float64, then
+    one rounding to fp32."""
+    alphas_cumprod = alphas_cumprod_table(timesteps, given_betas, beta_schedule, linear_start, linear_end, cosine_s)
     a = torch.from_numpy(np.sqrt(alphas_cumprod)).to(torch.float32)
     s = torch.from_numpy(np.sqrt(1.0 - alphas_cumprod)).to(torch.float32)
     return a, s
@@ -80,21 +96,30 @@ class DDPMB200(nn.Module):
                  channel_multipliers: Tuple[int, ...] = (1, 2, 4, 4), ema_decay: Optional[float] = None, parameterization: str = "eps",
                  condition_model: Optional[str] = None, timesteps: int = 1000, given_betas: Optional[np.ndarray] = None,
                  beta_schedule: str = "linear", linear_start: float = 1.0e-4, linear_end: float = 2.0e-2, cosine_s: float = 8.0e-3,
-                 learn_log_var: bool = False, **unet_kwargs: Any) -> None:
+                 learn_log_var: bool = False, sampler: str = "ddim", sampler_config: Optional[Dict[str, Any]] = None,
+                 **unet_kwargs: Any) -> None:
         super().__init__()
         what = "DDPMB200"
         refused = [(parameterization != "eps", f"parameterization={parameterization!r} (eps only)"),
                    (learn_log_var, "learn_log_var (a learned log-variance)"), (ema_decay is not None, "ema_decay (EMA)"),
-                   (condition_model is not None, "condition_model (pass the encoded context as cond)")]
+                   (condition_model not in (None, IDENTITY_CONDITION_MODEL),
+                    "condition_model (pass the encoded context as cond, with condition_model None or \"identity\")")]
         for bad, option in refused:
             if bad:
                 raise NotImplementedError(f"{what}: {option} is not supported")
+        _check_sampler(sampler)
         self.img_size = img_size
         self.in_channels, self.out_channels = in_channels, out_channels
         self.unet = UNetDiffuserB200(in_channels, out_channels, num_heads=num_heads, channel_multipliers=channel_multipliers,
                                      **unet_kwargs)
         a, s = noise_tables(timesteps, given_betas, beta_schedule, linear_start, linear_end, cosine_s)
         self.t = int(a.shape[0])
+        # the reference's float64 buffer, read by the sampler's host tables: a plain attribute, so it stays on the host and out of
+        # the state_dict
+        self.alphas_cumprod = torch.from_numpy(alphas_cumprod_table(timesteps, given_betas, beta_schedule, linear_start, linear_end,
+                                                                    cosine_s))
+        # _initialize_condition_model (ddpm.py:573-585): "identity" is nn.Identity, which has no state
+        self.condition_model: Optional[nn.Module] = nn.Identity() if condition_model == IDENTITY_CONDITION_MODEL else None
         self.register_buffer("sqrt_alphas_cumprod", a, persistent=False)
         self.register_buffer("sqrt_one_minus_alphas_cumprod", s, persistent=False)
         grads = enable_grad_arena(self.unet)
@@ -102,6 +127,8 @@ class DDPMB200(nn.Module):
         self.geo = self.engine = grads  # what dp reads: buckets(), reducer, shrink_next
         self.grad_arena = grads
         self.last_bad_flag: Optional[Tensor] = None
+        self.sampler: DDIMSamplerB200
+        self.switch_sampler(sampler, sampler_config)
 
     def _noised(self, net: Tensor, noise: Optional[Tensor], timesteps: Optional[Tensor]) -> Tuple[Tensor, Tensor, Tensor]:
         what = "DDPMB200"
@@ -133,3 +160,37 @@ class DDPMB200(nn.Module):
         if red is not None:
             self.grad_arena.check()
         return loss.detach()
+
+    # sampling (DDPM.generate_z / decode / sample / get_cond / switch_sampler, ddpm.py:264-356)
+
+    def switch_sampler(self, sampler: str, sampler_config: Optional[Dict[str, Any]] = None) -> None:
+        """Replace the sampler: "ddim" with ``DDIMSamplerB200``'s keywords; any other name raises ``NotImplementedError``."""
+        _check_sampler(sampler)
+        old = getattr(self, "sampler", None)
+        if old is not None:
+            old.release()
+        self.sampler = DDIMSamplerB200(self, **(sampler_config or {}))
+
+    def get_cond(self, cond: Any) -> Any:
+        if self.condition_model is None:
+            raise ValueError("should not call `get_cond` when `condition_model` is not provided")
+        return self.condition_model(cond)
+
+    def decode(self, z: Tensor, *, cond: Optional[Any] = None, num_steps: Optional[int] = None, start_step: Optional[int] = None,
+               verbose: bool = False, **kwargs: Any) -> Tensor:
+        """The sampler's loop from the fp32 latent z [B, in_channels, H, W] (CUDA, contiguous), conditioned on ``cond`` (an
+        encoded context [B, Tk, context_dim], or None).  ``kwargs`` override the sampler's keywords for this call."""
+        return self.sampler.sample(z, cond=cond, num_steps=num_steps, start_step=start_step, verbose=verbose, **kwargs)
+
+    def sample(self, num_samples: int, *, cond: Optional[Any] = None, num_steps: Optional[int] = None,
+               start_step: Optional[int] = None, clip_output: bool = True, verbose: bool = False,
+               kwargs: Optional[Dict[str, Any]] = None, **other_kw: Any) -> Tensor:
+        """``num_samples`` latents from ``torch.randn`` [n, in_channels, img_size, img_size] on the parameters' device (the current
+        CUDA generator), then ``decode``, then clipped to [-1, 1] unless ``clip_output`` is False."""
+        kw = dict(other_kw)
+        if kwargs is not None:
+            kw.update(kwargs)
+        device = next(self.unet.parameters()).device
+        z = torch.randn((num_samples, self.in_channels, self.img_size, self.img_size), dtype=torch.float32, device=device)
+        sampled = self.decode(z, cond=cond, num_steps=num_steps, start_step=start_step, verbose=verbose, **kw)
+        return torch.clip(sampled, -1.0, 1.0) if clip_output else sampled

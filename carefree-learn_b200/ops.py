@@ -886,12 +886,15 @@ def _layout(what: str, name: str, t: Tensor, dtypes: Tuple[torch.dtype, ...]) ->
     return cl and not t.is_contiguous()
 
 
-def pad_channels(x: Tensor, cp: int) -> Tensor:
+def pad_channels(x: Tensor, cp: int, *, out: Optional[Tensor] = None) -> Tensor:
     """x fp32 or bf16 [B, C, H, W] (contiguous NCHW or channels-last) -> bf16 [B, H, W, cp] with channels >= C zero: the
-    round-to-nearest-even cast autocast applies, then zero padding to a width the convolutions take."""
+    round-to-nearest-even cast autocast applies, then zero padding to a width the convolutions take.  ``out``: write there
+    (contiguous bf16 [B, H, W, cp]) instead of a new tensor."""
     cl = _layout("pad_channels", "x", x, (_F32, _BF16))
     B, C, H, W = x.shape
-    out = torch.empty((B, H, W, cp), dtype=torch.bfloat16, device=x.device)
+    if out is None:
+        out = torch.empty((B, H, W, cp), dtype=torch.bfloat16, device=x.device)
+    _check("pad_channels", "out", out, _BF16, (B, H, W, cp))
     call("b200_pad_channels_bf16", x.data_ptr(), int(x.dtype == _F32), int(cl), out.data_ptr(), B, C, H, W, cp, _stream())
     return out
 
@@ -936,3 +939,35 @@ def noise_prediction_loss(pred: Tensor, noise: Tensor, *, grad_out: Optional[Ten
     call("b200_noise_prediction_loss_bf16", pred.data_ptr(), noise.data_ptr(), int(noise.dtype == _F32), _ptr(loss), _ptr(dpred),
          _ptr(grad_out), B, N, _stream())
     return loss if grad_out is None else dpred
+
+
+def ddim_step(eps: Tensor, eps_uncond: Optional[Tensor], guidance_scale: float, x: Tensor, noise: Tensor, coef: Tensor,
+              ts_table: Tensor, temperature: float, step_dev: Tensor, bad_flag: Tensor, next_in: Tensor, next_ts: Tensor, *,
+              increment: bool = True) -> None:
+    """One DDIM step in place (include/b200_cflearn_ext.h, ``b200_ddim_step_bf16``): eps (and eps_uncond, or None) bf16
+    [B, C, H, W] with dense channels-last strides (the UNet's output, or a batch half of it); x, noise fp32 contiguous NCHW
+    [B, C, H, W]; coef fp32 [S, 5] and ts_table int64 [S] (``ddim.DDIMTables``); step_dev and bad_flag int32 [1]; next_in bf16
+    [copies B, H, W, Cp] and next_ts int64 [copies B], copies 1 or 2.  ``increment``: advance step_dev after the step."""
+    what = "ddim_step"
+    _check(what, "x", x, _F32, (None, None, None, None))
+    B, C, H, W = x.shape
+    _check(what, "noise", noise, _F32, (B, C, H, W))
+    for name, e in (("eps", eps), ("eps_uncond", eps_uncond)):
+        if e is None and name == "eps_uncond":
+            continue
+        if not (e.is_cuda and e.dtype == _BF16 and e.shape == (B, C, H, W) and e.is_contiguous(memory_format=torch.channels_last)):
+            got = f"{e.dtype} {list(e.shape)} with strides {list(e.stride())} on {e.device}"
+            raise B200Error(f"{what}: {name} must be a CUDA bf16 tensor [{B}, {C}, {H}, {W}] with dense channels-last strides (got {got})")
+    _check(what, "coef", coef, _F32, (None, 5))
+    S = coef.shape[0]
+    _check(what, "ts_table", ts_table, torch.int64, (S,))
+    _check(what, "step_dev", step_dev, torch.int32, (1,))
+    _check(what, "bad_flag", bad_flag, torch.int32, (1,))
+    _check(what, "next_in", next_in, _BF16, (None, H, W, None))
+    copies = next_in.shape[0] // B
+    if copies not in (1, 2) or next_in.shape[0] != copies * B:
+        raise B200Error(f"{what}: next_in must hold 1 or 2 copies of the batch ([B or 2B, H, W, Cp]), got {list(next_in.shape)}")
+    _check(what, "next_ts", next_ts, torch.int64, (copies * B,))
+    call("b200_ddim_step_bf16", eps.data_ptr(), _ptr(eps_uncond), float(guidance_scale), x.data_ptr(), noise.data_ptr(), coef.data_ptr(),
+         ts_table.data_ptr(), S, float(temperature), step_dev.data_ptr(), int(increment), bad_flag.data_ptr(), next_in.data_ptr(),
+         next_ts.data_ptr(), copies, B, C, H, W, next_in.shape[3], _stream())

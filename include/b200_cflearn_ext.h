@@ -98,6 +98,22 @@ int b200_q_sample_pad_bf16(const float* x0, const float* noise, int channels_las
                            const float* sqrt_alphas_cumprod, const float* sqrt_one_minus_alphas_cumprod, long long T, int* bad_flag,
                            void* out, int B, int C, int H, int W, int Cp, cudaStream_t stream);
 
+/* One DDIM denoising step (DDIMSampler, cflearn/modules/multimodal/diffusion/samplers/ddim.py:195-239, with the classifier-free
+ * guidance of samplers/schema.py:215-255), which also writes the stem's input for the next step.  step = *step_dev (int32, only
+ * read by the step) picks coef[step] = {s1m, sqrt_a, sqrt_ap, c_dir, sigma} (fp32 [S, 5]) and for every element, with e the
+ * bf16 eps (dense channels-last [B, H, W, C], UNetDiffuserB200's output layout):
+ *   guided (eps_uncond, the same layout, given and guidance_scale != 1):  e = bf16(u + bf16(scale bf16(e - u))), u = eps_uncond;
+ *   x <- ((sqrt_ap ((x - s1m e) / sqrt_a)) + c_dir e) + (sigma noise) temperature
+ * in fp32, every operation rounded, no contraction.  x and noise: fp32 [B, C, H, W], dense NCHW; x is updated in place.  When
+ * step + 1 < S: next_in (bf16 [copies B, H, W, Cp], dense) gets bf16(x) in channels < C and +0 in channels C..Cp of each of its
+ * copies (1 or 2; 2 needs eps_uncond), and next_ts (int64 [copies B]) gets ts_table[step + 1] (ts_table: int64 [S]).  A counter
+ * outside [0, S) reads no table entry: it sets *bad_flag = 1 (never cleared here), x becomes NaN and nothing else is written.
+ * increment = 1 then adds 1 to *step_dev in a second, one-thread launch.  0 < C <= Cp, Cp % 8 == 0, H * W < 2^31,
+ * 2 B * H * W * Cp <= 2^38. */
+int b200_ddim_step_bf16(const void* eps, const void* eps_uncond, float guidance_scale, float* x, const float* noise, const float* coef,
+                        const long long* ts_table, int S, float temperature, int* step_dev, int increment, int* bad_flag,
+                        void* next_in, long long* next_ts, int copies, int B, int C, int H, int W, int Cp, cudaStream_t stream);
+
 /* ---------------------------------------------------------------------------------------------------------
  * AdamW on the flat fp32 arenas (torch.optim.AdamW without amsgrad; the zoo's DDPM trains with "adamw",
  * cflearn/optimizers.py:31): b200_adam_step / b200_adam_step_dev with decoupled weight decay, in torch.optim.AdamW's order:
