@@ -110,6 +110,7 @@ EXT_SIGNATURES: Dict[str, Any] = {
                                     c_int, c_int, _P]),
     "b200_adamw_step": (c_int, [_P, _P, _P, _P, _LL, c_float, c_float, c_float, c_float, c_float, c_int, _P, _P]),
     "b200_adamw_step_dev": (c_int, [_P, _P, _P, _P, _LL, _P, _P, c_int, _P]),
+    "b200_softmax_rows_bf16": (c_int, [_P, _LL, _P, _LL, c_int, c_int, c_float, _P]),
 }
 
 _lib: Optional[ctypes.CDLL] = None

@@ -521,10 +521,11 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                         const int cpb = p.conv_cin / BK;
                         const int tap = kb / cpb, c0 = (kb - tap * cpb) * BK;
                         const int hw = p.conv_h * p.conv_w, q0 = m0 - cls * p.class_stride;
-                        const int bimg = q0 / hw, y0 = (q0 - bimg * hw) / p.conv_w;
+                        const int bimg = q0 / hw, q = q0 - bimg * hw, y0 = q / p.conv_w;
+                        const int x0 = q - y0 * p.conv_w;  // 0 unless a row is wider than a tile (then a multiple of 128)
                         int dx, dy;
                         conv_tap(p.conv_kind, cls, tap, dx, dy);
-                        tma_load_4d(a_dst, &tmA, &full_bar[stage], c0, dx, y0 * conv_ys(p.conv_kind) + dy, bimg);
+                        tma_load_4d(a_dst, &tmA, &full_bar[stage], c0, x0 * conv_ys(p.conv_kind) + dx, y0 * conv_ys(p.conv_kind) + dy, bimg);
                     } else if constexpr (!TA) {
                         tma_load_2d(a_dst, &tmA, &full_bar[stage], kb * BK, m0);
                     } else {
@@ -888,14 +889,16 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
         uint64_t d[2], s[1];
         uint32_t bx[2];
         if (cg != nullptr && cg->mode == 1) {
-            // channels-last activation [B, H, W, Cin]: dims {Cin, W, H, B}; box = 64 channels x 128 consecutive pixels
-            const int hb = cg->H < BM / cg->W ? cg->H : BM / cg->W;      // image rows per tile
-            const int nb = BM / (cg->W * hb);                             // images per tile (> 1 only when H * W < 128)
+            // channels-last activation [B, H, W, Cin]: dims {Cin, W, H, B}; box = 64 channels x 128 consecutive pixels: whole
+            // rows when W divides 128, else (W = 128 times a power of 2) 128 pixels of one row
+            const int wb = cg->W < BM ? cg->W : BM;                                         // pixels of a row per tile
+            const int hb = cg->W >= BM ? 1 : (cg->H < BM / cg->W ? cg->H : BM / cg->W);      // image rows per tile
+            const int nb = BM / (wb * hb);                                // images per tile (> 1 only when H * W < 128)
             const uint32_t st = conv_ys(cg->kind);
             const uint64_t sw = st * static_cast<uint64_t>(cg->W), sh = st * static_cast<uint64_t>(cg->H);
             uint64_t d4[4] = {static_cast<uint64_t>(cg->Cin), sw, sh, static_cast<uint64_t>(cg->B)};
             uint64_t s4[3] = {static_cast<uint64_t>(cg->Cin) * 2, sw * cg->Cin * 2, sh * sw * cg->Cin * 2};
-            uint32_t b4[4] = {BK, static_cast<uint32_t>(sw), st * hb, static_cast<uint32_t>(nb)};
+            uint32_t b4[4] = {BK, st * wb, st * hb, static_cast<uint32_t>(nb)};
             const uint32_t es[4] = {1, st, st, 1};
             if ((rc = make_tmap(&tmA, A, 2, 4, d4, s4, b4, 128, es)) != 0) return rc;
         } else {
@@ -966,6 +969,12 @@ extern "C" int b200_gemm_bf16(const void* A, long long lda, int a_mn_major, cons
     return gemm_dispatch(A, lda, a_mn_major, B, ldb, b_mn_major, M, N, K, epilogue, bias, out0, out1, aux, ldo, splits, max_ctas, stream, nullptr);
 }
 
+// Widths of 128 times a power of 2 (256, 512, ...: the KL decoder's wide images) take tiles of 128 pixels of one row; the
+// narrower widths that divide 128 keep tiles of whole rows.  The power of 2 is a policy, not a correctness condition: any
+// multiple of 128 keeps every tile inside one row and would tile the same way.  It keeps the admitted widths to those the
+// decoder's levels produce (W = 384, a 768 px image's, stays refused with the rest of that geometry).
+static bool wide_rows(int W) { return W > BM && W % BM == 0 && ((W / BM) & (W / BM - 1)) == 0; }
+
 // 3x3 convolution, stride 1, zero padding 1, on channels-last bf16 activations, as an implicit GEMM on the wgmma main loop:
 //   out[b, y, x, co] = epilogue( sum_{ky,kx,ci} x[b, y+ky-1, x+kx-1, ci] * w[co, ky, kx, ci] )
 // x: [B, H, W, Cin]; w_packed: [Cout, 9 * Cin] (tap-major: k = (ky * 3 + kx) * Cin + ci); out / aux: [B*H*W, ldo].
@@ -978,9 +987,11 @@ extern "C" int b200_conv3x3_nhwc_bf16(const void* x, const void* w_packed, const
                                       int B, int H, int W, int Cin, int Cout, int epilogue, cudaStream_t stream) {
     if (B <= 0 || H <= 0 || W <= 0 || Cin <= 0 || Cout <= 0) return refuse(B200_ERR_ARG, "conv3x3", "non-positive size");
     if (Cin % BK != 0) return refuse(B200_ERR_ARG, "conv3x3", "Cin must be a multiple of 64");
-    if (W > BM || BM % W != 0) return refuse(B200_ERR_ARG, "conv3x3", "the image width must divide 128");
-    const int hb = H < BM / W ? H : BM / W;
-    if (H % hb != 0 || BM % (W * hb) != 0) return refuse(B200_ERR_ARG, "conv3x3", "H must be a multiple of 128 / W (or H * W must divide 128)");
+    if (!wide_rows(W)) {
+        if (W > BM || BM % W != 0) return refuse(B200_ERR_ARG, "conv3x3", "the image width must divide 128 or be 128 times a power of 2");
+        const int hb = H < BM / W ? H : BM / W;
+        if (H % hb != 0 || BM % (W * hb) != 0) return refuse(B200_ERR_ARG, "conv3x3", "H must be a multiple of 128 / W (or H * W must divide 128)");
+    }
     const ConvGeom cg{B, H, W, Cin, 1, CONV_S1};
     const long long M = static_cast<long long>(B) * H * W;
     if (M > 0x7fffffffll) return refuse(B200_ERR_ARG, "conv3x3", "too many pixels");
@@ -1010,15 +1021,19 @@ extern "C" int b200_conv3x3_wgrad_nhwc_bf16(const void* dy, long long ld_dy, con
 // resampling convolutions (include/b200_cflearn_ext.h): the same main loop with other tap tables and output addressing
 // ------------------------------------------------------------------------------------------------
 // The size checks every resampling entry shares.  (H, W) is the lower-resolution side; (h, w) the grid the GEMM tiles;
-// red / outc: the reduction's and the output's channels.
-static int check_resample(const char* entry, int B, int H, int W, int red, int outc, bool even, int h, int w) {
+// red / outc: the reduction's and the output's channels.  wide: the grid may also be 128 times a power of 2 wide (forward entries
+// whose tiles need no whole rows).
+static int check_resample(const char* entry, int B, int H, int W, int red, int outc, bool even, int h, int w, bool wide = false) {
     if (B <= 0 || H <= 0 || W <= 0 || red <= 0 || outc <= 0) return refuse(B200_ERR_ARG, entry, "non-positive size");
     if (even && (H % 2 != 0 || W % 2 != 0)) return refuse(B200_ERR_ARG, entry, "H and W must be even");
     if (red % BK != 0) return refuse(B200_ERR_ARG, entry, "the reduction's channel count must be a multiple of 64");
     if (outc % 8 != 0) return refuse(B200_ERR_ARG, entry, "the output's channel count must be a multiple of 8");
-    if (w > BM || BM % w != 0) return refuse(B200_ERR_ARG, entry, "the grid width must divide 128");
-    const int hb = h < BM / w ? h : BM / w;
-    if (h % hb != 0 || BM % (w * hb) != 0) return refuse(B200_ERR_ARG, entry, "the grid height must be a multiple of 128 / width (or height * width must divide 128)");
+    if (!(wide && wide_rows(w))) {
+        if (w > BM || BM % w != 0)
+            return refuse(B200_ERR_ARG, entry, wide ? "the grid width must divide 128 or be 128 times a power of 2" : "the grid width must divide 128");
+        const int hb = h < BM / w ? h : BM / w;
+        if (h % hb != 0 || BM % (w * hb) != 0) return refuse(B200_ERR_ARG, entry, "the grid height must be a multiple of 128 / width (or height * width must divide 128)");
+    }
     if (4ll * B * (2 * H) * (2 * W) > 0x7fffffffll) return refuse(B200_ERR_ARG, entry, "too many pixels");
     return 0;
 }
@@ -1059,7 +1074,7 @@ extern "C" int b200_conv3x3_s2_wgrad_nhwc_bf16(const void* dy, long long ld_dy, 
 
 extern "C" int b200_conv3x3_up2_nhwc_bf16(const void* x, const void* w_packed, const void* bias, void* out0, const void* aux, long long ldo,
                                           int B, int H, int W, int Cin, int Cout, int epilogue, cudaStream_t stream) {
-    if (const int rc = check_resample("conv3x3_up2", B, H, W, Cin, Cout, false, H, W)) return rc;
+    if (const int rc = check_resample("conv3x3_up2", B, H, W, Cin, Cout, false, H, W, true)) return rc;
     const ConvGeom cg{B, H, W, Cin, 1, CONV_UP2};
     return gemm_dispatch(x, Cin, 0, w_packed, 9ll * Cin, 0, class_m(cg), Cout, 9 * Cin, epilogue, bias, out0, nullptr, aux, ldo, 1, 0,
                          stream, &cg);

@@ -1434,3 +1434,53 @@ extern "C" int b200_fill_f32(float* dst, float value, long long n, cudaStream_t 
     fill_f32_kernel<<<static_cast<unsigned>((thr + 255) / 256), 256, 0, stream>>>(dst, value, n);
     return check_launch("fill_f32");
 }
+
+// ------------------------------------------------------------------------------------------------
+// row softmax of the KL decoder's single-head spatial attention (include/b200_cflearn_ext.h)
+// ------------------------------------------------------------------------------------------------
+namespace b200 {
+
+constexpr int SOFTMAX_THREADS = 256;
+
+// the block's max or sum of v (every thread gets it), reduced in a fixed order
+template <bool kMax>
+__device__ __forceinline__ float softmax_block_reduce(float v, float* red) {
+    v = kMax ? warp_max(v) : warp_sum(v);
+    const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+    if (lane == 0) red[warp] = v;
+    __syncthreads();
+    v = lane < SOFTMAX_THREADS / 32 ? red[lane] : (kMax ? -INFINITY : 0.f);
+    v = kMax ? warp_max(v) : warp_sum(v);
+    __syncthreads();  // red is reused by the next reduction
+    return v;
+}
+
+// One block per row: m = max_c s[c], l = sum_c exp(scale (s[c] - m)), p[c] = bf16(exp(scale (s[c] - m)) / l).  Two reads of the
+// fp32 row (the second mostly from L2), one bf16 write.
+__global__ void __launch_bounds__(SOFTMAX_THREADS) softmax_rows_kernel(const float* __restrict__ s, long long lds, __nv_bfloat16* __restrict__ p,
+                                                                       long long ldp, int cols, float scale) {
+    __shared__ float red[SOFTMAX_THREADS / 32];
+    const float* row = s + static_cast<long long>(blockIdx.x) * lds;
+    __nv_bfloat16* out = p + static_cast<long long>(blockIdx.x) * ldp;
+    float m = -INFINITY;
+    for (int c = threadIdx.x; c < cols; c += SOFTMAX_THREADS) m = fmaxf(m, row[c]);
+    m = softmax_block_reduce<true>(m, red);
+    float l = 0.f;
+    for (int c = threadIdx.x; c < cols; c += SOFTMAX_THREADS) l += expf(scale * (row[c] - m));
+    l = softmax_block_reduce<false>(l, red);
+    for (int c = threadIdx.x; c < cols; c += SOFTMAX_THREADS) out[c] = __float2bfloat16_rn(expf(scale * (row[c] - m)) / l);
+}
+
+}  // namespace b200
+
+extern "C" int b200_softmax_rows_bf16(const float* s, long long lds, void* p_bf16, long long ldp, int rows, int cols, float scale,
+                                      cudaStream_t stream) {
+    const char* E = "softmax_rows";
+    if (rows <= 0 || cols <= 0) return refuse(B200_ERR_ARG, E, "non-positive size");
+    if (!(scale > 0.f) || isinf(scale)) return refuse(B200_ERR_ARG, E, "scale must be positive and finite");
+    if (lds < cols || ldp < cols) return refuse(B200_ERR_ARG, E, "lds / ldp < cols");
+    if (!s || !p_bf16) return refuse(B200_ERR_ARG, E, "null pointer");
+    if (!aligned(4, {s}) || !aligned(2, {p_bf16})) return refuse(B200_ERR_ALIGN, E, "s not 4-byte / p not 2-byte aligned");
+    softmax_rows_kernel<<<rows, SOFTMAX_THREADS, 0, stream>>>(s, lds, reinterpret_cast<__nv_bfloat16*>(p_bf16), ldp, cols, scale);
+    return check_launch(E);
+}

@@ -971,3 +971,19 @@ def ddim_step(eps: Tensor, eps_uncond: Optional[Tensor], guidance_scale: float, 
     call("b200_ddim_step_bf16", eps.data_ptr(), _ptr(eps_uncond), float(guidance_scale), x.data_ptr(), noise.data_ptr(), coef.data_ptr(),
          ts_table.data_ptr(), S, float(temperature), step_dev.data_ptr(), int(increment), bad_flag.data_ptr(), next_in.data_ptr(),
          next_ts.data_ptr(), copies, B, C, H, W, next_in.shape[3], _stream())
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# the KL-f8 autoencoder's single-head spatial attention (include/b200_cflearn_ext.h)
+# ----------------------------------------------------------------------------------------------------------------
+def softmax_rows(s: Tensor, scale: float, *, out: Optional[Tensor] = None) -> Tensor:
+    """p = bf16(softmax(scale * s, dim=-1)) of s fp32 [rows, cols] (unit inner stride), in fp32 with a fixed reduction order.
+    ``out``: write there (bf16 [rows, cols], unit inner stride) instead of a new tensor with 16-byte aligned rows."""
+    what = "softmax_rows"
+    lds = _check(what, "s", s, _F32, view=True)
+    rows, cols = s.shape
+    if out is None:
+        out = torch.empty((rows, (cols + 7) // 8 * 8), dtype=torch.bfloat16, device=s.device)[:, :cols]
+    ldp = _check(what, "out", out, _BF16, (rows, cols), view=True)
+    call("b200_softmax_rows_bf16", s.data_ptr(), lds, out.data_ptr(), ldp, rows, cols, float(scale), _stream())
+    return out

@@ -331,7 +331,8 @@ int b200_fill_f32(float* dst, float value, long long n, cudaStream_t stream);
 /* ---------------------------------------------------------------------------------------------------------
  * 3x3 convolution (stride 1, zero padding 1) on channels-last bf16 activations as an IMPLICIT GEMM on the wgmma main
  * loop: x [B, H, W, Cin], w_packed [Cout, 9 * Cin] (k = (ky * 3 + kx) * Cin + ci), bias bf16 [Cout] or NULL,
- * out0 / aux [B*H*W, ldo].  Cin % 64 == 0; W divides 128 and H is a multiple of 128 / W (or H * W divides 128).
+ * out0 / aux [B*H*W, ldo].  Cin % 64 == 0; W divides 128 and H is a multiple of 128 / W (or H * W divides 128), or W is 128
+ * times a power of 2 (256, 512, ...; each 128-pixel tile is then part of one image row).
  * epilogue: B200_EPI_BIAS_BF16, B200_EPI_BIAS_RESID_F32, B200_EPI_BIAS_RESID_CLAMP_BF16 (aux bf16 [B*H*W, ldo]) or
  * B200_EPI_BIAS_ADD_PER_IMAGE_BF16 (aux bf16 [B, ldo]).  No im2col matrix exists: each (tap, 64-channel) k-block is ONE
  * TMA box of the activation shifted by the tap, its halo zero-filled by the TMA unit.

@@ -22,7 +22,8 @@ extern "C" {
  * Geometry: H and W are the sizes of the lower-resolution side (the input of the stride-2 convolution is H x W and its output
  * H/2 x W/2; the upsampling convolution's input is H x W and its output 2H x 2W).  Write h x w for the grid the GEMM tiles:
  * H/2 x W/2 for the stride-2 convolution and its input gradient, H x W for the upsampling convolution.  Then w divides 128 and
- * h is a multiple of 128 / w (or h * w divides 128), the rule of b200_conv3x3_nhwc_bf16.  The weight gradient needs, on its
+ * h is a multiple of 128 / w (or h * w divides 128), the rule of b200_conv3x3_nhwc_bf16; the upsampling convolution also takes
+ * a w of 128 times a power of 2, as that entry does (the KL-f8 decoder's 128 -> 256 and 256 -> 512).  The weight gradient needs, on its
  * h x w grid, w dividing 64 and h * w a multiple of 64.  Channel counts: the reduction's channels (Cin of a forward, Cout of an
  * input gradient) are a multiple of 64, the output's a multiple of 8.  Sizes are positive; H and W of the stride-2 entries
  * are even.  The six resampling layers of SD-v1.5 at 512 px (H x W, Cin = Cout: 64 x 64 / 320, 32 x 32 / 640, 16 x 16 / 1280
@@ -124,6 +125,16 @@ int b200_adamw_step(float* params, const float* grads, float* exp_avg, float* ex
                     float beta2, float eps, float weight_decay, int step, int* step_dev, cudaStream_t stream);
 int b200_adamw_step_dev(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n, const float* hyper_dev,
                         int* step_dev, int increment, cudaStream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------
+ * Row softmax of the KL-f8 autoencoder's single-head SpatialAttention (cflearn/modules/core/attentions.py:330-370, sdp_attn
+ * with one head of width C over the H * W pixels), between the GEMMs S = Q K^T (fp32 out) and O = P V:
+ *   p[r][c] = bf16( exp(scale (s[r][c] - m_r)) / l_r ),  m_r = max_c s[r][c],  l_r = sum_c exp(scale (s[r][c] - m_r))
+ * in fp32, every row reduced in a fixed order (bit-identical run to run).  s: fp32 [rows, lds]; p: bf16 [rows, ldp];
+ * rows, cols > 0, lds >= cols, ldp >= cols, scale > 0 and finite.  One launch.
+ * --------------------------------------------------------------------------------------------------------- */
+int b200_softmax_rows_bf16(const float* s, long long lds, void* p, long long ldp, int rows, int cols, float scale,
+                           cudaStream_t stream);
 
 #ifdef __cplusplus
 }
