@@ -466,11 +466,15 @@ def gemm_epilogue(epi, t, aux=None):
     raise ValueError(f"no reference for epilogue {epi}")
 
 
-def adam(p, g, m, v, steps, lr, b1, b2, eps, wd, grad_scale=1.0):
-    """Adam with L2 weight decay (torch.optim.Adam's update) over the step numbers ``steps``: (params, exp_avg, exp_avg_sq)."""
+def adam(p, g, m, v, steps, lr, b1, b2, eps, wd, grad_scale=1.0, decoupled=False):
+    """Adam with L2 weight decay (torch.optim.Adam's update) over the step numbers ``steps``: (params, exp_avg, exp_avg_sq).
+    ``decoupled``: AdamW (torch.optim.AdamW's update), p <- p (1 - lr wd) first and no L2 term.  grad_scale multiplies only the
+    gradient."""
     p, m, v = p.to(F64).clone(), m.to(F64).clone(), v.to(F64).clone()
     for t in steps:
-        gg = g.to(F64) * grad_scale + wd * p
+        if decoupled:
+            p = p * (1 - lr * wd)
+        gg = g.to(F64) * grad_scale + (0.0 if decoupled else wd * p)
         m = b1 * m + (1 - b1) * gg
         v = b2 * v + (1 - b2) * gg * gg
         p = p - lr / (1 - b1 ** t) * m / (v.sqrt() / math.sqrt(1 - b2 ** t) + eps)

@@ -24,7 +24,7 @@ from cflearn_b200 import B200Error, ops  # noqa: E402
 from cflearn_b200.autoencoder import AttentionAutoEncoderKLB200, spatial_attention  # noqa: E402
 from _refs import (assert_bf16_close, assert_ulp, bf16, conv3x3, conv3x3_up2, exact_conv_operands, exponents, first_bad,  # noqa: E402
                    groupnorm, relerr)
-from test_kernel_footprint_gpu import Case, S, assert_equal, call, rand  # noqa: E402
+from test_kernel_footprint_gpu import Case, S, assert_equal, call, covers, rand  # noqa: E402
 import ae_oracle as ao  # noqa: E402
 
 DEV = "cuda"
@@ -102,6 +102,7 @@ def test_groupnorm_at_512px_batch_8(silu):
 
 
 # ---- 3. softmax and attention ----------------------------------------------------------------------------------------------------------
+@covers("b200_softmax_rows_bf16")
 @pytest.mark.gpu
 @pytest.mark.parametrize("rows,cols,lds,ldp", [(3, 1, 1, 8), (130, 1000, 1003, 1008), (64, 4096, 4096, 4096)])
 def test_softmax_rows(rows, cols, lds, ldp):

@@ -1,8 +1,8 @@
 """DDIM sampling on an H100 (pytest -m gpu): b200_ddim_step_bf16 bit for bit against the oracle's step in torch ops on CUDA at
-every step of a 50-step schedule, guided and not, on inputs with signed zeros, large magnitudes and bf16 ties, and its
-out-of-range counter; DDPMB200.decode bit for bit against oracle/ddim_oracle.py's loop driving the same native UNet, across the
-golden fixture's case matrix and at SD-v1.5, including the generator state after the call; the graph cache; and a graphed
-training step unchanged by sampling between its steps."""
+every step of a 50-step schedule, guided and not, on inputs with signed zeros, large magnitudes and bf16 ties, its out-of-range
+counter, and its footprint behind guarded buffers; DDPMB200.decode bit for bit against oracle/ddim_oracle.py's loop driving the
+same native UNet, across the golden fixture's case matrix and at SD-v1.5, including the generator state after the call; the
+graph cache; and a graphed training step unchanged by sampling between its steps."""
 import json
 import os
 import sys
@@ -22,6 +22,7 @@ from cflearn_b200.ddpm import DDPMB200, alphas_cumprod_table  # noqa: E402
 from cflearn_b200.optim import ArenaAdamW  # noqa: E402
 from cflearn_b200.trainer import B200TrainStep  # noqa: E402
 import ddim_oracle  # noqa: E402
+from test_kernel_footprint_gpu import Case, S as current_stream, call, covers, rand  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda", 0)
@@ -128,6 +129,58 @@ def test_out_of_range_counter_sets_the_flag_and_poisons_x(counter):
     ops.ddim_step(ec, eu, 7.5, x, noise, coef.to(DEV), ts.to(DEV), 1.0, step, bad, next_in, next_ts, increment=False)
     assert int(bad.item()) == 1 and torch.isnan(x).all()
     assert int(step.item()) == counter and not next_in.any() and (next_ts == -7).all()
+
+
+# (B, C, H, W, Cp) of the noising kernel's footprint: C = 4 in one group of many; odd C with a half-real last pair; two real groups
+DDIM_SHAPES = [(2, 4, 8, 16, 64), (3, 5, 6, 7, 24), (2, 9, 3, 5, 16)]
+DDIM_STEPS = 7
+
+
+@covers("b200_ddim_step_bf16")
+@pytest.mark.parametrize("increment", [0, 1])
+@pytest.mark.parametrize("counter", [0, 3, DDIM_STEPS - 1, -1, DDIM_STEPS])
+@pytest.mark.parametrize("copies,scale", [(1, 7.5), (2, 7.5), (2, 1.0)], ids=["unguided", "guided", "guided_scale_1"])
+@pytest.mark.parametrize("B,C,H,W,Cp", DDIM_SHAPES)
+def test_ddim_step_footprint(B, C, H, W, Cp, copies, scale, counter, increment):
+    """Guarded buffers (test_kernel_footprint_gpu): coef [S, 5] has poison rows at -1 and S, so a read of either NaNs x.  In range,
+    x is the oracle's step bit for bit, and next_in / next_ts are written in full, or, on the last step, left exactly as they were.
+    Out of range, only x (NaN), the flag and the counter change.  The counter ends at its start plus increment."""
+    ts, coef = step_tables(torch.from_numpy(alphas_cumprod_table(1000)), "uniform", DDIM_STEPS, 0.7)
+    temperature = 1.3
+    x, noise, ec, eu = _step_inputs(B, C, H, W, copies == 2, seed=B * 100 + C)
+    ok = 0 <= counter < DDIM_STEPS
+    writes_next = ok and counter + 1 < DDIM_STEPS
+    rows = lambda v: v.permute(0, 2, 3, 1).reshape(-1, C)  # noqa: E731  ([B, C, H, W] view of channels-last memory -> [B H W, C])
+    c = Case(f"ddim_step {B}x{C}x{H}x{W} Cp {Cp} copies {copies} scale {scale} counter {counter} increment {increment}")
+    ge = c.input("eps", rows(ec))
+    gu = c.input("eps_uncond", rows(eu)) if eu is not None else None
+    gx = c.inout("x", x.reshape(B * C, H * W))
+    gn = c.input("noise", noise.reshape(B * C, H * W))
+    gc, gts = c.input("coef", coef), c.input("ts_table", ts)
+    step = c.inout("step_dev", torch.tensor([counter], dtype=torch.int32))
+    flag = c.inout("bad_flag", torch.zeros(1, dtype=torch.int32))
+    n_in = copies * B * H * W
+    prior_in, prior_ts = rand((n_in, Cp), 7), torch.arange(copies * B, dtype=torch.int64) - 7
+    if writes_next:
+        nin, nts = c.output("next_in", n_in, Cp, dtype=torch.bfloat16), c.output("next_ts", 1, copies * B, dtype=torch.int64)
+    else:
+        nin, nts = c.inout("next_in", prior_in), c.inout("next_ts", prior_ts)
+    r = c.run(lambda: call("b200_ddim_step_bf16", ge.ptr(), gu.ptr() if gu else None, scale, gx.ptr(), gn.ptr(), gc.ptr(), gts.ptr(),
+                           DDIM_STEPS, temperature, step.ptr(), increment, flag.ptr(), nin.ptr(), nts.ptr(), copies, B, C, H, W, Cp,
+                           current_stream()), nan_ok=() if ok else ("x",))
+    assert r["step_dev"].item() == counter + increment and r["bad_flag"].item() == int(not ok), c.name
+    if ok:
+        ref = _oracle_step(x, noise, ec, eu, scale, coef[counter], temperature)
+        assert torch.equal(_bits(r["x"]), _bits(ref.reshape(B * C, H * W).cpu())), f"{c.name}: x"
+    else:
+        assert torch.isnan(r["x"]).all(), f"{c.name}: x"
+    if writes_next:
+        want = F.pad(ref.to(torch.bfloat16).permute(0, 2, 3, 1), (0, Cp - C)).repeat(copies, 1, 1, 1).reshape(n_in, Cp).cpu()
+        assert torch.equal(_bits(r["next_in"]), _bits(want)), f"{c.name}: next_in"
+        assert (r["next_ts"] == ts[counter + 1]).all(), f"{c.name}: next_ts"
+    else:
+        assert torch.equal(_bits(r["next_in"]), _bits(prior_in)), f"{c.name}: next_in"
+        assert torch.equal(r["next_ts"].view(-1), prior_ts), f"{c.name}: next_ts"
 
 
 # ---- decode against the oracle loop on the same native UNet ------------------------------------------------------------------------------

@@ -1,7 +1,7 @@
-"""DDPMB200 on an H100 (pytest -m gpu): the fused noising kernel bit for bit against eager's q_sample, the gradient arena bit for
-bit against the UNet's autograd gradients (stored and use_checkpoint, small and SD-v1.5), gradient accumulation in the arena,
-train_step against torch noising + the UNet + the loss, ArenaAdamW in lock-step with torch.optim.AdamW, and the graphed step
-against the eager one."""
+"""DDPMB200 on an H100 (pytest -m gpu): the fused noising kernel bit for bit against eager's q_sample and behind guarded buffers,
+the gradient arena bit for bit against the UNet's autograd gradients (stored and use_checkpoint, small and SD-v1.5), gradient
+accumulation in the arena, train_step against torch noising + the UNet + the loss, ArenaAdamW in lock-step with
+torch.optim.AdamW, and the graphed step against the eager one."""
 import json
 import os
 import shutil
@@ -21,6 +21,7 @@ from cflearn_b200.ddpm import DDPMB200, noise_tables  # noqa: E402
 from cflearn_b200.optim import ArenaAdamW  # noqa: E402
 from cflearn_b200.trainer import B200TrainStep  # noqa: E402
 from cflearn_b200.unet import UNetDiffuserB200, enable_grad_arena, noise_prediction_loss  # noqa: E402
+from test_kernel_footprint_gpu import Case, S, call, covers  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda", 0)
@@ -99,6 +100,44 @@ def test_q_sample_pad_bad_timestep_sets_the_flag():
     assert torch.equal(_bits(out[good]), _bits(want))
     for b in (1, 3, 5):
         assert torch.isnan(out[b, ..., :3].float()).all() and (_bits(out[b, ..., 3:]) == 0).all()
+
+
+# (B, C, H, W, Cp): one group of 8 channels with C = 4 and many groups; odd C, whose last pair holds one real channel
+# (c + 1 < C fails); odd C across two real groups
+Q_SAMPLE_SHAPES = [(2, 4, 8, 16, 64), (3, 5, 6, 7, 24), (2, 9, 3, 5, 16)]
+Q_SAMPLE_T = 37
+
+
+@covers("b200_q_sample_pad_bf16")
+@pytest.mark.parametrize("timesteps", ["in_range", "out_of_range", "flag_already_set"])
+@pytest.mark.parametrize("channels_last", [0, 1])
+@pytest.mark.parametrize("B,C,H,W,Cp", Q_SAMPLE_SHAPES)
+def test_q_sample_pad_footprint(B, C, H, W, Cp, channels_last, timesteps):
+    """Guarded buffers (test_kernel_footprint_gpu): the tables are [T] with poison on both sides, so a read of entry -1 or T NaNs
+    an image; every image with a timestep in range is eager's bit for bit.  Timesteps 0 and T - 1 are in every in-range batch;
+    out of range, image 1 has T (and image 2, if any, -1).  The flag is only ever set, never cleared."""
+    a, s = noise_tables(timesteps=Q_SAMPLE_T)
+    g = torch.Generator().manual_seed(B * 100 + C)
+    x0 = torch.randn(B, C, H, W, generator=g) * 3
+    noise = torch.randn(B, C, H, W, generator=g)
+    t = torch.tensor([0, Q_SAMPLE_T - 1, 17][:B])
+    if timesteps == "out_of_range":
+        t[1:] = torch.tensor([Q_SAMPLE_T, -1][:B - 1])
+    good = (t >= 0) & (t < Q_SAMPLE_T)
+    layout = (lambda v: v.permute(0, 2, 3, 1)) if channels_last else (lambda v: v)
+    c = Case(f"q_sample_pad {B}x{C}x{H}x{W} Cp {Cp} cl {channels_last} {timesteps}")
+    gx, gn = c.input("x0", layout(x0).reshape(1, -1)), c.input("noise", layout(noise).reshape(1, -1))
+    gt, ga, gs = c.input("timesteps", t), c.input("sqrt_alphas_cumprod", a), c.input("sqrt_one_minus_alphas_cumprod", s)
+    flag = c.inout("bad_flag", torch.tensor([int(timesteps == "flag_already_set")], dtype=torch.int32))
+    out = c.output("out", B * H * W, Cp, dtype=torch.bfloat16)
+    r = c.run(lambda: call("b200_q_sample_pad_bf16", gx.ptr(), gn.ptr(), channels_last, gt.ptr(), ga.ptr(), gs.ptr(), Q_SAMPLE_T,
+                           flag.ptr(), out.ptr(), B, C, H, W, Cp, S()), nan_ok=("out",) if timesteps == "out_of_range" else ())
+    assert r["bad_flag"].item() == int(timesteps != "in_range"), c.name
+    got = r["out"].view(B, H, W, Cp)
+    want = _torch_q_sample_pad(x0[good].to(DEV), noise[good].to(DEV), t[good].to(DEV), a.to(DEV), s.to(DEV), Cp).cpu()
+    assert torch.equal(_bits(got[good]), _bits(want)), c.name
+    for b in torch.nonzero(~good).flatten().tolist():
+        assert torch.isnan(got[b, ..., :C].float()).all() and (_bits(got[b, ..., C:]) == 0).all(), f"{c.name}: image {b}"
 
 
 # ---- the gradient arena ----------------------------------------------------------------------------------------------------------------

@@ -11,8 +11,11 @@ NaN, so a report can tell "never written" from "read the poison".  After a call:
   - every value matches a float64 CPU reference of the same operation.
 Every case runs twice, the second time with a different sentinel, and both results must be bit-identical.
 
-The calls go straight to the C-ABI (the ``ops`` wrappers pick leading dims and workspaces themselves)."""
+The calls go straight to the C-ABI (the ``ops`` wrappers pick leading dims and workspaces themselves).  The entry points of the
+companion header include/b200_cflearn_ext.h have their cases beside their other tests (EXT_CASE_MODULES); the coverage check
+imports those modules, so one ``@covers`` table spans both headers."""
 import ctypes
+import importlib
 import math
 
 import pytest
@@ -192,11 +195,16 @@ def call(name, *args):
 # ------------------------------------------------------------------------------------------------------------------------
 # value checks (the float64 references of _refs.py, on the CPU)
 # ------------------------------------------------------------------------------------------------------------------------
-def assert_close(got, ref, what, rtol, atol_rel=0.0):
+def within(got, ref, rtol, atol_rel=0.0):
+    """Elementwise |got - ref| <= rtol |ref| + atol_rel max |ref| (+ 1e-30), the bound of assert_close."""
     g, r = got.double(), ref.double()
     tol = rtol * r.abs() + atol_rel * r.abs().max().clamp_min(1e-30) + 1e-30
-    pos = first_bad(~((g - r).abs() <= tol))
-    assert pos is None, f"{what}: element {pos} = {g[pos].item()} vs reference {r[pos].item()}"
+    return (g - r).abs() <= tol
+
+
+def assert_close(got, ref, what, rtol, atol_rel=0.0):
+    pos = first_bad(~within(got, ref, rtol, atol_rel))
+    assert pos is None, f"{what}: element {pos} = {got.double()[pos].item()} vs reference {ref.double()[pos].item()}"
 
 
 def grad_err(got, ref, whole):
@@ -1087,40 +1095,118 @@ def test_symmetric_xent_footprint(Bn):
 # ------------------------------------------------------------------------------------------------------------------------
 # optimizer and element-wise helpers
 # ------------------------------------------------------------------------------------------------------------------------
-@covers("b200_adam_step", "b200_adam_step_dev")
-@pytest.mark.gpu
-@pytest.mark.parametrize("variant", ["host_step", "step_dev", "hyper_dev"])
-@pytest.mark.parametrize("n", [4, 1028])
-def test_adam_footprint(n, variant):
-    lr, b1, b2, eps, wd, gs = 1e-2, 0.8, 0.99, 1e-6, 0.05, 0.5
+ADAM_HYPER = (1e-2, 0.8, 0.99, 1e-6, 0.05, 0.5)  # lr, beta1, beta2, eps, weight_decay, grad_scale (hyper_dev only)
+ADAM_VARIANTS = ["host_step", "step_dev", "hyper_dev"]
+ADAM_SIZES = [(4, "randn"), (1028, "randn"), (1028, "sweep")]
+ADAM_TOL = {"params": 1e-6, "exp_avg": 1e-5, "exp_avg_sq": 1e-5}  # rtol; atol 1e-6 max |ref| for all three
+
+
+def _adam_inputs(n, grads):
+    """(params, grads, exp_avg, exp_avg_sq, scale) of an Adam case.  "sweep": element i's gradient and first moment times
+    scale_i = 2^e_i, e_i from -40 to 40, its second moment times scale_i^2, every 7th gradient exactly 0 and every 14th element's
+    moments too.  Below about 2^-20, eps dominates the denominator."""
     p0, g = rand((n,), 201, dtype=torch.float32), rand((n,), 202, dtype=torch.float32)
     m0 = rand((n,), 203, 0.1, dtype=torch.float32)
     v0 = rand((n,), 204, 0.1, dtype=torch.float32).abs()
-    c = Case(f"adam {variant} n {n}")
+    scale = torch.ones(n, dtype=torch.float64)
+    if grads == "sweep":
+        scale = torch.exp2(torch.linspace(-40, 40, n, dtype=torch.float64).round())
+        g, m0, v0 = (g * scale).float(), (m0 * scale).float(), (v0 * scale * scale).float()  # exact: powers of 2
+        g[::7] = 0.0
+        m0[::14] = 0.0
+        v0[::14] = 0.0
+    return p0, g, m0, v0, scale
+
+
+def _adam_steps(variant):
+    """The step numbers the case's five calls run with (hyper_dev's last call does not increment: step 6 twice)."""
+    return [3, 4, 5, 6, 7] if variant != "hyper_dev" else [3, 4, 5, 6, 6]
+
+
+def _adam_case(n, grads, variant, decoupled):
+    lr, b1, b2, eps, wd, gs = ADAM_HYPER
+    p0, g, m0, v0, scale = _adam_inputs(n, grads)
+    entry = "b200_adamw_step" if decoupled else "b200_adam_step"
+    c = Case(f"{entry[5:]} {variant} n {n} {grads}")
     gg = c.input("grads", g)
     p, m, v = c.inout("params", p0), c.inout("exp_avg", m0), c.inout("exp_avg_sq", v0)
     step = c.inout("step_dev", torch.tensor([2], dtype=torch.int32))
     hyper = c.input("hyper", torch.tensor([lr, b1, b2, eps, wd, gs], dtype=torch.float32))
 
     def launch():
-        L = _cabi.lib()
         for k in range(5):
             if variant == "host_step":
-                _cabi.check(L.b200_adam_step(p.ptr(), gg.ptr(), m.ptr(), v.ptr(), n, lr, b1, b2, eps, wd, 3 + k, None, S()), "adam_step")
+                call(entry, p.ptr(), gg.ptr(), m.ptr(), v.ptr(), n, lr, b1, b2, eps, wd, 3 + k, None, S())
             elif variant == "step_dev":
-                _cabi.check(L.b200_adam_step(p.ptr(), gg.ptr(), m.ptr(), v.ptr(), n, lr, b1, b2, eps, wd, 0, step.ptr(), S()), "adam_step")
-            else:  # the last call does not increment: step 7 twice
-                _cabi.check(L.b200_adam_step_dev(p.ptr(), gg.ptr(), m.ptr(), v.ptr(), n, hyper.ptr(), step.ptr(), int(k < 4), S()),
-                            "adam_step_dev")
+                call(entry, p.ptr(), gg.ptr(), m.ptr(), v.ptr(), n, lr, b1, b2, eps, wd, 0, step.ptr(), S())
+            else:
+                call(entry + "_dev", p.ptr(), gg.ptr(), m.ptr(), v.ptr(), n, hyper.ptr(), step.ptr(), int(k < 4), S())
 
     r = c.run(launch)
-    steps = [3, 4, 5, 6, 7] if variant != "hyper_dev" else [3, 4, 5, 6, 6]
     want_step = {"host_step": 2, "step_dev": 7, "hyper_dev": 6}[variant]
     assert r["step_dev"].item() == want_step
-    rp, rm, rv = adam(p0, g, m0, v0, steps, lr, b1, b2, eps, wd, gs if variant == "hyper_dev" else 1.0)
-    assert_close(r["params"].view(-1), rp, c.name + " params", rtol=1e-6, atol_rel=1e-6)
-    assert_close(r["exp_avg"].view(-1), rm, c.name + " exp_avg", rtol=1e-5, atol_rel=1e-6)
-    assert_close(r["exp_avg_sq"].view(-1), rv, c.name + " exp_avg_sq", rtol=1e-5, atol_rel=1e-6)
+    rp, rm, rv = adam(p0, g, m0, v0, _adam_steps(variant), lr, b1, b2, eps, wd, gs if variant == "hyper_dev" else 1.0,
+                      decoupled=decoupled)
+    assert_close(r["params"].view(-1), rp, c.name + " params", ADAM_TOL["params"], 1e-6)
+    # the moments in units of their element's scale (exact), so that the sweep's small elements are held as tightly as its large ones
+    assert_close(r["exp_avg"].view(-1) / scale, rm / scale, c.name + " exp_avg", ADAM_TOL["exp_avg"], 1e-6)
+    assert_close(r["exp_avg_sq"].view(-1) / scale ** 2, rv / scale ** 2, c.name + " exp_avg_sq", ADAM_TOL["exp_avg_sq"], 1e-6)
+
+
+@covers("b200_adam_step", "b200_adam_step_dev")
+@pytest.mark.gpu
+@pytest.mark.parametrize("variant", ADAM_VARIANTS)
+@pytest.mark.parametrize("n,grads", ADAM_SIZES, ids=["4", "1028", "1028-sweep"])
+def test_adam_footprint(n, grads, variant):
+    _adam_case(n, grads, variant, decoupled=False)
+
+
+@covers("b200_adamw_step", "b200_adamw_step_dev")
+@pytest.mark.gpu
+@pytest.mark.parametrize("variant", ADAM_VARIANTS)
+@pytest.mark.parametrize("n,grads", ADAM_SIZES, ids=["4", "1028", "1028-sweep"])
+def test_adamw_footprint(n, grads, variant):
+    _adam_case(n, grads, variant, decoupled=True)
+
+
+ADAMW_MISTAKES = ["L2 decay", "decay after the update", "no decay", "decay scaled by grad_scale", "decay using lr / bc1"]
+
+
+def _adamw_mistake(p, g, m, v, steps, lr, b1, b2, eps, wd, gs, mistake):
+    """AdamW in float64 with one plausible implementation mistake: the params the kernel would return."""
+    if mistake == "L2 decay":
+        return adam(p, g, m, v, steps, lr, b1, b2, eps, wd, gs)[0]
+    p, m, v = p.double(), m.double(), v.double()
+    for t in steps:
+        bc1 = 1 - b1 ** t
+        keep = {"decay after the update": 1.0, "no decay": 1.0, "decay scaled by grad_scale": 1 - lr * wd * gs,
+                "decay using lr / bc1": 1 - lr / bc1 * wd}[mistake]
+        p = p * keep
+        gg = g.double() * gs
+        m = b1 * m + (1 - b1) * gg
+        v = b2 * v + (1 - b2) * gg * gg
+        p = p - lr / bc1 * m / (v.sqrt() / math.sqrt(1 - b2 ** t) + eps)
+        if mistake == "decay after the update":
+            p = p * (1 - lr * wd)
+    return p
+
+
+@pytest.mark.parametrize("variant", ADAM_VARIANTS)
+@pytest.mark.parametrize("n,grads", ADAM_SIZES[1:], ids=["1028", "1028-sweep"])
+def test_adamw_footprint_tolerance_rejects_plausible_mistakes(n, grads, variant):
+    """CPU: on test_adamw_footprint's own inputs, steps and tolerance, each mistake moves many params out of the bound (the decay
+    scaled by grad_scale differs only where grad_scale is not 1: hyper_dev), so loosening the tolerance fails here first."""
+    lr, b1, b2, eps, wd, gs = ADAM_HYPER
+    gs = gs if variant == "hyper_dev" else 1.0
+    p0, g, m0, v0, _ = _adam_inputs(n, grads)
+    steps = _adam_steps(variant)
+    ref = adam(p0, g, m0, v0, steps, lr, b1, b2, eps, wd, gs, decoupled=True)[0]
+    for mistake in ADAMW_MISTAKES:
+        if mistake == "decay scaled by grad_scale" and gs == 1.0:
+            continue
+        got = _adamw_mistake(p0, g, m0, v0, steps, lr, b1, b2, eps, wd, gs, mistake)
+        caught = int((~within(got, ref, ADAM_TOL["params"], 1e-6)).sum())
+        assert caught >= n // 4, f"{mistake} ({variant}, {grads}): only {caught} of {n} params outside the tolerance"
 
 
 @covers("b200_cast_f32_to_bf16", "b200_fill_f32")
@@ -1186,11 +1272,18 @@ def test_groupnorm_footprint(B, HW, C, silu, accumulate):
 # ------------------------------------------------------------------------------------------------------------------------
 # CPU checks: the table covers every entry point, and the guard bookkeeping reports what it should
 # ------------------------------------------------------------------------------------------------------------------------
+# the modules that hold the footprint cases of the companion header's entry points (include/b200_cflearn_ext.h); importing one
+# registers its @covers
+EXT_CASE_MODULES = ("test_resample_gpu", "test_unet_gpu", "test_autoencoder_gpu", "test_ddpm_gpu", "test_ddim_gpu")
+
+
 def test_every_compute_entry_point_has_a_footprint_case():
-    entries = set(_cabi.SIGNATURES) - NOT_FOOTPRINT
-    missing = sorted(entries - COVERED)
+    for name in EXT_CASE_MODULES:
+        importlib.import_module(name)
+    abi = set(_cabi.SIGNATURES) | set(_cabi.EXT_SIGNATURES)
+    missing = sorted(abi - NOT_FOOTPRINT - COVERED)
     assert not missing, f"C-ABI entry points without a footprint case: {missing}"
-    stale = sorted(COVERED - set(_cabi.SIGNATURES)) + sorted(NOT_FOOTPRINT - set(_cabi.SIGNATURES))
+    stale = sorted(COVERED - abi) + sorted(NOT_FOOTPRINT - abi)
     assert not stale, f"names that are not C-ABI entry points: {stale}"
 
 

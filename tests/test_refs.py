@@ -107,6 +107,21 @@ def test_float64_references_match_torch():
     p, m, v = refs.adam(p0, grad, zeros, zeros, [1, 2, 3, 4], 1e-2, 0.8, 0.99, 1e-6, 0.05)
     assert torch.allclose(p, pt.detach(), rtol=1e-12, atol=1e-14)
     assert torch.allclose(m, opt.state[pt]["exp_avg"], rtol=1e-12) and torch.allclose(v, opt.state[pt]["exp_avg_sq"], rtol=1e-12)
+    # AdamW (decoupled decay) against torch.optim.AdamW, from nonzero moments at step 3 as the footprint case starts; a scaled
+    # gradient is the same update on the scaled gradient, the decay untouched
+    m0 = 0.1 * torch.randn(50, generator=g2, dtype=F64)
+    v0 = (0.1 * torch.randn(50, generator=g2, dtype=F64)) ** 2
+    for gs in (1.0, 0.5):
+        pt = p0.clone().requires_grad_(True)
+        opt = torch.optim.AdamW([pt], lr=1e-2, betas=(0.8, 0.99), eps=1e-6, weight_decay=0.05)
+        opt.state[pt] = {"step": torch.tensor(2.0), "exp_avg": m0.clone(), "exp_avg_sq": v0.clone()}
+        for _ in range(4):
+            pt.grad = grad * gs
+            opt.step()
+        p, m, v = refs.adam(p0, grad, m0, v0, [3, 4, 5, 6], 1e-2, 0.8, 0.99, 1e-6, 0.05, gs, decoupled=True)
+        assert torch.allclose(p, pt.detach(), rtol=1e-12, atol=1e-14)
+        assert torch.allclose(m, opt.state[pt]["exp_avg"], rtol=1e-12) and torch.allclose(v, opt.state[pt]["exp_avg_sq"], rtol=1e-12)
+        assert not torch.allclose(p, refs.adam(p0, grad, m0, v0, [3, 4, 5, 6], 1e-2, 0.8, 0.99, 1e-6, 0.05, gs)[0], rtol=1e-6)
 
 
 def test_attention_bounds():

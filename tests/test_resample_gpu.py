@@ -22,7 +22,7 @@ from cflearn_b200 import ops  # noqa: E402
 from cflearn_b200.unet_blocks import ResDownsampleB200, ResUpsampleB200, ResidualBlockWithTimeEmbeddingB200  # noqa: E402
 from _refs import (bf16, conv3x3_s2, conv3x3_s2_dgrad, conv3x3_s2_wgrad, conv3x3_up2, exact_ints, exact_scaled, exponents,  # noqa: E402
                    first_bad, relerr)
-from test_kernel_footprint_gpu import Case, S, assert_equal, call, rand  # noqa: E402
+from test_kernel_footprint_gpu import Case, S, assert_equal, call, covers, rand  # noqa: E402
 
 DEV = "cuda"
 F64 = torch.float64
@@ -159,6 +159,7 @@ def test_random_kernels(B, H, W, Cin, Cout):
 
 
 # ---- 3. footprint ---------------------------------------------------------------------------------------------------------------
+@covers("b200_conv3x3_s2_nhwc_bf16", "b200_conv3x3_up2_nhwc_bf16")
 @pytest.mark.gpu
 @pytest.mark.parametrize("entry", ["b200_conv3x3_s2_nhwc_bf16", "b200_conv3x3_up2_nhwc_bf16"])
 @pytest.mark.parametrize("epi", [0, 2, 10, 11])
@@ -190,6 +191,7 @@ def test_resample_conv_footprint(entry, epi):
     assert first_bad(~ok) is None, f"{c.name}: element {first_bad(~ok)}"
 
 
+@covers("b200_conv3x3_s2_dgrad_nhwc_bf16")
 @pytest.mark.gpu
 def test_down_dgrad_footprint():
     B, H, W, Cin, Cout = 3, 16, 16, 200, 64
@@ -203,6 +205,7 @@ def test_down_dgrad_footprint():
                    c.name)
 
 
+@covers("b200_conv3x3_s2_wgrad_nhwc_bf16")
 @pytest.mark.gpu
 def test_down_wgrad_footprint():
     B, H, W, Cin, Cout = 3, 16, 16, 64, 200
@@ -226,6 +229,7 @@ def test_down_wgrad_footprint():
         assert first_bad(bad) is None, f"{c.name}: split {sp} element {first_bad(bad)}"
 
 
+@covers("b200_upsample_nearest2x_bf16", "b200_sum2x2_bf16")
 @pytest.mark.gpu
 @pytest.mark.parametrize("entry", ["b200_upsample_nearest2x_bf16", "b200_sum2x2_bf16"])
 def test_copy_footprint(entry):

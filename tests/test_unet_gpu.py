@@ -24,7 +24,7 @@ import cflearn_b200  # noqa: F401,E402
 from cflearn_b200 import ops  # noqa: E402
 from cflearn_b200.unet import UNetDiffuserB200, head_conv, head_conv_bwd, noise_prediction_loss, stem_conv, stem_conv_bwd  # noqa: E402
 from _refs import bf16, conv3x3, conv3x3_dgrad, conv3x3_wgrad, exact_ints, exact_scaled, relerr  # noqa: E402
-from test_kernel_footprint_gpu import Case, S, assert_equal, call  # noqa: E402
+from test_kernel_footprint_gpu import Case, S, assert_equal, call, covers  # noqa: E402
 
 DEV = "cuda"
 F64 = torch.float64
@@ -66,6 +66,7 @@ def test_pad_channels_is_torchs_cast(dtype, fmt, C, B):
     assert (_bits(out[..., C:]) == 0).all()  # +0, not -0
 
 
+@covers("b200_pad_channels_bf16")
 @pytest.mark.gpu
 @pytest.mark.parametrize("x_f32,cl", [(1, 0), (1, 1), (0, 0), (0, 1)])
 def test_pad_channels_footprint(x_f32, cl):
@@ -183,6 +184,7 @@ def test_loss_is_deterministic():
     assert torch.equal(_bits(a[0]), _bits(b[0])) and torch.equal(_bits(a[1]), _bits(b[1]))
 
 
+@covers("b200_noise_prediction_loss_bf16")
 @pytest.mark.gpu
 @pytest.mark.parametrize("noise_f32", [1, 0])
 def test_loss_footprint(noise_f32):
