@@ -20,7 +20,8 @@ from torch import Tensor
 
 from . import ops
 from ._cabi import B200Error
-from .vit import ParamArena, TeTEncoderB200, ViTEncoderB200
+from .arena import ArenaModule, ParamArena
+from .vit import TeTEncoderB200, ViTEncoderB200
 
 
 def l2_normalize(t: Tensor) -> Tensor:
@@ -138,7 +139,7 @@ def symmetric_cross_entropy(logits_per_image: Tensor) -> Tensor:
     return _SymmetricXentFn.apply(logits_per_image)
 
 
-class CLIPB200(nn.Module):
+class CLIPB200(ArenaModule):
     def __init__(self, img_size: int = 224, latent_dim: int = 512, *, use_vision: bool = True, in_channels: int = 3,
                  vision_latent_dim: int = 768, vision_patch_size: int = 32, vision_num_heads: int = 12, vision_num_layers: int = 12,
                  vision_norm_eps: float = 1.0e-5, vision_feedforward_activation: str = "quick_gelu", use_text: bool = True,
@@ -178,14 +179,13 @@ class CLIPB200(nn.Module):
                 "text_projection.weight": self.text_projection.weight, "text_projection.bias": self.text_projection.bias}
         self.glue = ParamArena([(k, tuple(p.shape)) for k, p in glue.items()])
         self.glue.attach(glue)
-        self.comm: Any = None  # dp.NativeComm when data parallel (dp.attach_native_reducers)
 
-    # ---- what the optimizer / the data-parallel layer iterate over --------------------------------------------------
-    def towers(self) -> List[nn.Module]:
-        return [self.vit, self.text_transformer]
-
+    # ---- the trainer seam's contract (arena.ArenaModule): the glue arena is exchanged through ``comm`` by train_step ----
     def arenas(self) -> List[ParamArena]:
         return [self.vit.arena, self.text_transformer.arena, self.glue]
+
+    def exchanges(self) -> List[Any]:
+        return [self.vit.engine, self.text_transformer.engine]
 
     def _collect_glue_grads(self) -> None:
         """autograd hands the loose parameters' gradients over as separate tensors: move them into the glue arena.  Once they

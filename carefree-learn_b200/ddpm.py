@@ -21,7 +21,7 @@ than "identity" (pass the encoded context as ``cond``) and samplers other than "
 """
 from __future__ import annotations
 
-from typing import Any, Dict, Optional, Tuple
+from typing import Any, Dict, List, Optional, Tuple
 
 import numpy as np
 import torch
@@ -30,6 +30,7 @@ from torch import Tensor, nn
 from . import ops
 from .ddim import DDIMSamplerB200
 from ._cabi import B200Error
+from .arena import ArenaModule
 from .unet import PAD_CHANNELS, UNetDiffuserB200, enable_grad_arena, noise_prediction_loss
 
 PREDICTIONS_KEY = "predictions"  # cflearn/constants.py
@@ -80,7 +81,7 @@ def noise_tables(timesteps: int = 1000, given_betas: Optional[np.ndarray] = None
     return a, s
 
 
-class DDPMB200(nn.Module):
+class DDPMB200(ArenaModule):
     """Drop-in for the training forward of cflearn's ``DDPM`` with an SD-style ``UNetDiffuser`` on the native kernels (CUDA only).
 
     ``forward(net, cond)``: DDPM.forward's dict {predictions, noise, timesteps} for the fp32 latent ``net`` [B, C, H, W] and the
@@ -122,13 +123,13 @@ class DDPMB200(nn.Module):
         self.condition_model: Optional[nn.Module] = nn.Identity() if condition_model == IDENTITY_CONDITION_MODEL else None
         self.register_buffer("sqrt_alphas_cumprod", a, persistent=False)
         self.register_buffer("sqrt_one_minus_alphas_cumprod", s, persistent=False)
-        grads = enable_grad_arena(self.unet)
-        self.arena = grads.arena
-        self.geo = self.engine = grads  # what dp reads: buckets(), reducer, shrink_next
-        self.grad_arena = grads
-        self.last_bad_flag: Optional[Tensor] = None
+        self.grad_arena = enable_grad_arena(self.unet)
+        self.arena = self.grad_arena.arena
         self.sampler: DDIMSamplerB200
         self.switch_sampler(sampler, sampler_config)
+
+    def exchanges(self) -> List[Any]:
+        return [self.grad_arena]
 
     def _noised(self, net: Tensor, noise: Optional[Tensor], timesteps: Optional[Tensor]) -> Tuple[Tensor, Tensor, Tensor]:
         what = "DDPMB200"
@@ -153,7 +154,7 @@ class DDPMB200(nn.Module):
         x, noise, timesteps = self._noised(net, noise, timesteps)
         loss = noise_prediction_loss(self.unet.forward_padded(x, timesteps, cond), noise)
         loss.backward()  # the gradients land in the arena; buckets start their all-reduce as they complete
-        red = self.engine.reducer
+        red = self.grad_arena.reducer
         if red is not None:
             red.finish()
         self.grad_arena.end_backward()

@@ -39,8 +39,8 @@ def shard_indices(n: int, rank: int, world: int) -> range:
 
 
 class GradBucketReducer:
-    """Bucketed gradient averaging over ``torch.distributed``.  ``buckets`` (``ViTGeometry.buckets()``): for each point
-    of the engine's backward that calls ``ready``, the parameter keys of each arena span complete there."""
+    """Bucketed gradient averaging over ``torch.distributed``.  ``buckets`` (an exchange site's ``buckets()``): for each point
+    of backward that calls ``ready``, the parameter keys of each arena span complete there."""
 
     def __init__(self, arena, buckets: Dict[BucketKey, List[List[str]]], process_group=None):
         self.arena = arena
@@ -193,71 +193,57 @@ class NativeBucketReducer(GradBucketReducer):
         return self.comm_stream
 
 
-def attach_native_reducer(module, comm: NativeComm) -> NativeBucketReducer:
-    """Overlapped, capturable gradient averaging for a ViTEncoderB200 / VanillaClassifierB200."""
-    module.arena.ensure()
-    red = NativeBucketReducer(module.arena, module.geo.buckets(), comm, module.engine)
-    module.engine.reducer = red
-    return red
-
-
-def _towers(module) -> List[Any]:
-    """The sub-modules that own a fused engine: the module itself (ViT encoder / classifier / text encoder) or CLIP's towers."""
-    if hasattr(module, "towers"):
-        return list(module.towers())
-    return [module]
-
-
 def attach_native_reducers(module, comm: NativeComm) -> List[NativeBucketReducer]:
-    """Bucket reducers on every tower of ``module``; a module with loose parameters outside the towers (CLIP: logit_scale,
-    token embedding, text projection) all-reduces them itself through ``module.comm`` at the end of its ``train_step``."""
+    """Overlapped, capturable gradient averaging: a bucket reducer on every exchange site of ``module``
+    (``arena.ArenaModule.exchanges``), and ``module.comm`` for the gradients no site covers (CLIP's loose parameters, which
+    its ``train_step`` all-reduces itself)."""
     reds = []
-    for t in _towers(module):
-        red = t.engine.reducer
+    for site in module.exchanges():
+        red = site.reducer
         if not isinstance(red, NativeBucketReducer) or red.comm is not comm:
-            red = attach_native_reducer(t, comm)
+            site.arena.ensure()
+            red = site.reducer = NativeBucketReducer(site.arena, site.buckets(), comm, site)
         reds.append(red)
-    if hasattr(module, "towers"):
-        module.comm = comm
+    module.comm = comm
     return reds
 
 
 def detach_reducers(module) -> None:
-    for t in _towers(module):
-        t.engine.reducer = None
+    """No gradient exchange: every site's reducer and ``module.comm`` cleared."""
+    for site in module.exchanges():
+        site.reducer = None
+    module.comm = None
 
 
 @contextlib.contextmanager
 def no_sync(module):
-    """Backward without the gradient exchange, like DDP's ``no_sync``: inside, the towers' bucket reducers and a module's
-    all-reduce of its loose parameters (``module.comm``) are switched off.  Gradient accumulation runs every micro-batch
-    of a window but the last inside it, so the window's sum is exchanged once, by its last backward."""
-    towers = _towers(module)
-    reducers = [t.engine.reducer for t in towers]
-    comm = getattr(module, "comm", None)
+    """Backward without the gradient exchange, like DDP's ``no_sync``: inside, the bucket reducers and a module's all-reduce
+    of its loose parameters (``module.comm``) are switched off.  Gradient accumulation runs every micro-batch of a window
+    but the last inside it, so the window's sum is exchanged once, by its last backward."""
+    sites = module.exchanges()
+    reducers = [site.reducer for site in sites]
+    comm = module.comm
     try:
         detach_reducers(module)
-        if hasattr(module, "towers"):
-            module.comm = None
         yield
     finally:
-        for t, red in zip(towers, reducers):
-            t.engine.reducer = red
-        if hasattr(module, "towers"):
-            module.comm = comm
+        for site, red in zip(sites, reducers):
+            site.reducer = red
+        module.comm = comm
 
 
-def attach_reducer(module, process_group=None) -> GradBucketReducer:
-    """Enable overlapped gradient averaging for a ViTEncoderB200 / VanillaClassifierB200."""
-    module.arena.ensure()
-    red = GradBucketReducer(module.arena, module.geo.buckets(), process_group)
-    module.engine.reducer = red
-    return red
+def attach_reducer(module, process_group=None) -> List[GradBucketReducer]:
+    """Overlapped gradient averaging over ``torch.distributed``: a bucket reducer on every exchange site of ``module``."""
+    reds = []
+    for site in module.exchanges():
+        site.arena.ensure()
+        site.reducer = GradBucketReducer(site.arena, site.buckets(), process_group)
+        reds.append(site.reducer)
+    return reds
 
 
 def broadcast_parameters(module, src: int = 0, process_group=None) -> None:
     """Identical replicas at start (what DDP's constructor does): one broadcast per flat fp32 arena."""
-    arenas = list(module.arenas()) if hasattr(module, "arenas") else [module.arena]
-    for a in arenas:
+    for a in module.arenas():
         a.ensure()
         dist.broadcast(a.flat, src=src, group=process_group)

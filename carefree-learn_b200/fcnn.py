@@ -18,7 +18,7 @@ import torch.nn as nn
 from torch import Tensor
 
 from . import ops
-from .vit import ParamArena, _register_dotted
+from .arena import ArenaModule, ParamArena, register_dotted
 
 
 def _spec(input_dim: int, output_dim: int, hidden_units: List[int], bias: bool) -> List[Tuple[str, Tuple[int, ...]]]:
@@ -55,7 +55,7 @@ class _FCNNFn(torch.autograd.Function):
         return (None, None) + grads
 
 
-class FCNNB200(nn.Module):
+class FCNNB200(ArenaModule):
     def __init__(self, input_dim: int, output_dim: int, hidden_units: Optional[List[int]] = None, *,
                  mapping_type: str = "basic", bias: bool = True, activation: str = "ReLU", batch_norm: bool = False,
                  dropout: float = 0.0, rank: Optional[int] = None, rank_ratio: Optional[float] = None):
@@ -86,11 +86,14 @@ class FCNNB200(nn.Module):
                 bound = 1.0 / math.sqrt(self.dims[-2])
                 nn.init.uniform_(t, -bound, bound)
             p = nn.Parameter(t)
-            _register_dotted(self, key, p)
+            register_dotted(self, key, p)
             params[key] = p
         self.arena.attach(params)
         self._woff = [self.arena.offsets[k] for k, _ in spec if k.endswith("weight")]
         self._boff = [self.arena.offsets[k] for k, _ in spec if k.endswith("bias")] if bias else [-1] * (n + 1)
+
+    def exchanges(self) -> List[Any]:
+        raise NotImplementedError("FCNNB200 has no bucketed gradient exchange: its whole backward is one fused launch")
 
     # ---- kernel launch ------------------------------------------------------------------------------------------
     def _launch(self, x: Tensor, *, y: Optional[Tensor] = None, dpred: Optional[Tensor] = None, grads: Optional[Tensor] = None,

@@ -52,8 +52,7 @@ class ArenaAdam(torch.optim.Optimizer):
         self.exp_avg_sqs: List[Tensor] = []
 
     def arenas(self) -> List[Any]:
-        m = self.module
-        return list(m.arenas()) if hasattr(m, "arenas") else [m.arena]
+        return self.module.arenas()
 
     @property
     def exp_avg(self) -> Optional[Tensor]:
@@ -182,6 +181,13 @@ class ArenaAdam(torch.optim.Optimizer):
         self.hyper_dev[5:6].copy_(self._clip_dev.reshape(1))
         return norm
 
+    def reset_grad_scale(self) -> None:
+        """For steps that do not clip after steps that did: ``clip_grad_norm_`` left its last coefficient in the device's
+        ``grad_scale`` slot, so hand the slot back to the host's value (1), which the next ``sync_hyper`` writes."""
+        if self._clip_dev is not None:
+            self._clip_dev = None
+            self._hyper_sent = None
+
     def state_dict(self) -> Dict[str, Any]:
         step = int(self.step_dev.item()) if self.step_dev is not None else self.step_count
         g = self.param_groups[0]
@@ -222,8 +228,8 @@ class ArenaAdamW(ArenaAdam):
 
 
 class GraphedTrainStep:
-    """Whole training step of a B200 module (``VanillaClassifierB200`` or ``CLIPB200``) as one CUDA graph with static
-    input / loss buffers.
+    """Whole training step of a B200 module (an ``arena.ArenaModule``: ``VanillaClassifierB200``, ``CLIPB200``, ``DDPMB200``)
+    as one CUDA graph with static input / loss buffers.
 
     ``step(*inputs)`` copies the batch into the static buffers (device->device or pinned-host->device, on the current
     stream), replays the graph and returns the static loss tensor (fp32 scalar, on the device).  The warm-up runs needed
@@ -232,7 +238,8 @@ class GraphedTrainStep:
     Data parallel (``comm``: a ``dp.NativeComm``): the graph also holds the gradient exchange -- the model's bucket
     reducers launch ``ncclAllReduce`` per transformer block on a forked stream as soon as that block's gradients are
     complete -- and the Adam update behind the join.  ``inputs``: the static input tensors (default: an image batch
-    [batch, C, S, S] fp32 and int64 labels [batch, 1] for the classifier).
+    [batch, C, S, S] fp32 and int64 labels [batch, 1] for the classifier).  ``clip_norm > 0``: the exchanged gradients are
+    clipped to that global L2 norm before Adam (``ArenaAdam.clip_grad_norm_``, in the graph).
 
     ``grad_accumulate=K``: one optimizer update per K calls of ``step`` (the reference's ``TrainerConfig.grad_accumulate``).
     Every call runs forward, loss and a backward that adds to the gradient arenas, which are zeroed (one ``fill`` launch per
@@ -240,7 +247,7 @@ class GraphedTrainStep:
     ``updated`` says whether the last call did.  K = 1 is the single graph described above."""
 
     def __init__(self, model: Any, optimizer: ArenaAdam, batch: int, warmup: int = 2, comm: Any = None, flat: bool = False,
-                 inputs: Optional[List[Tensor]] = None, grad_accumulate: int = 1):
+                 inputs: Optional[List[Tensor]] = None, grad_accumulate: int = 1, clip_norm: float = 0.0):
         if grad_accumulate < 1:
             raise ValueError(f"grad_accumulate must be >= 1, got {grad_accumulate}")
         if not optimizer.capturable:
@@ -250,6 +257,7 @@ class GraphedTrainStep:
         self.world = 1 if comm is None else comm.world
         self.comm = comm
         self.accumulate = int(grad_accumulate)
+        self.clip_norm = float(clip_norm)
         self.micro = 0  # calls of the current window so far
         self.updated = False
         # flat=True (A/B switch): the graph stops after backward; ONE all-reduce per gradient arena and Adam are
@@ -260,10 +268,10 @@ class GraphedTrainStep:
         for a in arenas:
             a.ensure()
         dev = arenas[0].flat.device
+        if self.clip_norm <= 0.0:
+            optimizer.reset_grad_scale()
         if self.flat or self.world == 1:
             dp.detach_reducers(model)
-            if hasattr(model, "comm"):
-                model.comm = None
         else:
             dp.attach_native_reducers(model, comm)
         if inputs is None:
@@ -322,15 +330,13 @@ class GraphedTrainStep:
             self.optimizer.zero_grad()
         with contextlib.nullcontext() if update else dp.no_sync(self.model):
             loss = self.model.train_step(*self.inputs)  # DP: the reducers all-reduce bucket by bucket inside backward
-        hook = getattr(self.model, "clip_norm_hook", None)
-        if update and hook is not None and not self.flat:
-            hook()  # device-side clip coefficient (trainer.B200TrainStep): captured with the step
         if update and not self.flat:
+            if self.clip_norm > 0.0:
+                self.optimizer.clip_grad_norm_(self.clip_norm)  # device-side clip coefficient: captured with the step
             self.optimizer.step()
         self.loss.copy_(loss)
-        flag = getattr(self.model, "last_bad_flag", None)
-        if flag is not None:
-            self.bad_label.copy_(flag)
+        if self.model.last_bad_flag is not None:
+            self.bad_label.copy_(self.model.last_bad_flag)
 
     def step(self, *inputs: Tensor) -> Tensor:
         self.optimizer.sync_hyper()  # lr schedule: 24 bytes host->device when (and only when) a value changed
@@ -348,9 +354,8 @@ class GraphedTrainStep:
         if self.flat:
             for a in self.optimizer.arenas():
                 self.comm.allreduce_(a.grad, average=True)
-            hook = getattr(self.model, "clip_norm_hook", None)
-            if hook is not None:
-                hook()  # (clipping sees the AVERAGED gradients, as under DDP)
+            if self.clip_norm > 0.0:
+                self.optimizer.clip_grad_norm_(self.clip_norm)  # (clipping sees the AVERAGED gradients, as under DDP)
             self.optimizer.step()
         return self.loss
 

@@ -53,16 +53,16 @@ class B200TrainStep:
         if self.clip_norm > 0.0 and not optimizer.capturable:
             raise ValueError("clip_norm > 0 needs ArenaAdam(capturable=True)")
         if graph:
-            if self.clip_norm > 0.0:
-                # the clip coefficient is computed between backward and Adam: both live inside the captured step
-                model.clip_norm_hook = lambda: optimizer.clip_grad_norm_(self.clip_norm)
             if batch is None and static_inputs is None:
                 raise ValueError("graph=True needs the batch size (or the static input tensors)")
             self._graph = GraphedTrainStep(model, optimizer, batch or static_inputs[0].shape[0], comm=comm, inputs=static_inputs,
                                            flat=flat,  # flat: ONE all-reduce behind the graph instead of in-graph buckets
-                                           grad_accumulate=self.accumulate)
-        elif comm is not None and comm.world > 1:
-            dp.attach_native_reducers(model, comm)
+                                           grad_accumulate=self.accumulate, clip_norm=self.clip_norm)
+        else:
+            if self.clip_norm <= 0.0:
+                optimizer.reset_grad_scale()
+            if comm is not None and comm.world > 1:
+                dp.attach_native_reducers(model, comm)
 
     def close(self) -> None:
         """Destroy the captured graph (must happen before the communicator it captured is closed)."""

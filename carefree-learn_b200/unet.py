@@ -34,6 +34,7 @@ from torch import Tensor, nn
 
 from . import checkpoint, ops
 from ._cabi import B200Error
+from .arena import ParamArena
 from .attention import _bf, _check_cuda
 from .spatial_transformer import SpatialTransformerB200
 from .unet_blocks import (ResDownsampleB200, ResidualBlockWithTimeEmbeddingB200, ResUpsampleB200, _bias_rows, _nhwc,
@@ -422,14 +423,14 @@ def bucket_plan(unet: UNetDiffuserB200) -> List[Tuple[str, List[str]]]:
 
 
 class UNetGradArena:
-    """The UNet's parameters in one ``vit.ParamArena`` laid out by ``bucket_plan``, each parameter carrying a
+    """The UNet's parameters in one ``arena.ParamArena`` laid out by ``bucket_plan``, each parameter carrying a
     ``checkpoint.GradSlot``: every op's backward writes its parameter gradients straight into their views (overwriting, or adding
     while the parameters hold gradients, ``ParamArena.claim_grads``), and ``p.grad`` is the view.  When a bucket's last gradient
     is written it is handed to ``reducer.ready`` (``dp.NativeBucketReducer``), which all-reduces it on a side stream while
     backward goes on; the persistent kernels launched next then leave the communicator's SMs free (``shrink_next``).
 
-    It offers what ``dp`` reads of a transformer engine (``buckets()``, ``reducer``, ``shrink_next``), so the DDPM module hands
-    it out as both its ``geo`` and its ``engine``.
+    It is the DDPM module's one exchange site (``arena.ArenaModule.exchanges``): ``arena``, ``buckets()``, ``reducer`` and
+    ``shrink_next``.
 
     The arena is built on the parameters' device by its first ``arena.ensure()`` (the UNet's forward calls ``begin``, which
     does it, and rebuilds it after ``.to(device)``), so a module constructed on the host holds no second copy there.  Each forward
@@ -437,8 +438,6 @@ class UNetGradArena:
     since (``check``)."""
 
     def __init__(self, unet: UNetDiffuserB200) -> None:
-        from .vit import ParamArena
-
         params = dict(unet.named_parameters())
         self.plan = bucket_plan(unet)
         self.arena = ParamArena([(k, tuple(params[k].shape)) for _, keys in self.plan for k in keys], bf16_shadow=False)

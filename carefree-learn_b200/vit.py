@@ -16,7 +16,6 @@ backward is still running.
 """
 from __future__ import annotations
 
-import math
 from typing import Any, Dict, List, Optional, Tuple, Union
 
 import torch
@@ -25,133 +24,10 @@ from torch import Tensor
 
 from . import ops
 from ._cabi import B200Error
+from .arena import ArenaModule, ParamArena, register_dotted
 
 PREDICTIONS_KEY = "predictions"  # cflearn/constants.py:6
 LATENT_KEY = "latent"
-
-_ALIGN = 64  # elements; keeps every view 16-byte aligned in both the fp32 and the bf16 arena
-
-
-def _padded(shape: Tuple[int, ...]) -> int:
-    return (math.prod(shape) + _ALIGN - 1) // _ALIGN * _ALIGN
-
-
-# -----------------------------------------------------------------------------------------------------------------
-# parameter arena
-# -----------------------------------------------------------------------------------------------------------------
-class ParamArena:
-    """Flat fp32 parameters + bf16 shadow + flat fp32 gradients, addressed by reference ``state_dict`` key.  ``bf16_shadow=False``:
-    no shadow (a module whose ops cast their own weights)."""
-
-    def __init__(self, spec: List[Tuple[str, Tuple[int, ...]]], bf16_shadow: bool = True):
-        self.spec = list(spec)
-        self.bf16_shadow = bf16_shadow
-        self.offsets: Dict[str, int] = {}
-        off = 0
-        for key, shape in self.spec:
-            self.offsets[key] = off
-            off += _padded(shape)
-        self.total = off
-        self.shapes = dict(self.spec)
-        self.flat: Optional[Tensor] = None
-        self.flat_bf16: Optional[Tensor] = None
-        self.grad: Optional[Tensor] = None
-        self.params: Dict[str, nn.Parameter] = {}
-        self._bf16_version = -1
-
-    def view(self, flat: Tensor, key: str) -> Tensor:
-        off = self.offsets[key]
-        shape = self.shapes[key]
-        return flat[off : off + math.prod(shape)].view(shape)
-
-    def attach(self, params: Dict[str, nn.Parameter]) -> None:
-        self.params = params
-        self.rebuild()
-
-    def rebuild(self) -> None:
-        """(Re)create the arenas on the parameters' current device and re-point every parameter into them."""
-        first = next(iter(self.params.values()))
-        dev = first.device
-        flat = torch.zeros(self.total, dtype=torch.float32, device=dev)
-        with torch.no_grad():
-            for key, p in self.params.items():
-                v = self.view(flat, key)
-                v.copy_(p.data.to(torch.float32))
-                p.data = v
-        self.flat = flat
-        self.flat_bf16 = torch.zeros(self.total, dtype=torch.bfloat16, device=dev) if dev.type == "cuda" and self.bf16_shadow else None
-        self.grad = torch.zeros(self.total, dtype=torch.float32, device=dev)
-        self._bf16_version = -1
-
-    def ensure(self) -> None:
-        """Cheap aliasing check: ``module.to(device)`` / ``load_state_dict(assign=True)`` break the views.  An arena whose
-        parameters were given but not yet attached (``flat`` None) is built here, on their device."""
-        if self.flat is None:
-            self.rebuild()
-            return
-        base = self.flat.data_ptr()
-        ok = True
-        for key, p in self.params.items():
-            if p.data_ptr() != base + 4 * self.offsets[key] or p.device != self.flat.device:
-                ok = False
-                break
-        if not ok:
-            self.rebuild()
-
-    def refresh_bf16(self) -> None:
-        """fp32 -> bf16 shadow of ALL parameters in one launch (what autocast's per-op weight casts amount to)."""
-        assert self.flat is not None and self.flat_bf16 is not None
-        ops.cast_bf16(self.flat, self.flat_bf16)
-
-    def w(self, key: str) -> Tensor:  # bf16 view
-        return self.view(self.flat_bf16, key)
-
-    def p(self, key: str) -> Tensor:  # fp32 view
-        return self.view(self.flat, key)
-
-    def g(self, key: str, arena: Optional[Tensor] = None) -> Tensor:  # fp32 grad view
-        return self.view(self.grad if arena is None else arena, key)
-
-    def span(self, keys: List[str]) -> Tuple[int, int]:
-        """[lo, hi) of the arena holding ``keys``, which are consecutive in the layout (one all-reduce bucket)."""
-        return self.offsets[keys[0]], self.offsets[keys[-1]] + _padded(self.shapes[keys[-1]])
-
-    def claim_grads(self, keys: List[str]) -> bool:
-        """Before a backward over ``keys``: whether it adds to the gradient arena in place (``True``: eager's ``p.grad += g``)
-        or overwrites it.  It overwrites while no parameter holds a gradient.  Once one does (gradient accumulation), every
-        ``p.grad`` that is not yet its arena view is folded in first -- a missing one as zeros, any other tensor copied -- so
-        that the arena holds every gradient the backward adds to.  After ``publish_grads`` the gradients are live (each
-        ``p.grad`` its arena view) and the next backward accumulates with no extra pass."""
-        if all(self.params[k].grad is None for k in keys):
-            return False
-        with torch.no_grad():
-            for key in keys:
-                p, v = self.params[key], self.view(self.grad, key)
-                if p.grad is None:
-                    ops.fill_f32(v, 0.0)
-                elif p.grad.data_ptr() != v.data_ptr():
-                    v.copy_(p.grad)
-        return True
-
-    def publish_grads(self, keys: List[str]) -> None:
-        """Make each ``p.grad`` of ``keys`` its view of the gradient arena (no copies)."""
-        for key in keys:
-            p = self.params[key]
-            v = self.view(self.grad, key)
-            if p.grad is None or p.grad.data_ptr() != v.data_ptr():
-                p.grad = v
-
-
-def _register_dotted(root: nn.Module, key: str, param: nn.Parameter) -> None:
-    parts = key.split(".")
-    mod = root
-    for name in parts[:-1]:
-        child = mod._modules.get(name)
-        if child is None:
-            child = nn.Module()
-            mod.add_module(name, child)
-        mod = child
-    mod.register_parameter(parts[-1], param)
 
 
 # -----------------------------------------------------------------------------------------------------------------
@@ -286,11 +162,15 @@ class ViTEngine:
     def __init__(self, geo: ViTGeometry, arena: ParamArena):
         self.geo = geo
         self.arena = arena
-        self.reducer = None  # set by dp.attach_reducer / dp.attach_native_reducer
+        self.reducer = None  # set by dp.attach_reducer / dp.attach_native_reducers
         # uint8 [B, S, S, C] inputs: {"division": 255.0, "mean": [...], "std": [...]} = the reference's static_normalize +
         # imagenet / affine normalisation blocks (data/blocks/cv/normalize.py); None: division by 255 only
         self.input_pipeline: Optional[Dict[str, Any]] = None
         self.shrink_next = 0  # SMs to leave free for an in-flight bucket all-reduce when launching the next GEMM (dp.py)
+
+    def buckets(self) -> Dict[Union[int, str], List[List[str]]]:
+        """The gradient exchange's buckets (``ViTGeometry.buckets``): this engine is an exchange site of its model."""
+        return self.geo.buckets()
 
     # ---- stages (also the units of the teacher-forced parity tests, tests/test_taps_gpu.py) --------------------
     def stem_forward(self, x: Tensor) -> Tuple[Optional[Tensor], Tensor]:
@@ -632,7 +512,7 @@ def _check_common(name: str, latent_dim: int, *, default_heads: int, norm_kwargs
     return dict(eps=eps, embedding_norm_eps=emb_eps, activation=fk.get("activation", "GELU"))
 
 
-class _FusedStack(nn.Module):
+class _FusedStack(ArenaModule):
     """What ``ViTEncoderB200`` and ``TeTEncoderB200`` share: parameters in one arena, one engine, one autograd node."""
 
     def _build(self, geo: ViTGeometry, embedding_norm: Optional[nn.Module], defer_head: bool = False) -> None:
@@ -647,7 +527,7 @@ class _FusedStack(nn.Module):
                 p.data.copy_(getattr(embedding_norm, key.rsplit(".", 1)[1]).data)
             params[key] = p
             if not (defer_head and key.startswith("head.linear")):
-                _register_dotted(self, key, p)
+                register_dotted(self, key, p)
         self.geo = geo
         self.arena = ParamArena(spec)
         self.arena.attach(params)
@@ -772,7 +652,7 @@ class TeTEncoderB200(_FusedStack):
         return self._run(net)
 
 
-class VanillaClassifierB200(nn.Module):
+class VanillaClassifierB200(ArenaModule):
     """Drop-in for ``cv_clf`` with ``encoder="vit"`` (cv/classifier/vanilla.py:16-66): ``{"predictions": logits}``.
 
     Module tree and ``state_dict`` layout are the reference's: the encoder is the sub-module ``encoder``
@@ -797,9 +677,8 @@ class VanillaClassifierB200(nn.Module):
         self.img_size = img_size
         self.encoder = ViTEncoderB200(**cfg, _num_classes=num_classes, _defer_head=True)
         for key in ("head.linear.weight", "head.linear.bias"):  # registered after `encoder`: the reference's key order
-            _register_dotted(self, key, self.encoder.arena.params[key])
+            register_dotted(self, key, self.encoder.arena.params[key])
         self.num_classes = num_classes
-        self.last_bad_flag: Optional[Tensor] = None  # int32[1] on the device, written by the loss of the last train_step
         self._bad_host: Optional[Tensor] = None
         self._bad_event: Optional[torch.cuda.Event] = None
         self._register_load_state_dict_pre_hook(self._accept_bare_encoder_keys)

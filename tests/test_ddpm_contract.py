@@ -174,15 +174,15 @@ def test_check_refuses_a_skipped_or_repeated_exchange():
     assert ga._buckets["head"].size == len(dict(bucket_plan(m.unet))["head"]) - 1
 
 
-def test_optimizers_and_dp_accept_the_module():
+def test_optimizers_and_dp_accept_the_module_through_its_grad_arena():
     m, _ = _ddpm("unet_small64_state_dict_keys.json")
     opt = ArenaAdamW(m, lr=1e-4)
     assert opt.weight_decay == 0.01 and opt.decoupled and not ArenaAdam.decoupled
     assert opt.arenas() == [m.arena]
     dp.detach_reducers(m)
-    assert m.engine.reducer is None
+    assert m.grad_arena.reducer is None
     with dp.no_sync(m):
-        assert m.engine.reducer is None
+        assert m.grad_arena.reducer is None
 
 
 # ---- the three entries' argument contracts ----------------------------------------------------------------------------------------------
@@ -243,8 +243,8 @@ def _worker(rank, world, port, q):
         torch.manual_seed(rank)  # different replicas until the broadcast
         m, _ = _ddpm("unet_small64_state_dict_keys.json")
         dp.broadcast_parameters(m)
-        red = dp.GradBucketReducer(m.arena, m.geo.buckets())
-        m.engine.reducer = red
+        red = dp.GradBucketReducer(m.arena, m.grad_arena.buckets())
+        m.grad_arena.reducer = red
         # every parameter's gradient as its backward would leave it: rank r writes (r + 1) x its flat index, bucket by bucket
         idx = torch.arange(m.arena.total, dtype=torch.float32)
         for name, keys in bucket_plan(m.unet):
@@ -257,7 +257,7 @@ def _worker(rank, world, port, q):
         dist.destroy_process_group()
 
 
-def test_world2_gloo_unet_buckets_average_the_arena():
+def test_world2_gloo_grad_arena_buckets_average_the_arena():
     world, port = 2, 29581
     ctx = mp.get_context("spawn")
     q = ctx.Queue()

@@ -13,7 +13,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 import cflearn_b200  # noqa: F401,E402
-from cflearn_b200 import dp, vit  # noqa: E402
+from cflearn_b200 import dp  # noqa: E402
+from cflearn_b200.arena import ParamArena  # noqa: E402
 from cflearn_b200.optim import GraphedTrainStep  # noqa: E402
 from cflearn_b200.trainer import B200TrainStep  # noqa: E402
 
@@ -23,35 +24,36 @@ class _Comm:
     ctas = 0
 
 
-class _Geo:
+class _Site:
+    """An exchange site: its arena, its buckets and the reducer ``dp`` puts on it."""
+
+    reducer = None
+    shrink_next = 0
+
+    def __init__(self):
+        self.arena = ParamArena([("w", (4,))])
+        self.arena.attach({"w": torch.nn.Parameter(torch.zeros(4))})
+
     def buckets(self):
         return {"stem": [["w"]]}
 
 
-class _Engine:
-    reducer = None
-    shrink_next = 0
-
-
-class _Tower:
-    def __init__(self):
-        self.arena = vit.ParamArena([("w", (4,))])
-        self.arena.attach({"w": torch.nn.Parameter(torch.zeros(4))})
-        self.geo, self.engine = _Geo(), _Engine()
-
-
 class _Model:
-    """CLIP-shaped: a tower whose backward runs the bucket reducer, and loose parameters all-reduced through ``comm``."""
+    """CLIP-shaped: an exchange site whose backward runs the bucket reducer, and loose parameters all-reduced through
+    ``comm``."""
 
     def __init__(self, log):
-        self.log, self.tower, self.comm = log, _Tower(), None
+        self.log, self.site, self.comm = log, _Site(), None
 
-    def towers(self):
-        return [self.tower]
+    def arenas(self):
+        return [self.site.arena]
+
+    def exchanges(self):
+        return [self.site]
 
     def train_step(self, x):
         self.log.append(("backward", int(x)))
-        if self.tower.engine.reducer is not None:
+        if self.site.reducer is not None:
             self.log.append(("bucket_exchange", int(x)))
         if self.comm is not None:
             self.log.append(("glue_exchange", int(x)))
@@ -105,7 +107,7 @@ def _calls_of(log):
     return out
 
 
-def test_k3_updates_clips_schedules_and_exchanges_on_every_third_micro_batch():
+def test_k3_updates_clips_schedules_and_exchanges_every_site_on_every_third_micro_batch():
     log, updated, model = _run(3, 10, comm=_Comm())
     calls = _calls_of(log)
     assert [i for i, u in enumerate(updated, 1) if u] == [3, 6, 9]
@@ -119,10 +121,10 @@ def test_k3_updates_clips_schedules_and_exchanges_on_every_third_micro_batch():
         if update:
             assert c == ["backward", "bucket_exchange", "glue_exchange", "clip", "step", "sched"], c
     # the exchange is switched off only for the micro-steps: the reducer and the communicator are back afterwards
-    assert model.tower.engine.reducer is not None and model.comm is not None
+    assert model.site.reducer is not None and model.comm is not None
 
 
-def test_k1_is_one_update_per_call():
+def test_k1_is_one_update_per_call_with_exchange_sites():
     log, updated, _ = _run(1, 3)
     assert updated == [True, True, True]
     calls = _calls_of(log)
@@ -132,15 +134,15 @@ def test_k1_is_one_update_per_call():
     assert _calls_of(log)[2] == ["zero_grad", "backward", "bucket_exchange", "glue_exchange", "clip", "step", "sched"]
 
 
-def test_no_sync_restores_the_exchange_after_an_error():
+def test_no_sync_restores_every_exchange_site_after_an_error():
     model = _Model([])
     dp.attach_native_reducers(model, _Comm())
-    red, comm = model.tower.engine.reducer, model.comm
+    red, comm = model.site.reducer, model.comm
     with pytest.raises(RuntimeError):
         with dp.no_sync(model):
-            assert model.tower.engine.reducer is None and model.comm is None
+            assert model.site.reducer is None and model.comm is None
             raise RuntimeError("backward failed")
-    assert model.tower.engine.reducer is red and model.comm is comm
+    assert model.site.reducer is red and model.comm is comm
 
 
 @pytest.mark.parametrize("K", [0, -1])

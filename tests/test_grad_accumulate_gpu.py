@@ -67,13 +67,9 @@ def case(name, batch, n):
     return make, [tuple(t.to(DEV) for t in b) for b in batches]
 
 
-def arenas(m):
-    return list(m.arenas()) if hasattr(m, "arenas") else [m.arena]
-
-
 def assert_sum(m, expected):
     """Every arena equals ``expected`` exactly, but CLIP's token embedding (fp32 atomics: see the module docstring)."""
-    for a, want in zip(arenas(m), expected):
+    for a, want in zip(m.arenas(), expected):
         if "token_embedding.weight" not in a.params:
             assert torch.equal(a.grad, want), (a.grad - want).abs().max().item()
             continue
@@ -93,14 +89,14 @@ def test_accumulated_arena_is_the_fp32_sum_of_fresh_backwards(name):
     for b in batches:
         m.zero_grad(set_to_none=True)  # an overwriting backward
         m.train_step(*b)
-        fresh.append([a.grad.clone() for a in arenas(m)])
+        fresh.append([a.grad.clone() for a in m.arenas()])
     expected = [(g1 + g2) + g3 for g1, g2, g3 in zip(*fresh)]
     m.zero_grad(set_to_none=True)
     for b in batches:  # the first overwrites, the next two add in place
         m.train_step(*b)
     torch.cuda.synchronize()
     assert_sum(m, expected)
-    for a in arenas(m):
+    for a in m.arenas():
         assert all(p.grad.data_ptr() == a.g(k).data_ptr() for k, p in a.params.items())
     # the graphed seam over one window: the arenas are zeroed, the three micro-steps add, the closing one also steps Adam
     # (which reads the gradients but leaves them in place)

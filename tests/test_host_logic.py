@@ -198,7 +198,7 @@ def _worker(rank, world, port, total, q):
     with torch.no_grad():
         m.arena.flat.add_(rank)  # replicas differ until the broadcast
     dp.broadcast_parameters(m, src=0)
-    red = dp.attach_reducer(m)
+    (red,) = dp.attach_reducer(m)
     g = m.arena.grad
     g.copy_(torch.arange(g.numel(), dtype=torch.float32) * (rank + 1))
     # the engine signals buckets in backward order: tail, blocks L-1..0, stem
@@ -210,7 +210,7 @@ def _worker(rank, world, port, total, q):
     dist.destroy_process_group()
 
 
-def test_world2_gloo_bucket_allreduce_matches_mean():
+def test_world2_gloo_attached_reducers_average_to_the_mean():
     world, port = 2, 29577
     ctx = mp.get_context("spawn")
     q = ctx.Queue()

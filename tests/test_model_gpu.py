@@ -552,6 +552,33 @@ def test_trainer_seam_matches_reference_update_sequence():
         assert torch.allclose(pa, pe, rtol=1e-5, atol=1e-7), k  # and the lock-step run IS the eager run of (a)
 
 
+def test_graphed_step_without_clipping_ignores_an_earlier_clipping_step():
+    """A graphed ``B200TrainStep(clip_norm=0)`` on a model and optimizer that a clipping graphed step was built on before does
+    not clip: its parameters equal, bit for bit, those of the same run on a fresh model and optimizer."""
+    from cflearn_b200.optim import ArenaAdam
+    from cflearn_b200.trainer import B200TrainStep
+
+    cfg = vo.vit_config("vit_tiny")
+    sd = vo.init_state_dict(cfg, seed=0)
+    batches = [vo.synthetic_batch(cfg, 4, seed=20 + i) for i in range(3)]
+
+    def run_unclipped(m, opt):
+        step = B200TrainStep(m, opt, clip_norm=0.0, graph=True, batch=4)
+        for x, y in batches:
+            step.step(x.to(DEV), y.to(DEV))
+        torch.cuda.synchronize()
+        step.close()
+
+    m = build(cfg, sd)
+    opt = ArenaAdam(m, lr=1e-3, capturable=True)
+    B200TrainStep(m, opt, clip_norm=0.05, graph=True, batch=4).close()  # its warm-up clips, then restores the state
+    run_unclipped(m, opt)
+    fresh = build(cfg, sd)
+    run_unclipped(fresh, ArenaAdam(fresh, lr=1e-3, capturable=True))
+    for (k, p), (_, q) in zip(m.named_parameters(), fresh.named_parameters()):
+        assert torch.equal(p, q), k
+
+
 @pytest.mark.parametrize("B,H,W,Cin,Cout", [(2, 64, 64, 320, 320), (2, 16, 16, 640, 1280)])
 def test_unet_res_block_forward_matches_oracle(B, H, W, Cin, Cout):
     """SURVEY.md N3, first composed block: ResidualBlockWithTimeEmbedding forward on the native kernels (GroupNorm+SiLU, 3x3

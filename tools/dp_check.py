@@ -66,7 +66,7 @@ def main():
         m = build(cfg, sd, dev)
         dp.broadcast_parameters(m)
         if mode == "eager" and K == 1:
-            dp.attach_native_reducer(m, comm)
+            dp.attach_native_reducers(m, comm)
             m.train_step(xs, ys)
         elif mode == "eager":
             seam = B200TrainStep(m, ArenaAdam(m, lr=0.0), comm=comm, grad_accumulate=K)
@@ -86,7 +86,7 @@ def main():
         assert torch.equal(ref, g_dp), f"{mode}: ranks disagree after the all-reduce"
         if rank == 0:
             results[mode] = ((g_dp - g_one).norm() / g_one.norm()).item()
-        m.engine.reducer = None
+        dp.detach_reducers(m)
         if mode != "eager":
             gs.release()  # (ncclCommDestroy below waits for every graph that captured the communicator)
         del m

@@ -86,7 +86,7 @@ def main():
         assert torch.equal(ref, g_dp), f"{mode}: ranks disagree after the all-reduce"
         if rank == 0:
             results[mode] = ((g_dp - g_one).norm() / g_one.norm()).item()
-        m.engine.reducer = None
+        dp.detach_reducers(m)
         if gs is not None:
             gs.release()  # (ncclCommDestroy below waits for every graph that captured the communicator)
         del m
